@@ -2,7 +2,7 @@
 """Headline benchmark of the dense-retrieval hot path (BASELINE.json):
 
   metric  : queries/sec, top-1000 over an 8.8M x 768 corpus (configs[1]: bert-base 768-d, 6 980 queries,
-            brute force on 1 x B200); with --gpus N the same corpus is row-sharded over N GPUs and searched through
+            brute force on 1 x H100); with --gpus N the same corpus is row-sharded over N GPUs and searched through
             om_index_search_sharded (collectives inside the library, NCCL over NVLink) -> strong scaling.
   also    : passages encoded/sec (bert-base / t5-base / bert-large, L=128, batch 256 per GPU), the contrastive loss,
             the C4 train step, the C5-sized shard (2.625 M x 1024), the streaming regime, and the eager-PyTorch GPU
@@ -12,6 +12,7 @@
   python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
   python bench.py --impl reference ...      # CPU arm: faiss if importable, else the oracle port, on a bounded sample
   python bench.py --workload c5 --gpus 8    # configs[4]: 21 M x 1024 row-sharded 8-way (2.625 M rows per GPU)
+  python bench.py ... --dump-outputs DIR    # also write the last timed step's (D, I) for a fixed query sample as .npy
 
 A step = one search of the whole query batch against the HBM-resident corpus (value: inputs resident in HBM;
 e2e: host fp32 queries in, host (D, I) out, copies inside the timed region).  Synthetic data: corpus and
@@ -39,6 +40,28 @@ WORKLOADS = {
 }
 
 
+DUMP_QUERIES = 2048         # (D, I) rows written by --dump-outputs: 2048 x 1000 x (4 + 8) B = 24.6 MB at k = 1000
+DUMP_BYTES = 60 * 2 ** 20   # ... and never more than this (D + I of the sample; the row list adds <= 16 KB): <= 64 MB
+
+
+def dump_rows(nq, k):
+    """Query rows in the --dump-outputs sample: DUMP_QUERIES, fewer when 12 * k bytes per row would exceed DUMP_BYTES."""
+    return max(1, min(nq, DUMP_QUERIES, DUMP_BYTES // (12 * k)))
+
+
+def dump_outputs(out_dir, D, I, nq, seed=20240917):
+    """D [nq, k] fp32 and I [nq, k] int64 (device tensors) -> out_dir/{search_D,search_I,query_rows}.npy for a seeded,
+    sorted sample of dump_rows(nq, k) query rows; ids are stored as float64 (exact below 2**53)."""
+    import numpy as np
+    import torch
+    rows = np.sort(np.random.default_rng(seed).permutation(nq)[:dump_rows(nq, D.shape[1])])
+    sel = torch.from_numpy(rows).to(D.device)
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "search_D.npy"), D.index_select(0, sel).cpu().numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "search_I.npy"), I.index_select(0, sel).cpu().numpy().astype(np.float64))
+    np.save(os.path.join(out_dir, "query_rows.npy"), rows.astype(np.float64))
+
+
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -56,6 +79,10 @@ def parse_args():
     ap.add_argument("--skip-train", action="store_true")
     ap.add_argument("--skip-eager", action="store_true")
     ap.add_argument("--skip-parity", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's search result (D float32, I as float64) for a fixed, "
+                         "seeded sample of up to %d queries (fewer for large k: at most %d MB) to DIR/*.npy"
+                         % (DUMP_QUERIES, DUMP_BYTES >> 20))
     args = ap.parse_args()
     w = WORKLOADS[args.workload]
     args.corpus = args.corpus or w["corpus"]
@@ -71,7 +98,8 @@ def measured_peaks():
         return {"tflops": float(p.get("bf16_tflops_sustained", p.get("bf16_tflops", 1400.0))), "hbm": float(p["hbm_gbs"]),
                 "burst": float(p.get("bf16_tflops", 0.0)) or None,
                 "source": "MEASURED_PEAKS.json bf16_tflops_sustained (of measured)"}
-    return {"tflops": 1400.0, "hbm": 6650.0, "burst": None, "source": "B200_PROFILING.md fallback (of fallback)"}
+    return {"tflops": 989.0, "hbm": 3350.0, "burst": None,
+            "source": "H100 SXM data-sheet peaks (dense BF16, HBM3 at 700 W), not measured"}
 
 
 class ClockSampler:
@@ -272,6 +300,7 @@ def main():
 
     def fill_index(d, lo, hi, seed_base):
         idx_ = FlatIPIndex(d)
+        idx_.reserve_rows(hi - lo)  # size the shard once: growing it chunk by chunk would need old + new copies at once
         chunk = 550_000
         for c0 in range(lo, hi, chunk):
             n = min(chunk, hi - c0)
@@ -346,6 +375,8 @@ def main():
     idx.set_param("profile", 0)
     ms_per_step = total_ms / args.steps
     qps = nq / (ms_per_step * 1e-3)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["D"], last["I"], nq)
 
     e2e_ms = timed(e2e_step, args.steps, min(args.warmup, 2)) / args.steps
     e2e_qps = nq / (e2e_ms * 1e-3)
@@ -368,7 +399,7 @@ def main():
             sweep_bytes = (hi - lo) * d * 2.0
             for snq in (1, 16, 64):
                 qs = q_dev[:snq].contiguous()
-                sms_ = timed(lambda: idx.search_device(qs, 100), 10, 3) / 10
+                sms_ = timed(lambda: idx.search_device(qs, 100), args.steps, 3) / args.steps
                 case = {"ms": sms_, "queries_per_s": world * snq / (sms_ * 1e-3), "achieved_gbs": sweep_bytes / (sms_ * 1e-3) / 1e9}
                 case["frac_of_hbm_peak"] = case["achieved_gbs"] / peaks["hbm"]
                 streaming["cases"]["nq=%d" % snq] = case
@@ -379,7 +410,7 @@ def main():
     eager = {}
     if not args.skip_eager and not args.skip_encode:
         try:
-            eager["search"] = eager_search(torch, idx, q_dev, k, hi - lo, total_rows, timed)
+            eager["search"] = eager_search(torch, idx, q_dev, k, hi - lo, total_rows, timed, args.steps)
         except Exception as e:
             eager["search"] = {"error": "%s: %s" % (type(e).__name__, e)}
 
@@ -391,12 +422,12 @@ def main():
     encode = loss_obj = train_obj = c5_obj = None
     if not args.skip_encode:
         encode = encoder_legs(torch, synthetic, CudaEncoder, args, timed, world, rank, dev, peaks, eager if not args.skip_eager else None)
-        loss_obj = loss_leg(torch, timed, dev, eager if not args.skip_eager else None)
+        loss_obj = loss_leg(torch, timed, dev, eager if not args.skip_eager else None, args.steps)
         if not args.skip_train:
-            train_obj = train_leg(torch, synthetic, timed, world, rank, dev)
+            train_obj = train_leg(torch, synthetic, timed, world, rank, dev, args.steps)
         if args.workload == "c2" and world == 1:
             try:
-                c5_obj = c5_shard_leg(torch, fill_index, timed, nq, k, dev, peaks)
+                c5_obj = c5_shard_leg(torch, fill_index, timed, nq, k, dev, peaks, args.steps)
             except Exception as e:
                 c5_obj = {"error": "%s: %s" % (type(e).__name__, e)}
 
@@ -409,14 +440,6 @@ def main():
     scan_s = acc["scan_ns"] * 1e-9
     achieved = scan_flops / scan_s / 1e12 if scan_s > 0 else None
     traffic = traffic_note = None
-    tpath = os.path.join(ROOT, "profiles", "scan_traffic.json")
-    if os.path.exists(tpath) and world == 1 and args.workload == "c2":
-        with open(tpath) as f:
-            tj = json.load(f)
-        traffic = tj.get("dram_bytes_per_launch")
-        traffic_note = "%s: %.3g B DRAM vs %.3g B algorithmic (x%.3f); %s (constant from that ncu capture, not measured in this run)" % (
-            tj.get("launch"), traffic, tj.get("algorithmic_bytes_per_launch"), tj.get("ratio_traffic_over_algorithmic"),
-            tj.get("source"))
     phase = {p: acc[p + "_ns"] / 1e6 / args.steps for p in ("scan", "select", "finalize", "other")}
     line = {
         "metric": wl["metric"], "value": qps, "unit": "queries/s", "n_gpus": world,
@@ -424,7 +447,7 @@ def main():
         "scaling": wl["scaling"], "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": "%s: top-%d over %d x %d fp32 corpus resident in HBM, %d queries per step"
                                % (wl["name"], k, total_rows, d, nq), "corpus_rows": total_rows, "rows_per_gpu": n_local, "dim": d,
-                   "k": k, "nq": nq, "candidate_stage": "fp16 tensor-core scan on CTA pairs (tcgen05 cta_group::2, fp32 accumulate) + fp32 re-score + exactness "
+                   "k": k, "nq": nq, "candidate_stage": "fp16 tensor-core scan on 2-CTA clusters (wgmma, fp32 accumulate, corpus tiles multicast) + fp32 re-score + exactness "
                    "certificate (escalation: 4096-wide list, then exact fp32 scan)", "rounds": rounds,
                    "parallelism": ("index row-sharded x%d, om_index_search_sharded: shard-sized candidate lists, ONE packed NCCL "
                                    "all-gather per query chunk (scores | ids | floors | error norms), merge + certificate on "
@@ -437,7 +460,7 @@ def main():
         "roofline": {"bound": "tensor", "achieved": achieved, "peak": peaks["tflops"], "unit": "TFLOP/s",
                      "frac": achieved / peaks["tflops"] if achieved else None, "traffic": traffic,
                      "traffic_note": traffic_note, "frac_of_burst_peak": achieved / peaks["burst"] if achieved and peaks["burst"] else None,
-                     "kernel": "gemm2_tn_kernel<5,1,8,EpiScan,F16> (CTA pairs, cta_group::2; fused Q*X^T + top-k filter)",
+                     "kernel": "gemm_bf16_tn_kernel<128,3,M_FASTEST,EpiScan,F16,CLUSTER=2> (wgmma; fused Q*X^T + top-k filter)",
                      "note": "2*nq*rows*d FLOPs per sweep / CUDA-event time of the scan launches on the launching "
                              "stream; " + peaks["source"],
                      "phase_ms_per_step": {"scan": phase["scan"], "select": phase["select"], "finalize_rescore": phase["finalize"],
@@ -544,7 +567,7 @@ def check_search_parity(torch, dist, idx, comm, q_dev, D, I, k, lo, rank, world,
     return out
 
 
-def eager_search(torch, idx, q_dev, k, n_local, total_rows, timed):
+def eager_search(torch, idx, q_dev, k, n_local, total_rows, timed, steps):
     """Chunked torch.matmul + topk over a bounded slice of the fp32 master rows (TF32 on = what a PyTorch user gets
     with torch.set_float32_matmul_precision('high')), extrapolated linearly in rows."""
     x = idx.master_rows()
@@ -567,7 +590,7 @@ def eager_search(torch, idx, q_dev, k, n_local, total_rows, timed):
         return best_s, best_i
 
     try:
-        ms = timed(step, 2, 1) / 2
+        ms = timed(step, steps, 1) / steps
     finally:
         torch.backends.cuda.matmul.allow_tf32 = prev
     full_ms = ms * (total_rows / rows)
@@ -581,7 +604,7 @@ def eager_search(torch, idx, q_dev, k, n_local, total_rows, timed):
 # ------------------------------------------------------------------------------------------------------------------
 def encoder_legs(torch, synthetic, CudaEncoder, args, timed, world, rank, dev, peaks, eager):
     B, L = args.encode_batch, 128
-    steps = max(args.steps, 5)
+    steps = args.steps
 
     def flops(spec):
         H = spec["hidden"]
@@ -687,9 +710,9 @@ def timed_local(torch, fn, steps, warmup):
     return e0.elapsed_time(e1) / steps
 
 
-def loss_leg(torch, timed, dev, eager):
+def loss_leg(torch, timed, dev, eager, steps):
     """contrastive loss fwd+bwd (C4): local negatives [64, 768] x [512, 768] and the cross-device-at-8 shape
-    [512, 768] x [4096, 768]; one cooperative tcgen05 kernel per call (latency-bound: reported in microseconds)"""
+    [512, 768] x [4096, 768]; one cooperative wgmma kernel per call (latency-bound: reported in microseconds)"""
     from openmatch_b200 import _lib as om_lib
     lib = om_lib.load()
     loss_obj = {"metric": "contrastive loss fwd+bwd latency", "unit": "us", "kernel_launches_per_call": 1, "shapes": {}}
@@ -707,7 +730,7 @@ def loss_leg(torch, timed, dev, eager):
                     xq.data_ptr(), xp.data_ptr(), om_lib.OM_BF16, bq, bp, 768, None, om_lib.OM_REDUCE_MEAN, 1.0,
                     lo_t.data_ptr(), dxq.data_ptr(), dxp.data_ptr(), None, om_lib.current_stream_ptr()))
 
-        us = timed(loss_step, 3, 3) / 3 / reps * 1e3
+        us = timed(loss_step, steps, 3) / steps / reps * 1e3
         import ctypes
         ph = (ctypes.c_uint64 * 4)()
         om_lib.check(lib.om_debug_loss_phase_ns(ph))
@@ -724,12 +747,12 @@ def loss_leg(torch, timed, dev, eager):
                     s = a @ b.T
                     torch.nn.functional.cross_entropy(s.float(), tgt).backward()
 
-            eus = timed_local(torch, eager_step, 3, 3) / reps * 1e3
+            eus = timed_local(torch, eager_step, steps, 3) / reps * 1e3
             eager.setdefault("loss", {})[name] = {"us": eus, "what": "bf16 matmul + F.cross_entropy(fp32) + autograd backward (eager)"}
     return loss_obj
 
 
-def train_leg(torch, synthetic, timed, world, rank, dev):
+def train_leg(torch, synthetic, timed, world, rank, dev, steps):
     """contrastive training step (C4): bert-base, 64 queries (L=32) x 8 passages (L=128) per GPU, bf16 autocast.
     Encoder forward/backward = the HF torch module under autograd (our encoder kernels are forward-only, DESIGN
     section 6); loss forward+backward = loss_fused_kernel; AdamW step included; DDP all-reduce when world > 1; with
@@ -760,7 +783,7 @@ def train_leg(torch, synthetic, timed, world, rank, dev):
                 opt.step()
                 opt.zero_grad(set_to_none=True)
 
-            tr_ms = timed(train_step, 5, 3) / 5
+            tr_ms = timed(train_step, steps, 3) / steps
             obj = {"value": world * 64 / (tr_ms * 1e-3), "unit": "queries/s", "ms_per_step": tr_ms,
                    "tflops_per_gpu": flop / (tr_ms * 1e-3) / 1e12}
             if not xdev:
@@ -776,7 +799,7 @@ def train_leg(torch, synthetic, timed, world, rank, dev):
         return {"error": "%s: %s" % (type(e).__name__, e)}
 
 
-def c5_shard_leg(torch, fill_index, timed, nq, k, dev, peaks):
+def c5_shard_leg(torch, fill_index, timed, nq, k, dev, peaks, steps):
     """One C5 shard on this GPU: 2.625 M x 1024 (= 21 M / 8), 6 980 queries, top-1000 (configs[4] per-GPU work;
     `bench.py --workload c5 --gpus 8` runs the whole 21 M corpus)."""
     n, d = 2_625_000, 1024
@@ -796,12 +819,12 @@ def c5_shard_leg(torch, fill_index, timed, nq, k, dev, peaks):
 
     for _ in range(2):
         idx.search_device(q, k, out=out)
-    ms = timed(step, 3, 0) / 3
-    ach = 2.0 * nq * n * d * 3 / (scan_ns * 1e-9) / 1e12
+    ms = timed(step, steps, 0) / steps
+    ach = 2.0 * nq * n * d * steps / (scan_ns * 1e-9) / 1e12
     out = {"rows": n, "dim": d, "nq": nq, "k": k, "ms_per_step": ms, "queries_per_s": nq / (ms * 1e-3),
            "roofline": {"bound": "tensor", "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"],
-                        "scan_ms_per_step": scan_ns / 1e6 / 3},
-           "uncertified_queries_per_step": unc / 3,
+                        "scan_ms_per_step": scan_ns / 1e6 / steps},
+           "uncertified_queries_per_step": unc / steps,
            "ceiling_note": "compute ceiling for 21M x 1024 on 8 GPUs at this per-shard time: %.0f queries/s" % (nq / (ms * 1e-3))}
     del idx
     torch.cuda.empty_cache()

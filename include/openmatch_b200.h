@@ -1,4 +1,4 @@
-/* openmatch_b200 — C ABI of the B200-native dense-retrieval hot path (libopenmatch_b200.so).
+/* openmatch_b200 — C ABI of the H100-native dense-retrieval hot path (libopenmatch_b200.so).
  *
  * The reference (thunlp/OpenMatch, 100 % Python) has no FFI layer; the seams where its hot path crosses
  * into third-party compute are three Python call sites, and each entry point below replaces one of them
@@ -18,7 +18,7 @@
  * passes raw pointers (host or device as stated) plus a CUDA stream handle (cudaStream_t cast to void*,
  * NULL = legacy default stream); the library owns only its opaque handles.  One process drives one GPU;
  * a handle is not thread-safe, distinct handles are.  There is no CPU fallback: every compute entry
- * point fails with OM_ENODEVICE when no sm_100 device is present.
+ * point fails with OM_ENODEVICE when no sm_90 device is present.
  */
 #ifndef OPENMATCH_B200_H_
 #define OPENMATCH_B200_H_
@@ -160,7 +160,7 @@ int om_search_floor_bins(void);
  * "certify" (default 1; 0 = skip the exactness certificate and its escalation: top-k of the fp16 candidate stage),
  * "exact_only" (1 = answer every query with the exact fp32 CUDA-core scan; testing),
  * "debug_stage_scores" (1 = D holds candidate-stage scores instead of fp32 re-scores; error-model measurement),
- * "pair_scan" (default 1: the scan GEMM runs on CTA pairs, tcgen05 cta_group::2; 0 = single-CTA tiles),
+ * "pair_scan" (default 1: the scan GEMM runs on 2-CTA clusters sharing each corpus tile; 0 = single-CTA tiles),
  * "profile" (1 = bracket every kernel launch of a search with CUDA events on the launching stream). */
 int om_index_set_param(om_index* idx, const char* name, int64_t value);
 /* Statistics of the last search: "rounds", "overflow_retries", "candidates" (per query capacity),

@@ -1,5 +1,5 @@
 """Drop-in alias: ``import openmatch`` / ``python -m openmatch.driver.build_index`` resolve to the
-B200-native implementation in ``openmatch_b200`` (same module, class and function names as
+H100-native (sm_90a) implementation in ``openmatch_b200`` (same module, class and function names as
 thunlp/OpenMatch's ``src/openmatch`` for the dense-retrieval hot path)."""
 import importlib
 import sys

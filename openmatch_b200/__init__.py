@@ -1,4 +1,4 @@
-"""openmatch_b200 — B200-native (sm_100a) dense-retrieval hot path behind OpenMatch's own entry points.
+"""openmatch_b200 — H100-native (sm_90a) dense-retrieval hot path behind OpenMatch's own entry points.
 
 Host side mirrors the reference package layout (``modeling``, ``retriever``, ``loss``, ``driver``,
 ``arguments``, ``utils``); the three hot steps run in hand-written CUDA behind the C ABI declared in

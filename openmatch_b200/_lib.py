@@ -1,7 +1,7 @@
 """ctypes binding of libopenmatch_b200.so (C ABI declared in include/openmatch_b200.h).
 
 There is no CPU fallback: if the shared library is missing this module raises at import of the symbol
-table, and every compute entry point raises RuntimeError when no sm_100 device is present.
+table, and every compute entry point raises RuntimeError when no sm_90 device is present.
 """
 from __future__ import annotations
 

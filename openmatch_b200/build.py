@@ -1,4 +1,4 @@
-"""In-tree build of libopenmatch_b200.so (nvcc, sm_100a only).  `python -m openmatch_b200.build [--force]`.
+"""In-tree build of libopenmatch_b200.so (nvcc, sm_90a only).  `python -m openmatch_b200.build [--force]`.
 
 The library is pure CUDA C++ behind a C ABI (include/openmatch_b200.h); PyTorch is not involved in the
 build.  Objects are compiled in parallel, one translation unit per hot-path step.
@@ -17,7 +17,8 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libopenmatch_b200.so")
 OBJ_DIR = os.path.join(os.path.dirname(HERE), "build", "obj")
 SOURCES = ["api.cu", "search.cu", "encoder.cu", "loss.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 
 def _nvcc() -> str:
@@ -58,7 +59,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if force or _stale(LIB_PATH, objs):
         # link next to the target and rename: the library in the tree is always complete (it ships with repo snapshots)
         tmp = LIB_PATH + ".tmp.%d" % os.getpid()
-        cmd = [nvcc, "-shared", "-o", tmp] + objs + ["-gencode", "arch=compute_100a,code=sm_100a"]
+        cmd = [nvcc, "-shared", "-o", tmp] + objs + ARCH
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s\n%s" % (r.stdout, r.stderr))

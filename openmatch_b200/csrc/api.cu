@@ -29,8 +29,8 @@ int device_sm_count() {
     cudaGetLastError();
     return fail(OM_ENODEVICE, "cudaGetDeviceProperties failed: %s", cudaGetErrorString(e));
   }
-  if (p.major != 10)
-    return fail(OM_ENODEVICE, "device %d is sm_%d%d; libopenmatch_b200 is built for sm_100a (B200) only", dev, p.major,
+  if (p.major != 9 || p.minor != 0)
+    return fail(OM_ENODEVICE, "device %d is sm_%d%d; libopenmatch_b200 is built for sm_90a (H100) only", dev, p.major,
                 p.minor);
   cached_dev = dev;
   cached_sms = p.multiProcessorCount;

@@ -37,7 +37,7 @@ static inline int fail(int code, const char* fmt, ...) {
     if (rc__ < 0) return rc__;  \
   } while (0)
 
-// Number of SMs of the current device (cached); negative OM_E* when no usable sm_100 device exists.
+// Number of SMs of the current device (cached); negative OM_E* when no usable sm_90 device exists.
 int device_sm_count();
 
 static inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }

@@ -1,4 +1,4 @@
-// B200-native encoder forward behind DRModel.encode (src/openmatch/modeling/dense_retrieval_model.py:133-155):
+// H100-native encoder forward behind DRModel.encode (src/openmatch/modeling/dense_retrieval_model.py:133-155):
 // HF BertModel (post-LN, GELU-erf) or T5EncoderModel (pre-RMSNorm, ReLU, shared relative position bias)
 // -> 'first' / 'mean' pooling (:145-150, src/openmatch/utils.py:233-235) -> bias-free LinearHead
 // (src/openmatch/modeling/linear.py:19,22-23) -> F.normalize (:153-154).
@@ -9,15 +9,15 @@
 //        LN(s) W^T = rstd * (s Wf^T) + (W beta + b),   Wf = W diag(gamma) with every row centred (sum_i Wf[j, i] = 0,
 //        which makes the "- rstd * mean * rowsum" term vanish; RMSNorm has no mean, rows stay as they are),
 // and into the residual read of the GEMM that produces the next s:
-//   QKV    tcgen05 GEMM [T,H]x[3I,H]^T on bf16(s) and the folded weights; epilogue: rstd[row] * acc + folded bias
+//   QKV    wgmma GEMM [T,H]x[3I,H]^T on bf16(s) and the folded weights; epilogue: rstd[row] * acc + folded bias
 //          -> bf16 Q|K [T,2I] and V transposed [I, T]
-//   ATTN   one CTA per (128-row tile, head): S = Q K^T (tcgen05, TMEM) -> masked softmax in registers
-//          (thread = query row) -> P (bf16, 128B-swizzled smem) -> O = P V (tcgen05) -> ctx bf16 [T,I]
-//   OPROJ  tcgen05 GEMM [T,I]x[H,I]^T, epilogue (EpiResidNorm): s' = acc + bias + LN(s) (BERT) / + s (T5), written in
+//   ATTN   one CTA per (128-row tile, head), one warpgroup, 64 query rows at a time: S = Q K^T (wgmma, registers) ->
+//          masked softmax on the accumulator fragments -> P (bf16, registers) -> O = P V (wgmma) -> ctx bf16 [T,I]
+//   OPROJ  wgmma GEMM [T,I]x[H,I]^T, epilogue (EpiResidNorm): s' = acc + bias + LN(s) (BERT) / + s (T5), written in
 //          place as fp32 (TMA load + TMA store of the residual tile) and as bf16, row statistics of s' accumulated
-//   FFN1   tcgen05 GEMM [T,H]x[F,H]^T on bf16(s') and folded weights; epilogue: rstd[row] * acc + folded bias, GELU(erf) /
+//   FFN1   wgmma GEMM [T,H]x[F,H]^T on bf16(s') and folded weights; epilogue: rstd[row] * acc + folded bias, GELU(erf) /
 //          ReLU -> bf16 [T,F]
-//   FFN2   tcgen05 GEMM [T,F]x[H,F]^T, epilogue (EpiResidNorm) like OPROJ -> next layer's s
+//   FFN2   wgmma GEMM [T,F]x[H,F]^T, epilogue (EpiResidNorm) like OPROJ -> next layer's s
 // One norm kernel runs after the last layer (last_hidden_state for pooling).  Activations feeding tensor cores are
 // bf16; the residual stream, normalisation statistics, softmax, pooling, head and L2-normalisation are fp32.
 #include <math.h>
@@ -30,7 +30,6 @@
 
 #include "common.h"
 #include "gemm.cuh"
-#include "gemm2sm.cuh"
 
 namespace om {
 
@@ -42,11 +41,10 @@ constexpr float kLog2e = 1.4426950408889634f;
 // ===================================================================================================
 // GEMM epilogues
 // ===================================================================================================
-// GELU(x) = x/2 (1 + erf(x / sqrt 2)) for two elements per instruction (FFMA2): the FFN1 epilogue is ISSUE-bound
-// (with erff() / a 13-term rational it needed more issue cycles per tile than the tensor cores need for the
-// tile's MMAs), so erf is the cheapest approximation that is invisible after bf16 rounding of the output:
+// GELU(x) = x/2 (1 + erf(x / sqrt 2)) for an element pair: the FFN1 epilogue is issue-bound, so erf is the cheapest
+// approximation that is invisible after bf16 rounding of the output:
 // z P(z^2) / Q(z^2) on [-4, 4], P cubic, Q cubic with Q >= 1, fitted against math.erf: max |err| 2.1e-5
-// (bf16 output rounding is 2e-3 relative); 6 FFMA2 + 1 MUFU.RCP per element pair half.
+// (bf16 output rounding is 2e-3 relative); 6 FFMA + 1 MUFU.RCP per element.
 __device__ __forceinline__ float rcp_approx(float x) {
   float y;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -74,7 +72,7 @@ enum { ACT_NONE = 0, ACT_GELU = 1, ACT_RELU = 2 };
 // The statistics arrive as kStatParts partial (sum, sumsq) pairs per row — one per (column tile, epilogue column group)
 // of the GEMM that produced the row, summed here in a fixed order (deterministic, no atomics); unused slots hold zeros.
 // LayerNorm: var = E[x^2] - mean^2 (fp32; clamped at 0), RMSNorm: mean = 0.  stats == nullptr: identity (rstd 1, rm 0).
-constexpr int kStatParts = 8;
+constexpr int kStatParts = 16;
 struct RowNorm {
   const float* stats;  // [T, kStatParts, 2] or nullptr
   float inv_h, eps;
@@ -103,7 +101,7 @@ struct RowNorm {
 
 // Coalescing stage for bf16 epilogue outputs.  A thread owns one accumulator ROW, so a direct 16-byte store
 // per lane touches 32 different cache lines per warp instruction and the SM's load/store unit — not the tensor
-// core — bounds the GEMM (measured: tensor pipe ~50 % with direct stores, 92 % with no stores).  Instead two
+// core — bounds the GEMM.  Instead two
 // consecutive 32-column chunks (= 128 bytes per row) are written into a warp-private 4 KB shared-memory tile
 // in the TMA SWIZZLE_128B layout (16-byte pieces XOR-ed with row & 7) and ONE lane issues a TMA store of the
 // 32-row x 64-column box: no LSU work for the global write, rows beyond M are clipped by the tensor map.
@@ -278,8 +276,8 @@ struct EpiQKV {
 // A thread owns an accumulator ROW, so touching global memory directly would cost one cache line per lane and
 // instruction; instead each warp moves its 32-row x 32-column chunks through shared memory with TMA:
 //   TMA load  s[32 rows, 32 cols] fp32 -> 4 KB tile (SWIZZLE_128B; the first chunk of a tile is requested before the
-//             accumulator wait, the residual of the NEXT tile is pulled into L2 a tile ahead; one tile per warp: the
-//             shared memory a second one would take buys the mainloop its 4th ring stage, worth more — measured)
+//             tile's mainloop, the residual of the NEXT tile is pulled into L2 a tile ahead; one tile per warp: the
+//             shared memory a second one would take is what the mainloop's ring and the staged accumulator need)
 //   in place  thread r rewrites row r of the tile (16-byte pieces XOR-ed with r & 7: conflict-free) and writes bf16(s')
 //             into a 2 KB tile (SWIZZLE_64B: 64-byte rows, also conflict-free)
 //   TMA store both tiles; rows >= M are clipped by the tensor maps.
@@ -296,7 +294,6 @@ struct EpiResidNorm {
   int bn;            // tile width (BN of the GEMM): geometry of the static tile schedule, for the L2 prefetch below
   static constexpr int kPasses = 1;
   static constexpr bool kPrefetch = true;
-  static constexpr bool kRolled = true;  // one copy of chunk() in the kernel (gemm.cuh)
   static constexpr int kF32Tile = 4096, kBf16Tile = 2048, kPerWarp = kF32Tile + kBf16Tile;
   static constexpr int kMaxN = 1024;     // per-column constants staged in shared memory: 2 * kMaxN floats
   __host__ __device__ static constexpr int smem_bytes(int epi_warps) { return epi_warps * kPerWarp + 1024 + 2 * kMaxN * 4; }
@@ -345,7 +342,7 @@ struct EpiResidNorm {
     s.slot = n_blk * parts + s.group;
     // The residual of the tile this CTA processes NEXT (static schedule: tile + gridDim.x, n fastest) is pulled into L2
     // now, a whole tile ahead: its TMA loads then cost an L2 hit instead of an exposed HBM round trip per chunk.
-    if (bn > 0 && (threadIdx.x & 31) == 0) {  // bn == 0: CTA-pair schedule, no look-ahead
+    if (bn > 0 && (threadIdx.x & 31) == 0) {  // bn == 0: no look-ahead
       const int num_n = (N + bn - 1) / bn, num_m = (M + kBlockM - 1) / kBlockM;
       const int next = m_blk * num_n + n_blk + static_cast<int>(gridDim.x);
       if (next < num_m * num_n) {
@@ -621,12 +618,11 @@ struct AttnParams {
   __nv_bfloat16* ctx;             // [T, I]
 };
 
-// P (32 KB) overwrites the Q and K tiles, which are dead once S = Q K^T has completed; O overwrites the first
-// 64 TMEM columns of S, dead once the softmax has read it: 52 KB smem + 128 TMEM columns per CTA -> 4 CTAs/SM.
-constexpr int kAttnSmemQ = 0, kAttnSmemK = 16384, kAttnSmemV = 32768, kAttnSmemP = 0;
-constexpr int kAttnSmemMisc = 49152;  // kb[128] f32, rel[256] f32, barriers, tmem slot
-constexpr int kAttnTmemCols = 128;
-constexpr int kAttnSmemBytes = kAttnSmemMisc + 512 + 1024 + 64 + 1024;
+// Q, K and V^T of a tile in shared memory (48 KB, TMA, 128B-swizzled); S, P and O never leave registers.
+constexpr int kAttnSmemQ = 0, kAttnSmemK = 16384, kAttnSmemV = 32768;
+constexpr int kAttnSmemMisc = 49152;  // kb[4] u32, rel[256] f32, barrier
+constexpr int kAttnSmemBytes = kAttnSmemMisc + 16 + 1024 + 64 + 1024;
+constexpr int kAttnCtasPerSm = 3;
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -634,194 +630,166 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-__global__ void __launch_bounds__(128, 4)
+// S = Q_h K^T for the 64 query rows [64 h, +64) of the tile: 4 wgmma m64n128k16 (K = head dim 64)
+__device__ __forceinline__ void attn_scores(float (&s)[64], uint32_t qa, uint32_t ka) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    wgmma_m64n128k16_bf16<0, 0>(s, wgmma_desc(qa + k * 32, kDescKMajorSW128), wgmma_desc(ka + k * 32, kDescKMajorSW128),
+                                k != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+}
+// O (+)= P V for the same 64 rows: P from registers (the probabilities in s, packed to bf16 as the A fragment of each
+// 16-key step), V^T [64 dims, 128 keys] as two K-major boxes of 64 keys
+__device__ __forceinline__ void attn_pv(float (&o)[32], const float (&s)[64], uint32_t va, uint32_t accumulate) {
+  uint32_t a[8][4];
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk) {
+    a[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+    a[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+    a[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+    a[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+  }
+  wgmma_fence();
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk)
+    wgmma_m64n64k16_bf16_rs(o, a[kk], wgmma_desc(va + (kk >> 2) * 8192 + (kk & 3) * 32, kDescKMajorSW128),
+                            (accumulate | kk) != 0 ? 1u : 0u);
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+}
+__device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+__device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// Fragment coordinates (see ptx.cuh): element 4 j + e of a thread's accumulator is row rr[e >> 1], column 8 j + 2 (lane % 4)
+// + (e & 1) of the 64-row block.
+__global__ void __launch_bounds__(128, kAttnCtasPerSm)
 attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p, int n_tiles,
             int n_heads) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* s_kb = reinterpret_cast<float*>(smem + kAttnSmemMisc);
-  float* s_rel = s_kb + 128;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_rel + 256);  // [0] load, [1] S ready, [2] O ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint32_t* s_kb = reinterpret_cast<uint32_t*>(smem + kAttnSmemMisc);
+  float* s_rel = reinterpret_cast<float*>(s_kb + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_rel + 256);  // [0] loads
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (tid == 0) {
     tma_prefetch_desc(&tmQK);
     tma_prefetch_desc(&tmVt);
     mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&bars[2], 1);
     fence_barrier_init();
   }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, kAttnTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-  // Persistent CTA (grid = 4 per SM): barriers, tensor memory and descriptors are set up once; work items are
-  // (tile, head) pairs taken head-fastest, so that the CTAs running at the same time read the same token rows of qk
-  // (neighbouring 128-byte slices of one DRAM page instead of one slice from each of many pages).
+  // Persistent CTA: work items are (tile, head) pairs taken head-fastest, so that the CTAs running at the same time read
+  // the same token rows of qk (neighbouring 128-byte slices of one DRAM page instead of one slice from each of many pages).
   const int n_items = n_tiles * n_heads;
+  const bool has_rel = p.relbias_log2 != nullptr;
+  const uint32_t qa = smem_u32(smem + kAttnSmemQ), ka = smem_u32(smem + kAttnSmemK), va = smem_u32(smem + kAttnSmemV);
   uint32_t par = 0;
 #pragma unroll 1
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, par ^= 1u) {
-  const int tile = item / n_heads, head = item - tile * n_heads;
-  const int row0 = tile * p.Tvalid_rows;  // first token of this tile
-  if (tid == 0) {  // shared memory and tensor memory of the previous item are free (trailing barrier): loads go out first
-    mbar_arrive_expect_tx(&bars[0], 3 * 16384);
-    tma_load_2d(smem + kAttnSmemQ, &tmQK, &bars[0], head * kHeadDim, row0);
-    tma_load_2d(smem + kAttnSmemK, &tmQK, &bars[0], p.I + head * kHeadDim, row0);
-    tma_load_2d(smem + kAttnSmemV, &tmVt, &bars[0], tile * 128, head * kHeadDim);
-    tma_load_2d(smem + kAttnSmemV + 8192, &tmVt, &bars[0], tile * 128 + 64, head * kHeadDim);
-  }
-  {
-    const int tok = row0 + tid;
-    // key validity as 4 x 32-bit words (bit c%32 of word c/32): one ballot per warp
-    const bool key_ok = (tid < p.Tvalid_rows && tok < p.T) && p.kmask[tok] == 0.f;
-    const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
-    if ((tid & 31) == 0) reinterpret_cast<uint32_t*>(s_kb)[warp] = bits;
-    if (p.relbias_log2) {
-      for (int i = tid; i < 2 * kMaxL - 1; i += 128) s_rel[i] = p.relbias_log2[head * (2 * kMaxL - 1) + i];
+    const int tile = item / n_heads, head = item - tile * n_heads;
+    const int row0 = tile * p.Tvalid_rows;  // first token of this tile
+    if (tid == 0) {  // shared memory of the previous item is free (trailing barrier): loads go out first
+      mbar_arrive_expect_tx(&bars[0], 3 * 16384);
+      tma_load_2d(smem + kAttnSmemQ, &tmQK, &bars[0], head * kHeadDim, row0);
+      tma_load_2d(smem + kAttnSmemK, &tmQK, &bars[0], p.I + head * kHeadDim, row0);
+      tma_load_2d(smem + kAttnSmemV, &tmVt, &bars[0], tile * 128, head * kHeadDim);
+      tma_load_2d(smem + kAttnSmemV + 8192, &tmVt, &bars[0], tile * 128 + 64, head * kHeadDim);
     }
-  }
-  __syncthreads();  // key bits / relative bias of this item are in place
-
-  if (tid == 0) {
-    mbar_wait(&bars[0], par, 10);
-    tc_fence_after_sync();
-    constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128);
-    const uint32_t qa = smem_u32(smem + kAttnSmemQ), ka = smem_u32(smem + kAttnSmemK);
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      umma_bf16_ss(tmem_base, umma_smem_desc(qa + k * 32, kDescKMajorSW128),
-                   umma_smem_desc(ka + k * 32, kDescKMajorSW128), idesc_s, k != 0 ? 1u : 0u);
-    umma_commit(&bars[1]);
-  }
-  mbar_wait_warp(&bars[1], par, 11);
-  tc_fence_after_sync();
-
-  // ---- softmax: thread r owns query row r of the tile ----
-  const int r = tid;
-  const bool row_valid = r < p.Tvalid_rows && row0 + r < p.T;
-  const int seq = r / p.L;
-  const int c_lo = row_valid ? seq * p.L : 0, c_hi = row_valid ? c_lo + p.L : 0;
-  // this row may attend key c iff the key is valid AND belongs to the row's own sequence [c_lo, c_hi)
-  uint32_t allow[4];
-#pragma unroll
-  for (int w = 0; w < 4; ++w) {
-    const int lo = c_lo - 32 * w, hi = c_hi - 32 * w;  // range relative to word w
-    const uint32_t ge = lo <= 0 ? 0xffffffffu : (lo >= 32 ? 0u : (0xffffffffu << lo));
-    const uint32_t lt = hi >= 32 ? 0xffffffffu : (hi <= 0 ? 0u : (0xffffffffu >> (32 - hi)));
-    allow[w] = reinterpret_cast<const uint32_t*>(s_kb)[w] & ge & lt;
-  }
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
-  const bool has_rel = p.relbias_log2 != nullptr;
-  float m = __int_as_float(0xff800000);
-#pragma unroll
-  for (int c4 = 0; c4 < 4; ++c4) {
-    uint32_t raw[32];
-    tmem_ld_32x32b_x32(taddr + c4 * 32, raw);
-    tmem_ld_wait();
-    const uint32_t aw = allow[c4];
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      const int c = c4 * 32 + i;
-      float s = __uint_as_float(raw[i]) * p.scale_log2;
-      if (has_rel) s += s_rel[c - r + (kMaxL - 1)];
-      if (!(aw & (1u << i))) s = __int_as_float(0xff800000);
-      m = fmaxf(m, s);
+    {
+      const int tok = row0 + tid;
+      // key validity as 4 x 32-bit words (bit c%32 of word c/32): one ballot per warp
+      const bool key_ok = (tid < p.Tvalid_rows && tok < p.T) && p.kmask[tok] == 0.f;
+      const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
+      if (lane == 0) s_kb[warp] = bits;
+      if (has_rel) {
+        for (int i = tid; i < 2 * kMaxL - 1; i += 128) s_rel[i] = p.relbias_log2[head * (2 * kMaxL - 1) + i];
+      }
     }
-  }
-  const bool dead = !(m > __int_as_float(0xff800000));  // every key masked (padding row)
-  const float mm = dead ? 0.f : m;
-  float sum = 0.f;
-  uint8_t* sP = smem + kAttnSmemP;
-  const float neg_mm = -mm;
-#pragma unroll
-  for (int c4 = 0; c4 < 4; ++c4) {
-    uint32_t raw[32];
-    tmem_ld_32x32b_x32(taddr + c4 * 32, raw);
-    tmem_ld_wait();
-    const uint32_t aw = dead ? 0u : allow[c4];
-    uint32_t packed[16];
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      float pv[2];
+    __syncthreads();  // key bits / relative bias of this item are in place
+    mbar_wait_warp(&bars[0], par, 10);
+
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+      float sc[64];
+      attn_scores(sc, qa + h * 8192, ka);
+      // ---- softmax on the fragments: this thread holds columns 8 j + 2 (lane % 4) + {0, 1} of two query rows ----
+      int rr[2], c_lo[2], c_hi[2];
+      bool valid[2];
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
-        const int c = c4 * 32 + i + u;
-        float s = fmaf(__uint_as_float(raw[i + u]), p.scale_log2, neg_mm);
-        if (has_rel) s += s_rel[c - r + (kMaxL - 1)];
-        pv[u] = (aw & (1u << (i + u))) ? ex2_approx(s) : 0.f;
+        rr[u] = h * 64 + 16 * warp + (lane >> 2) + 8 * u;
+        valid[u] = rr[u] < p.Tvalid_rows && row0 + rr[u] < p.T;
+        // this row may attend key c iff the key is valid AND belongs to the row's own sequence [c_lo, c_hi)
+        c_lo[u] = valid[u] ? (rr[u] / p.L) * p.L : 0;
+        c_hi[u] = valid[u] ? c_lo[u] + p.L : 0;
       }
-      sum += pv[0] + pv[1];
-      packed[i >> 1] = pack_bf16x2(pv[0], pv[1]);
-    }
-    // P[r, c4*32 .. +32) -> K-major SWIZZLE_128B layout: block = c / 64, 16-B chunk j XOR (r & 7)
-    uint8_t* blk = sP + (c4 >> 1) * 16384 + r * 128;
+      float m[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
 #pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      const int chunk = ((c4 & 1) * 4 + j) ^ (r & 7);
-      *reinterpret_cast<uint4*>(blk + chunk * 16) =
-          make_uint4(packed[4 * j], packed[4 * j + 1], packed[4 * j + 2], packed[4 * j + 3]);
-    }
-  }
-  const float inv = sum > 0.f ? 1.0f / sum : 0.f;
-  fence_proxy_async_smem();  // generic-proxy smem writes -> visible to the tensor core (async proxy)
-  tc_fence_before_sync();
-  __syncthreads();
-
-  if (tid == 0) {
-    tc_fence_after_sync();
-    constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64);
-    const uint32_t pa = smem_u32(sP), va = smem_u32(smem + kAttnSmemV);
+      for (int j = 0; j < 16; ++j)
 #pragma unroll
-    for (int k = 0; k < 8; ++k)
-      umma_bf16_ss(tmem_base, umma_smem_desc(pa + (k >> 2) * 16384 + (k & 3) * 32, kDescKMajorSW128),
-                   umma_smem_desc(va + (k >> 2) * 8192 + (k & 3) * 32, kDescKMajorSW128), idesc_o, k != 0 ? 1u : 0u);
-    umma_commit(&bars[2]);
-  }
-  mbar_wait_warp(&bars[2], par, 12);
-  tc_fence_after_sync();
-#pragma unroll 1
-  for (int c2 = 0; c2 < 2; ++c2) {
-    uint32_t raw[32];
-    tmem_ld_32x32b_x32(taddr + c2 * 32, raw);
-    tmem_ld_wait();
-    if (row_valid) {
-      uint4* dst = reinterpret_cast<uint4*>(p.ctx + static_cast<int64_t>(row0 + r) * p.I + head * kHeadDim + c2 * 32);
+        for (int e = 0; e < 4; ++e) {
+          const int u = e >> 1, c = 8 * j + 2 * (lane & 3) + (e & 1);
+          float v = sc[4 * j + e] * p.scale_log2;
+          if (has_rel) v += s_rel[c - rr[u] + (kMaxL - 1)];
+          const bool ok = c >= c_lo[u] && c < c_hi[u] && ((s_kb[c >> 5] >> (c & 31)) & 1u);
+          v = ok ? v : __int_as_float(0xff800000);
+          sc[4 * j + e] = v;
+          m[u] = fmaxf(m[u], v);
+        }
+      float sum[2] = {0.f, 0.f};
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        uint32_t w[4];
+      for (int u = 0; u < 2; ++u) {
+        m[u] = quad_max(m[u]);
+        if (!(m[u] > __int_as_float(0xff800000))) m[u] = 0.f;  // every key masked (padding row): all p = 0
+      }
 #pragma unroll
-        for (int u = 0; u < 4; ++u)
-          w[u] = pack_bf16x2(__uint_as_float(raw[8 * j + 2 * u]) * inv, __uint_as_float(raw[8 * j + 2 * u + 1]) * inv);
-        dst[j] = make_uint4(w[0], w[1], w[2], w[3]);
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float pv = ex2_approx(sc[4 * j + e] - m[e >> 1]);  // ex2(-inf) = 0 for masked keys
+          sc[4 * j + e] = pv;
+          sum[e >> 1] += pv;
+        }
+      float o[32];
+      attn_pv(o, sc, va, 0u);
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const float tot = quad_sum(sum[u]);
+        const float inv = tot > 0.f ? 1.0f / tot : 0.f;
+        if (valid[u]) {
+          __nv_bfloat16* dst = p.ctx + static_cast<int64_t>(row0 + rr[u]) * p.I + head * kHeadDim + 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+            *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(o[4 * j + 2 * u] * inv, o[4 * j + 2 * u + 1] * inv);
+        }
       }
     }
-  }
-  // the next item's TMA loads overwrite Q / K / V and its first MMA overwrites S: every thread must be done with O
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
+    // the next item's TMA loads overwrite Q / K / V: every warp must be done with its wgmma reads
+    __syncthreads();
   }  // item loop
-  if (warp == 0) tmem_dealloc(tmem_base, kAttnTmemCols);
 }
 
 // ---------------------------------------------------------------------------------------------------
 // Sequences longer than one tile (L = 256 / 384 / 512, multiples of 128): one CTA per (128-row query tile, head)
-// loops over the sequence's 128-key tiles with an online softmax:  S_j = Q K_j^T (tcgen05 -> TMEM) -> running
-// max / sum in registers (thread = query row) -> P_j (bf16, swizzled smem) -> O_j = P_j V_j (tcgen05 -> TMEM) ->
-// acc = acc * alpha + O_j in registers.  Q stays in smem; K_j / V_j are re-loaded by TMA per iteration.
+// loops over the sequence's 128-key tiles with an online softmax, 64 query rows at a time:  S_j = Q K_j^T (wgmma) ->
+// running max / sum per row on the fragments -> P_j (bf16, registers) -> O = O * alpha + P_j V_j (wgmma, accumulating in
+// registers).  Q stays in smem; K_j / V_j are re-loaded by TMA per iteration.
 // ---------------------------------------------------------------------------------------------------
-constexpr int kAttnLongSmemQ = 0, kAttnLongSmemK = 16384, kAttnLongSmemV = 32768, kAttnLongSmemP = 49152;
-constexpr int kAttnLongSmemMisc = 81920;  // rel[1024] f32, key bits [4 tiles x 4 words], barriers, tmem slot
-constexpr int kAttnLongTmemCols = 256;    // S_j: columns [0, 128); O_j: columns [128, 192)
-constexpr int kAttnLongSmemBytes = kAttnLongSmemMisc + 4096 + 64 + 64 + 64 + 1024;
+constexpr int kAttnLongSmemQ = 0, kAttnLongSmemK = 16384, kAttnLongSmemV = 32768;
+constexpr int kAttnLongSmemMisc = 49152;  // rel[1024] f32, key bits [4 tiles x 4 words], barrier
+constexpr int kAttnLongSmemBytes = kAttnLongSmemMisc + 4096 + 64 + 64 + 1024;
 
 __global__ void __launch_bounds__(128, 2)
 attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p) {
@@ -829,10 +797,9 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* s_rel = reinterpret_cast<float*>(smem + kAttnLongSmemMisc);
   uint32_t* s_kb = reinterpret_cast<uint32_t*>(s_rel + 1024);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_kb + 16);  // [0] loads, [1] S ready, [2] O ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_kb + 16);  // [0] loads
 
-  const int tid = threadIdx.x, warp = tid >> 5;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, head = blockIdx.y;
   const int nk = p.L / 128;                 // key tiles per sequence
   const int row0 = qt * 128;                // first token of this query tile
@@ -843,156 +810,104 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
     tma_prefetch_desc(&tmQK);
     tma_prefetch_desc(&tmVt);
     mbar_init(&bars[0], 1);
-    mbar_init(&bars[1], 1);
-    mbar_init(&bars[2], 1);
     fence_barrier_init();
-  }
-  if (warp == 0) {
-    tmem_alloc(tmem_slot, kAttnLongTmemCols);
-    tmem_relinquish();
   }
   for (int j = 0; j < nk; ++j) {  // key validity of every key tile of the sequence: one ballot per warp and tile
     const int tok = (kt0 + j) * 128 + tid;
     const bool key_ok = tok < p.T && p.kmask[tok] == 0.f;
     const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
-    if ((tid & 31) == 0) s_kb[j * 4 + warp] = bits;
+    if (lane == 0) s_kb[j * 4 + warp] = bits;
   }
   if (p.relbias_log2) {
     for (int i = tid; i < 2 * kMaxLongL - 1; i += 128) s_rel[i] = p.relbias_log2[head * (2 * kMaxLongL - 1) + i];
   }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(warp * 32) << 16);
 
-  const int r = tid;
-  const bool row_valid = row0 + r < p.T;
   const bool has_rel = p.relbias_log2 != nullptr;
-  const int rel0 = (kMaxLongL - 1) - (qpos0 + r);  // + key position = index into s_rel
-  float m_run = __int_as_float(0xff800000), sum = 0.f;
-  float acc[kHeadDim];
+  const uint32_t qa = smem_u32(smem + kAttnLongSmemQ), ka = smem_u32(smem + kAttnLongSmemK),
+                 va = smem_u32(smem + kAttnLongSmemV);
+  int rr[2][2];
+  bool valid[2][2];
+  float m_run[2][2], sum[2][2], o[2][32];
 #pragma unroll
-  for (int i = 0; i < kHeadDim; ++i) acc[i] = 0.f;
-  uint8_t* sP = smem + kAttnLongSmemP;
+  for (int h = 0; h < 2; ++h) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      rr[h][u] = h * 64 + 16 * warp + (lane >> 2) + 8 * u;
+      valid[h][u] = row0 + rr[h][u] < p.T;
+      m_run[h][u] = __int_as_float(0xff800000);
+      sum[h][u] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[h][i] = 0.f;
+  }
 
 #pragma unroll 1
   for (int j = 0; j < nk; ++j) {
-    const uint32_t par = static_cast<uint32_t>(j & 1);
     if (tid == 0) {
-      // K / V of the previous iteration are dead: S_{j-1} and O_{j-1} have completed (every thread waited on them)
+      // K / V of the previous iteration are dead: every warp passed the trailing barrier of that iteration
       mbar_arrive_expect_tx(&bars[0], (j == 0 ? 3 : 2) * 16384);
       if (j == 0) tma_load_2d(smem + kAttnLongSmemQ, &tmQK, &bars[0], head * kHeadDim, row0);
       tma_load_2d(smem + kAttnLongSmemK, &tmQK, &bars[0], p.I + head * kHeadDim, (kt0 + j) * 128);
       tma_load_2d(smem + kAttnLongSmemV, &tmVt, &bars[0], (kt0 + j) * 128, head * kHeadDim);
       tma_load_2d(smem + kAttnLongSmemV + 8192, &tmVt, &bars[0], (kt0 + j) * 128 + 64, head * kHeadDim);
-      mbar_wait(&bars[0], par, 13);
-      tc_fence_after_sync();
-      constexpr uint32_t idesc_s = umma_idesc_bf16(128, 128);
-      const uint32_t qa = smem_u32(smem + kAttnLongSmemQ), ka = smem_u32(smem + kAttnLongSmemK);
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        umma_bf16_ss(tmem_base, umma_smem_desc(qa + k * 32, kDescKMajorSW128),
-                     umma_smem_desc(ka + k * 32, kDescKMajorSW128), idesc_s, k != 0 ? 1u : 0u);
-      umma_commit(&bars[1]);
     }
-    mbar_wait_warp(&bars[1], par, 14);
-    tc_fence_after_sync();
-
-    // ---- running max over this key tile ----
-    float m_j = __int_as_float(0xff800000);
+    mbar_wait_warp(&bars[0], static_cast<uint32_t>(j & 1), 13);
 #pragma unroll
-    for (int c4 = 0; c4 < 4; ++c4) {
-      uint32_t raw[32];
-      tmem_ld_32x32b_x32(taddr + c4 * 32, raw);
-      tmem_ld_wait();
-      const uint32_t aw = row_valid ? s_kb[j * 4 + c4] : 0u;
+    for (int h = 0; h < 2; ++h) {
+      float sc[64];
+      attn_scores(sc, qa + h * 8192, ka);
+      float m_j[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
 #pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        float sc = __uint_as_float(raw[i]) * p.scale_log2;
-        if (has_rel) sc += s_rel[rel0 + j * 128 + c4 * 32 + i];
-        if (!(aw & (1u << i))) sc = __int_as_float(0xff800000);
-        m_j = fmaxf(m_j, sc);
-      }
-    }
-    const float m_new = fmaxf(m_run, m_j);
-    const bool dead = !(m_new > __int_as_float(0xff800000));  // no allowed key seen so far
-    const float mm = dead ? 0.f : m_new;
-    const float alpha = (m_run > __int_as_float(0xff800000)) ? ex2_approx(m_run - mm) : 0.f;
-    m_run = m_new;
-    sum *= alpha;
-    const float neg_mm = -mm;
+      for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
-    for (int c4 = 0; c4 < 4; ++c4) {
-      uint32_t raw[32];
-      tmem_ld_32x32b_x32(taddr + c4 * 32, raw);
-      tmem_ld_wait();
-      const uint32_t aw = (row_valid && !dead) ? s_kb[j * 4 + c4] : 0u;
-      uint32_t packed[16];
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        float pv[2];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          float sc = fmaf(__uint_as_float(raw[i + u]), p.scale_log2, neg_mm);
-          if (has_rel) sc += s_rel[rel0 + j * 128 + c4 * 32 + i + u];
-          pv[u] = (aw & (1u << (i + u))) ? ex2_approx(sc) : 0.f;
+        for (int e = 0; e < 4; ++e) {
+          const int u = e >> 1, c = 8 * jj + 2 * (lane & 3) + (e & 1);
+          float v = sc[4 * jj + e] * p.scale_log2;
+          if (has_rel) v += s_rel[(kMaxLongL - 1) - (qpos0 + rr[h][u]) + j * 128 + c];
+          const bool ok = valid[h][u] && ((s_kb[j * 4 + (c >> 5)] >> (c & 31)) & 1u);
+          v = ok ? v : __int_as_float(0xff800000);
+          sc[4 * jj + e] = v;
+          m_j[u] = fmaxf(m_j[u], v);
         }
-        sum += pv[0] + pv[1];
-        packed[i >> 1] = pack_bf16x2(pv[0], pv[1]);
+      float alpha[2], mm[2];
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const float m_new = fmaxf(m_run[h][u], quad_max(m_j[u]));
+        mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new : 0.f;  // no allowed key seen so far: all p = 0
+        alpha[u] = (m_run[h][u] > __int_as_float(0xff800000)) ? ex2_approx(m_run[h][u] - mm[u]) : 0.f;
+        m_run[h][u] = m_new;
+        sum[h][u] *= alpha[u];
       }
-      uint8_t* blk = sP + (c4 >> 1) * 16384 + r * 128;  // K-major SWIZZLE_128B, see attn_kernel
 #pragma unroll
-      for (int q4 = 0; q4 < 4; ++q4) {
-        const int chunk = ((c4 & 1) * 4 + q4) ^ (r & 7);
-        *reinterpret_cast<uint4*>(blk + chunk * 16) =
-            make_uint4(packed[4 * q4], packed[4 * q4 + 1], packed[4 * q4 + 2], packed[4 * q4 + 3]);
-      }
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float pv = ex2_approx(sc[4 * jj + e] - mm[e >> 1]);
+          sc[4 * jj + e] = pv;
+          sum[h][e >> 1] += pv;
+        }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[h][i] *= alpha[(i >> 1) & 1];
+      attn_pv(o[h], sc, va, 1u);
     }
-    fence_proxy_async_smem();
-    tc_fence_before_sync();
-    __syncthreads();
-
-    if (tid == 0) {
-      tc_fence_after_sync();
-      constexpr uint32_t idesc_o = umma_idesc_bf16(128, 64);
-      const uint32_t pa = smem_u32(sP), va = smem_u32(smem + kAttnLongSmemV);
-#pragma unroll
-      for (int k = 0; k < 8; ++k)
-        umma_bf16_ss(tmem_base + 128, umma_smem_desc(pa + (k >> 2) * 16384 + (k & 3) * 32, kDescKMajorSW128),
-                     umma_smem_desc(va + (k >> 2) * 8192 + (k & 3) * 32, kDescKMajorSW128), idesc_o, k != 0 ? 1u : 0u);
-      umma_commit(&bars[2]);
-    }
-    mbar_wait_warp(&bars[2], par, 15);
-    tc_fence_after_sync();
-#pragma unroll
-    for (int c2 = 0; c2 < 2; ++c2) {
-      uint32_t raw[32];
-      tmem_ld_32x32b_x32(taddr + 128 + c2 * 32, raw);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) acc[c2 * 32 + i] = fmaf(acc[c2 * 32 + i], alpha, __uint_as_float(raw[i]));
-    }
-    tc_fence_before_sync();  // the next iteration's MMAs overwrite S (after this thread's reads above)
+    __syncthreads();  // the next iteration's TMA loads overwrite K / V
   }
 
-  const float inv = sum > 0.f ? 1.0f / sum : 0.f;
-  if (row_valid) {
-    uint4* dst = reinterpret_cast<uint4*>(p.ctx + static_cast<int64_t>(row0 + r) * p.I + head * kHeadDim);
 #pragma unroll
-    for (int q8 = 0; q8 < 8; ++q8) {
-      uint32_t w[4];
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
-      for (int u = 0; u < 4; ++u) w[u] = pack_bf16x2(acc[8 * q8 + 2 * u] * inv, acc[8 * q8 + 2 * u + 1] * inv);
-      dst[q8] = make_uint4(w[0], w[1], w[2], w[3]);
+    for (int u = 0; u < 2; ++u) {
+      const float tot = quad_sum(sum[h][u]);
+      const float inv = tot > 0.f ? 1.0f / tot : 0.f;
+      if (valid[h][u]) {
+        __nv_bfloat16* dst = p.ctx + static_cast<int64_t>(row0 + rr[h][u]) * p.I + head * kHeadDim + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jj) =
+              pack_bf16x2(o[h][4 * jj + 2 * u] * inv, o[h][4 * jj + 2 * u + 1] * inv);
+      }
     }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 0) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, kAttnLongTmemCols);
-  }
 }
 
 // ===================================================================================================
@@ -1560,33 +1475,16 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   const int rms = bert ? 0 : 1;
   const RowNorm normA{e->stats[0], inv_h, d.ln_eps, rms}, normB{e->stats[1], inv_h, d.ln_eps, rms};
   const RowNorm ident{nullptr, inv_h, d.ln_eps, rms};
-  // wide GEMMs (QKV, FFN1: N >= 2 H, plain bf16 epilogues): CTA pairs (cta_group::2, 256 x 256 tiles: half the operand
-  // bytes per SM and FLOP; 1 700 vs 1 595 TFLOP/s on the FFN1 shape, profiles/r02_2sm_product_core.log), single-CTA
-  // tiles when the device cannot host a pair
-  static const bool pair_gemm = getenv("OM_ENCODER_SINGLE_CTA") == nullptr;  // measurement switch, read once
+  // 128 x 128 tiles, 3-stage ring: the staged fp32 accumulator tile (66 KB) and the functors' shared memory leave room for
+  // three 32 KB stages within the 227 KB an H100 block may use.  8 epilogue warps = 2 column groups per tile ->
+  // (H / 128) * 2 <= kStatParts statistics slots for the residual GEMMs.
   auto wide_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, int M, int N, const auto& epi) -> cudaError_t {
-    cudaError_t err = cudaErrorNotSupported;
-    if (pair_gemm) err = launch_gemm2<5, false, 8>(A, K, W, K, M, N, K, epi, sms, st);
-    if (err == cudaErrorNotSupported) err = launch_gemm<256, 4, false, 8>(A, K, W, K, M, N, K, epi, sms, st);
-    return err;
+    return launch_gemm<128, 3, false>(A, K, W, K, M, N, K, epi, sms, st);
   };
-  // residual GEMMs (N = H): 192-wide tiles divide 768 into 4 (1024 tiles = 6.9 waves of 3/4-size tiles instead of 5.2
-  // waves of full tiles); 8 epilogue warps = 2 column groups per tile -> (H / BN) * 2 <= kStatParts statistics slots
-  // CTA pairs: 256-wide tiles with 8 epilogue warps (two column groups) fit next to a 5-stage ring of 32 KB stages
-  // (bert-base 6.59 vs 6.80 ms, bert-large 20.4 vs 21.7 ms per batch of 256: profiles/r02_encoder_pair_resid_probe.log)
-  auto resid_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, EpiResidNorm epi) -> cudaError_t {
-    if (pair_gemm && ((H + 255) / 256) * 2 <= kStatParts) {
-      EpiResidNorm e2 = epi;
-      e2.parts = 2;
-      e2.bn = 0;
-      const cudaError_t err = launch_gemm2<5, false, 8>(A, K, W, K, T, H, K, e2, sms, st);
-      if (err != cudaErrorNotSupported) return err;
-    }
-    if (H % 192 == 0) return launch_gemm<192, 4, false, 8>(A, K, W, K, T, H, K, epi, sms, st);
-    epi.parts = 1;  // 256-wide tiles: a 4-stage ring leaves room for 4 epilogue warps (one column group)
-    return launch_gemm<256, 4, false, 4>(A, K, W, K, T, H, K, epi, sms, st);
+  auto resid_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, const EpiResidNorm& epi) -> cudaError_t {
+    return launch_gemm<128, 3, false>(A, K, W, K, T, H, K, epi, sms, st);
   };
-  if ((H % 192 == 0 ? H / 192 : (H + 255) / 256) * 2 > kStatParts)
+  if (((H + 127) / 128) * 2 > kStatParts)
     return fail(OM_EINVAL, "om_encode: hidden=%d needs more statistics slots than kStatParts", H);
   for (int li = 0; li < d.layers; ++li) {
     const LayerW& w = e->layers[li];
@@ -1596,19 +1494,17 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
     const float* b_in = bert ? (li == 0 ? e->emb_b : e->layers[li - 1].ln2_b) : nullptr;
     {
       EpiQKV epi{tmQKout, e->qk, e->vt, e->Tld, bert ? w.bqkv_fold : nullptr, T, 2 * I, ap.Tvalid_rows, normA};
-      // (192-wide tiles with 12 epilogue warps measured 3 % slower here and on FFN1: r02 tile A/B in profiles/README.md)
       cudaError_t err = wide_gemm(e->xb, H, w.wqkv, T, 3 * I, epi);
       if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
     }
     if (long_seq)
       attn_long_kernel<<<dim3(n_tiles, d.heads), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap);
     else
-      attn_kernel<<<std::min(n_tiles * d.heads, sms * 4), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap, n_tiles, d.heads);
+      attn_kernel<<<std::min(n_tiles * d.heads, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap, n_tiles, d.heads);
     OM_CUDA(cudaGetLastError());
     {
       // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
-      EpiResidNorm epi{tmS, tmXb, bert ? w.bo : nullptr, bert ? normA : ident, g_in, b_in, e->stats[1], 2, T, H,
-                       H % 192 == 0 ? 192 : 256};
+      EpiResidNorm epi{tmS, tmXb, bert ? w.bo : nullptr, bert ? normA : ident, g_in, b_in, e->stats[1], 2, T, H, 128};
       cudaError_t err = resid_gemm(e->ctx, I, w.wo, epi);
       if (err != cudaSuccess) return fail(OM_ECUDA, "O-proj GEMM launch failed: %s", cudaGetErrorString(err));
     }
@@ -1625,8 +1521,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
     }
     {
       // s <- inter W2^T + b2 + LN_attn(s) (BERT) / + s (T5); statistics -> stats[0] (the next layer's input)
-      EpiResidNorm epi{tmS, tmXb, bert ? w.b2 : nullptr, bert ? normB : ident, w.ln1_g, w.ln1_b, e->stats[0], 2, T, H,
-                       H % 192 == 0 ? 192 : 256};
+      EpiResidNorm epi{tmS, tmXb, bert ? w.b2 : nullptr, bert ? normB : ident, w.ln1_g, w.ln1_b, e->stats[0], 2, T, H, 128};
       cudaError_t err = resid_gemm(e->inter, F, w.w2, epi);
       if (err != cudaSuccess) return fail(OM_ECUDA, "FFN2 GEMM launch failed: %s", cudaGetErrorString(err));
     }

@@ -1,20 +1,22 @@
-// Persistent, warp-specialised tcgen05 GEMM core for sm_100a:   C[m, n] = sum_k A[m, k] * B[n, k]
-// (both operands K-major bf16, fp32 accumulation in tensor memory).  This one mainloop serves the
-// three hot steps: encoder linear layers (A = activations [T, H], B = nn.Linear weight [out, in]),
-// brute-force search (A = queries [nq, d], B = corpus rows [N, d]) and contrastive logits (Q * P^T).
+// Persistent, warp-specialised wgmma GEMM core for sm_90a:   C[m, n] = sum_k A[m, k] * B[n, k]
+// (both operands K-major bf16 — or IEEE half with F16 — fp32 accumulation).  This one mainloop serves the three hot
+// steps: encoder linear layers (A = activations [T, H], B = nn.Linear weight [out, in]), brute-force search (A = queries
+// [nq, d], B = corpus rows [N, d]) and contrastive logits (Q * P^T).
 //
-//   warp 0 (one elected lane)  TMA producer : global -> STAGES-deep smem ring (128B-swizzled boxes)
-//   warp 1 (one elected lane)  MMA issuer   : tcgen05.mma 128 x BN x 16, accumulators in TMEM,
-//                                             double-buffered (2 x BN columns)
-//   warp 2                     TMEM allocator
-//   warps 4..4+EPI_WARPS       epilogue     : tcgen05.ld -> registers -> Epi functor (fused op).
-//                                             EPI_WARPS = 4: one thread per accumulator row; 8 / 16: two / four
-//                                             threads per row, each owning a column group of the tile (math-
-//                                             heavy epilogues such as bias + erf-GELU need the extra warps to
-//                                             hide TMEM-load and MUFU latency)
+//   warp 0 (one lane)       TMA producer : global -> STAGES-deep smem ring (128B-swizzled boxes)
+//   warps 1..3              idle (they pad the producer role to a whole warpgroup, so the consumers start at warp 4)
+//   warps 4..11             two consumer warpgroups: warpgroup g issues wgmma m64 x BN x 16 for rows [64 g, 64 g + 64) of
+//                           the 128-row tile, accumulating in registers; then both write their accumulators into a
+//                           padded fp32 tile in shared memory and run the epilogue functor on it with the row-per-thread
+//                           mapping of the functor contract below (thread <-> accumulator row, 32-column chunks)
 //
-// Pipelines: smem full/empty (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue); static persistent
-// tile schedule (tile = blockIdx.x + i * gridDim.x).
+// Pipelines: smem full/empty (TMA <-> consumers, released per k block one wgmma group late); the staged accumulator
+// tile is handed over with two named barriers per tile.  Tile schedule: static (tile = blockIdx.x + i * gridDim.x) or
+// dynamic (claimed from a global counter by the producer, published through a 4-deep smem ring).
+//
+// CLUSTER = 2: two CTAs of a cluster own vertically adjacent 128-row tiles that share the same B tile; each CTA loads
+// its own A tile and one half of B, multicast into both CTAs' shared memory, so every B byte crosses L2 -> SM once per
+// pair.  Static tile schedule over pair tiles.
 #pragma once
 #include <type_traits>
 
@@ -25,67 +27,70 @@ namespace om {
 
 constexpr int kBlockM = 128;
 constexpr int kBlockK = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kGemmProducerThreads = 128;  // warps 0..3: TMA, MMA, TMEM alloc, idle
+constexpr int kWgmmaK = 16;
+constexpr int kGemmProducerThreads = 128;  // warpgroup 0: TMA producer + idle warps
+constexpr int kGemmEpiWarps = 8;           // two consumer warpgroups
 
 template <int BN, int STAGES>
 struct GemmCfg {
-  static_assert(BN == 64 || BN == 128 || BN == 192 || BN == 256, "BN must be 64, 128, 192 or 256");
+  static_assert(BN == 128, "BN must be 128 (one wgmma m64n128 per consumer warpgroup)");
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kBBytes = BN * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kBarOffset = STAGES * kStageBytes;
-  static constexpr int kEpiOffset = kBarOffset + 1024;         // epilogue scratch starts 1024-B aligned (TMA store)
-  static constexpr int kSmemBytes = kEpiOffset + 1024;         // + slack for 1024-B alignment of the base
-  static constexpr int kTmemCols = BN <= 64 ? 128 : (BN <= 128 ? 256 : 512);  // power of two >= 2 * BN
+  static constexpr int kAccPitch = BN + 4;                    // floats per staged row: conflict-free row reads
+  static constexpr int kAccOffset = STAGES * kStageBytes;     // staged fp32 accumulator tile [128][kAccPitch]
+  static constexpr int kBarOffset = kAccOffset + kBlockM * kAccPitch * 4;
+  static constexpr int kEpiOffset = kBarOffset + 1024;        // epilogue scratch starts 1024-B aligned (TMA store)
+  static constexpr int kSmemBytes = kEpiOffset + 1024;        // + slack for 1024-B alignment of the base
+  static_assert(kBarOffset % 1024 == 0, "barrier block must stay 1024-B aligned");
 };
 
-// Epilogue functor contract (all methods __device__, called by the epilogue threads; thread <-> row (half)):
+// Epilogue functor contract (all methods __device__, called by the 256 epilogue threads; thread <-> row (half)):
 //   struct State;                                             per-thread, per-tile scratch
-//   void begin(State&, int row, int m_blk, int n_blk) const;  once per tile
+//   void begin(State&, int row, int m_blk, int n_blk) const;  once per tile, before the tile's mainloop
 //   void chunk(State&, int row, int col0, const float (&v)[32]) const;   v = C[row, col0 .. col0+31]
 //   void end(State&, int row) const;                           once per tile
 //   static constexpr bool kPrefetch = false;                   true: prefetch(State&, row, col0) is called for the
-//        thread's first chunk BEFORE waiting on the accumulator, and chunk(..., int next_col0) receives the
-//        column of the thread's next chunk (-1: none) so that global operands (residual) are always one
-//        chunk ahead of the math
+//        thread's first chunk BEFORE the tile's mainloop, and chunk(..., int next_col0) receives the column of the
+//        thread's next chunk (-1: none) so that global operands (residual) are always one chunk ahead of the math
 //   __host__ __device__ static constexpr int smem_bytes(int epi_warps);            > 0: that much dynamic smem is reserved for the functor
 //        and handed over through bind(State&, uint8_t* smem, int epilogue_thread_index) once per thread; the
 //        State object persists across the thread's tiles and finish(State&) is called after the last one
-//   end() runs AFTER the thread's warp has released the accumulator buffer: long-latency tails (atomics,
-//        global stores) placed there overlap the next tile's MMAs
+//   end() runs right after the thread's last chunk: long-latency tails (atomics, global stores) placed there overlap the
+//        next tile's mainloop
 //   static constexpr int kPasses = 1;                          2: the accumulator tile may be read twice:
 //        chunk(..., int pass) runs for pass 0; if need_pass(State&, 1) (warp-uniform) is true, between(State&,
-//        row) and a second sweep with pass 1 follow (TMEM re-reads are cheap; the search filter uses this as
-//        its overflow path when a thread finds more survivors than its stash holds)
+//        row) and a second sweep with pass 1 follow (the staged tile stays in shared memory until every epilogue thread
+//        is done; the search filter uses this as its overflow path when a thread finds more survivors than its stash holds)
 // Rows >= M and columns >= N contain zeros (TMA out-of-bounds fill) and must be masked by the functor.
+// Named barrier 1 is the functors'; the core uses barrier 2.
 
-// Epi::kRolled (optional, default false): see the epilogue loop
-template <class Epi, class = void>
-struct epi_rolled : std::false_type {};
-template <class Epi>
-struct epi_rolled<Epi, std::void_t<decltype(Epi::kRolled)>> : std::bool_constant<Epi::kRolled> {};
+template <int BN, bool F16>
+__device__ __forceinline__ void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t accumulate) {
+  if constexpr (F16) wgmma_m64n128k16_f16<0, 0>(acc, da, db, accumulate);
+  else wgmma_m64n128k16_bf16<0, 0>(acc, da, db, accumulate);
+}
 
-template <int BN, int STAGES, bool M_FASTEST, int EPI_WARPS, class Epi, bool F16 = false>
-__global__ void __launch_bounds__(kGemmProducerThreads + 32 * EPI_WARPS, 1)
+template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16, int CLUSTER>
+__global__ void __launch_bounds__(kGemmProducerThreads + 32 * kGemmEpiWarps, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
                     int K, const __grid_constant__ Epi epi, int* tile_counter) {
   using Cfg = GemmCfg<BN, STAGES>;
+  static_assert(CLUSTER == 1 || CLUSTER == 2, "CLUSTER: 1 or 2");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOffset);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;
-  uint64_t* tempty_bar = tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty_bar + 2);
-  uint8_t* epi_smem = smem + Cfg::kEpiOffset;  // Epi::smem_bytes() of scratch owned by the epilogue functor
-  // dynamic tile scheduler (tile_counter != nullptr): the producer claims tile indices from a global counter
-  // and publishes them to the MMA and epilogue roles through a 4-deep smem ring
+  // dynamic tile scheduler (tile_counter != nullptr, CLUSTER == 1): the producer claims tile indices from a global
+  // counter and publishes them to the consumer warps through a 4-deep smem ring
   constexpr int kSched = 4;
-  uint64_t* sfull_bar = reinterpret_cast<uint64_t*>(tmem_slot + 2);
+  uint64_t* sfull_bar = empty_bar + STAGES;
   uint64_t* sempty_bar = sfull_bar + kSched;
   volatile int* tile_ring = reinterpret_cast<volatile int*>(sempty_bar + kSched);
-  const bool dyn = tile_counter != nullptr;
+  uint8_t* epi_smem = smem + Cfg::kEpiOffset;  // Epi::smem_bytes() of scratch owned by the epilogue functor
+  const bool dyn = CLUSTER == 1 && tile_counter != nullptr;
+  const uint32_t rank = CLUSTER > 1 ? cluster_ctarank() : 0u;
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = static_cast<int>(threadIdx.x & 31);
@@ -97,43 +102,36 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tfull_bar[i], 1);
-      mbar_init(&tempty_bar[i], EPI_WARPS);  // one arrive per epilogue warp
+      mbar_init(&empty_bar[i], kGemmEpiWarps * CLUSTER);  // every consumer warp of every CTA that writes this stage
     }
     for (int i = 0; i < kSched; ++i) {
       mbar_init(&sfull_bar[i], 1);
-      mbar_init(&sempty_bar[i], 1 + EPI_WARPS);  // MMA thread + one lane per epilogue warp
+      mbar_init(&sempty_bar[i], kGemmEpiWarps);  // one lane per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
+  if constexpr (CLUSTER > 1) cluster_sync_all();  // the peer's barriers exist before any multicast or remote arrive
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
 
   const int num_m = (M + kBlockM - 1) / kBlockM;
   const int num_n = (N + BN - 1) / BN;
-  const int num_tiles = num_m * num_n;
+  const int num_mt = (num_m + CLUSTER - 1) / CLUSTER;  // tile rows of the schedule (pairs of 128-row tiles: CLUSTER 2)
+  const int num_tiles = num_mt * num_n;
   const int num_k = (K + kBlockK - 1) / kBlockK;
+  const int first_tile = CLUSTER > 1 ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
+  const int tile_step = CLUSTER > 1 ? static_cast<int>(cluster_count_x()) : static_cast<int>(gridDim.x);
 
   if (warp == 0) {
     if (lane == 0) {
       // ------------------------------ TMA producer ------------------------------
       uint32_t stage = 0, phase = 0, sslot = 0, sphase = 0;
-      int tile = blockIdx.x;
+      int tile = first_tile;
       if (dyn) {
         tile = atomicAdd(tile_counter, 1);
         if (tile >= num_tiles) tile = -1;
       }
       while (true) {
-        if (dyn) {  // publish (also the -1 sentinel) to the consumer roles
+        if (dyn) {  // publish (also the -1 sentinel) to the consumer warps
           mbar_wait(&sempty_bar[sslot], sphase ^ 1u, 5);
           tile_ring[sslot] = tile;
           mbar_arrive(&sfull_bar[sslot]);
@@ -146,15 +144,21 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
           break;
         }
         // claim the next tile now; the atomic's round trip overlaps this tile's loads
-        int next = dyn ? atomicAdd(tile_counter, 1) : tile + static_cast<int>(gridDim.x);
-        const int m_blk = M_FASTEST ? tile % num_m : tile / num_n;
-        const int n_blk = M_FASTEST ? tile / num_m : tile % num_n;
+        int next = dyn ? atomicAdd(tile_counter, 1) : tile + tile_step;
+        const int m_blk = (M_FASTEST ? tile % num_mt : tile / num_n) * CLUSTER + static_cast<int>(rank);
+        const int n_blk = M_FASTEST ? tile / num_mt : tile % num_n;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u, 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           tma_load_2d(sa, &tmA, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n_blk * BN);
+          if constexpr (CLUSTER > 1) {
+            constexpr int kHalf = BN / CLUSTER;
+            tma_load_2d_multicast(sa + Cfg::kABytes + rank * kHalf * 128, &tmB, &full_bar[stage], kb * kBlockK,
+                                  n_blk * BN + static_cast<int>(rank) * kHalf, static_cast<uint16_t>((1u << CLUSTER) - 1u));
+          } else {
+            tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n_blk * BN);
+          }
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1u;
@@ -163,63 +167,19 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         tile = (dyn && next >= num_tiles) ? -1 : next;
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ------------------------------ MMA issuer ------------------------------
-      // F16: both operands IEEE half instead of bf16 (same instruction, same rate, 3 more significand bits)
-      constexpr uint32_t idesc = F16 ? umma_idesc_f16(kBlockM, BN) : umma_idesc_bf16(kBlockM, BN);
-      uint32_t stage = 0, phase = 0, sslot = 0, sphase = 0;
-      int it = 0;
-      for (int tile = blockIdx.x;; tile += gridDim.x, ++it) {
-        if (dyn) {
-          mbar_wait(&sfull_bar[sslot], sphase, 6);
-          const int t = tile_ring[sslot];
-          mbar_arrive(&sempty_bar[sslot]);
-          if (++sslot == kSched) {
-            sslot = 0;
-            sphase ^= 1u;
-          }
-          if (t < 0) break;
-        } else if (tile >= num_tiles) {
-          break;
-        }
-        const uint32_t as = it & 1, aphase = (it >> 1) & 1;
-        mbar_wait(&tempty_bar[as], aphase ^ 1u, 2);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = tmem_base + as * BN;
-        for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&full_bar[stage], phase, 3);
-          tc_fence_after_sync();
-          const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes);
-          const uint32_t b_addr = a_addr + Cfg::kABytes;
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = umma_smem_desc(a_addr + k * kUmmaK * 2, kDescKMajorSW128);
-            const uint64_t db = umma_smem_desc(b_addr + k * kUmmaK * 2, kDescKMajorSW128);
-            umma_bf16_ss(d_tmem, da, db, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);  // frees the smem slot once these MMAs have read it
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
-        }
-        umma_commit(&tfull_bar[as]);  // accumulator complete -> epilogue
-      }
-    }
   } else if (warp >= 4) {
-    // ------------------------------ epilogue ------------------------------
-    static_assert(EPI_WARPS == 4 || EPI_WARPS == 8 || EPI_WARPS == 12 || EPI_WARPS == 16, "EPI_WARPS: 4, 8, 12 or 16");
-    const int ew = (warp - 4) & 3;      // == warp % 4: the TMEM lane quarter this warp may access
-    const int half = (warp - 4) >> 2;   // column group (of EPI_WARPS / 4) owned by this warp
-    static_assert((BN / 32) % (EPI_WARPS / 4) == 0, "column chunks must split evenly over the epilogue warps");
-    constexpr int kChunks = BN / 32 / (EPI_WARPS / 4);
-    int it = 0;
+    // ------------------------------ consumers: wgmma + epilogue ------------------------------
+    const int et = static_cast<int>(threadIdx.x) - kGemmProducerThreads;  // 0 .. 255
+    const int wg = et >> 7;                  // consumer warpgroup = rows [64 wg, +64) of the MMA tile
+    const int ew = (warp - 4) & 3;           // epilogue: rows [32 ew, +32) of the tile
+    const int half = (warp - 4) >> 2;        // epilogue: column group of the tile
+    constexpr int kChunks = BN / 32 / 2;
     typename Epi::State st;  // lives across tiles: functors may keep work in flight from one tile to the next
-    if constexpr (Epi::smem_bytes(EPI_WARPS) > 0)
-      epi.bind(st, epi_smem, static_cast<int>(threadIdx.x) - kGemmProducerThreads);
-    uint32_t sslot = 0, sphase = 0;
-    for (int tile = blockIdx.x;; tile += gridDim.x, ++it) {
+    if constexpr (Epi::smem_bytes(kGemmEpiWarps) > 0) epi.bind(st, epi_smem, et);
+    uint32_t stage = 0, phase = 0, sslot = 0, sphase = 0;
+    // staging coordinates of this thread's accumulator fragment
+    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2), fcol = 2 * (lane & 3);
+    for (int tile = first_tile;; tile += tile_step) {
       if (dyn) {
         mbar_wait_warp(&sfull_bar[sslot], sphase, 7);
         tile = tile_ring[sslot];
@@ -233,15 +193,58 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       } else if (tile >= num_tiles) {
         break;
       }
-      const int m_blk = M_FASTEST ? tile % num_m : tile / num_n;
-      const int n_blk = M_FASTEST ? tile / num_m : tile % num_n;
-      const uint32_t as = it & 1, aphase = (it >> 1) & 1;
+      const int m_blk = (M_FASTEST ? tile % num_mt : tile / num_n) * CLUSTER + static_cast<int>(rank);
+      const int n_blk = M_FASTEST ? tile / num_mt : tile % num_n;
       const int row = m_blk * kBlockM + ew * 32 + lane;
       epi.begin(st, row, m_blk, n_blk);
-      if constexpr (Epi::kPrefetch) epi.prefetch(st, row, n_blk * BN + half * kChunks * 32);  // before the wait
-      mbar_wait_warp(&tfull_bar[as], aphase, 4);
-      tc_fence_after_sync();
-      const uint32_t taddr = tmem_base + as * BN + (static_cast<uint32_t>(ew * 32) << 16);
+      if constexpr (Epi::kPrefetch) epi.prefetch(st, row, n_blk * BN + half * kChunks * 32);
+
+      // mainloop: one wgmma group per k block in flight; a stage is released once the group after it was issued
+      float acc[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait_warp(&full_bar[stage], phase, 3);
+        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes) + wg * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+          wgmma_tile_k16<BN, F16>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
+                                  wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();
+          if (lane == 0) {
+            mbar_arrive(&empty_bar[prev_stage]);
+            if constexpr (CLUSTER > 1) mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
+          }
+        }
+        prev_stage = stage;
+        if (++stage == STAGES) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (num_k > 0 && lane == 0) {
+        mbar_arrive(&empty_bar[prev_stage]);
+        if constexpr (CLUSTER > 1) mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
+      }
+
+      // stage the accumulators: every epilogue thread has finished reading the previous tile
+      named_bar_sync(2, 32 * kGemmEpiWarps);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        *reinterpret_cast<float2*>(acc_tile + frow * Cfg::kAccPitch + 8 * j + fcol) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(acc_tile + (frow + 8) * Cfg::kAccPitch + 8 * j + fcol) =
+            make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+      }
+      named_bar_sync(2, 32 * kGemmEpiWarps);
+
+      const float* my_row = acc_tile + (ew * 32 + lane) * Cfg::kAccPitch;
 #pragma unroll 1
       for (int pass = 0; pass < Epi::kPasses; ++pass) {
         if constexpr (Epi::kPasses > 1) {
@@ -250,74 +253,33 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
             epi.between(st, row);
           }
         }
-        // Software-pipelined TMEM reads: the load of chunk c+1 is in flight while chunk c is processed.  The
-        // loop stays ROLLED over chunk pairs (two register buffers): fully unrolling it made the scan kernel
-        // 30 K SASS instructions and instruction-fetch bound (2.3x slower).
         const int c0 = half * kChunks;
-        auto run = [&](const uint32_t (&rb)[32], int c, bool has_next) {
+#pragma unroll 1
+        for (int c = c0; c < c0 + kChunks; ++c) {
           float v[32];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(rb[i]);
+          for (int i = 0; i < 8; ++i) {
+            const float4 t = *reinterpret_cast<const float4*>(my_row + c * 32 + 4 * i);
+            v[4 * i] = t.x, v[4 * i + 1] = t.y, v[4 * i + 2] = t.z, v[4 * i + 3] = t.w;
+          }
+          const bool has_next = c + 1 < c0 + kChunks;
           if constexpr (Epi::kPasses > 1)
             epi.chunk(st, row, n_blk * BN + c * 32, v, pass);
           else if constexpr (Epi::kPrefetch)
             epi.chunk(st, row, n_blk * BN + c * 32, v, has_next ? n_blk * BN + (c + 1) * 32 : -1);
           else
             epi.chunk(st, row, n_blk * BN + c * 32, v);
-        };
-        if constexpr (epi_rolled<Epi>::value) {
-          // heavy epilogues (hundreds of instructions per chunk): ONE copy of the chunk code, chunks processed in a rolled
-          // loop; the exposed TMEM-load latency (~100 cycles per chunk) is noise next to the chunk's own work, while
-          // three inlined copies (double-buffered loads + tail) made the kernel 4.7 K instructions and fetch-bound
-          uint32_t ra[32];
-#pragma unroll 1
-          for (int c = c0; c < c0 + kChunks; ++c) {
-            tmem_ld_32x32b_x32(taddr + c * 32, ra);
-            tmem_ld_wait();
-            run(ra, c, c + 1 < c0 + kChunks);
-          }
-          continue;
-        }
-        uint32_t ra[32], rb[32];
-        tmem_ld_32x32b_x32(taddr + c0 * 32, ra);
-        if constexpr (kChunks == 1) {
-          tmem_ld_wait();
-          run(ra, c0, false);
-        } else {
-#pragma unroll 1
-          for (int c = c0; c + 1 < c0 + kChunks; c += 2) {
-            tmem_ld_wait();
-            tmem_ld_32x32b_x32(taddr + (c + 1) * 32, rb);
-            run(ra, c, true);
-            tmem_ld_wait();
-            const bool more = c + 2 < c0 + kChunks;
-            if (more) tmem_ld_32x32b_x32(taddr + (c + 2) * 32, ra);
-            run(rb, c + 1, more);
-          }
-          if constexpr (kChunks % 2 == 1) {  // odd tail (e.g. BN = 192 with 8 epilogue warps: 3 chunks each)
-            tmem_ld_wait();
-            run(ra, c0 + kChunks - 1, false);
-          }
         }
       }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
       epi.end(st, row);
     }
-    if constexpr (Epi::smem_bytes(EPI_WARPS) > 0) epi.finish(st);  // drain whatever the functor still has in flight
+    if constexpr (Epi::smem_bytes(kGemmEpiWarps) > 0) epi.finish(st);  // drain whatever the functor still has in flight
   }
 
-  tc_fence_before_sync();
   __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, Cfg::kTmemCols);
-  }
+  if constexpr (CLUSTER > 1) cluster_sync_all();  // the peer may still be signalling this CTA's barriers
 }
 
-// Host launcher.  A: [M, K] bf16 row pitch lda elements; B: [N, K] bf16 row pitch ldb elements.
-// Returns cudaSuccess / a CUDA error; tensor-map failures map to cudaErrorInvalidValue.
 // Pool of tile counters for the dynamic scheduler: launch i uses counter i % 64 (zeroed on the launching stream
 // just before the kernel), so up to 64 dynamically scheduled GEMMs may be in flight.
 static inline int* next_tile_counter(cudaStream_t stream) {
@@ -329,11 +291,13 @@ static inline int* next_tile_counter(cudaStream_t stream) {
   return c;
 }
 
-// dynamic_sched: claim tiles from a global counter instead of the static blockIdx + i * gridDim order.  With
-// the static order CTAs drift apart over thousands of tiles and stop sharing operand tiles in L2 (measured on
-// the search scan: 143 GB of DRAM reads for a 6.4 GB shard); the dynamic order keeps all CTAs on neighbouring
-// tiles.
-template <int BN, int STAGES, bool M_FASTEST, int EPI_WARPS, class Epi, bool F16 = false>
+// Host launcher.  A: [M, K] row pitch lda elements; B: [N, K] row pitch ldb elements (bf16, or IEEE half with F16).
+// Returns cudaSuccess / a CUDA error; tensor-map failures map to cudaErrorInvalidValue.
+// dynamic_sched: claim tiles from a global counter instead of the static blockIdx + i * gridDim order, which keeps all
+// CTAs on neighbouring tiles (with the static order CTAs drift apart over thousands of tiles and stop sharing operand
+// tiles in L2).  CLUSTER = 2 (CTA pairs sharing B by multicast) always uses the static order; it returns
+// cudaErrorNotSupported if no cluster of the kernel fits on the device.
+template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16 = false, int CLUSTER = 1>
 static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
                                       const Epi& epi, int num_sms, cudaStream_t stream, bool dynamic_sched = false) {
   using Cfg = GemmCfg<BN, STAGES>;
@@ -341,26 +305,54 @@ static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B,
   CUtensorMap tmA, tmB;
   if (make_tmap_bf16_2d(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, kBlockK, kBlockM) != 0)
     return cudaErrorInvalidValue;
-  if (make_tmap_bf16_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, kBlockK, BN) != 0)
+  if (make_tmap_bf16_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, kBlockK, BN / CLUSTER) != 0)
     return cudaErrorInvalidValue;
-  auto kern = gemm_bf16_tn_kernel<BN, STAGES, M_FASTEST, EPI_WARPS, Epi, F16>;
+  auto kern = gemm_bf16_tn_kernel<BN, STAGES, M_FASTEST, Epi, F16, CLUSTER>;
+  const int smem_bytes = Cfg::kSmemBytes + Epi::smem_bytes(kGemmEpiWarps);
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::kSmemBytes + Epi::smem_bytes(EPI_WARPS));
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_bytes);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const int num_tiles = ((M + kBlockM - 1) / kBlockM) * ((N + BN - 1) / BN);
-  const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-  int* counter = nullptr;
-  if (dynamic_sched) {
-    counter = next_tile_counter(stream);
-    if (!counter) return cudaErrorMemoryAllocation;
+  const int num_m = (M + kBlockM - 1) / kBlockM;
+  const int num_tiles = ((num_m + CLUSTER - 1) / CLUSTER) * ((N + BN - 1) / BN);
+  const int threads = kGemmProducerThreads + 32 * kGemmEpiWarps;
+  if constexpr (CLUSTER > 1) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(threads);
+    cfg.dynamicSmemBytes = smem_bytes;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CLUSTER;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    // the persistent schedule wants every cluster co-resident (a second wave of clusters would double the run time)
+    static int max_clusters = 0;  // per instantiation
+    if (!max_clusters) {
+      cfg.gridDim = dim3(CLUSTER * (num_sms / CLUSTER));
+      int n = 0;
+      cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
+      if (e != cudaSuccess) return e;
+      if (n < 1) return cudaErrorNotSupported;
+      max_clusters = n < num_sms / CLUSTER ? n : num_sms / CLUSTER;
+    }
+    const int clusters = num_tiles < max_clusters ? num_tiles : max_clusters;
+    cfg.gridDim = dim3(CLUSTER * clusters);
+    return cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, epi, static_cast<int*>(nullptr));
+  } else {
+    const int grid = num_tiles < num_sms ? num_tiles : num_sms;
+    int* counter = nullptr;
+    if (dynamic_sched) {
+      counter = next_tile_counter(stream);
+      if (!counter) return cudaErrorMemoryAllocation;
+    }
+    kern<<<grid, threads, smem_bytes, stream>>>(tmA, tmB, M, N, K, epi, counter);
+    return cudaGetLastError();
   }
-  kern<<<grid, kGemmProducerThreads + 32 * EPI_WARPS, Cfg::kSmemBytes + Epi::smem_bytes(EPI_WARPS), stream>>>(tmA, tmB, M, N, K,
-                                                                                                     epi, counter);
-  return cudaGetLastError();
 }
 
 // --------------------------------------------------------------------------------------------------

@@ -1,11 +1,11 @@
-// In-batch-negatives contrastive loss, forward + backward, as ONE persistent tcgen05 kernel, replacing
+// In-batch-negatives contrastive loss, forward + backward, as ONE persistent wgmma kernel, replacing
 //   logits = x @ y.T ; F.cross_entropy(logits, target)          src/openmatch/loss.py:7-15
 //   scores = q_reps @ p_reps.T ; CrossEntropyLoss(mean)          src/openmatch/modeling/dense_retrieval_model.py:113-122
 // and their autograd backward (~8 PyTorch launches forward, as many backward).
 //
 // loss_fused_kernel: cooperative grid (<= 1 CTA per SM), phases separated by grid barriers; every GEMM runs on the
-// tcgen05 pipeline of gemm.cuh's design (TMA -> 4-stage smem ring -> tcgen05.mma 128x128x16 -> TMEM -> tcgen05.ld
-// epilogue), with the pipeline state carried from phase to phase:
+// pipeline of gemm.cuh's design (TMA -> 4-stage smem ring -> one consumer warpgroup issuing wgmma 2 x (64x128x16), fp32
+// accumulators in registers -> stores), with the pipeline state carried from phase to phase:
 //   PREP    fp32 (or unaligned) inputs only: Q, P -> bf16 row-major copies.  Aligned bf16 inputs are read in place.
 //   LOGITS  S = Q P^T, fp32 [nq, np]                      (A = Q, B = P, both K-major)
 //   SOFTMAX one warp per query row, the row in registers: log-sum-exp (fp32), loss_i = lse_i - s_i,t_i,
@@ -17,6 +17,7 @@
 // or G is ever written.
 #include <algorithm>
 #include <cstdlib>
+#include <type_traits>
 
 #include "common.h"
 #include "gemm.cuh"
@@ -27,7 +28,12 @@ namespace om {
 #define OM_LOSS_STAGES 4
 #endif
 constexpr int kLossBN = 128, kLossStages = OM_LOSS_STAGES, kLossThreads = 256;
-using LossCfg = GemmCfg<kLossBN, kLossStages>;
+struct LossCfg {
+  static constexpr int kABytes = kBlockM * kBlockK * 2;
+  static constexpr int kStageBytes = kABytes + kLossBN * kBlockK * 2;
+  static constexpr int kBarOffset = kLossStages * kStageBytes;
+  static constexpr int kSmemBytes = kBarOffset + 1024 + 1024;  // barriers + slack for 1024-B alignment of the base
+};
 
 // [0] logits (Q, P)   [1] dQ (G, P)   [2] dP (G, Q); 128-B swizzle; K-major operands: boxes {64 k, 128 rows},
 // MN-major operands: boxes {64 mn, 64 k} (two per stage)
@@ -92,27 +98,33 @@ __device__ __forceinline__ void grid_sync(unsigned* bar) {
   __syncthreads();
 }
 
-constexpr int kStgPitch = 36, kStgFloats = 32 * kStgPitch;  // epilogue staging tile per warp: 32 x 32 fp32, padded rows
-constexpr int kLossSmemBytes = LossCfg::kSmemBytes + 4 * kStgFloats * 4;
+constexpr int kLossSmemBytes = LossCfg::kSmemBytes;
 
 struct LossSmem {
   uint8_t* ring;
-  float* stage;
-  uint64_t *full_bar, *empty_bar, *tfull_bar, *tempty_bar;
-  uint32_t tmem_base;
+  uint64_t *full_bar, *empty_bar;
 };
-struct Pipe {  // per-thread pipeline position, carried across the GEMM phases (every role advances identically)
+struct Pipe {  // per-thread pipeline position, carried across the GEMM phases (producer and consumers advance identically)
   uint32_t stage = 0, phase = 0;
-  int it = 0;
 };
 
 // MN-major operand tile in shared memory: two TMA boxes {64 mn, 64 k} back to back.  Inside a box the 64 mn elements
 // of one k are a 128-byte row, 8 such rows form a 1024-byte swizzle atom (stride between 8-k groups, SBO = 1024 B);
-// the second 64 mn elements live in the second box (LBO = 8192 B).  One MMA (K = 16) consumes two 8-k groups, so the
-// descriptor start address advances by 2048 B per MMA.
+// the second 64 mn elements live in the second box (LBO = 8192 B).  One wgmma (K = 16) consumes two 8-k groups, so the
+// descriptor start address advances by 2048 B per instruction.
 constexpr uint32_t kMnBoxBytes = 64 * kBlockK * 2;
 constexpr int kMaxSplit = 4;  // K slices per output tile of the split GEMM
-constexpr uint64_t kDescMNMajorSW128 = umma_smem_desc_base(kMnBoxBytes, 1024, kSwizzle128B);
+constexpr uint64_t kDescMNMajorSW128 = wgmma_desc_base(kMnBoxBytes, 1024);
+
+// 64 x 128 x 16 step of the 64-row half `h` of the tile; A_MN / B_MN: operand stored MN-major
+template <bool A_MN, bool B_MN>
+__device__ __forceinline__ void loss_mma_k16(float (&acc)[64], uint32_t a_addr, uint32_t b_addr, int h, int k,
+                                             uint32_t accumulate) {
+  // K-major: the half is 64 rows further (8 KB), a K step 32 B; MN-major: the half is the second box (8 KB), a K step 2 KB
+  const uint64_t da = wgmma_desc(a_addr + h * 8192 + k * (A_MN ? 2048 : 32), A_MN ? kDescMNMajorSW128 : kDescKMajorSW128);
+  const uint64_t db = wgmma_desc(b_addr + k * (B_MN ? 2048 : 32), B_MN ? kDescMNMajorSW128 : kDescKMajorSW128);
+  wgmma_m64n128k16_bf16<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da, db, accumulate);
+}
 
 // One GEMM of the kernel: C[M, N] fp32 (row pitch ldc) = A B^T with A [M, K], B [N, K]; a_mn / b_mn say that the
 // operand is stored [K, M] / [K, N] (MN-major) instead of K-major.  S > 1 splits K into S slices (see gemm_phase).
@@ -176,98 +188,79 @@ __device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const Los
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {  // MMA issuer
-      const uint32_t idesc = umma_idesc_bf16(kBlockM, kLossBN, g.a_mn ? 1u : 0u, g.b_mn ? 1u : 0u);
-      const uint64_t a_base = g.a_mn ? kDescMNMajorSW128 : kDescKMajorSW128;
-      const uint64_t b_base = g.b_mn ? kDescMNMajorSW128 : kDescKMajorSW128;
-      const uint32_t a_step = g.a_mn ? kUmmaK * 128u : kUmmaK * 2u, b_step = g.b_mn ? kUmmaK * 128u : kUmmaK * 2u;
-      int tslot = g.tb;
-      for (int item = first; item < num_items; item += G, ++pipe.it, tslot += 8) {
-        const uint32_t as = pipe.it & 1, aphase = (pipe.it >> 1) & 1;
-        mbar_wait(&sm.tempty_bar[as], aphase ^ 1u, 2);
-        tc_fence_after_sync();
-        const uint32_t d_tmem = sm.tmem_base + as * kLossBN;
-        const int ks = item % S, kb_begin = ks * kper, kb_end = min(num_k, kb_begin + kper);
-        for (int kb = kb_begin; kb < kb_end; ++kb) {
-          mbar_wait(&sm.full_bar[pipe.stage], pipe.phase, 3);
-          tc_fence_after_sync();
-          if (kb == kb_begin) OM_TRACE(tslot + 1);
-          const uint32_t a_addr = smem_u32(sm.ring + pipe.stage * LossCfg::kStageBytes);
-          const uint32_t b_addr = a_addr + LossCfg::kABytes;
-#pragma unroll
-          for (int k = 0; k < kBlockK / kUmmaK; ++k) {
-            const uint64_t da = umma_smem_desc(a_addr + k * a_step, a_base);
-            const uint64_t db = umma_smem_desc(b_addr + k * b_step, b_base);
-            umma_bf16_ss(d_tmem, da, db, idesc, ((kb - kb_begin) | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&sm.empty_bar[pipe.stage]);
-          if (++pipe.stage == kLossStages) {
-            pipe.stage = 0;
-            pipe.phase ^= 1u;
-          }
-        }
-        umma_commit(&sm.tfull_bar[as]);
-        OM_TRACE(tslot + 2);
-      }
-    }
-  } else if (warp >= 4) {  // epilogue: warp w owns TMEM lanes [32 (w % 4), +32) = rows of the tile
+  } else if (warp >= 4) {  // consumer warpgroup: wgmma for both 64-row halves of the tile, then stores
     const int ew = warp & 3;
     int tslot = (ew == 0 && lane == 0) ? g.tb : -1000;
-    for (int item = first; item < num_items; item += G, ++pipe.it, tslot += 8) {
+    for (int item = first; item < num_items; item += G, tslot += 8) {
       const int tile = item / S, ks = item - tile * S;
       const int m_blk = tile / num_n, n_blk = tile % num_n;
-      const uint32_t as = pipe.it & 1, aphase = (pipe.it >> 1) & 1;
+      const int kb_begin = ks * kper, kb_end = min(num_k, kb_begin + kper);
       float* Cw = S > 1 ? g.part + static_cast<int64_t>(ks) * M * ldc : g.C;
-      mbar_wait_warp(&sm.tfull_bar[as], aphase, 4);
-      tc_fence_after_sync();
+      float acc[2][64];
+      uint32_t prev_stage = 0;
+      for (int kb = kb_begin; kb < kb_end; ++kb) {
+        mbar_wait_warp(&sm.full_bar[pipe.stage], pipe.phase, 3);
+        if (kb == kb_begin) OM_TRACE(tslot + 1);
+        const uint32_t a_addr = smem_u32(sm.ring + pipe.stage * LossCfg::kStageBytes);
+        const uint32_t b_addr = a_addr + LossCfg::kABytes;
+        // operand majors are immediates of the instruction: one fully unrolled k block per layout
+        auto issue = [&](auto a_mn, auto b_mn) {
+#pragma unroll
+          for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+            const uint32_t accum = ((kb - kb_begin) | k) != 0 ? 1u : 0u;
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              loss_mma_k16<decltype(a_mn)::value, decltype(b_mn)::value>(acc[h], a_addr, b_addr, h, k, accum);
+          }
+        };
+        wgmma_fence();
+        if (!g.a_mn && !g.b_mn) issue(std::false_type{}, std::false_type{});
+        else if (!g.a_mn) issue(std::false_type{}, std::true_type{});
+        else if (g.b_mn) issue(std::true_type{}, std::true_type{});
+        else issue(std::true_type{}, std::false_type{});
+        wgmma_commit();
+        if (kb > kb_begin) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(&sm.empty_bar[prev_stage]);
+        }
+        prev_stage = pipe.stage;
+        if (++pipe.stage == kLossStages) {
+          pipe.stage = 0;
+          pipe.phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc[0]);
+      wgmma_fence_regs(acc[1]);
+      if (lane == 0) mbar_arrive(&sm.empty_bar[prev_stage]);
       OM_TRACE(tslot + 3);
-      const uint32_t taddr = sm.tmem_base + as * kLossBN + (static_cast<uint32_t>(ew * 32) << 16);
-      // accumulator chunk (lane = row, 32 columns) -> warp-private staging tile -> global rows: every store
-      // instruction writes four complete 128-byte lines (16-byte pieces of a line from 32 different rows would make
-      // L2 fetch every sector from HBM before merging the write)
-      float* stg = sm.stage + ew * kStgFloats;
-      const bool vec = (ldc & 3) == 0 && (reinterpret_cast<uintptr_t>(Cw) & 15) == 0;
-      const int rr = lane >> 3, cc = (lane & 7) * 4, row_base = m_blk * kBlockM + ew * 32;
-#pragma unroll 1
-      for (int c = 0; c < kLossBN / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld_32x32b_x32(taddr + c * 32, r);
-        tmem_ld_wait();
-        __syncwarp();  // the previous chunk has been read out of the staging tile
+      // fragments -> global: every quad of lanes writes 32 consecutive bytes of a row (whole sectors)
+      const bool vec = (ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(Cw) & 7) == 0;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          *reinterpret_cast<float4*>(stg + lane * kStgPitch + 4 * j) =
-              make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                          __uint_as_float(r[4 * j + 3]));
-        __syncwarp();
-        const int col = n_blk * kLossBN + c * 32 + cc;
+      for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int rw = row_base + i * 4 + rr;
-          const float4 v = *reinterpret_cast<const float4*>(stg + (i * 4 + rr) * kStgPitch + cc);
-          if (rw < M) {
-            float* out = Cw + static_cast<int64_t>(rw) * ldc + col;
-            if (vec && col + 4 <= N) {
-              *reinterpret_cast<float4*>(out) = v;
+        for (int u = 0; u < 2; ++u) {
+          const int rw = m_blk * kBlockM + h * 64 + ew * 16 + (lane >> 2) + 8 * u;
+          if (rw >= M) continue;
+          float* out = Cw + static_cast<int64_t>(rw) * ldc;
+#pragma unroll
+          for (int j = 0; j < kLossBN / 8; ++j) {
+            const int col = n_blk * kLossBN + 8 * j + 2 * (lane & 3);
+            const float v0 = acc[h][4 * j + 2 * u], v1 = acc[h][4 * j + 2 * u + 1];
+            if (vec && col + 2 <= N) {
+              *reinterpret_cast<float2*>(out + col) = make_float2(v0, v1);
             } else {
-              if (col < N) out[0] = v.x;
-              if (col + 1 < N) out[1] = v.y;
-              if (col + 2 < N) out[2] = v.z;
-              if (col + 3 < N) out[3] = v.w;
+              if (col < N) out[col] = v0;
+              if (col + 1 < N) out[col + 1] = v1;
             }
           }
         }
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&sm.tempty_bar[as]);
       OM_TRACE(tslot + 4);
       if (S > 1) {
         // all S slices of a tile run at the same time on different CTAs: each waits for the others and then adds
         // the S partials of ITS share of the warp's 32 rows, in slice order
         __threadfence();  // this lane's partial rows are visible before the counter moves
-        __syncwarp();
+        named_bar_sync(5, 128);  // ... and those of the whole warpgroup (a warp stored rows of other warps' shares)
         unsigned* arrive = &g.sem[(tile * 4 + ew) * 2];
         if (lane == 0) {
           atomicAdd(arrive, 1u);
@@ -373,12 +366,8 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   LossSmem sm;
   sm.ring = smem;
-  sm.stage = reinterpret_cast<float*>(smem + LossCfg::kEpiOffset);
   sm.full_bar = reinterpret_cast<uint64_t*>(smem + LossCfg::kBarOffset);
   sm.empty_bar = sm.full_bar + kLossStages;
-  sm.tfull_bar = sm.empty_bar + kLossStages;
-  sm.tempty_bar = sm.tfull_bar + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm.tempty_bar + 2);
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = static_cast<int>(threadIdx.x & 31);
   const int G = static_cast<int>(gridDim.x);
@@ -392,22 +381,11 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kLossStages; ++i) {
       mbar_init(&sm.full_bar[i], 1);
-      mbar_init(&sm.empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&sm.tfull_bar[i], 1);
-      mbar_init(&sm.tempty_bar[i], 4);  // one arrive per epilogue warp
+      mbar_init(&sm.empty_bar[i], 4);  // one arrive per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, LossCfg::kTmemCols);
-    tmem_relinquish();
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  sm.tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
   Pipe pipe;
 
   // ------------------------------ PREP ------------------------------
@@ -560,13 +538,6 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
   }
   if (warp >= 4 && lane == 0) atomicMax(&a.ts[4], global_timer_ns());
   if (warp == 4 && lane == 0) OM_TRACE(61);
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after_sync();
-    tmem_dealloc(sm.tmem_base, LossCfg::kTmemCols);
-  }
 }
 
 struct LossWs {

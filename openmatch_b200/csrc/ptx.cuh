@@ -1,5 +1,6 @@
-// Inline-PTX primitives for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma /
-// commit / ld), UMMA shared-memory + instruction descriptors.  Hand-written; no CUTLASS dependency.
+// Inline-PTX primitives for sm_90a: mbarrier, TMA (cp.async.bulk.tensor, with cluster multicast), wgmma
+// (warpgroup MMA, operands in shared memory or A in registers) and its shared-memory matrix descriptors.
+// Hand-written; no CUTLASS dependency.
 //
 // Every blocking wait is bounded: a wait that exceeds OM_WAIT_TIMEOUT_CYCLES records a diagnostic
 // code in the translation unit's fault word and returns; every other waiter then bails out as soon as
@@ -78,7 +79,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parity, uint32_t site) {
   // try_wait suspends the thread in hardware until the phase completes or a time limit expires, so this
   // loop is not a busy spin.  The fault word (a global load, ~1 us) and the clock are consulted only every
-  // 1024 wake-ups: polling them on every iteration added a DRAM round trip to every pipeline hand-off.
+  // 1024 wake-ups: polling them on every iteration would add a DRAM round trip to every pipeline hand-off.
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -101,7 +102,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
 }
 // Warp-collective wait for consumer warps: lane 0 polls (with a short sleep between probes), the rest of the
 // warp parks at __syncwarp.  Hundreds of threads spinning on try_wait compete with the TMA/MMA threads for
-// the barrier unit: measured 2x slowdown of the scan kernel when all 256 epilogue threads polled.
+// the barrier unit.
 __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity, uint32_t site) {
 #ifdef OM_EPI_ALL_LANES_WAIT
   if (!mbar_try_wait(bar, parity)) {
@@ -190,91 +191,108 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   return p;
 }
 
-// ----------------------------------------------------------------------------------------------
-// tcgen05: tensor memory allocation, MMA issue, commit, TMEM loads
-// ----------------------------------------------------------------------------------------------
-// Whole-warp collective. ncols: power of two in [32, 512]. The base TMEM address lands in *dst_smem.
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-               "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single-thread issue. accumulate==0 overwrites D.
-__device__ __forceinline__ void umma_bf16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                             uint32_t accumulate) {
+
+// TMA load of one box into the same shared-memory offset of every CTA in `cta_mask` (cluster multicast); the
+// transaction bytes complete on the mbarrier at the same offset in each destination CTA.
+__device__ __forceinline__ void tma_load_2d_multicast(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
+                                                      int32_t c1, uint16_t cta_mask) {
   asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}\n"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
+      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
+      " [%0], [%1, {%3, %4}], [%2], %5;"
+      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
+      "h"(cta_mask)
       : "memory");
 }
-// Arrive (count 1) on `bar` once all previously issued tcgen05.mma of this thread have completed.
-// Implies tcgen05.fence::before_thread_sync.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-// Warp-collective: lane t receives 32 consecutive fp32 columns of TMEM lane (lane_base + t).
-__device__ __forceinline__ void tmem_ld_32x32b_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ----------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layout per PTX ISA "tcgen05 matrix descriptor" / "instruction descriptor")
+// clusters
 // ----------------------------------------------------------------------------------------------
-// Shared-memory operand descriptor.
-//   [0,14)  start address >> 4        [16,30) leading byte offset >> 4     [32,46) stride byte offset >> 4
-//   [46,48) descriptor version (1 on sm_100)   [49,52) base offset   [61,64) swizzle (2 = 128 B)
-__host__ __device__ constexpr uint64_t umma_smem_desc_base(uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                           uint32_t layout_type) {
-  return (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16) |
-         (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 46) |
-         (static_cast<uint64_t>(layout_type & 7u) << 61);
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
 }
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr, uint64_t base) {
+__device__ __forceinline__ uint32_t cluster_id_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ uint32_t cluster_count_x() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
+  return r;
+}
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at the address of `bar` in the shared memory of the cluster's CTA `rank`
+__device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n"
+      ::"r"(smem_u32(bar)), "r"(rank)
+      : "memory");
+}
+
+// ----------------------------------------------------------------------------------------------
+// wgmma: warpgroup (4 warps, 128 threads) MMA, fp32 accumulators in registers
+// ----------------------------------------------------------------------------------------------
+// Accumulator fragment of an m64nN tile for thread t of the warpgroup (warp w = t / 32, lane l):
+//   d[4 j + 0, 1] = C[16 w + l / 4,     8 j + 2 (l % 4) + {0, 1}]
+//   d[4 j + 2, 3] = C[16 w + l / 4 + 8, 8 j + 2 (l % 4) + {0, 1}]
+// The A register fragment of an m64k16 step has the same shape: a[0..3] = packed (d[0,1]), (d[2,3]), (d[4,5]), (d[6,7])
+// of the two 8-column blocks that make up the 16 columns.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// Keeps the compiler from moving accumulator reads / writes across an asynchronous wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// Shared-memory matrix descriptor (sm_90):
+//   [0,14) start address >> 4   [16,30) leading byte offset >> 4   [32,46) stride byte offset >> 4   [62,64) swizzle (1 = 128 B)
+__host__ __device__ constexpr uint64_t wgmma_desc_base(uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  return (static_cast<uint64_t>((lbo_bytes >> 4) & 0x3fffu) << 16) |
+         (static_cast<uint64_t>((sbo_bytes >> 4) & 0x3fffu) << 32) | (1ull << 62);
+}
+__device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr, uint64_t base) {
   return base | static_cast<uint64_t>((smem_addr & 0x3ffffu) >> 4);
 }
-constexpr uint32_t kSwizzle128B = 2;  // UMMA layout_type encoding
-// K-major operand, rows of 64 bf16 (=128 B) swizzled in 8-row / 1024-B atoms (what a TMA box of
-// {64 elems, R rows} with CU_TENSOR_MAP_SWIZZLE_128B produces): SBO = 1024 B between 8-row groups.
-constexpr uint64_t kDescKMajorSW128 = umma_smem_desc_base(16, 1024, kSwizzle128B);
+// K-major operand, rows of 64 bf16 (= 128 B) swizzled in 8-row / 1024-B atoms (what a TMA box of {64 elems, R rows}
+// with CU_TENSOR_MAP_SWIZZLE_128B produces): SBO = 1024 B between 8-row groups; the leading offset is unused.  A K step
+// of 16 elements advances the start address by 32 B.
+constexpr uint64_t kDescKMajorSW128 = wgmma_desc_base(16, 1024);
 
-// Instruction descriptor for kind::f16 with BF16 A/B, FP32 accumulate.
-//   [4,6) D fmt (1=f32)  [7,10) A fmt (1=bf16)  [10,13) B fmt  [15] A major (0=K)  [16] B major
-//   [17,23) N>>3   [24,29) M>>4
-// A and B in IEEE fp16 (format code 0), fp32 accumulate, K-major operands
-__host__ __device__ constexpr uint32_t umma_idesc_f16(uint32_t M, uint32_t N) {
-  return (1u << 4) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// TA / TB: 0 = operand K-major, 1 = MN-major (transposed).  accumulate == 0 overwrites d.
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_bf16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
 }
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N, uint32_t a_mn_major = 0,
-                                                       uint32_t b_mn_major = 0) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-         ((M >> 4) << 24);
+template <int TA, int TB>
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, %67, %68;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate), "n"(TA), "n"(TB));
+}
+__device__ __forceinline__ void wgmma_m64n64k16_bf16_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate));
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -284,29 +302,10 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-// Packed fp32x2 arithmetic (sm_100: FFMA2 — two fp32 FMAs per issue slot); used by issue-bound epilogues.
-__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  unsigned long long r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;"
-      : "=l"(r)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)),
-        "l"(*reinterpret_cast<unsigned long long*>(&c)));
-  return *reinterpret_cast<float2*>(&r);
-}
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  unsigned long long r;
-  asm("mul.rn.f32x2 %0, %1, %2;"
-      : "=l"(r)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&r);
-}
-__device__ __forceinline__ float2 add2(float2 a, float2 b) {
-  unsigned long long r;
-  asm("add.rn.f32x2 %0, %1, %2;"
-      : "=l"(r)
-      : "l"(*reinterpret_cast<unsigned long long*>(&a)), "l"(*reinterpret_cast<unsigned long long*>(&b)));
-  return *reinterpret_cast<float2*>(&r);
-}
+// fp32 pairs, element-wise (two FFMA each)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 splat2(float x) { return make_float2(x, x); }
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

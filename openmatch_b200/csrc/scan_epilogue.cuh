@@ -1,5 +1,4 @@
-// Fused top-k filter epilogue of the search scan GEMM + candidate key encoding (shared by search.cu and the
-// bring-up probe selftest_gemm.cu).
+// Fused top-k filter epilogue of the search scan GEMM + candidate key encoding.
 #pragma once
 #include <string.h>
 
@@ -43,10 +42,7 @@ __host__ __device__ __forceinline__ float key_score(unsigned long long k) {
 // ---------------------------------------------------------------------------------------------------
 // fused scan epilogue
 // ---------------------------------------------------------------------------------------------------
-// Filter shape: one 32-column max (3-input max tree), then a 32-bit mask and a 31-SEL select tree per survivor.  Three
-// alternative shapes (group maxima of 8 columns with 8-bit masks, rolled or unrolled; warp-cooperative extraction with
-// shuffles + ballot) were measured in round 2 against this one at five survivor densities: all within +-1 %
-// (profiles/r02_scan_variants_selftest.log), the warp-cooperative one 13 % slower at high density — removed.
+// Filter shape: one 32-column max (3-input max tree), then a 32-bit mask and a 31-SEL select tree per survivor.
 template <bool DENSE, int EPI_THREADS = 256>
 struct EpiScan {
   const float* thr;          // [nq] strict lower bound per query
@@ -154,7 +150,7 @@ struct EpiScan {
     if (!(mx > t)) return;  // common case: nothing in this chunk beats the threshold
     // Survivor path.  Kept deliberately COMPACT (a bit mask + a short loop with a select tree instead of 32
     // unrolled predicated blocks): it is executed rarely per warp, so its instructions are cold in the
-    // instruction cache and every extra cache line costs hundreds of cycles (measured ~1000 cycles per
+    // instruction cache and every extra cache line costs hundreds of cycles (~1000 cycles per
     // survivor with the unrolled form).
     uint32_t mask = 0;
 #pragma unroll

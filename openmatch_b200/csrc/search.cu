@@ -1,15 +1,15 @@
-// Exact inner-product top-k over an HBM-resident flat index — the B200 replacement of
+// Exact inner-product top-k over an HBM-resident flat index — the H100 replacement of
 // faiss.IndexFlatIP.{add,search,reset} as the reference uses it
 // (src/openmatch/retriever/dense_retriever.py:38-41,105,133-137,180) and of the IndexShards merge behind
 // index_cpu_to_gpu_multiple(shard=True) (:43-58).
 //
 // Storage per index shard: fp32 master rows [n, d] (what index.add received; used for exact re-scoring)
 // plus an fp16 scan copy [n, dpad] (tensor-core operand; IEEE half keeps 3 more significand bits than bf16 at the
-// same tcgen05 rate, which is what makes the exactness certificate below affordable).
+// same tensor-core rate, which is what makes the exactness certificate below affordable).
 //
 // search(q, k):
-//   1. SCAN    fp16 Q * X^T on tcgen05 (gemm.cuh mainloop) with the top-k filter fused into the epilogue:
-//              scores never leave TMEM/registers; a thread owns one query row, compares its 32-column chunk
+//   1. SCAN    fp16 Q * X^T on wgmma (gemm.cuh mainloop) with the top-k filter fused into the epilogue:
+//              scores never leave the SM (registers / shared memory); a thread owns one query row, compares its 32-column chunk
 //              against that query's running threshold and appends the rare survivors
 //              (key = orderable(score) << 32 | ~row) to the query's candidate list in HBM.
 //              The corpus is swept in rounds of geometrically growing size; after each round
@@ -38,7 +38,6 @@
 
 #include "common.h"
 #include "gemm.cuh"
-#include "gemm2sm.cuh"
 #include "nccl_dyn.h"
 #include "scan_epilogue.cuh"
 
@@ -707,10 +706,10 @@ struct om_index {
   int64_t rescore_slack = -1;
   int force_safe = 0;
   int dynamic_sched = 1;  // claim scan tiles from a global counter (keeps CTAs on neighbouring corpus tiles)
-  int pair_scan = 1;      // scan GEMM on CTA pairs (cta_group::2, gemm2sm.cuh); 0 = the single-CTA core of gemm.cuh
-  int growth = 0;         // each round scans (growth - 1) x the rows seen so far; 0 = auto: 2 for query batches (measured
-                          // best at nq = 6 980: fewest filter survivors), 8 for <= 256 queries (HBM-bound streaming
-                          // regime: 5 instead of 13 dependent scan + select launch pairs over 8.8 M rows)
+  int pair_scan = 1;      // scan GEMM on 2-CTA clusters sharing each corpus tile by TMA multicast; 0 = single-CTA tiles
+  int growth = 0;         // each round scans (growth - 1) x the rows seen so far; 0 = auto: 2 for query batches (fewest
+                          // filter survivors), 8 for <= 256 queries (HBM-bound streaming regime: 5 instead of 13
+                          // dependent scan + select launch pairs over 8.8 M rows)
   int certify = 1;        // 0: legacy behaviour (top-k of the half-precision candidate stage, no proof)
   int exact_only = 0;     // 1: answer every query with the exact fp32 scan (testing / reference timing)
   int stage_scores = 0;   // 1: emit candidate-stage scores instead of fp32 re-scores (measuring the error model)
@@ -757,7 +756,7 @@ static int index_grow(om_index* ix, int64_t need) {
 
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
-  return static_cast<int>(std::min<int64_t>(std::max<int64_t>(g, 1), 148 * 16));
+  return static_cast<int>(std::min<int64_t>(std::max<int64_t>(g, 1), 132 * 16));
 }
 
 extern "C" {
@@ -1077,19 +1076,19 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         cudaError_t e = cudaErrorNotSupported;
         const bool dynsched = ix->dynamic_sched != 0;
         const int ncols = static_cast<int>(step);
-        // CTA pairs own 256 query rows per tile: with <= 128 queries the peer's half would be padding (and the sweep is
-        // HBM-bound there: the single-CTA ring keeps more corpus bytes in flight per SM)
+        // a 2-CTA cluster owns 2 x 128 query rows per tile: with <= 128 queries the peer's half would be padding (and the sweep is
+        // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing)
         const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
         if (first) {
           EpiScan<true> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          if (pair) e = launch_gemm2<5, true, 8, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
-          if (e == cudaErrorNotSupported)  // no CTA pair fits (a device without two free SMs per TPC)
-            e = launch_gemm<256, 4, true, 8, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
+          if (pair) e = launch_gemm<128, 3, true, EpiScan<true>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
+          if (e == cudaErrorNotSupported)  // no 2-CTA cluster fits on the device
+            e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
         } else {
           EpiScan<false> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          if (pair) e = launch_gemm2<5, true, 8, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
+          if (pair) e = launch_gemm<128, 3, true, EpiScan<false>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
           if (e == cudaErrorNotSupported)
-            e = launch_gemm<256, 4, true, 8, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
+            e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
         }
         if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
       } else {

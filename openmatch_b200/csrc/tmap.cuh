@@ -28,7 +28,7 @@ static inline PFN_tmapEncodeTiled tmap_encode_fn() {
 
 // 2-D row-major bf16 tensor [rows, inner] with row pitch `row_stride_bytes` (multiple of 16), tiled into
 // boxes of {box_inner (= 64 elements = 128 B), box_rows (<= 256)} with the 128-byte swizzle — the layout
-// tcgen05.mma consumes as a K-major SWIZZLE_128B operand.  Out-of-bounds elements read as zero.
+// wgmma consumes as a K-major SWIZZLE_128B operand.  Out-of-bounds elements read as zero.
 // Returns 0 on success, else the CUresult (or -1 when the driver entry point is unavailable).
 // (also used for TMA stores: box {64, 32} of a bf16 output matrix)
 static inline int make_tmap_bf16_2d(CUtensorMap* out, const void* gptr, uint64_t inner, uint64_t rows,

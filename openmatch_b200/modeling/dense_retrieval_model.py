@@ -5,7 +5,7 @@
 
 Two execution paths, chosen per call:
   * inference (no autograd: ``DRModelForInference``, or ``DRModel`` in eval mode under ``torch.no_grad``):
-    the whole encode -> pool -> head -> normalise sequence runs in the hand-written sm_100a encoder
+    the whole encode -> pool -> head -> normalise sequence runs in the hand-written sm_90a encoder
     (``openmatch_b200.encoder.CudaEncoder`` -> csrc/encoder.cu).  CUDA tensors only, no fallback.
   * training (autograd needed): the HF module runs under PyTorch autograd (the CUDA encoder is
     forward-only); scores, log-softmax, loss and the rep gradients come from the fused loss kernel
@@ -120,7 +120,7 @@ class DRModel(nn.Module):
             # decoder last_hidden_state[:, 0].  The decoder is outside the CUDA encoder (GTR / --encoder_only is the hot
             # path, SURVEY 8(a4)), so this mode runs the HF module on the GPU — for training and for inference alike.
             if not getattr(self, "_warned_decoder_path", False):
-                logger.warning("encoder-decoder T5 pooling runs the HuggingFace module (not the sm_100a encoder); "
+                logger.warning("encoder-decoder T5 pooling runs the HuggingFace module (not the sm_90a encoder); "
                                "use --encoder_only for the accelerated path")
                 self._warned_decoder_path = True
             dec = torch.zeros((items["input_ids"].shape[0], 1), dtype=torch.long, device=items["input_ids"].device)

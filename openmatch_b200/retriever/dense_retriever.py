@@ -4,10 +4,10 @@
 ``SuccessiveRetriever``; ``FaissRetriever`` is the successor repo's name for the same class.
 
 What changed underneath:
-  * embeddings come from the sm_100a encoder and are written straight into this rank's HBM index shard
+  * embeddings come from the sm_90a encoder and are written straight into this rank's HBM index shard
     (zero-copy ``reserve_rows``/``commit_rows``); one D2H copy per *corpus* (for the reference-compatible
     pickle), not one blocking ``.cpu()`` per batch (reference :81);
-  * the index is ``openmatch_b200.index.FlatIPIndex`` (fused tcgen05 scan + top-k) instead of faiss;
+  * the index is ``openmatch_b200.index.FlatIPIndex`` (fused wgmma scan + top-k) instead of faiss;
     with ``world_size > 1`` every rank keeps the rows it encoded, searches all queries against its shard and
     the per-shard top-k lists are all-gathered over NCCL and merged (the reference instead idles all ranks
     but 0 and lets faiss shard inside one process, :43-58,200-203);

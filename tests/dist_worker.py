@@ -65,7 +65,7 @@ assert (I == I0).all() and (D == D0).all(), "sharded integer search differs from
 report.append("integer exact")
 
 # ---- 2. Gaussian data: identical to the unsharded index, eps-valid vs float64, all ranks agree ----
-n, d, nq, k = 200000, 256, 300, 1000  # > 128 queries: the scan runs on CTA pairs
+n, d, nq, k = 200000, 256, 300, 1000  # > 128 queries: the scan runs on 2-CTA clusters
 x = rng.standard_normal((n, d), dtype=np.float32)
 q = rng.standard_normal((nq, d), dtype=np.float32)
 idx = sharded(x, uneven(n))

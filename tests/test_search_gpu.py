@@ -457,7 +457,7 @@ def test_more_queries_than_one_chunk(om):
 @pytest.mark.parametrize("n,d,nq,k", [(70001, 72, 300, 50), (40000, 768, 129, 1000), (9000, 64, 257, 10),
                                        (300000, 128, 513, 100)])
 def test_pair_scan_and_single_cta_scan_agree(om, n, d, nq, k):
-    # > 128 queries: the scan GEMM runs on CTA pairs (tcgen05 cta_group::2, 256 x 256 tiles, dynamic pair scheduler);
+    # > 128 queries: the scan GEMM runs on 2-CTA clusters (2 x 128 query rows per tile, corpus tile multicast to both);
     # "pair_scan" = 0 selects the single-CTA core.  Same candidates, same answer, bit for bit, and equal to the oracle.
     rng = np.random.default_rng(n + nq)
     x, q = _int_data(rng, n, d, -5, 5), _int_data(rng, nq, d, -5, 5)

@@ -1,5 +1,5 @@
 """Build-index throughput through the public API (SURVEY 8(f1)): a synthetic PRE-TOKENISED corpus (int32 .npy memory map,
-`PretokenizedDataset`) -> `Retriever.build_all` (block ingest: pinned staging, async H2D, sm_100a encoder writing straight
+`PretokenizedDataset`) -> `Retriever.build_all` (block ingest: pinned staging, async H2D, sm_90a encoder writing straight
 into the HBM index shard) -> reference-format embedding file.  Prints one JSON line.
   python tools/ingest_bench.py [n_passages=1000000] [batch=256] [L=128]
 """

@@ -26,12 +26,13 @@ for _ in range(5):
                                                  dp.data_ptr() if which != "dq" else None, None,
                                                  om_lib.current_stream_ptr()))
 torch.cuda.synchronize()
-buf = np.zeros((148, 64), np.uint64)
-raw.om_debug_loss_trace(buf.ctypes.data_as(ctypes.c_void_p), 148)
+ctas = min(om_lib.check(lib.om_device_sm_count()), 160)  # the loss grid is at most one CTA per SM; the trace holds 160
+buf = np.zeros((ctas, 64), np.uint64)
+raw.om_debug_loss_trace(buf.ctypes.data_as(ctypes.c_void_p), ctas)
 t = buf.astype(np.int64)
 t0 = t[:, 60].min()
 rel = np.where(t >= t0, t - t0, -1)
-names = ["tma0", "full0", "commit", "tfull", "stored", "fenced", "reduced", "-"]
+names = ["tma0", "full0", "-", "mma_done", "stored", "fenced", "reduced", "-"]
 np.set_printoptions(linewidth=250)
 print("which =", which, " grads start spread (ns):", int(t[:, 60].max() - t0), " end (slot 61): min/max",
       int(rel[:, 61].min()), int(rel[:, 61].max()))
@@ -41,5 +42,5 @@ for item in range(5):
         ok = col[col >= 0]
         if ok.size:
             print("item %d %-8s n=%3d  min %6d  med %6d  max %6d" % (item, names[e], ok.size, ok.min(), int(np.median(ok)), ok.max()))
-for c in (0, 1, 40, 95, 96, 120, 147):
+for c in sorted({0, 1, ctas // 3, ctas // 2, ctas - 1}):
     print("cta", c, rel[c, :48].reshape(6, 8)[:, :7].tolist(), "end", rel[c, 61])
