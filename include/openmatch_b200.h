@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define OM_ABI_VERSION 1
+#define OM_ABI_VERSION 2
 
 enum { OM_OK = 0, OM_EINVAL = -1, OM_ECUDA = -2, OM_ENOMEM = -3, OM_ENODEVICE = -4, OM_ESTATE = -5, OM_EFAULT = -6 };
 
@@ -133,27 +133,6 @@ void om_comm_destroy(om_comm* comm);
 int om_index_search_sharded(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D,
                             int64_t* I, om_memkind out_kind, int64_t id_offset, void* stream);
 
-/* Three-phase variant for row-sharded indexes (one shard per process, at most 16384 queries per round trip).
- * Replaces the per-shard full top-k that faiss IndexShards computes before merging (dense_retriever.py:43-58):
- * the shards agree on a per-query score floor first, so each one re-scores and ships ~k / n_shards rows.
- *   begin : fp16 tensor-core scan of the local shard.  local_range (device fp32 [2, nq]) receives per query the local
- *           (k + slack)-th best candidate-stage score (row 0; -inf when the shard has fewer rows) and the local best
- *           (row 1).  The caller MAX-reduces it over the shards.
- *   count : local_hist (device int32 [nq, om_search_floor_bins()]) receives the histogram of the local
- *           candidates over equal-width bins of [global_range[0][q], global_range[1][q]].  The caller SUM-reduces.
- *   finish: re-scores in fp32 only the local candidates in or above the bin holding the global (k + slack)-th
- *           score (every member of the global top-k is among them) and writes them sorted to device D fp32
- *           [nq, k] / I int64 [nq, k], padded with -FLT_MAX / -1.  global_hist == NULL: floor = global_range[0];
- *           global_range == NULL: no pruning.  kept_max (device int32, nullable) receives the longest valid prefix
- *           over the queries, so the caller can exchange [nq, kept_max] instead of [nq, k].
- * These are the uncertified building blocks (the caller reduces between the phases, e.g. over gloo in the CPU
- * protocol test); om_index_search_sharded runs the same phases plus the certificate and its escalation. */
-int om_index_search_begin(om_index* idx, const void* q, om_memkind q_kind, int nq, int k, float* local_range,
-                          void* stream);
-int om_index_search_count(om_index* idx, const float* global_range, int* local_hist, void* stream);
-int om_index_search_finish(om_index* idx, const float* global_range, const int* global_hist, float* D, int64_t* I,
-                           int64_t id_offset, int* kept_max, void* stream);
-int om_search_floor_bins(void);
 /* Tunables: "rescore_slack" (extra candidate-stage rows kept per query; default max(128, k/5)),
  * "force_safe_rounds" (1 = always use the overflow-proof fixed-size round schedule; testing),
  * "round_growth" (2..8: each scan round covers (g-1) x the rows already seen; default 0 = auto: 2, or 8 for <= 256 queries),
@@ -172,12 +151,10 @@ int64_t om_index_get_stat(const om_index* idx, const char* name);
 void om_index_destroy(om_index* idx);
 
 /* Exchange step of the row-sharded search: merge `nparts` per-shard results laid out as
- * D_parts [nparts, nq, k], I_parts [nparts, nq, k] (device) into the global top-k by (score desc, id asc);
- * ids < 0 are padding.  Matches merge semantics of faiss IndexShards / utils.py:215-229. */
-int om_topk_merge(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k, float* D, int64_t* I,
-                  void* stream);
-/* Same with input lists of width k_in (e.g. the kept_max prefix of om_index_search_finish) and k_out results;
- * more than 8192 entries per query (nparts * k_in) are merged hierarchically. */
+ * D_parts [nparts, nq, k_in], I_parts [nparts, nq, k_in] (device) into the global top-k_out by (score desc, id asc);
+ * ids < 0 are padding.  Matches merge semantics of faiss IndexShards / utils.py:215-229.  Input lists may be
+ * narrower than the output (k_in < k_out); more than 8192 entries per query (nparts * k_in) are merged
+ * hierarchically. */
 int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k_in, int k_out, float* D,
                     int64_t* I, void* stream);
 

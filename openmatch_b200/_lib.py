@@ -52,14 +52,9 @@ SIGNATURES = {
     "om_comm_destroy": (None, [c_void_p]),
     "om_index_search_sharded": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                         c_int64, c_void_p]),
-    "om_index_search_begin": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
-    "om_index_search_count": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
-    "om_index_search_finish": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int64, c_void_p, c_void_p]),
-    "om_search_floor_bins": (c_int, []),
     "om_index_set_param": (c_int, [c_void_p, c_char_p, c_int64]),
     "om_index_get_stat": (c_int64, [c_void_p, c_char_p]),
     "om_index_destroy": (None, [c_void_p]),
-    "om_topk_merge": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "om_topk_merge_n": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "om_contrastive_loss_fwd_bwd": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_float,
                                             c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -83,7 +78,7 @@ def load():
         fn = getattr(lib, name)  # AttributeError here == header/library mismatch
         fn.restype = res
         fn.argtypes = args
-    if lib.om_abi_version() != 1:
+    if lib.om_abi_version() != 2:
         raise RuntimeError("libopenmatch_b200.so ABI version mismatch")
     _lib = lib
     return lib

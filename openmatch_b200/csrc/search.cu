@@ -184,99 +184,30 @@ __global__ void __launch_bounds__(256) select_kernel(unsigned long long* cand, i
   }
 }
 
-// Equal-width score bins shared by every shard of a sharded search (same inputs -> same bin on every rank).
-constexpr int kFloorBins = 256;
-struct FloorBins {
-  float lo, scale;  // bin = floor((s - lo) * scale), clamped to [0, kFloorBins - 1]; s < lo -> -1
-  __device__ static FloorBins make(float lo, float hi) {
-    FloorBins f;
-    f.lo = lo;
-    const float w = hi - lo;
-    f.scale = (w > 0.f && w < 3.0e38f) ? static_cast<float>(kFloorBins) / w : 0.f;  // lo = -inf / hi <= lo: one bin
-    return f;
-  }
-  __device__ int bin(float s) const {
-    if (s < lo) return -1;
-    if (!(scale > 0.f)) return 0;
-    const float t = (s - lo) * scale;
-    return t >= static_cast<float>(kFloorBins - 1) ? kFloorBins - 1 : static_cast<int>(t);
-  }
-};
-
-// Lowest bin b with count(bins >= b) >= kp (0 when the lists hold fewer than kp rows: no pruning), computed by one
-// warp from a query's reduced histogram: lane l owns bins [l * per, (l + 1) * per); suffix sums over the lanes.
-__device__ __forceinline__ int warp_min_bin(const int* __restrict__ hrow, int kp, int lane) {
-  constexpr int per = kFloorBins / 32;
-  int h[per], sum = 0;
-#pragma unroll
-  for (int j = 0; j < per; ++j) {
-    h[j] = hrow[lane * per + j];
-    sum += h[j];
-  }
-  int suffix = sum;  // sum over lanes >= this one
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int v = __shfl_down_sync(0xffffffffu, suffix, o);
-    if (lane + o < 32) suffix += v;
-  }
-  int run = suffix - sum;  // count in the bins above this lane's
-  int mine = 0;
-  const bool owner = run < kp && kp <= suffix;  // at most one lane
-  if (owner) {
-    int b = per - 1;
-#pragma unroll
-    for (int j = per - 1; j >= 0; --j) {
-      if (run < kp) b = j;
-      run += h[j];
-    }
-    mine = lane * per + b;
-  }
-  const unsigned who = __ballot_sync(0xffffffffu, owner);
-  return who ? __shfl_sync(0xffffffffu, mine, __ffs(who) - 1) : 0;
-}
-
-// FINAL: one CTA per query: exact fp32 re-score of the surviving candidates against the master rows,
-// sort by (score desc, row asc), emit top-k.
-__global__ void __launch_bounds__(256) finalize_kernel(const unsigned long long* cand, const int* count, int C,
-                                                       const float* __restrict__ qf, const float* __restrict__ xf,
-                                                       int d, int k, float* D, int64_t* I, int64_t id_offset,
-                                                       const float* __restrict__ range, const int* __restrict__ ghist,
-                                                       int nq_total, int kp, int* kept_max, int k_out, int* exceed,
-                                                       int stage_scores) {
+// FINAL: one CTA per query: exact fp32 re-score of the candidates against the master rows,
+// sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row gathers are HBM-bound and
+// want every warp resident.
+__global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long long* cand, const int* count, int C,
+                                                          const float* __restrict__ qf, const float* __restrict__ xf,
+                                                          int d, float* D, int64_t* I, int64_t id_offset, int k_out,
+                                                          int stage_scores) {
   extern __shared__ unsigned long long fsm[];
   const int q = blockIdx.x;
-  int cnt = count[q];
+  const int cnt = count[q];
   int P = 2;
   while (P < cnt) P <<= 1;
   unsigned long long* skeys = fsm;
   float* sq = reinterpret_cast<float*>(fsm + P);
   for (int i = threadIdx.x; i < d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q) * d + i];
+  for (int i = cnt + threadIdx.x; i < P; i += blockDim.x) skeys[i] = 0ull;
+  __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const unsigned long long* mine = cand + static_cast<size_t>(q) * C;
-  // sharded search: only candidates in or above the histogram bin that holds the global kp-th bf16-stage score
-  // can be in the global top-k; the others are not re-scored
-  __shared__ int s_minbin;
-  __shared__ int s_n;
-  FloorBins fb{__int_as_float(0xff800000), 0.f};
-  if (range) fb = FloorBins::make(range[q], range[nq_total + q]);
-  if (threadIdx.x == 0) {
-    s_minbin = 0;
-    s_n = 0;
-  }
-  __syncthreads();
-  if (range && ghist && warp == 0) {
-    const int mb = warp_min_bin(ghist + static_cast<size_t>(q) * kFloorBins, kp, lane);
-    if (lane == 0) s_minbin = mb;
-  }
-  __syncthreads();
-  const int minbin = s_minbin;
   for (int j = warp; j < cnt; j += nw) {
-    if (range && fb.bin(key_score(mine[j])) < minbin) continue;
     const uint32_t row = key_row(mine[j]);
-    const float* x = xf + static_cast<size_t>(row) * d;
     float acc = 0.f;
     if ((d & 3) == 0) {
-      const float4* x4 = reinterpret_cast<const float4*>(x);
+      const float4* x4 = reinterpret_cast<const float4*>(xf) + static_cast<size_t>(row) * (d >> 2);
       const float4* q4 = reinterpret_cast<const float4*>(sq);
       for (int i = lane; i < (d >> 2); i += 32) {
         const float4 a = __ldg(x4 + i), b = q4[i];
@@ -286,78 +217,26 @@ __global__ void __launch_bounds__(256) finalize_kernel(const unsigned long long*
         acc = fmaf(a.w, b.w, acc);
       }
     } else {
+      const float* x = xf + static_cast<size_t>(row) * d;
       for (int i = lane; i < d; i += 32) acc = fmaf(__ldg(x + i), sq[i], acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
     if (stage_scores) acc = key_score(mine[j]);  // debug: report the candidate-stage score instead
-    if (lane == 0) skeys[atomicAdd(&s_n, 1)] = make_key(acc, row);  // compacted: the sort covers survivors only
+    if (lane == 0) skeys[j] = make_key(acc, row);
   }
   __syncthreads();
-  const int n = s_n;
-  int P2 = 2;
-  while (P2 < n) P2 <<= 1;
-  for (int i = n + threadIdx.x; i < P2; i += blockDim.x) skeys[i] = 0ull;
-  __syncthreads();
-  bitonic_sort_desc(skeys, P2, threadIdx.x, blockDim.x);
-  // k_out <= k entries are written per query (row pitch k_out): the sharded exchange ships a fixed-width prefix
+  bitonic_sort_desc(skeys, P, threadIdx.x, blockDim.x);
+  // k_out entries are written per query (row pitch k_out): the sharded exchange ships a fixed-width prefix
   for (int r = threadIdx.x; r < k_out; r += blockDim.x) {
     float s = -FLT_MAX;
     int64_t id = -1;
-    if (r < n) {
+    if (r < cnt) {
       s = key_score(skeys[r]);
       id = id_offset + static_cast<int64_t>(key_row(skeys[r]));
     }
     D[static_cast<size_t>(q) * k_out + r] = s;
     I[static_cast<size_t>(q) * k_out + r] = id;
-  }
-  // longest valid prefix over the queries: lets the caller exchange [nq, kept] instead of [nq, k]
-  if (kept_max && threadIdx.x == 0 && n > 0) atomicMax(kept_max, n < k ? n : k);
-  // a list longer than the shipped prefix: the caller must redo the exchange at full width
-  if (exceed && threadIdx.x == 0 && (n < k ? n : k) > k_out) *exceed = 1;
-}
-
-// COUNT (sharded search): histogram of this shard's surviving candidates over kFloorBins equal-width score bins
-// spanning [range[0][q], range[1][q]] = (best local floor, best local score) over the shards.
-__global__ void __launch_bounds__(256) floor_hist_kernel(const unsigned long long* cand, const int* count, int C,
-                                                         const float* __restrict__ range, int nq, int* hist) {
-  __shared__ int sh[kFloorBins];
-  const int q = blockIdx.x;
-  for (int i = threadIdx.x; i < kFloorBins; i += blockDim.x) sh[i] = 0;
-  __syncthreads();
-  const FloorBins fb = FloorBins::make(range[q], range[nq + q]);
-  const int cnt = count[q];
-  const unsigned long long* mine = cand + static_cast<size_t>(q) * C;
-  for (int j = threadIdx.x; j < cnt; j += blockDim.x) {
-    const int b = fb.bin(key_score(mine[j]));
-    if (b >= 0) atomicAdd(&sh[b], 1);
-  }
-  __syncthreads();
-  for (int i = threadIdx.x; i < kFloorBins; i += blockDim.x) hist[static_cast<size_t>(q) * kFloorBins + i] = sh[i];
-}
-
-// per query: {kp-th (floor) and best bf16-stage score} of this shard's candidate list -> range[0][q], range[1][q]
-__global__ void __launch_bounds__(256) local_range_kernel(const unsigned long long* cand, const int* count,
-                                                          const float* thr, int C, int nq, int has_floor,
-                                                          float* range, const float* gstats) {
-  __shared__ float smax[8];
-  const int q = blockIdx.x;
-  const int cnt = count[q];
-  const unsigned long long* mine = cand + static_cast<size_t>(q) * C;
-  float m = __int_as_float(0xff800000);
-  for (int j = threadIdx.x; j < cnt; j += blockDim.x) m = fmaxf(m, key_score(mine[j]));
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0) smax[threadIdx.x >> 5] = m;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    for (int i = 1; i < 8; ++i) m = fmaxf(m, smax[i]);
-    range[q] = has_floor ? thr[q] : __int_as_float(0xff800000);  // a floor needs k + slack local rows
-    range[nq + q] = m;
-    if (q == 0 && gstats) {  // MAX-reduced together with the ranges: every shard certifies against the global maxima
-      range[2 * nq] = gstats[0];
-      range[2 * nq + 1] = gstats[1];
-    }
   }
 }
 
@@ -683,7 +562,6 @@ struct DevBuf {  // grow-only device scratch
 // One pass of the pipeline (scan -> select -> re-score [-> exchange -> merge] -> certify) over nq device-resident
 // queries; all pointers are carved from the index's level workspace.
 struct Level {
-  bool valid = false;  // three-phase API: a search is in progress
   int nq = 0, k = 0, kp = 0, kp_target = 0, C = 0, growth = 2, mode = 0, world = 1, kc = 0, nqc_max = 0;
   const float* qf = nullptr;  // [nq, d] fp32 (not owned by the workspace)
   __half* qh = nullptr;       // [nq, dpad] scan operand
@@ -705,7 +583,6 @@ struct om_index {
   float* gstats = nullptr;  // device [2]: max ||x||, max ||x - x_h|| over the committed rows (float bit patterns)
   int64_t rescore_slack = -1;
   int force_safe = 0;
-  int dynamic_sched = 1;  // claim scan tiles from a global counter (keeps CTAs on neighbouring corpus tiles)
   int pair_scan = 1;      // scan GEMM on 2-CTA clusters sharing each corpus tile by TMA multicast; 0 = single-CTA tiles
   int growth = 0;         // each round scans (growth - 1) x the rows seen so far; 0 = auto: 2 for query batches (fewest
                           // filter survivors), 8 for <= 256 queries (HBM-bound streaming regime: 5 instead of 13
@@ -714,7 +591,7 @@ struct om_index {
   int exact_only = 0;     // 1: answer every query with the exact fp32 scan (testing / reference timing)
   int stage_scores = 0;   // 1: emit candidate-stage scores instead of fp32 re-scores (measuring the error model)
   int64_t st_rounds = 0, st_retries = 0, st_capacity = 0, st_launches = 0;
-  int64_t st_flagged = 0, st_flagged_wide = 0, st_exact = 0, st_wide_exchange = 0;
+  int64_t st_flagged = 0, st_flagged_wide = 0, st_exact = 0;
   // optional per-phase device timing (CUDA events on the launching stream), enabled by set_param("profile", 1)
   int profile = 0;
   double st_scan_us = 0, st_select_us = 0, st_final_us = 0, st_other_us = 0;
@@ -723,7 +600,6 @@ struct om_index {
   size_t ev_used = 0;
   DevBuf ws, ows, sws;  // level workspace / whole-search staging / escalation sub-batch
   int* h_status = nullptr;  // pinned host mirror of Level::status
-  Level plan;               // state between om_index_search_begin and om_index_search_finish
 };
 
 static int index_grow(om_index* ix, int64_t need) {
@@ -798,7 +674,6 @@ int om_index_dim(const om_index* ix) { return ix ? ix->d : 0; }
 int om_index_reset(om_index* ix) {
   if (!ix) return fail(OM_EINVAL, "om_index_reset: null index");
   ix->n = 0;
-  ix->plan.valid = false;  // a search begun on the old contents cannot be finished
   OM_CUDA(cudaMemset(ix->gstats, 0, 2 * sizeof(float)));
   return 0;
 }
@@ -867,8 +742,6 @@ int om_index_set_param(om_index* ix, const char* name, int64_t value) {
   } else if (!strcmp(name, "round_growth")) {
     if (value != 0 && (value < 2 || value > 8)) return fail(OM_EINVAL, "round_growth must be 0 (auto) or in [2, 8]");
     ix->growth = static_cast<int>(value);
-  } else if (!strcmp(name, "dynamic_sched")) {
-    ix->dynamic_sched = value != 0;
   } else if (!strcmp(name, "pair_scan")) {
     ix->pair_scan = value != 0;
   } else if (!strcmp(name, "profile")) {
@@ -894,7 +767,6 @@ int64_t om_index_get_stat(const om_index* ix, const char* name) {
   if (!strcmp(name, "uncertified")) return ix->st_flagged;
   if (!strcmp(name, "uncertified_wide")) return ix->st_flagged_wide;
   if (!strcmp(name, "exact_queries")) return ix->st_exact;
-  if (!strcmp(name, "wide_exchanges")) return ix->st_wide_exchange;
   if (!strcmp(name, "scan_ns")) return static_cast<int64_t>(ix->st_scan_us * 1e3);
   if (!strcmp(name, "select_ns")) return static_cast<int64_t>(ix->st_select_us * 1e3);
   if (!strcmp(name, "finalize_ns")) return static_cast<int64_t>(ix->st_final_us * 1e3);
@@ -981,7 +853,6 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   if (d > 16384) return fail(OM_EINVAL, "om_index_search: d > 16384 unsupported");
   if (k > kMaxCandidates) return fail(OM_EINVAL, "om_index_search: k = %d exceeds %d", k, kMaxCandidates);
   OM_TRY(once_attrs());
-  L.valid = false;
   L.qf = qf;
   L.nq = nq;
   L.k = k;
@@ -1074,7 +945,6 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
       if (L.mode == 0) {
         const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
         cudaError_t e = cudaErrorNotSupported;
-        const bool dynsched = ix->dynamic_sched != 0;
         const int ncols = static_cast<int>(step);
         // a 2-CTA cluster owns 2 x 128 query rows per tile: with <= 128 queries the peer's half would be padding (and the sweep is
         // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing)
@@ -1083,12 +953,12 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
           EpiScan<true> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           if (pair) e = launch_gemm<128, 3, true, EpiScan<true>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
           if (e == cudaErrorNotSupported)  // no 2-CTA cluster fits on the device
-            e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
+            e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         } else {
           EpiScan<false> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           if (pair) e = launch_gemm<128, 3, true, EpiScan<false>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
           if (e == cudaErrorNotSupported)
-            e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, dynsched);
+            e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         }
         if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
       } else {
@@ -1115,15 +985,14 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
 }
 
 int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int64_t* I, int k_out, int64_t id_offset,
-                   const float* range, const int* ghist, int* kept_max, int* exceed, cudaStream_t st) {
+                   cudaStream_t st) {
   int P2 = 2;
   while (P2 < L.kp) P2 <<= 1;
   const size_t fin_smem = static_cast<size_t>(P2) * 8 + static_cast<size_t>(ix->d) * 4;
   {
     Timed t(ix, st, 2);
     finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, L.qf + static_cast<size_t>(q0) * ix->d, ix->xf, ix->d,
-                                                L.k, D, I, id_offset, range, ghist, nqc, L.kp_target, kept_max, k_out,
-                                                exceed, ix->stage_scores);
+                                                D, I, id_offset, k_out, ix->stage_scores);
   }
   OM_CUDA(cudaGetLastError());
   ix->st_launches += 1;
@@ -1140,7 +1009,7 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
 int merge_parts(const float* Dp, const int64_t* Ip, int64_t stride_d, int64_t stride_i, int nparts, int nq, int k_in,
                 int k_out, float* D, int64_t* I, cudaStream_t st) {
   OM_TRY(once_attrs());
-  if (k_in > 8192) return fail(OM_EINVAL, "om_topk_merge: k_in = %d exceeds 8192", k_in);
+  if (k_in > 8192) return fail(OM_EINVAL, "om_topk_merge_n: k_in = %d exceeds 8192", k_in);
   if (static_cast<int64_t>(nparts) * k_in <= 8192) {
     int P = 2;
     while (P < nparts * k_in) P <<= 1;
@@ -1179,7 +1048,7 @@ int exchange_chunk(om_index* ix, om_comm* comm, const Level& L, int q0, int nqc,
   const int W = comm->world;
   const ExchangeBlock b = exchange_block(nqc, L.kc);
   OM_TRY(finalize_chunk(ix, L, q0, nqc, reinterpret_cast<float*>(L.send), reinterpret_cast<int64_t*>(L.send + b.off_i), L.kc,
-                        id_offset, nullptr, nullptr, nullptr, nullptr, st));
+                        id_offset, st));
   {
     Timed t(ix, st, 3);
     OM_CUDA(cudaMemcpyAsync(L.send + b.off_floor, L.thr, static_cast<size_t>(nqc) * 4, cudaMemcpyDeviceToDevice, st));
@@ -1212,7 +1081,7 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
         OM_TRY(exchange_chunk(ix, comm, L, q0, nqc, dD, dI, id_offset, st));
       else
         OM_TRY(finalize_chunk(ix, L, q0, nqc, dD + static_cast<size_t>(q0) * L.k, dI + static_cast<size_t>(q0) * L.k, L.k,
-                              id_offset, nullptr, nullptr, nullptr, nullptr, st));
+                              id_offset, st));
       if (certify) {
         Timed t(ix, st, 3);
         const ExchangeBlock b = exchange_block(nqc, L.kc);
@@ -1256,9 +1125,8 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   NvtxRange nvtx("om.search");
   const int d = ix->d;
   const int world = comm ? comm->world : 1;
-  ix->plan.valid = false;  // the level workspace is about to be reused
   ix->st_rounds = ix->st_retries = ix->st_launches = 0;
-  ix->st_flagged = ix->st_flagged_wide = ix->st_exact = ix->st_wide_exchange = 0;
+  ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
   ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
   ix->ev_used = 0;
   // whole-search staging: queries (if they arrive from the host), results (if they leave to the host), flag list
@@ -1419,80 +1287,12 @@ extern "C" int om_index_search_sharded(om_index* ix, om_comm* comm, const void* 
   return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, static_cast<cudaStream_t>(stream));
 }
 
-// ---- three-phase building blocks (one shard per call; the caller reduces between the phases) ----------------------
-extern "C" int om_index_search_begin(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* local_range,
-                                     void* stream) {
-  if (!ix || nq <= 0 || !q || !local_range || k <= 0) return fail(OM_EINVAL, "om_index_search_begin: bad arguments");
-  if (nq > kQueryChunk) return fail(OM_EINVAL, "om_index_search_begin: at most %d queries per call", kQueryChunk);
-  const int sms = device_sm_count();
-  if (sms < 0) return sms;
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  // the queries must outlive this call (finish re-scores against them): keep a copy in the staging buffer
-  OM_TRY(ix->ows.reserve(round_up(static_cast<size_t>(nq) * ix->d * 4, 256)));
-  OM_CUDA(cudaMemcpyAsync(ix->ows.p, q, static_cast<size_t>(nq) * ix->d * 4,
-                          q_kind == OM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
-  ix->st_rounds = ix->st_retries = ix->st_launches = 0;
-  const int64_t slack = ix->rescore_slack >= 0 ? ix->rescore_slack : std::max<int64_t>(128, k / 5);
-  Level& L = ix->plan;
-  OM_TRY(level_prepare(ix, L, static_cast<const float*>(ix->ows.p), nq, k,
-                       static_cast<int>(std::min<int64_t>(static_cast<int64_t>(k) + slack, kMaxCandidates)), 0, 1, st));
-  bool safe = ix->force_safe != 0;
-  for (int attempt = 0;; ++attempt) {
-    OM_CUDA(cudaMemsetAsync(L.status, 0, 32, st));
-    OM_TRY(sweep_chunk(ix, L, 0, nq, safe, sms, st));
-    OM_CUDA(cudaMemcpyAsync(ix->h_status, L.status, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    OM_CUDA(cudaStreamSynchronize(st));
-    const unsigned int fault = read_clear_dev_fault();
-    if (fault) return fail(OM_EFAULT, "scan kernel pipeline fault 0x%08x", fault);
-    if (!ix->h_status[0]) break;
-    if (safe || attempt > 0) return fail(OM_EFAULT, "candidate list overflow in the overflow-proof schedule (bug)");
-    safe = true;
-    ix->st_retries++;
-  }
-  local_range_kernel<<<nq, 256, 0, st>>>(L.cand, L.count, L.thr, L.C, nq, ix->n >= L.kp_target ? 1 : 0, local_range, nullptr);
-  OM_CUDA(cudaGetLastError());
-  ix->st_launches += 1;
-  L.valid = true;
-  return 0;
-}
-
-extern "C" int om_index_search_count(om_index* ix, const float* global_range, int* local_hist, void* stream) {
-  if (!ix || !global_range || !local_hist) return fail(OM_EINVAL, "om_index_search_count: bad arguments");
-  if (!ix->plan.valid) return fail(OM_ESTATE, "om_index_search_count: no search in progress (call om_index_search_begin)");
-  const Level& L = ix->plan;
-  floor_hist_kernel<<<L.nq, 256, 0, static_cast<cudaStream_t>(stream)>>>(L.cand, L.count, L.C, global_range, L.nq, local_hist);
-  OM_CUDA(cudaGetLastError());
-  ix->st_launches += 1;
-  return 0;
-}
-
-extern "C" int om_index_search_finish(om_index* ix, const float* global_range, const int* global_hist, float* D,
-                                      int64_t* I, int64_t id_offset, int* kept_max, void* stream) {
-  if (!ix || !D || !I || (global_hist && !global_range)) return fail(OM_EINVAL, "om_index_search_finish: bad arguments");
-  if (!ix->plan.valid) return fail(OM_ESTATE, "om_index_search_finish: no search in progress (call om_index_search_begin)");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  Level& L = ix->plan;
-  L.valid = false;
-  if (kept_max) OM_CUDA(cudaMemsetAsync(kept_max, 0, sizeof(int), st));
-  OM_TRY(finalize_chunk(ix, L, 0, L.nq, D, I, L.k, id_offset, global_range, global_hist, kept_max, nullptr, st));
-  OM_CUDA(cudaStreamSynchronize(st));
-  if (ix->profile) collect_profile(ix);
-  return 0;
-}
-
-extern "C" int om_search_floor_bins(void) { return kFloorBins; }
-
 extern "C" int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k_in, int k_out,
                                float* D, int64_t* I, void* stream) {
   if (nparts <= 0 || nq < 0 || k_in <= 0 || k_out <= 0 || !D_parts || !I_parts || !D || !I)
-    return fail(OM_EINVAL, "om_topk_merge: bad arguments");
+    return fail(OM_EINVAL, "om_topk_merge_n: bad arguments");
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
   const int64_t stride = static_cast<int64_t>(nq) * k_in;
   return merge_parts(D_parts, I_parts, stride, stride, nparts, nq, k_in, k_out, D, I, static_cast<cudaStream_t>(stream));
-}
-
-extern "C" int om_topk_merge(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k, float* D,
-                             int64_t* I, void* stream) {
-  return om_topk_merge_n(D_parts, I_parts, nparts, nq, k, k, D, I, stream);
 }

@@ -8,7 +8,7 @@ All arithmetic runs in libopenmatch_b200.so (csrc/search.cu); this file only mar
 from __future__ import annotations
 
 import ctypes
-from typing import Optional, Tuple
+from typing import Tuple
 
 import numpy as np
 import torch
@@ -30,7 +30,6 @@ class FlatIPIndex:
         _lib.check(self._lib.om_index_create(int(d), ctypes.byref(h)))
         self._h = h
         self.d = int(d)
-        self._pending = None  # (nq, k, device) between search_begin and search_finish
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -119,45 +118,6 @@ class FlatIPIndex:
         kind = _lib.OM_DEVICE if D_out.is_cuda else _lib.OM_HOST
         _lib.check(self._lib.om_index_search_sharded(self._h, comm._h, q_host.data_ptr(), _lib.OM_HOST, nq, int(k),
                                                      D_out.data_ptr(), I_out.data_ptr(), kind, int(id_offset), _stream()))
-
-    def search_begin(self, q: torch.Tensor, k: int) -> torch.Tensor:
-        """Phase 1 of the sharded search: bf16 scan of the local shard; returns the per-query (local floor, local
-        best) bf16-stage scores as a CUDA fp32 [2, nq] tensor, to be MAX-reduced over the shards."""
-        q = q.contiguous().float()
-        self._check_shape(q.shape)
-        rng = torch.empty((2, q.shape[0]), dtype=torch.float32, device=q.device)
-        _lib.check(self._lib.om_index_search_begin(self._h, q.data_ptr(), _lib.OM_DEVICE, q.shape[0], int(k),
-                                                   rng.data_ptr(), _stream()))
-        self._pending = (q.shape[0], int(k), q.device)
-        return rng
-
-    def _require_pending(self, what: str):
-        if self._pending is None:
-            raise RuntimeError("%s: no search in progress (call search_begin first)" % what)
-        return self._pending
-
-    def search_count(self, global_range: torch.Tensor) -> torch.Tensor:
-        """Phase 2: histogram (CUDA int32 [nq, bins]) of the local candidates over the reduced score range, to be
-        SUM-reduced over the shards."""
-        nq, _, dev = self._require_pending("search_count")
-        hist = torch.empty((nq, self._lib.om_search_floor_bins()), dtype=torch.int32, device=dev)
-        _lib.check(self._lib.om_index_search_count(self._h, global_range.data_ptr(), hist.data_ptr(), _stream()))
-        return hist
-
-    def search_finish(self, global_range: Optional[torch.Tensor], global_hist: Optional[torch.Tensor] = None,
-                      id_offset: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        """Phase 3: fp32 re-score of the local candidates at or above the agreed floor -> (D [nq, k], I [nq, k],
-        kept [1] int32 = longest valid prefix over the queries), all on the device."""
-        nq, k, dev = self._require_pending("search_finish")
-        self._pending = None
-        D = torch.empty((nq, k), dtype=torch.float32, device=dev)
-        I = torch.empty((nq, k), dtype=torch.int64, device=dev)
-        kept = torch.empty((1,), dtype=torch.int32, device=dev)
-        _lib.check(self._lib.om_index_search_finish(
-            self._h, None if global_range is None else global_range.data_ptr(),
-            None if global_hist is None else global_hist.data_ptr(), D.data_ptr(), I.data_ptr(), int(id_offset),
-            kept.data_ptr(), _stream()))
-        return D, I, kept
 
     def search_pinned(self, q_host: torch.Tensor, k: int, D_host: torch.Tensor, I_host: torch.Tensor,
                       id_offset: int = 0) -> None:
@@ -257,49 +217,15 @@ def merge_topk_device(D_parts: torch.Tensor, I_parts: torch.Tensor, k: int) -> T
     return D, I
 
 
-def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offset: int, group=None, merge=None):
-    """Row-sharded exact search.  With a real ``FlatIPIndex`` on a NCCL process group the whole sequence (scan,
-    collectives, re-score, merge, exactness certificate) runs inside the library on the current stream
-    (``om_index_search_sharded``).  Otherwise — the CPU protocol test drives this function under gloo with the
-    oracle's restatement of the phases — the same phases are stepped from Python:
-      1. bf16 scan of the local shard                                    -> (floor, best) per query
-      2. all-reduce MAX [2, nq]; local histogram over the agreed range   -> all-reduce SUM [nq, 64]
-      3. fp32 re-score of the local candidates above the global floor (~k / world rows per query, not k)
-      4. all-reduce MAX of the longest kept prefix; all-gather of the [nq, kept] (score, id) lists; merge kernel.
-    Every rank returns the same global (D, I) [nq, k].  Without a process group: the single-shard call.
-    ``index`` only needs ``search_begin / search_count / search_finish`` (tests run this function on CPU under
-    gloo with the oracle's restatement of the three phases and the oracle's ``merge``)."""
+def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offset: int, group=None):
+    """Row-sharded exact search: every rank passes the same queries and its own shard's ``id_offset`` and receives
+    the same global (D, I) [nq, k].  Scan, exchange, merge and the exactness certificate run inside the library
+    (``om_index_search_sharded``) over the library's NCCL communicator for ``group``, which is created on first
+    use whatever the group's backend.  Without a process group, or with one rank: the single-shard search."""
     import torch.distributed as dist
     if not dist.is_initialized() or dist.get_world_size(group) == 1:
         return index.search_device(q, k, id_offset=id_offset)
-    if isinstance(index, FlatIPIndex) and merge is None and dist.get_backend(group) == "nccl":
-        return index.search_sharded_device(comm_for(group), q, k, id_offset)
-    if q.shape[0] > 16384:
-        D, I = index.search_device(q, k, id_offset=id_offset)
-        return exchange_and_merge(D, I, k, group, merge)
-    rng = index.search_begin(q, k)
-    dist.all_reduce(rng, op=dist.ReduceOp.MAX, group=group)
-    hist = index.search_count(rng)
-    dist.all_reduce(hist, op=dist.ReduceOp.SUM, group=group)
-    D, I, kept = index.search_finish(rng, hist, id_offset=id_offset)
-    dist.all_reduce(kept, op=dist.ReduceOp.MAX, group=group)
-    kc = min(k, max(32, -(-int(kept.item()) // 32) * 32))
-    return exchange_and_merge(D[:, :kc], I[:, :kc], k, group, merge)
-
-
-def exchange_and_merge(D_local: torch.Tensor, I_local: torch.Tensor, k: int, group=None, merge=None):
-    """Exchange step of the row-sharded search: all-gather the per-shard [nq, k] (score, global id) lists in
-    rank order (NCCL over NVLink on GPUs) and merge them by (score desc, id asc) on every rank.  ``merge``
-    defaults to the CUDA merge kernel; tests inject the oracle's merge to run this on CPU / gloo."""
-    import torch.distributed as dist
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    if world == 1:
-        return D_local, I_local
-    Dp = torch.empty((world,) + tuple(D_local.shape), dtype=D_local.dtype, device=D_local.device)
-    Ip = torch.empty((world,) + tuple(I_local.shape), dtype=I_local.dtype, device=I_local.device)
-    dist.all_gather(list(Dp.unbind(0)), D_local.contiguous(), group=group)  # views of one [W, nq, k] buffer
-    dist.all_gather(list(Ip.unbind(0)), I_local.contiguous(), group=group)
-    return (merge or merge_topk_device)(Dp, Ip, k)  # input lists may be narrower than k (pruned exchange)
+    return index.search_sharded_device(comm_for(group), q, k, id_offset)
 
 
 def shard_offsets(n_local: int, group=None):

@@ -14,7 +14,7 @@ Pinning status (see DESIGN.md "Oracle"):
     the search step parity is anchored on the reference's call sites only: **parity unpinned** w.r.t. faiss.
 """
 from .flat_index import (  # noqa: F401
-    FlatIPIndex, ShardPhases, flat_ip_search, merge_topk, merge_retrieval_results_by_score,
+    FlatIPIndex, flat_ip_search, merge_topk, merge_retrieval_results_by_score,
 )
 from .loss import contrastive_loss, contrastive_loss_fwd_bwd  # noqa: F401
 from .encoder import (  # noqa: F401

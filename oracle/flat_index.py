@@ -106,92 +106,6 @@ def merge_topk(parts, k: int):
     return outD, outI
 
 
-FLOOR_BINS = 256
-
-
-class ShardPhases:
-    """CPU restatement of the three-phase row-sharded search of ``openmatch_b200`` (csrc/search.cu
-    ``om_index_search_begin / _count / _finish``), used to check the protocol's host logic under gloo.
-
-    The role is the one faiss ``IndexShards`` plays behind ``index_cpu_to_gpu_multiple(shard=True)``
-    (dense_retriever.py:43-58); the protocol itself is ours: a candidate stage on fp16-rounded operands keeps
-    the local top-kp, the shards agree on a per-query floor through a MAX-reduced (floor, best) range and a
-    SUM-reduced histogram, and only candidates in or above the bin holding the global kp-th score are re-scored
-    in fp32 and exchanged.  Tensors in / out are torch CPU tensors so that ``torch.distributed`` can reduce them.
-    """
-
-    def __init__(self, x: np.ndarray, slack: int = 128):
-        self.x = np.ascontiguousarray(x, dtype=np.float32)
-        self.slack = slack
-
-    @staticmethod
-    def _f16(a: np.ndarray) -> np.ndarray:
-        """IEEE half rounding of the scan operands (csrc/search.cu rows_to_f16_kernel; finite values saturate)"""
-        return np.clip(np.ascontiguousarray(a, np.float32), -65504.0, 65504.0).astype(np.float16).astype(np.float32)
-
-    def search_begin(self, q, k: int):
-        import torch
-        self.q = np.ascontiguousarray(q.numpy() if hasattr(q, "numpy") else q, dtype=np.float32)
-        self.k = k
-        self.kp_target = min(k + max(self.slack, k // 5), 4096)
-        kp = min(self.kp_target, self.x.shape[0])
-        s = self._f16(self.q) @ self._f16(self.x).T if self.x.shape[0] else np.zeros((self.q.shape[0], 0), np.float32)
-        self.cand_s, self.cand_i = _topk_rows(s.astype(np.float32), kp) if kp else (s, s.astype(np.int64))
-        nq = self.q.shape[0]
-        rng = np.full((2, nq), -np.inf, np.float32)
-        if kp:
-            rng[1] = self.cand_s[:, 0]
-            if self.x.shape[0] >= self.kp_target:  # only a shard holding kp rows has a floor
-                rng[0] = self.cand_s[:, kp - 1]
-        return torch.from_numpy(rng)
-
-    @staticmethod
-    def _bins(s: np.ndarray, lo: np.ndarray, hi: np.ndarray) -> np.ndarray:
-        """float32 arithmetic of csrc/search.cu FloorBins: floor((s - lo) * (bins / (hi - lo))), clamped; s < lo -> -1"""
-        w = (hi - lo).astype(np.float32)
-        ok = (w > 0) & (w < np.float32(3.0e38))
-        with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
-            scale = np.where(ok, np.float32(FLOOR_BINS) / w, np.float32(0)).astype(np.float32)
-            t = ((s - lo[:, None]).astype(np.float32) * scale[:, None]).astype(np.float32)
-        b = np.where(t >= FLOOR_BINS - 1, FLOOR_BINS - 1, np.nan_to_num(t, nan=0.0, posinf=0.0, neginf=0.0).astype(np.int64))
-        b = np.where(ok[:, None], b, 0)
-        return np.where(s < lo[:, None], -1, b)
-
-    def search_count(self, grange):
-        import torch
-        g = grange.numpy()
-        b = self._bins(self.cand_s, g[0], g[1])
-        hist = np.zeros((self.q.shape[0], FLOOR_BINS), np.int32)
-        for r in range(b.shape[0]):
-            v = b[r][(b[r] >= 0) & (self.cand_i[r] >= 0)]
-            hist[r] = np.bincount(v, minlength=FLOOR_BINS)
-        return torch.from_numpy(hist)
-
-    def search_finish(self, grange, ghist, id_offset: int = 0):
-        import torch
-        nq, k = self.q.shape[0], self.k
-        D = np.full((nq, k), NEG_FILL, np.float32)
-        I = np.full((nq, k), -1, np.int64)
-        g = grange.numpy()
-        b = self._bins(self.cand_s, g[0], g[1])
-        kept = 0
-        for r in range(nq):
-            above = np.cumsum(ghist[r].numpy()[::-1])[::-1]  # above[b] = count in bins >= b
-            ok = np.flatnonzero(above >= self.kp_target)
-            minbin = int(ok.max()) if ok.size else 0
-            rows = self.cand_i[r][(b[r] >= minbin) & (self.cand_i[r] >= 0)]
-            if rows.size == 0:
-                continue
-            d, i = flat_ip_search(self.q[r:r + 1], self.x[rows], min(k, rows.size))
-            n = int((i[0] >= 0).sum())
-            # flat_ip_search orders ties by position in `rows`; restore (score desc, row asc)
-            ids = rows[i[0, :n]]
-            order = np.lexsort((ids, -d[0, :n].astype(np.float64)))
-            D[r, :n], I[r, :n] = d[0, :n][order], ids[order] + id_offset
-            kept = max(kept, n)
-        return torch.from_numpy(D), torch.from_numpy(I), torch.tensor([kept], dtype=torch.int32)
-
-
 class FlatIPIndex:
     """Duck-type of ``faiss.IndexFlatIP`` (the five members the reference touches)."""
 

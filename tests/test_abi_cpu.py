@@ -15,7 +15,7 @@ def _declared_symbols():
     return sorted(set(re.findall(r"\b(om_[a-z0-9_]+)\s*\(", text)))
 
 
-def test_header_symbols_are_exported_and_bound():
+def test_abi_v2_exports_and_binds_every_header_symbol():
     from openmatch_b200 import _lib
     if not os.path.exists(_lib.LIB_PATH):
         from openmatch_b200.build import build
@@ -26,7 +26,7 @@ def test_header_symbols_are_exported_and_bound():
     for name in declared:
         assert hasattr(lib, name), "library does not export %s" % name
         assert name in _lib.SIGNATURES, "ctypes binding lacks %s" % name
-    assert lib.om_abi_version() == 1
+    assert lib.om_abi_version() == 2
 
 
 @pytest.mark.skipif(torch.cuda.is_available(), reason="checks the no-GPU failure mode")

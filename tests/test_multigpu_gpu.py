@@ -1,7 +1,7 @@
 """GPU, real NCCL: spawns one rank per GPU (2 ranks) running tests/dist_worker.py when the box has >= 2 GPUs.
 On a single-GPU box the same library entry point (om_index_search_sharded) and the distributed loss are still
-exercised through a world-size-1 NCCL group, and the exchange arithmetic through logical shards
-(tests/test_search_gpu.py::test_three_phase_sharded_search_prunes_and_stays_exact)."""
+exercised through a world-size-1 NCCL group, and the merge of the exchanged lists through logical shards
+(tests/test_search_gpu.py::test_sharded_merge_matches_unsharded)."""
 import os
 import socket
 import subprocess

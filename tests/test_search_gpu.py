@@ -155,7 +155,8 @@ def test_normalized_embeddings(om):
 
 
 def test_sharded_merge_matches_unsharded(om):
-    # single-GPU "logical shards": 4 indexes over contiguous row ranges, merged through om_topk_merge
+    # single-GPU "logical shards": 4 indexes over contiguous row ranges, merged through om_topk_merge_n.  This is the
+    # single-GPU check of merge_kernel, the merge step of the row-sharded search: a world-size-1 group never merges.
     rng = np.random.default_rng(2)
     x, q = _int_data(rng, 8000, 64, -3, 3), _int_data(rng, 21, 64, -3, 3)
     k = 50
@@ -172,77 +173,6 @@ def test_sharded_merge_matches_unsharded(om):
     # and against the oracle's own merge
     D1, I1 = oracle.merge_topk([(a.cpu().numpy(), b.cpu().numpy()) for a, b in zip(Dp, Ip)], k)
     np.testing.assert_array_equal(I.cpu().numpy(), I1)
-
-
-@pytest.mark.parametrize("lo,hi,bounds", [(-3, 3, [0, 2500, 6100, 6150, 12000]), (-8, 8, [0, 3000, 6000, 9000, 12000]),
-                                          (0, 1, [0, 100, 11000, 11990, 12000])])
-def test_three_phase_sharded_search_prunes_and_stays_exact(om, lo, hi, bounds):
-    # logical shards on one GPU running the protocol the ranks run: begin on every shard -> MAX of the ranges ->
-    # count -> SUM of the histograms -> finish -> merge of the kept prefixes.  (0/1 data: massive score ties.)
-    rng = np.random.default_rng(12 + hi)
-    x, q = _int_data(rng, 12000, 64, lo, hi), _int_data(rng, 33, 64, lo, hi)
-    k = 100
-    qd = torch.from_numpy(q).cuda()
-    shards = []
-    for s in range(4):
-        idx = om.FlatIPIndex(64)
-        idx.add(x[bounds[s]:bounds[s + 1]])
-        shards.append(idx)
-    ranges = torch.stack([idx.search_begin(qd, k) for idx in shards])
-    small = [s for s in range(4) if bounds[s + 1] - bounds[s] < k + 128]
-    for s in small:  # fewer rows than k + slack: no local floor
-        assert torch.isinf(ranges[s, 0]).all() and (ranges[s, 0] < 0).all()
-    grange = ranges.max(dim=0).values
-    ghist = torch.stack([idx.search_count(grange) for idx in shards]).sum(dim=0, dtype=torch.int32)
-    assert (ghist.sum(dim=1) >= k + 128).all()
-    outs = [idx.search_finish(grange, ghist, id_offset=bounds[s]) for s, idx in enumerate(shards)]
-    kc = max(int(o[2].item()) for o in outs)
-    kept = sum(int((o[1] >= 0).sum()) for o in outs)
-    for o in outs:
-        assert int((o[1] >= 0).sum(dim=1).max()) == int(o[2].item())
-    if hi > 1:
-        assert kept < 33 * (k + 128) * 1.5, "histogram floor did not prune the per-shard lists (%d kept)" % kept
-    D, I = om.merge_topk_device(torch.stack([o[0][:, :kc] for o in outs]), torch.stack([o[1][:, :kc] for o in outs]), k)
-    D0, I0 = oracle.flat_ip_search(q, x, k)
-    np.testing.assert_array_equal(I.cpu().numpy(), I0)
-    np.testing.assert_array_equal(D.cpu().numpy(), D0)
-    # finish without begin is a state error; finish without a range / histogram = the plain per-shard top-k
-    with pytest.raises(RuntimeError):
-        shards[0].search_finish(grange, ghist)
-    shards[1].search_begin(qd, k)
-    Dn, In, _ = shards[1].search_finish(None, None, id_offset=bounds[1])
-    Dl, Il = shards[1].search_device(qd, k, id_offset=bounds[1])
-    assert torch.equal(In, Il) and torch.equal(Dn, Dl)
-
-
-def test_shard_phases_match_oracle_phase_by_phase(om):
-    # integer data: bf16-stage scores are exact, so every intermediate of the protocol must equal the oracle's
-    rng = np.random.default_rng(77)
-    x, q = _int_data(rng, 9000, 64, -4, 4), _int_data(rng, 17, 64, -4, 4)
-    k, bounds = 50, [0, 4000, 9000]
-    qd = torch.from_numpy(q).cuda()
-    cu, cpu = [], []
-    for s in range(2):
-        idx = om.FlatIPIndex(64)
-        idx.add(x[bounds[s]:bounds[s + 1]])
-        cu.append(idx)
-        cpu.append(oracle.ShardPhases(x[bounds[s]:bounds[s + 1]], slack=128))
-    r_cu = [i.search_begin(qd, k) for i in cu]
-    r_cpu = [o.search_begin(torch.from_numpy(q), k) for o in cpu]
-    for a, b in zip(r_cu, r_cpu):
-        assert torch.equal(a.cpu(), b)
-    grange = torch.stack(r_cpu).max(dim=0).values
-    h_cu = [i.search_count(grange.cuda()) for i in cu]
-    h_cpu = [o.search_count(grange) for o in cpu]
-    for a, b in zip(h_cu, h_cpu):
-        assert torch.equal(a.cpu(), b)
-    ghist = (h_cpu[0] + h_cpu[1]).to(torch.int32)
-    for s in range(2):
-        D, I, kept = cu[s].search_finish(grange.cuda(), ghist.cuda(), id_offset=bounds[s])
-        D0, I0, kept0 = cpu[s].search_finish(grange, ghist, id_offset=bounds[s])
-        assert int(kept.item()) == int(kept0.item())
-        np.testing.assert_array_equal(I.cpu().numpy(), I0.numpy())
-        np.testing.assert_array_equal(D.cpu().numpy(), D0.numpy())
 
 
 def test_zero_copy_ingest(om):
