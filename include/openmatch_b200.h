@@ -62,7 +62,7 @@ typedef struct om_encoder_desc {
   float ln_eps;             /* layer_norm_eps (1e-12 BERT) / layer_norm_epsilon (1e-6 T5) */
   int32_t pooling;          /* om_pooling: DRModel.pooling 'first' | 'mean' */
   int32_t has_head;         /* 1: bias-free LinearHead follows pooling */
-  int32_t head_out;         /* LinearHead output_dim (multiple of 8) */
+  int32_t head_out;         /* LinearHead output_dim (any positive width) */
   int32_t normalize;        /* 1: F.normalize(reps, dim=1) */
   int32_t rel_buckets;      /* T5 relative_attention_num_buckets (32) */
   int32_t rel_max_distance; /* T5 relative_attention_max_distance (128) */

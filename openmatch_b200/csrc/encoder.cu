@@ -532,6 +532,9 @@ __device__ __forceinline__ void raw_store(const float4 (&v)[kMaxVec], int nvec, 
 
 // BERT embeddings (modeling_bert.py:53-112): s = word[id] + type[tt] + pos[l], UN-normalised (fp32 + bf16) with its row
 // statistics; the embedding LayerNorm is applied by the first layer's QKV / O-proj epilogues like every other LayerNorm.
+// s is stored minus its row mean: only the embedding LayerNorm reads it, which is shift-invariant.  A common offset in
+// the embedding tables otherwise leaves rows whose mean is tens of times their standard deviation, and the bf16 copy that
+// the QKV GEMM reads (and the folded weights' rounding residue, scaled by mean / std) would bury the row's information.
 __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, const int64_t* tts, const float* word,
                                                          const float* type, const float* pos, int T, int L, int H, int vocab,
                                                          int type_vocab, float* out_f32, __nv_bfloat16* out_bf16,
@@ -554,6 +557,16 @@ __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, con
       const float4 p = *reinterpret_cast<const float4*>(pos + static_cast<int64_t>(l) * H + c);
       v[j] = make_float4((a.x + b.x) + p.x, (a.y + b.y) + p.y, (a.z + b.z) + p.z, (a.w + b.w) + p.w);
     }
+  float sum = 0.f;
+#pragma unroll
+  for (int j = 0; j < kMaxVec; ++j)
+    if (j < nvec) sum += (v[j].x + v[j].y) + (v[j].z + v[j].w);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+  const float mean = sum / H;
+#pragma unroll
+  for (int j = 0; j < kMaxVec; ++j)
+    if (j < nvec) v[j].x -= mean, v[j].y -= mean, v[j].z -= mean, v[j].w -= mean;
   raw_store(v, nvec, lane, out_f32 + static_cast<int64_t>(row) * H, out_bf16 + static_cast<int64_t>(row) * H);
   store_row_stats(v, nvec, lane, stats + static_cast<int64_t>(row) * (2 * kStatParts));
 }
@@ -577,7 +590,9 @@ __global__ void __launch_bounds__(128) t5_embed_kernel(const int64_t* ids, const
 // Weight folding (once, at om_encoder_finalize):  Wf[j, i] = bf16(W[j, i] * gamma[i] - centre * mean_i(W[j, i] * gamma[i]))
 // and bfold[j] = b[j] + sum_i W[j, i] * beta[i] (fp32, un-centred W).  With centred rows (LayerNorm) the mean term of the
 // folded normalisation vanishes identically:  sum_i s_i Wf[j, i] = sum_i (s_i - mean(s)) W[j, i] gamma[i]  (up to the bf16
-// rounding of Wf, ~1e-3 of a weight: below the bf16 rounding of the GEMM's output).  RMSNorm (T5): centre = 0, beta = none.
+// rounding of Wf, ~1e-3 of a weight, multiplied by mean(s) / std(s): below the bf16 rounding of the GEMM's output while
+// the rows of s are no further from zero mean than LN(s), which the centred embedding rows ensure, see bert_embed_kernel).
+// RMSNorm (T5): centre = 0, beta = none.
 // One warp per output row j.
 __global__ void __launch_bounds__(256) fold_norm_kernel(const float* __restrict__ W, const float* __restrict__ gamma,
                                                         const float* __restrict__ beta, const float* __restrict__ bias,

@@ -12,6 +12,13 @@ The encoder maths lives in an un-vendored dependency, HuggingFace ``transformers
 Explicit matmuls on plain tensors keyed by the HF ``state_dict`` names; no HF module is executed here.
 tests/test_oracle_pinning.py checks this file against the reference's own ``DRModelForInference`` (golden
 vectors in tests/golden/, made by tests/golden/make_golden.py inside the build container).
+
+``encode_reps`` computes in float32 by default.  ``dtype=torch.float64`` gives the high-precision yardstick the GPU
+numerics tests compare against; ``emulate_bf16=True`` additionally rounds to bf16 what the reference rounds under
+bf16 autocast (SURVEY section 8(d)): both operands of every matmul (activations, weights and biases), the output of
+every Linear and the probabilities P before P V.  Softmax, LayerNorm / RMSNorm, the residual stream and pooling stay in
+``dtype``.  ``probe(layer, logits)`` receives every layer's masked attention logits [B, heads, L, L] (float64, -inf at
+masked keys, natural-log units) so a test can check the attention statistics it claims to exercise.
 """
 from __future__ import annotations
 
@@ -37,13 +44,36 @@ class EncoderSpec:
     rel_max_distance: int = 128  # T5 only
 
 
-def _f32(t):
-    return t.detach().to(torch.float32)
+class _Num:
+    """Arithmetic of one oracle run: the compute dtype and whether matmuls see bf16-rounded operands (autocast)."""
+
+    def __init__(self, dtype=torch.float32, emulate_bf16=False, probe=None):
+        self.dtype, self.bf16, self.probe = dtype, emulate_bf16, probe
+
+    def t(self, t):
+        return t.detach().to(self.dtype)
+
+    def r(self, t):  # bf16 rounding of a matmul operand / Linear output (identity without emulation)
+        return t.to(torch.bfloat16).to(self.dtype) if self.bf16 else t
+
+    def mm(self, a, b):
+        return self.r(a) @ self.r(b)
+
+    def lin(self, x, w, b=None):  # F.linear under autocast: bf16 x, W, b; bf16 output
+        y = self.mm(x, self.t(w).T)
+        return self.r(y + self.r(self.t(b)) if b is not None else y)
+
+    def look(self, layer, logits):
+        if self.probe is not None:
+            self.probe(layer, logits.detach().to(torch.float64))
 
 
-def _key_mask(attention_mask: torch.Tensor) -> torch.Tensor:
+_F32 = _Num()
+
+
+def _key_mask(attention_mask: torch.Tensor, dtype=torch.float32) -> torch.Tensor:
     # additive key-padding mask [B, 1, 1, L]: 0 where attended, -inf where padded
-    m = torch.zeros(attention_mask.shape, dtype=torch.float32)
+    m = torch.zeros(attention_mask.shape, dtype=dtype)
     m = m.masked_fill(attention_mask == 0, float("-inf"))
     return m[:, None, None, :]
 
@@ -57,37 +87,39 @@ def _softmax_rows(s: torch.Tensor) -> torch.Tensor:
     return e / torch.where(z == 0, torch.ones_like(z), z)
 
 
-def bert_encode(sd: Dict[str, torch.Tensor], spec: EncoderSpec, input_ids, attention_mask, token_type_ids=None):
-    """``BertModel.forward`` -> last_hidden_state fp32 [B, L, H] (pooler skipped: OpenMatch ignores it)."""
+def bert_encode(sd: Dict[str, torch.Tensor], spec: EncoderSpec, input_ids, attention_mask, token_type_ids=None,
+                nm: _Num = _F32):
+    """``BertModel.forward`` -> last_hidden_state [B, L, H] (pooler skipped: OpenMatch ignores it)."""
     B, L = input_ids.shape
     H, nh = spec.hidden, spec.heads
     dh = H // nh
     if token_type_ids is None:
         token_type_ids = torch.zeros_like(input_ids)
-    emb = (_f32(sd["embeddings.word_embeddings.weight"])[input_ids]
-           + _f32(sd["embeddings.token_type_embeddings.weight"])[token_type_ids]
-           + _f32(sd["embeddings.position_embeddings.weight"])[torch.arange(L)][None])
-    h = F.layer_norm(emb, (H,), _f32(sd["embeddings.LayerNorm.weight"]), _f32(sd["embeddings.LayerNorm.bias"]),
+    emb = (nm.t(sd["embeddings.word_embeddings.weight"])[input_ids]
+           + nm.t(sd["embeddings.token_type_embeddings.weight"])[token_type_ids]
+           + nm.t(sd["embeddings.position_embeddings.weight"])[torch.arange(L)][None])
+    h = F.layer_norm(emb, (H,), nm.t(sd["embeddings.LayerNorm.weight"]), nm.t(sd["embeddings.LayerNorm.bias"]),
                      spec.ln_eps)
-    mask = _key_mask(attention_mask)
+    mask = _key_mask(attention_mask, nm.dtype)
     for i in range(spec.layers):
         p = f"encoder.layer.{i}."
 
         def lin(x, name):
-            return x @ _f32(sd[p + name + ".weight"]).T + _f32(sd[p + name + ".bias"])
+            return nm.lin(x, sd[p + name + ".weight"], sd[p + name + ".bias"])
 
         def heads(x):
             return x.view(B, L, nh, dh).permute(0, 2, 1, 3)
 
         q, k, v = (heads(lin(h, "attention.self." + n)) for n in ("query", "key", "value"))
-        s = q @ k.transpose(-1, -2) * (dh ** -0.5) + mask
-        ctx = (_softmax_rows(s) @ v).permute(0, 2, 1, 3).reshape(B, L, H)
+        s = nm.mm(q, k.transpose(-1, -2)) * (dh ** -0.5) + mask
+        nm.look(i, s)
+        ctx = nm.mm(_softmax_rows(s), v).permute(0, 2, 1, 3).reshape(B, L, H)
         h = F.layer_norm(lin(ctx, "attention.output.dense") + h, (H,),
-                         _f32(sd[p + "attention.output.LayerNorm.weight"]),
-                         _f32(sd[p + "attention.output.LayerNorm.bias"]), spec.ln_eps)
+                         nm.t(sd[p + "attention.output.LayerNorm.weight"]),
+                         nm.t(sd[p + "attention.output.LayerNorm.bias"]), spec.ln_eps)
         inter = F.gelu(lin(h, "intermediate.dense"))  # exact erf GELU (hidden_act="gelu")
-        h = F.layer_norm(lin(inter, "output.dense") + h, (H,), _f32(sd[p + "output.LayerNorm.weight"]),
-                         _f32(sd[p + "output.LayerNorm.bias"]), spec.ln_eps)
+        h = F.layer_norm(lin(inter, "output.dense") + h, (H,), nm.t(sd[p + "output.LayerNorm.weight"]),
+                         nm.t(sd[p + "output.LayerNorm.bias"]), spec.ln_eps)
     return h
 
 
@@ -109,63 +141,68 @@ def _rms(x, w, eps):
     return w * (x * torch.rsqrt(var + eps))
 
 
-def t5_encode(sd: Dict[str, torch.Tensor], spec: EncoderSpec, input_ids, attention_mask):
-    """``T5EncoderModel.forward`` -> last_hidden_state fp32 [B, L, H] (after final_layer_norm)."""
+def t5_encode(sd: Dict[str, torch.Tensor], spec: EncoderSpec, input_ids, attention_mask, nm: _Num = _F32):
+    """``T5EncoderModel.forward`` -> last_hidden_state [B, L, H] (after final_layer_norm)."""
     B, L = input_ids.shape
     H, nh = spec.hidden, spec.heads
     emb_key = "shared.weight" if "shared.weight" in sd else "encoder.embed_tokens.weight"
-    h = _f32(sd[emb_key])[input_ids]
-    dh = _f32(sd["encoder.block.0.layer.0.SelfAttention.q.weight"]).shape[0] // nh
+    h = nm.t(sd[emb_key])[input_ids]
+    dh = sd["encoder.block.0.layer.0.SelfAttention.q.weight"].shape[0] // nh
     pos = torch.arange(L)
     bucket = t5_relative_position_bucket(pos[None, :] - pos[:, None], spec.rel_buckets, spec.rel_max_distance)
-    rel = _f32(sd["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"])  # [buckets, heads]
+    rel = nm.t(sd["encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight"])  # [buckets, heads]
     bias = rel[bucket].permute(2, 0, 1)[None]  # [1, heads, L, L], shared by all layers
-    mask = _key_mask(attention_mask)
+    mask = _key_mask(attention_mask, nm.dtype)
     for i in range(spec.layers):
         p = f"encoder.block.{i}.layer."
-        x = _rms(h, _f32(sd[p + "0.layer_norm.weight"]), spec.ln_eps)
+        x = _rms(h, nm.t(sd[p + "0.layer_norm.weight"]), spec.ln_eps)
 
         def heads(t):
             return t.view(B, L, nh, dh).permute(0, 2, 1, 3)
 
-        q, k, v = (heads(x @ _f32(sd[p + f"0.SelfAttention.{n}.weight"]).T) for n in ("q", "k", "v"))
-        s = q @ k.transpose(-1, -2) + bias + mask  # no 1/sqrt(d) scaling in T5
-        ctx = (_softmax_rows(s) @ v).permute(0, 2, 1, 3).reshape(B, L, nh * dh)
-        h = h + ctx @ _f32(sd[p + "0.SelfAttention.o.weight"]).T
-        x = _rms(h, _f32(sd[p + "1.layer_norm.weight"]), spec.ln_eps)
+        q, k, v = (heads(nm.lin(x, sd[p + f"0.SelfAttention.{n}.weight"])) for n in ("q", "k", "v"))
+        s = nm.mm(q, k.transpose(-1, -2)) + bias + mask  # no 1/sqrt(d) scaling in T5
+        nm.look(i, s)
+        ctx = nm.mm(_softmax_rows(s), v).permute(0, 2, 1, 3).reshape(B, L, nh * dh)
+        h = h + nm.lin(ctx, sd[p + "0.SelfAttention.o.weight"])
+        x = _rms(h, nm.t(sd[p + "1.layer_norm.weight"]), spec.ln_eps)
         if p + "1.DenseReluDense.wi.weight" in sd:
-            inter = torch.relu(x @ _f32(sd[p + "1.DenseReluDense.wi.weight"]).T)
+            inter = torch.relu(nm.lin(x, sd[p + "1.DenseReluDense.wi.weight"]))
         else:  # gated-GELU variant (t5 v1.1): gelu_new(wi_0 x) * (wi_1 x)
-            g = x @ _f32(sd[p + "1.DenseReluDense.wi_0.weight"]).T
-            inter = F.gelu(g, approximate="tanh") * (x @ _f32(sd[p + "1.DenseReluDense.wi_1.weight"]).T)
-        h = h + inter @ _f32(sd[p + "1.DenseReluDense.wo.weight"]).T
-    return _rms(h, _f32(sd["encoder.final_layer_norm.weight"]), spec.ln_eps)
+            g = nm.lin(x, sd[p + "1.DenseReluDense.wi_0.weight"])
+            inter = nm.r(F.gelu(g, approximate="tanh") * nm.lin(x, sd[p + "1.DenseReluDense.wi_1.weight"]))
+        h = h + nm.lin(inter, sd[p + "1.DenseReluDense.wo.weight"])
+    return _rms(h, nm.t(sd["encoder.final_layer_norm.weight"]), spec.ln_eps)
 
 
-def pool_head_normalize(hidden, attention_mask, pooling: str, head_weight: Optional[torch.Tensor], normalize: bool):
+def pool_head_normalize(hidden, attention_mask, pooling: str, head_weight: Optional[torch.Tensor], normalize: bool,
+                        nm: _Num = _F32):
     """dense_retrieval_model.py:145-154 + utils.py:233-235 + linear.py:22-23."""
     if pooling == "first":
         reps = hidden[:, 0, :]
     elif pooling == "mean":
-        m = attention_mask.unsqueeze(-1).expand(hidden.size()).float()
+        m = attention_mask.unsqueeze(-1).expand(hidden.size()).to(hidden.dtype)
         reps = torch.sum(hidden * m, 1) / torch.clamp(m.sum(1), min=1e-9)
     else:
         raise ValueError("Unknown pooling type: {}".format(pooling))
     if head_weight is not None:
-        reps = reps @ _f32(head_weight).T
+        reps = nm.lin(reps, head_weight)
     if normalize:
         reps = F.normalize(reps, dim=1)
     return reps
 
 
-def encode_reps(sd, spec: EncoderSpec, input_ids, attention_mask, token_type_ids=None, head_weight=None):
-    """(hidden, reps) exactly as ``DRModel.encode`` returns them, in fp32 on CPU."""
+def encode_reps(sd, spec: EncoderSpec, input_ids, attention_mask, token_type_ids=None, head_weight=None,
+                dtype=torch.float32, emulate_bf16=False, probe=None):
+    """(hidden, reps) exactly as ``DRModel.encode`` returns them, in ``dtype`` on CPU (see the module docstring for
+    ``emulate_bf16`` and ``probe``)."""
+    nm = _Num(dtype, emulate_bf16, probe)
     with torch.no_grad():
         if spec.arch == "bert":
-            hidden = bert_encode(sd, spec, input_ids, attention_mask, token_type_ids)
+            hidden = bert_encode(sd, spec, input_ids, attention_mask, token_type_ids, nm)
         elif spec.arch == "t5":
-            hidden = t5_encode(sd, spec, input_ids, attention_mask)
+            hidden = t5_encode(sd, spec, input_ids, attention_mask, nm)
         else:
             raise ValueError(spec.arch)
-        reps = pool_head_normalize(hidden, attention_mask, spec.pooling, head_weight, spec.normalize)
+        reps = pool_head_normalize(hidden, attention_mask, spec.pooling, head_weight, spec.normalize, nm)
     return hidden, reps

@@ -36,6 +36,29 @@ def test_t5_encoder_matches_reference(golden_dir):
     np.testing.assert_allclose(reps.numpy(), z["reps"], rtol=2e-4, atol=2e-6)
 
 
+def test_float64_oracle_matches_reference(golden_dir):
+    # the float64 mode is the yardstick of tests/test_encoder_numerics_gpu.py: it must meet the golden vectors at the
+    # float32 mode's tolerances, and its bf16-autocast emulation must drift from it like autocast does (SURVEY 8(d))
+    cases = [("bert_small.npz", EncoderSpec("bert", 2, 128, 2, 512, 1e-12, pooling="first"), False),
+             ("t5_small.npz", EncoderSpec("t5", 2, 128, 2, 512, 1e-6, pooling="mean", normalize=True), True)]
+    for name, spec, head in cases:
+        z, sd = _load(golden_dir, name)
+        args = (sd, spec, torch.from_numpy(z["input_ids"]), torch.from_numpy(z["attention_mask"]),
+                torch.from_numpy(z["token_type_ids"]) if "token_type_ids" in z.files else None,
+                torch.from_numpy(z["head_weight"]) if head else None)
+        logits = []
+        hidden, reps = oracle.encode_reps(*args, dtype=torch.float64, probe=lambda i, s: logits.append((i, s)))
+        assert hidden.dtype == torch.float64 and reps.dtype == torch.float64
+        assert [i for i, _ in logits] == list(range(spec.layers))
+        assert all(s.dtype == torch.float64 and s.shape[1] == spec.heads for _, s in logits)
+        m = z["attention_mask"].astype(bool)
+        np.testing.assert_allclose(hidden.numpy()[m], z["hidden"][m], rtol=2e-4, atol=2e-5)
+        np.testing.assert_allclose(reps.numpy(), z["reps"], rtol=2e-4, atol=2e-5 if not head else 2e-6)
+        _, reps_bf16 = oracle.encode_reps(*args, dtype=torch.float64, emulate_bf16=True)
+        rel = float((reps_bf16 - reps).norm() / reps.norm())
+        assert 1e-4 < rel < 1e-2, "%s: bf16 emulation drift %.2e" % (name, rel)
+
+
 def test_t5_buckets_match_hf(golden_dir):
     z = np.load(os.path.join(golden_dir, "misc.npz"))
     got = oracle.t5_relative_position_bucket(torch.from_numpy(z["t5_bucket_rel"]), 32, 128).numpy()
