@@ -139,7 +139,8 @@ int om_index_search_sharded(om_index* idx, om_comm* comm, const void* q, om_memk
  * "certify" (default 1; 0 = skip the exactness certificate and its escalation: top-k of the fp16 candidate stage),
  * "exact_only" (1 = answer every query with the exact fp32 CUDA-core scan; testing),
  * "debug_stage_scores" (1 = D holds candidate-stage scores instead of fp32 re-scores; error-model measurement),
- * "pair_scan" (default 1: the scan GEMM runs on 2-CTA clusters sharing each corpus tile; 0 = single-CTA tiles),
+ * "pair_scan" (default 1: after the first round, batches of > 128 queries scan on 2-CTA clusters with 256-row corpus
+ *   tiles multicast to both CTAs and the top-k filter on the accumulator registers; 0 = single-CTA 128 x 128 tiles),
  * "profile" (1 = bracket every kernel launch of a search with CUDA events on the launching stream). */
 int om_index_set_param(om_index* idx, const char* name, int64_t value);
 /* Statistics of the last search: "rounds", "overflow_retries", "candidates" (per query capacity),

@@ -13,10 +13,6 @@
 // Pipelines: smem full/empty (TMA <-> consumers, released per k block one wgmma group late); the staged accumulator
 // tile is handed over with two named barriers per tile.  Tile schedule: static (tile = blockIdx.x + i * gridDim.x) or
 // dynamic (claimed from a global counter by the producer, published through a 4-deep smem ring).
-//
-// CLUSTER = 2: two CTAs of a cluster own vertically adjacent 128-row tiles that share the same B tile; each CTA loads
-// its own A tile and one half of B, multicast into both CTAs' shared memory, so every B byte crosses L2 -> SM once per
-// pair.  Static tile schedule over pair tiles.
 #pragma once
 #include <type_traits>
 
@@ -71,26 +67,24 @@ __device__ __forceinline__ void wgmma_tile_k16(float (&acc)[BN / 2], uint64_t da
   else wgmma_m64n128k16_bf16<0, 0>(acc, da, db, accumulate);
 }
 
-template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16, int CLUSTER>
+template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16>
 __global__ void __launch_bounds__(kGemmProducerThreads + 32 * kGemmEpiWarps, 1)
 gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, int M, int N,
                     int K, const __grid_constant__ Epi epi, int* tile_counter) {
   using Cfg = GemmCfg<BN, STAGES>;
-  static_assert(CLUSTER == 1 || CLUSTER == 2, "CLUSTER: 1 or 2");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* acc_tile = reinterpret_cast<float*>(smem + Cfg::kAccOffset);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::kBarOffset);
   uint64_t* empty_bar = full_bar + STAGES;
-  // dynamic tile scheduler (tile_counter != nullptr, CLUSTER == 1): the producer claims tile indices from a global
+  // dynamic tile scheduler (tile_counter != nullptr): the producer claims tile indices from a global
   // counter and publishes them to the consumer warps through a 4-deep smem ring
   constexpr int kSched = 4;
   uint64_t* sfull_bar = empty_bar + STAGES;
   uint64_t* sempty_bar = sfull_bar + kSched;
   volatile int* tile_ring = reinterpret_cast<volatile int*>(sempty_bar + kSched);
   uint8_t* epi_smem = smem + Cfg::kEpiOffset;  // Epi::smem_bytes() of scratch owned by the epilogue functor
-  const bool dyn = CLUSTER == 1 && tile_counter != nullptr;
-  const uint32_t rank = CLUSTER > 1 ? cluster_ctarank() : 0u;
+  const bool dyn = tile_counter != nullptr;
 
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = static_cast<int>(threadIdx.x & 31);
@@ -102,7 +96,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kGemmEpiWarps * CLUSTER);  // every consumer warp of every CTA that writes this stage
+      mbar_init(&empty_bar[i], kGemmEpiWarps);  // every consumer warp
     }
     for (int i = 0; i < kSched; ++i) {
       mbar_init(&sfull_bar[i], 1);
@@ -110,16 +104,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     }
     fence_barrier_init();
   }
-  if constexpr (CLUSTER > 1) cluster_sync_all();  // the peer's barriers exist before any multicast or remote arrive
   __syncthreads();
 
   const int num_m = (M + kBlockM - 1) / kBlockM;
   const int num_n = (N + BN - 1) / BN;
-  const int num_mt = (num_m + CLUSTER - 1) / CLUSTER;  // tile rows of the schedule (pairs of 128-row tiles: CLUSTER 2)
-  const int num_tiles = num_mt * num_n;
+  const int num_tiles = num_m * num_n;
   const int num_k = (K + kBlockK - 1) / kBlockK;
-  const int first_tile = CLUSTER > 1 ? static_cast<int>(cluster_id_x()) : static_cast<int>(blockIdx.x);
-  const int tile_step = CLUSTER > 1 ? static_cast<int>(cluster_count_x()) : static_cast<int>(gridDim.x);
+  const int first_tile = static_cast<int>(blockIdx.x);
+  const int tile_step = static_cast<int>(gridDim.x);
 
   if (warp == 0) {
     if (lane == 0) {
@@ -145,20 +137,14 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         }
         // claim the next tile now; the atomic's round trip overlaps this tile's loads
         int next = dyn ? atomicAdd(tile_counter, 1) : tile + tile_step;
-        const int m_blk = (M_FASTEST ? tile % num_mt : tile / num_n) * CLUSTER + static_cast<int>(rank);
-        const int n_blk = M_FASTEST ? tile / num_mt : tile % num_n;
+        const int m_blk = M_FASTEST ? tile % num_m : tile / num_n;
+        const int n_blk = M_FASTEST ? tile / num_m : tile % num_n;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u, 1);
           uint8_t* sa = smem + stage * Cfg::kStageBytes;
           mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
           tma_load_2d(sa, &tmA, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          if constexpr (CLUSTER > 1) {
-            constexpr int kHalf = BN / CLUSTER;
-            tma_load_2d_multicast(sa + Cfg::kABytes + rank * kHalf * 128, &tmB, &full_bar[stage], kb * kBlockK,
-                                  n_blk * BN + static_cast<int>(rank) * kHalf, static_cast<uint16_t>((1u << CLUSTER) - 1u));
-          } else {
-            tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n_blk * BN);
-          }
+          tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n_blk * BN);
           if (++stage == STAGES) {
             stage = 0;
             phase ^= 1u;
@@ -193,8 +179,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       } else if (tile >= num_tiles) {
         break;
       }
-      const int m_blk = (M_FASTEST ? tile % num_mt : tile / num_n) * CLUSTER + static_cast<int>(rank);
-      const int n_blk = M_FASTEST ? tile / num_mt : tile % num_n;
+      const int m_blk = M_FASTEST ? tile % num_m : tile / num_n;
+      const int n_blk = M_FASTEST ? tile / num_m : tile % num_n;
       const int row = m_blk * kBlockM + ew * 32 + lane;
       epi.begin(st, row, m_blk, n_blk);
       if constexpr (Epi::kPrefetch) epi.prefetch(st, row, n_blk * BN + half * kChunks * 32);
@@ -216,10 +202,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         wgmma_commit();
         if (kb > 0) {
           wgmma_wait<1>();
-          if (lane == 0) {
-            mbar_arrive(&empty_bar[prev_stage]);
-            if constexpr (CLUSTER > 1) mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
-          }
+          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
         }
         prev_stage = stage;
         if (++stage == STAGES) {
@@ -229,10 +212,7 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      if (num_k > 0 && lane == 0) {
-        mbar_arrive(&empty_bar[prev_stage]);
-        if constexpr (CLUSTER > 1) mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
-      }
+      if (num_k > 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       // stage the accumulators: every epilogue thread has finished reading the previous tile
       named_bar_sync(2, 32 * kGemmEpiWarps);
@@ -277,7 +257,6 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   }
 
   __syncthreads();
-  if constexpr (CLUSTER > 1) cluster_sync_all();  // the peer may still be signalling this CTA's barriers
 }
 
 // Pool of tile counters for the dynamic scheduler: launch i uses counter i % 64 (zeroed on the launching stream
@@ -295,9 +274,8 @@ static inline int* next_tile_counter(cudaStream_t stream) {
 // Returns cudaSuccess / a CUDA error; tensor-map failures map to cudaErrorInvalidValue.
 // dynamic_sched: claim tiles from a global counter instead of the static blockIdx + i * gridDim order, which keeps all
 // CTAs on neighbouring tiles (with the static order CTAs drift apart over thousands of tiles and stop sharing operand
-// tiles in L2).  CLUSTER = 2 (CTA pairs sharing B by multicast) always uses the static order; it returns
-// cudaErrorNotSupported if no cluster of the kernel fits on the device.
-template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16 = false, int CLUSTER = 1>
+// tiles in L2).
+template <int BN, int STAGES, bool M_FASTEST, class Epi, bool F16 = false>
 static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int M, int N, int K,
                                       const Epi& epi, int num_sms, cudaStream_t stream, bool dynamic_sched = false) {
   using Cfg = GemmCfg<BN, STAGES>;
@@ -305,9 +283,9 @@ static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B,
   CUtensorMap tmA, tmB;
   if (make_tmap_bf16_2d(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)lda * 2, kBlockK, kBlockM) != 0)
     return cudaErrorInvalidValue;
-  if (make_tmap_bf16_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, kBlockK, BN / CLUSTER) != 0)
+  if (make_tmap_bf16_2d(&tmB, B, (uint64_t)K, (uint64_t)N, (uint64_t)ldb * 2, kBlockK, BN) != 0)
     return cudaErrorInvalidValue;
-  auto kern = gemm_bf16_tn_kernel<BN, STAGES, M_FASTEST, Epi, F16, CLUSTER>;
+  auto kern = gemm_bf16_tn_kernel<BN, STAGES, M_FASTEST, Epi, F16>;
   const int smem_bytes = Cfg::kSmemBytes + Epi::smem_bytes(kGemmEpiWarps);
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
@@ -315,44 +293,16 @@ static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B,
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  const int num_m = (M + kBlockM - 1) / kBlockM;
-  const int num_tiles = ((num_m + CLUSTER - 1) / CLUSTER) * ((N + BN - 1) / BN);
+  const int num_tiles = ((M + kBlockM - 1) / kBlockM) * ((N + BN - 1) / BN);
   const int threads = kGemmProducerThreads + 32 * kGemmEpiWarps;
-  if constexpr (CLUSTER > 1) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(threads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = CLUSTER;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    // the persistent schedule wants every cluster co-resident (a second wave of clusters would double the run time)
-    static int max_clusters = 0;  // per instantiation
-    if (!max_clusters) {
-      cfg.gridDim = dim3(CLUSTER * (num_sms / CLUSTER));
-      int n = 0;
-      cudaError_t e = cudaOccupancyMaxActiveClusters(&n, kern, &cfg);
-      if (e != cudaSuccess) return e;
-      if (n < 1) return cudaErrorNotSupported;
-      max_clusters = n < num_sms / CLUSTER ? n : num_sms / CLUSTER;
-    }
-    const int clusters = num_tiles < max_clusters ? num_tiles : max_clusters;
-    cfg.gridDim = dim3(CLUSTER * clusters);
-    return cudaLaunchKernelEx(&cfg, kern, tmA, tmB, M, N, K, epi, static_cast<int*>(nullptr));
-  } else {
-    const int grid = num_tiles < num_sms ? num_tiles : num_sms;
-    int* counter = nullptr;
-    if (dynamic_sched) {
-      counter = next_tile_counter(stream);
-      if (!counter) return cudaErrorMemoryAllocation;
-    }
-    kern<<<grid, threads, smem_bytes, stream>>>(tmA, tmB, M, N, K, epi, counter);
-    return cudaGetLastError();
+  const int grid = num_tiles < num_sms ? num_tiles : num_sms;
+  int* counter = nullptr;
+  if (dynamic_sched) {
+    counter = next_tile_counter(stream);
+    if (!counter) return cudaErrorMemoryAllocation;
   }
+  kern<<<grid, threads, smem_bytes, stream>>>(tmA, tmB, M, N, K, epi, counter);
+  return cudaGetLastError();
 }
 
 // --------------------------------------------------------------------------------------------------

@@ -1,0 +1,308 @@
+// Search scan for query batches: fp16 Q * X^T on 2-CTA clusters with the top-k filter applied directly to the wgmma
+// accumulator registers.
+//
+//   tile        one cluster owns 256 queries x 256 corpus rows; CTA `rank` of the pair owns queries
+//               [128 (2 p + rank), +128) of pair row p and the whole 256-row corpus tile, K = d in 64-wide k blocks
+//   operands    each CTA TMA-loads its own 128-query box and one 128-row half of the corpus tile, multicast into both
+//               CTAs' shared memory; the two halves land back to back and form one K-major SW128 operand of 256 rows,
+//               so every corpus byte crosses L2 -> SM once per pair (32 KB per CTA and k block for 4.2 MFLOP)
+//   warp roles  warpgroup 0: one TMA producer lane (registers lowered to 40); warpgroups 1, 2: consumers (registers
+//               raised to 232), consumer g issues wgmma m64n256k16 for queries [64 g, +64) of the CTA's 128 and holds the
+//               64 x 256 fp32 accumulator tile in 128 registers per thread
+//   ring        kScanStages x 48 KB; a slot is released one wgmma group late on the empty barriers of BOTH CTAs (every
+//               consumer warp of the pair arrives on each), since the peer's producer writes half of every slot
+//   schedule    persistent, static, queries fastest: tile t -> pair row t % pairs, corpus tile t / pairs, so all
+//               clusters work on neighbouring corpus tiles and the corpus streams from HBM about once
+//   epilogue    no staging through shared memory: a thread owns two query rows (fragment rows l/4 and l/4 + 8 of its
+//               warp's 16) x 64 corpus columns (8 j + 2 (l % 4) + {0, 1}, j < 32).  One 64-value max per row against the
+//               query's strict threshold rejects the row in the common case; survivors go through a compact bit-mask
+//               loop into a per-thread, double-buffered shared-memory stash.  At the end of a tile the 4 lanes that share
+//               a row reserve their survivors' list slots with ONE atomicAdd (shuffle prefix for the lane offsets); the
+//               atomic's result is consumed one tile later, when the stash is copied to the candidate list, so its L2
+//               round trip hides behind a whole tile of MMA work.  Survivors beyond the stash (dense early rounds) take a
+//               synchronous atomicAdd and are stored at once.  Keys and the overflow flag are those of EpiScan.
+#pragma once
+#include <cuda_fp16.h>
+
+#include "scan_epilogue.cuh"
+
+namespace om {
+
+constexpr int kScanBlockN = 256;                             // corpus rows per tile
+constexpr int kScanStages = 3;  // 4 fit next to the stash too, but ran the C2 scan 2-4 % slower (H100 SXM, 700 W)
+constexpr int kScanABytes = kBlockM * kBlockK * 2;           // 16 KB: the CTA's 128 queries
+constexpr int kScanBBytes = kScanBlockN * kBlockK * 2;       // 32 KB: the pair's corpus tile (two multicast halves)
+constexpr int kScanStageBytes = kScanABytes + kScanBBytes;
+constexpr int kScanConsumers = 256;                          // two consumer warpgroups
+constexpr int kScanStash = 4;                                // survivors a thread parks per row and tile
+constexpr int kScanStashOffset = kScanStages * kScanStageBytes;
+constexpr int kScanStashBytes = 2 * 2 * kScanStash * kScanConsumers * 8;  // [buffer][row half][slot][thread] keys
+constexpr int kScanBarOffset = kScanStashOffset + kScanStashBytes;
+constexpr int kScanSmemBytes = kScanBarOffset + 2 * kScanStages * 8 + 1024;  // + slack for 1024-B alignment of the base
+static_assert(kScanSmemBytes <= 232448, "scan ring + stash exceed the 227 KB of shared memory an H100 block may use");
+
+// Value of fragment row H (0: l/4, 1: l/4 + 8) at bit i of the row's 64-bit survivor mask, i = 2 j + b <-> acc[4 j + 2 H + b],
+// for a run-time i without local memory: 6-level select tree (63 SEL).
+template <int H>
+__device__ __forceinline__ float scan_pick(const float (&acc)[128], int i) {
+  float a[32], b[16], c[8], d[4], e[2];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) a[j] = (i & 1) ? acc[4 * j + 2 * H + 1] : acc[4 * j + 2 * H];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) b[j] = (i & 2) ? a[2 * j + 1] : a[2 * j];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) c[j] = (i & 4) ? b[2 * j + 1] : b[2 * j];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) d[j] = (i & 8) ? c[2 * j + 1] : c[2 * j];
+#pragma unroll
+  for (int j = 0; j < 2; ++j) e[j] = (i & 16) ? d[2 * j + 1] : d[2 * j];
+  return (i & 32) ? e[1] : e[0];
+}
+
+// Filter of fragment row H of one tile: returns the number of survivors parked in the stash (<= kScanStash).
+// stash: this thread's slot 0 of (buffer, row H); slot j is at stash[j * kScanConsumers].
+template <int H>
+__device__ __forceinline__ int scan_filter_row(const float (&acc)[128], float t, int row, int lim, int q4, int col0,
+                                               unsigned long long* stash, unsigned long long* cand, int* count,
+                                               int* overflow, int C, uint32_t row_base) {
+  float mx = acc[2 * H];
+#pragma unroll
+  for (int j = 0; j < 32; ++j) mx = fmaxf(mx, fmaxf(acc[4 * j + 2 * H], acc[4 * j + 2 * H + 1]));
+  if (!(mx > t)) return 0;  // common case: nothing in this row's 64 columns beats the threshold
+  // Survivor path.  Kept deliberately COMPACT (a bit mask + a short loop with a select tree): it runs rarely per warp,
+  // so its instructions are cold in the instruction cache and every extra cache line costs hundreds of cycles.
+  uint32_t lo = 0, hi = 0;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) {
+    lo |= (acc[4 * (i >> 1) + 2 * H + (i & 1)] > t ? 1u : 0u) << i;
+    hi |= (acc[4 * (16 + (i >> 1)) + 2 * H + (i & 1)] > t ? 1u : 0u) << i;
+  }
+  unsigned long long mask = (static_cast<unsigned long long>(hi) << 32) | lo;
+  if (lim < kScanBlockN) {  // last corpus tile: columns >= lim hold TMA zero fill, and a zero can beat a negative threshold
+#pragma unroll 1
+    for (int i = 0; i < 64; ++i)
+      if (8 * (i >> 1) + 2 * q4 + (i & 1) >= lim) mask &= ~(1ull << i);
+  }
+  const int n = __popcll(mask);
+  int pos = 0;
+  if (n > kScanStash) {  // more than the stash holds: reserve the excess synchronously
+    pos = atomicAdd(count + row, n - kScanStash);
+    if (pos + (n - kScanStash) > C) *overflow = 1;
+  }
+  unsigned long long* mine = cand + static_cast<size_t>(row) * C;
+  int idx = 0;
+#pragma unroll 1
+  while (mask) {
+    const int i = __ffsll(static_cast<long long>(mask)) - 1;
+    mask &= mask - 1;
+    const unsigned long long key =
+        make_key(scan_pick<H>(acc, i), row_base + static_cast<uint32_t>(col0 + 8 * (i >> 1) + 2 * q4 + (i & 1)));
+    if (idx < kScanStash)
+      stash[idx * kScanConsumers] = key;
+    else if (pos + idx - kScanStash < C)
+      mine[pos + idx - kScanStash] = key;
+    ++idx;
+  }
+  return n < kScanStash ? n : kScanStash;
+}
+
+__global__ void __launch_bounds__(kGemmProducerThreads + kScanConsumers, 1)
+scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmX, int K,
+                 const float* __restrict__ thr, unsigned long long* cand, int* count, int* overflow, int nq, int n_cols,
+                 int C, uint32_t row_base) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned long long* stash = reinterpret_cast<unsigned long long*>(smem + kScanStashOffset);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kScanBarOffset);
+  uint64_t* empty_bar = full_bar + kScanStages;
+  const uint32_t rank = cluster_ctarank();
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = static_cast<int>(threadIdx.x & 31);
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmX);
+  }
+  if (warp == 1 && lane == 0) {
+    for (int i = 0; i < kScanStages; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2 * kScanConsumers / 32);  // every consumer warp of both CTAs
+    }
+    fence_barrier_init();
+  }
+  cluster_sync_all();  // the peer's barriers exist before any multicast or remote arrive
+
+  const int pairs = (nq + 2 * kBlockM - 1) / (2 * kBlockM);
+  const int num_tiles = pairs * ((n_cols + kScanBlockN - 1) / kScanBlockN);
+  const int num_k = (K + kBlockK - 1) / kBlockK;
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ------------------------------ TMA producer ------------------------------
+      uint32_t stage = 0, phase = 0;
+      for (int tile = static_cast<int>(cluster_id_x()); tile < num_tiles; tile += static_cast<int>(cluster_count_x())) {
+        const int m_blk = (tile % pairs) * 2 + static_cast<int>(rank);
+        const int n_blk = tile / pairs;
+        for (int kb = 0; kb < num_k; ++kb) {
+          mbar_wait(&empty_bar[stage], phase ^ 1u, 30);
+          uint8_t* sa = smem + stage * kScanStageBytes;
+          mbar_arrive_expect_tx(&full_bar[stage], kScanStageBytes);
+          tma_load_2d(sa, &tmQ, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
+          tma_load_2d_multicast(sa + kScanABytes + rank * (kScanBBytes / 2), &tmX, &full_bar[stage], kb * kBlockK,
+                                n_blk * kScanBlockN + static_cast<int>(rank) * (kScanBlockN / 2), static_cast<uint16_t>(3u));
+          if (++stage == kScanStages) {
+            stage = 0;
+            phase ^= 1u;
+          }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ------------------------------ consumers: wgmma + filter ------------------------------
+    const int et = static_cast<int>(threadIdx.x) - kGemmProducerThreads;  // 0 .. 255
+    const int wg = et >> 7;                                               // queries [64 wg, +64) of the CTA's 128
+    const int q4 = lane & 3;
+    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
+    uint32_t stage = 0, phase = 0;
+    int buf = 0;
+    // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
+    int p_n0 = 0, p_n1 = 0, p_excl0 = 0, p_excl1 = 0, p_pos0 = 0, p_pos1 = 0, p_row = 0, p_buf = 0;
+    auto drain = [&]() {
+      if (!__any_sync(0xffffffffu, (p_n0 | p_n1) != 0)) return;
+      const int b0 = __shfl_sync(0xffffffffu, p_pos0, lane & ~3) + p_excl0;
+      const int b1 = __shfl_sync(0xffffffffu, p_pos1, lane & ~3) + p_excl1;
+      const unsigned long long* s = stash + p_buf * (2 * kScanStash * kScanConsumers) + et;
+      unsigned long long* m0 = cand + static_cast<size_t>(p_row) * C;
+      unsigned long long* m1 = cand + static_cast<size_t>(p_row + 8) * C;
+      for (int j = 0; j < p_n0; ++j)
+        if (b0 + j < C) m0[b0 + j] = s[j * kScanConsumers];
+      for (int j = 0; j < p_n1; ++j)
+        if (b1 + j < C) m1[b1 + j] = s[(kScanStash + j) * kScanConsumers];
+      if ((p_n0 > 0 && b0 + p_n0 > C) || (p_n1 > 0 && b1 + p_n1 > C)) *overflow = 1;
+      p_n0 = p_n1 = 0;
+    };
+
+    for (int tile = static_cast<int>(cluster_id_x()); tile < num_tiles; tile += static_cast<int>(cluster_count_x())) {
+      const int m_blk = (tile % pairs) * 2 + static_cast<int>(rank);
+      const int n_blk = tile / pairs;
+      const int row0 = m_blk * kBlockM + frow, row1 = row0 + 8;
+      const float inf = __int_as_float(0x7f800000);
+      const float t0 = row0 < nq ? thr[row0] : inf, t1 = row1 < nq ? thr[row1] : inf;
+
+      // mainloop: one wgmma group per k block in flight; a stage is released once the group after it was issued
+      float acc[128];
+#pragma unroll
+      for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+      uint32_t prev_stage = 0;
+      for (int kb = 0; kb < num_k; ++kb) {
+        mbar_wait_warp(&full_bar[stage], phase, 31);
+        const uint32_t a_addr = smem_u32(smem + stage * kScanStageBytes) + wg * (64 * 128);
+        const uint32_t b_addr = smem_u32(smem + stage * kScanStageBytes + kScanABytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+          wgmma_m64n256k16_f16<0, 0>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
+                                     wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        if (kb > 0) {
+          wgmma_wait<1>();
+          if (lane == 0) {
+            mbar_arrive(&empty_bar[prev_stage]);
+            mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
+          }
+        }
+        prev_stage = stage;
+        if (++stage == kScanStages) {
+          stage = 0;
+          phase ^= 1u;
+        }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (num_k > 0 && lane == 0) {
+        mbar_arrive(&empty_bar[prev_stage]);
+        mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
+      }
+
+      // ------------------------------ filter on the fragments ------------------------------
+      drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
+      const int col0 = n_blk * kScanBlockN;
+      const int lim = n_cols - col0;
+      unsigned long long* sb = stash + buf * (2 * kScanStash * kScanConsumers) + et;
+      const int k0 = scan_filter_row<0>(acc, t0, row0, lim, q4, col0, sb, cand, count, overflow, C, row_base);
+      const int k1 = scan_filter_row<1>(acc, t1, row1, lim, q4, col0, sb + kScanStash * kScanConsumers, cand, count,
+                                        overflow, C, row_base);
+      if (__any_sync(0xffffffffu, (k0 | k1) != 0)) {
+        // quad aggregation: lanes 4 i .. 4 i + 3 share both rows; exclusive prefix per lane, one atomic per quad and row
+        int x0 = k0, x1 = k1;
+        int y0 = __shfl_up_sync(0xffffffffu, x0, 1, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 1, 4);
+        if (q4 >= 1) x0 += y0, x1 += y1;
+        y0 = __shfl_up_sync(0xffffffffu, x0, 2, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 2, 4);
+        if (q4 >= 2) x0 += y0, x1 += y1;
+        const int n0 = __shfl_sync(0xffffffffu, x0, lane | 3), n1 = __shfl_sync(0xffffffffu, x1, lane | 3);
+        if (q4 == 0) {
+          if (n0 > 0) p_pos0 = atomicAdd(count + row0, n0);  // result first used by the next drain()
+          if (n1 > 0) p_pos1 = atomicAdd(count + row1, n1);
+        }
+        p_n0 = k0;
+        p_n1 = k1;
+        p_excl0 = x0 - k0;
+        p_excl1 = x1 - k1;
+        p_row = row0;
+        p_buf = buf;
+        buf ^= 1;
+      }
+    }
+    drain();
+  }
+
+  __syncthreads();
+  cluster_sync_all();  // the peer may still be signalling this CTA's barriers or writing into its ring
+}
+
+// Host launcher.  Q: [nq, K] fp16 queries, row pitch ldq elements; X: [n_cols, K] fp16 corpus rows, row pitch ldx.
+// Survivors (score > thr[q]) are appended to cand[q * C ...] as make_key(score, row_base + column); a list that
+// would grow beyond C sets *overflow.  Returns cudaSuccess / a CUDA error; tensor-map failures map to
+// cudaErrorInvalidValue, and cudaErrorNotSupported means that no 2-CTA cluster of the kernel fits on the device.
+static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const __half* X, int64_t ldx, int nq, int n_cols,
+                                           int K, const float* thr, unsigned long long* cand, int* count, int* overflow,
+                                           int C, uint32_t row_base, int num_sms, cudaStream_t stream) {
+  if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
+  CUtensorMap tmQ, tmX;
+  if (make_tmap_bf16_2d(&tmQ, Q, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq * 2, kBlockK, kBlockM) != 0)
+    return cudaErrorInvalidValue;
+  if (make_tmap_bf16_2d(&tmX, X, (uint64_t)K, (uint64_t)n_cols, (uint64_t)ldx * 2, kBlockK, kScanBlockN / 2) != 0)
+    return cudaErrorInvalidValue;
+  cudaLaunchConfig_t cfg = {};
+  cfg.blockDim = dim3(kGemmProducerThreads + kScanConsumers);
+  cfg.dynamicSmemBytes = kScanSmemBytes;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  // the persistent schedule wants every cluster co-resident (a second wave of clusters would double the run time)
+  static int max_clusters = 0;
+  if (!max_clusters) {
+    cudaError_t e = cudaFuncSetAttribute(scan_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmemBytes);
+    if (e != cudaSuccess) return e;
+    cfg.gridDim = dim3(2 * (num_sms / 2));
+    int n = 0;
+    e = cudaOccupancyMaxActiveClusters(&n, scan_wide_kernel, &cfg);
+    if (e != cudaSuccess) return e;
+    if (n < 1) return cudaErrorNotSupported;
+    max_clusters = n < num_sms / 2 ? n : num_sms / 2;
+  }
+  const int pairs = (nq + 2 * kBlockM - 1) / (2 * kBlockM);
+  const int64_t num_tiles = static_cast<int64_t>(pairs) * ((n_cols + kScanBlockN - 1) / kScanBlockN);
+  const int clusters = num_tiles < max_clusters ? static_cast<int>(num_tiles) : max_clusters;
+  cfg.gridDim = dim3(2 * clusters);
+  return cudaLaunchKernelEx(&cfg, scan_wide_kernel, tmQ, tmX, K, thr, cand, count, overflow, nq, n_cols, C, row_base);
+}
+
+}  // namespace om

@@ -8,9 +8,10 @@
 // same tensor-core rate, which is what makes the exactness certificate below affordable).
 //
 // search(q, k):
-//   1. SCAN    fp16 Q * X^T on wgmma (gemm.cuh mainloop) with the top-k filter fused into the epilogue:
-//              scores never leave the SM (registers / shared memory); a thread owns one query row, compares its 32-column chunk
-//              against that query's running threshold and appends the rare survivors
+//   1. SCAN    fp16 Q * X^T on wgmma with the top-k filter fused into the epilogue (query batches: scan_gemm.cuh, 2-CTA
+//              clusters, filter on the accumulator registers; the first round and <= 128 queries: the gemm.cuh mainloop):
+//              scores never leave the SM (registers / shared memory); each query row's scores are compared against that
+//              query's running threshold and the rare survivors are appended
 //              (key = orderable(score) << 32 | ~row) to the query's candidate list in HBM.
 //              The corpus is swept in rounds of geometrically growing size; after each round
 //   2. SELECT  a per-query radix select keeps the best kp = k + slack candidates and publishes the kp-th score
@@ -40,6 +41,7 @@
 #include "gemm.cuh"
 #include "nccl_dyn.h"
 #include "scan_epilogue.cuh"
+#include "scan_gemm.cuh"
 
 namespace om {
 
@@ -583,7 +585,7 @@ struct om_index {
   float* gstats = nullptr;  // device [2]: max ||x||, max ||x - x_h|| over the committed rows (float bit patterns)
   int64_t rescore_slack = -1;
   int force_safe = 0;
-  int pair_scan = 1;      // scan GEMM on 2-CTA clusters sharing each corpus tile by TMA multicast; 0 = single-CTA tiles
+  int pair_scan = 1;      // > 128 queries: rounds after the first on the wide scan (scan_gemm.cuh); 0 = single-CTA tiles
   int growth = 0;         // each round scans (growth - 1) x the rows seen so far; 0 = auto: 2 for query batches (fewest
                           // filter survivors), 8 for <= 256 queries (HBM-bound streaming regime: 5 instead of 13
                           // dependent scan + select launch pairs over 8.8 M rows)
@@ -944,21 +946,21 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
       Timed t(ix, st, 0);
       if (L.mode == 0) {
         const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
-        cudaError_t e = cudaErrorNotSupported;
+        cudaError_t e;
         const int ncols = static_cast<int>(step);
         // a 2-CTA cluster owns 2 x 128 query rows per tile: with <= 128 queries the peer's half would be padding (and the sweep is
-        // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing)
+        // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
+        // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
         const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
         if (first) {
           EpiScan<true> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          if (pair) e = launch_gemm<128, 3, true, EpiScan<true>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
-          if (e == cudaErrorNotSupported)  // no 2-CTA cluster fits on the device
-            e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
+          e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
+        } else if (pair) {
+          e = launch_scan_wide(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C,
+                               static_cast<uint32_t>(pos), sms, st);
         } else {
           EpiScan<false> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          if (pair) e = launch_gemm<128, 3, true, EpiScan<false>, true, 2>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st);
-          if (e == cudaErrorNotSupported)
-            e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
+          e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         }
         if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
       } else {
