@@ -545,10 +545,11 @@ struct LossWs {
   size_t bytes = 0;
   unsigned* grid_bar = nullptr;  // persistent (self-resetting), zeroed once: [0] grid barrier, [64..] split-K counters,
                                  // last 64 bytes: phase timestamps
-  // tensor maps are rebuilt only when the problem or the workspace changes
+  // tensor maps are rebuilt only when an address or an extent they encode changes.  G's offset in the workspace
+  // depends on whether the caller keeps the logits (scores_out), so it is part of the key.
   LossMaps maps;
   const void* maps_base = nullptr;
-  const void *maps_q = nullptr, *maps_p = nullptr;
+  const void *maps_q = nullptr, *maps_p = nullptr, *maps_g = nullptr;
   int maps_nq = 0, maps_np = 0, maps_d = 0;
 };
 constexpr int kLossBarBytes = 65536, kLossSemSlots = (kLossBarBytes - 256 - 64) / 4;
@@ -668,8 +669,8 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
   const void* q_src = direct ? Q : static_cast<const void*>(a.qb);
   const void* p_src = direct ? P : static_cast<const void*>(a.pb);
   const uint64_t in_pitch = direct ? (uint64_t)d * 2 : (uint64_t)dpad * 2;
-  if (ws.maps_base != ws.p || ws.maps_q != q_src || ws.maps_p != p_src || ws.maps_nq != nq || ws.maps_np != np ||
-      ws.maps_d != d) {
+  if (ws.maps_base != ws.p || ws.maps_q != q_src || ws.maps_p != p_src || ws.maps_g != a.G || ws.maps_nq != nq ||
+      ws.maps_np != np || ws.maps_d != d) {
     const uint64_t un = (uint64_t)np, uq = (uint64_t)nq, ud = (uint64_t)d;
     int rc = 0;
     // K-major operands: box {64 k, 128 rows}; MN-major operands (the matrix as stored, K = its rows): box {64, 64}
@@ -683,6 +684,7 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
     ws.maps_base = ws.p;
     ws.maps_q = q_src;
     ws.maps_p = p_src;
+    ws.maps_g = a.G;
     ws.maps_nq = nq;
     ws.maps_np = np;
     ws.maps_d = d;

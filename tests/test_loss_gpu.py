@@ -35,7 +35,8 @@ def _rel(a, b):
                                              # np > 4096 / np % 4 != 0: looped softmax; ragged K slices of dQ
                                              (96, 4100, 200, torch.float32), (33, 2052, 72, torch.float32),
                                              (40, 1001, 136, torch.float32),
-                                             # bf16 rows that TMA cannot read in place (pitch not 16-byte aligned)
+                                             # bf16: a 72-byte row pitch is not 16-byte aligned, so the rows are
+                                             # copied; a 400-byte pitch is, so they are read in place
                                              (12, 24, 36, torch.bfloat16), (130, 1040, 200, torch.bfloat16)])
 def test_loss_and_grads_vs_oracle(L, nq, n_p, d, dtype):
     gen = torch.Generator().manual_seed(nq + d)
@@ -110,4 +111,7 @@ def test_upstream_gradient_scaling_and_errors(L):
     with pytest.raises(RuntimeError):
         L.SimpleContrastiveLoss()(torch.randn(4, 32), torch.randn(8, 32))  # CPU tensors: no CPU path
     bad = L.SimpleContrastiveLoss()(x, y, target=torch.tensor([0, 1, 99, 2], device="cuda"))
+    assert torch.isnan(bad)
+    # no ignore_index: PyTorch's -100 is out of range like any other (DESIGN section 6)
+    bad = L.SimpleContrastiveLoss()(x, y, target=torch.tensor([0, 1, -100, 2], device="cuda"))
     assert torch.isnan(bad)
