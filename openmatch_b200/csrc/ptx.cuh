@@ -225,12 +225,15 @@ __device__ __forceinline__ uint32_t cluster_count_x() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-// arrive on the mbarrier at the address of `bar` in the shared memory of the cluster's CTA `rank`
+// arrive on the mbarrier at the address of `bar` in the shared memory of the cluster's CTA `rank`.  Default semantics
+// (release at CTA scope), as for a ring slot that a peer's TMA refills: the arriving thread's only accesses to the slot
+// are wgmma reads, finished by wgmma.wait_group before the arrive.  `.release.cluster` would add a GPU-scope memory
+// barrier (MEMBAR.ALL.GPU) to every arrive, which waits for the thread's outstanding global stores and atomics.
 __device__ __forceinline__ void mbar_arrive_remote(uint64_t* bar, uint32_t rank) {
   asm volatile(
       "{\n\t.reg .b32 ra;\n\t"
       "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}\n"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}\n"
       ::"r"(smem_u32(bar)), "r"(rank)
       : "memory");
 }

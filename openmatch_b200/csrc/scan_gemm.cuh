@@ -1,18 +1,23 @@
-// Search scan for query batches: fp16 Q * X^T on 2-CTA clusters with the top-k filter applied directly to the wgmma
-// accumulator registers.
+// Search scan for query batches: fp16 Q * X^T on CQ x CX CTA clusters with the top-k filter applied directly to the
+// wgmma accumulator registers.
 //
-//   tile        one cluster owns 256 queries x 256 corpus rows; CTA `rank` of the pair owns queries
-//               [128 (2 p + rank), +128) of pair row p and the whole 256-row corpus tile, K = d in 64-wide k blocks
-//   operands    each CTA TMA-loads its own 128-query box and one 128-row half of the corpus tile, multicast into both
-//               CTAs' shared memory; the two halves land back to back and form one K-major SW128 operand of 256 rows,
-//               so every corpus byte crosses L2 -> SM once per pair (32 KB per CTA and k block for 4.2 MFLOP)
+//   tile        a cluster owns CQ x 128 queries x CX x 256 corpus rows; cluster rank r is CTA (a, b) = (r % CQ, r / CQ),
+//               which owns query box a (128 queries) x corpus tile b (256 rows), K = d in 64-wide k blocks
+//   operands    corpus tile b is needed by the CQ CTAs of column b and query box a by the CX CTAs of row a: each CTA
+//               TMA-loads a 256/CQ-row slice of its corpus tile and a 128/CX-row slice of its query box and multicasts
+//               each slice to the CTAs that share it.  Slices land back to back at the same offset in every destination
+//               (slice boundaries are multiples of the 8-row / 1 KB swizzle atom), so every CTA sees one K-major SW128
+//               operand of 128 rows (A) and one of 256 rows (B).  L2 -> SM bytes per CTA and k block: 16/CX + 32/CQ KB
+//               for 4.2 MFLOP
 //   warp roles  warpgroup 0: one TMA producer lane (registers lowered to 40); warpgroups 1, 2: consumers (registers
 //               raised to 232), consumer g issues wgmma m64n256k16 for queries [64 g, +64) of the CTA's 128 and holds the
 //               64 x 256 fp32 accumulator tile in 128 registers per thread
-//   ring        kScanStages x 48 KB; a slot is released one wgmma group late on the empty barriers of BOTH CTAs (every
-//               consumer warp of the pair arrives on each), since the peer's producer writes half of every slot
-//   schedule    persistent, static, queries fastest: tile t -> pair row t % pairs, corpus tile t / pairs, so all
-//               clusters work on neighbouring corpus tiles and the corpus streams from HBM about once
+//   ring        kScanStages x 48 KB; the producer of CTA c writes into every CTA of S(c) = {same a} U {same b}, so a slot
+//               is released one wgmma group late on the empty barriers of all of S(c) (ScanCluster)
+//   schedule    persistent, static, queries fastest: tile t -> query group t % qgroups, corpus group t / qgroups, so all
+//               clusters work on neighbouring corpus tiles and the corpus streams from HBM about once.  Every CTA runs
+//               every k block of every tile of its cluster, also when its corpus tile lies past n_cols or its query box
+//               is all padding (TMA zero fill, every column masked): its peers wait on its slices and releases
 //   epilogue    no staging through shared memory: a thread owns two query rows (fragment rows l/4 and l/4 + 8 of its
 //               warp's 16) x 64 corpus columns (8 j + 2 (l % 4) + {0, 1}, j < 32).  One 64-value max per row against the
 //               query's strict threshold rejects the row in the common case; survivors go through a compact bit-mask
@@ -29,9 +34,11 @@
 namespace om {
 
 constexpr int kScanBlockN = 256;                             // corpus rows per tile
-constexpr int kScanStages = 3;  // 4 fit next to the stash too, but ran the C2 scan 2-4 % slower (H100 SXM, 700 W)
+// 4 stages fit next to the stash too, but ran the C2 scan 2-4 % slower (H100 SXM, 700 W); at 400 W the largest C2 round
+// took 130.5 / 136.8 ms with 3 / 4 stages on 2x1 clusters
+constexpr int kScanStages = 3;
 constexpr int kScanABytes = kBlockM * kBlockK * 2;           // 16 KB: the CTA's 128 queries
-constexpr int kScanBBytes = kScanBlockN * kBlockK * 2;       // 32 KB: the pair's corpus tile (two multicast halves)
+constexpr int kScanBBytes = kScanBlockN * kBlockK * 2;       // 32 KB: the CTA's corpus tile
 constexpr int kScanStageBytes = kScanABytes + kScanBBytes;
 constexpr int kScanConsumers = 256;                          // two consumer warpgroups
 constexpr int kScanStash = 4;                                // survivors a thread parks per row and tile
@@ -106,16 +113,53 @@ __device__ __forceinline__ int scan_filter_row(const float (&acc)[128], float t,
   return n < kScanStash ? n : kScanStash;
 }
 
+// Cluster shape CQ x CX and the operand sharing it implies: the one place that knows which CTAs write into which ring
+// and who releases it.  CTA c = (a, b) multicasts its query slice to S_q(c) = {(a, b') : b' < CX} and its corpus slice
+// to S_x(c) = {(a', b) : a' < CQ}, so its producer writes into S(c) = S_q(c) U S_x(c), |S(c)| = CQ + CX - 1 CTAs.  A slot
+// of c's ring is written by the producers of S(c) (the relation is symmetric), so c's empty barrier counts the consumer
+// warps of all of S(c), and each consumer warp of c arrives on the empty barrier of every CTA in S(c).
+template <int CQ, int CX>
+struct ScanCluster {
+  static_assert((CQ == 2 || CQ == 4) && (CX == 1 || CX == 2), "scan cluster shapes: CQ in {2, 4}, CX in {1, 2}");
+  static constexpr int kSize = CQ * CX;
+  static constexpr int kShare = CQ + CX - 1;       // |S(c)|, c included
+  static constexpr int kQRows = kBlockM / CX;      // query rows of the slice a CTA loads per k block
+  static constexpr int kXRows = kScanBlockN / CQ;  // corpus rows of the slice a CTA loads per k block
+  static constexpr int kEmptyArrivals = kShare * (kScanConsumers / 32);
+  // rank of the j-th CTA of S(c) other than c, j < kShare - 1: the other CTAs of corpus column b, then those of query row a
+  __device__ static uint32_t peer_rank(uint32_t rank, int j) {
+    const uint32_t a = rank % CQ, b = rank / CQ;
+    if (j < CQ - 1) {
+      const uint32_t o = static_cast<uint32_t>(j);
+      return (o < a ? o : o + 1) + CQ * b;
+    }
+    const uint32_t o = static_cast<uint32_t>(j - (CQ - 1));
+    return a + CQ * (o < b ? o : o + 1);
+  }
+  __device__ static uint16_t q_mask(uint32_t rank) {  // S_q(c)
+    uint32_t m = 0;
+#pragma unroll
+    for (int b = 0; b < CX; ++b) m |= 1u << (rank % CQ + CQ * b);
+    return static_cast<uint16_t>(m);
+  }
+  __device__ static uint16_t x_mask(uint32_t rank) {  // S_x(c)
+    return static_cast<uint16_t>(((1u << CQ) - 1u) << (CQ * (rank / CQ)));
+  }
+};
+
+template <int CQ, int CX>
 __global__ void __launch_bounds__(kGemmProducerThreads + kScanConsumers, 1)
 scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmX, int K,
                  const float* __restrict__ thr, unsigned long long* cand, int* count, int* overflow, int nq, int n_cols,
                  int C, uint32_t row_base) {
+  using Cl = ScanCluster<CQ, CX>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   unsigned long long* stash = reinterpret_cast<unsigned long long*>(smem + kScanStashOffset);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kScanBarOffset);
   uint64_t* empty_bar = full_bar + kScanStages;
   const uint32_t rank = cluster_ctarank();
+  const int qa = static_cast<int>(rank % CQ), xb = static_cast<int>(rank / CQ);
   const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
   const int lane = static_cast<int>(threadIdx.x & 31);
 
@@ -125,32 +169,37 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   }
   if (warp == 1 && lane == 0) {
     for (int i = 0; i < kScanStages; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 2 * kScanConsumers / 32);  // every consumer warp of both CTAs
+      mbar_init(&full_bar[i], 1);  // the own producer's expect_tx; the bytes come from every producer of S(c)
+      mbar_init(&empty_bar[i], Cl::kEmptyArrivals);
     }
     fence_barrier_init();
   }
-  cluster_sync_all();  // the peer's barriers exist before any multicast or remote arrive
+  cluster_sync_all();  // every peer's barriers exist before any multicast or remote arrive
 
-  const int pairs = (nq + 2 * kBlockM - 1) / (2 * kBlockM);
-  const int num_tiles = pairs * ((n_cols + kScanBlockN - 1) / kScanBlockN);
+  const int qgroups = (nq + CQ * kBlockM - 1) / (CQ * kBlockM);
+  const int num_tiles = qgroups * ((n_cols + CX * kScanBlockN - 1) / (CX * kScanBlockN));
   const int num_k = (K + kBlockK - 1) / kBlockK;
 
   if (warp < 4) {
     setmaxnreg_dec<40>();
     if (warp == 0 && lane == 0) {
       // ------------------------------ TMA producer ------------------------------
+      const uint16_t qmask = Cl::q_mask(rank), xmask = Cl::x_mask(rank);
       uint32_t stage = 0, phase = 0;
       for (int tile = static_cast<int>(cluster_id_x()); tile < num_tiles; tile += static_cast<int>(cluster_count_x())) {
-        const int m_blk = (tile % pairs) * 2 + static_cast<int>(rank);
-        const int n_blk = tile / pairs;
+        const int m_blk = (tile % qgroups) * CQ + qa;
+        const int n_blk = (tile / qgroups) * CX + xb;
         for (int kb = 0; kb < num_k; ++kb) {
           mbar_wait(&empty_bar[stage], phase ^ 1u, 30);
           uint8_t* sa = smem + stage * kScanStageBytes;
           mbar_arrive_expect_tx(&full_bar[stage], kScanStageBytes);
-          tma_load_2d(sa, &tmQ, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d_multicast(sa + kScanABytes + rank * (kScanBBytes / 2), &tmX, &full_bar[stage], kb * kBlockK,
-                                n_blk * kScanBlockN + static_cast<int>(rank) * (kScanBlockN / 2), static_cast<uint16_t>(3u));
+          if constexpr (CX == 1)
+            tma_load_2d(sa, &tmQ, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
+          else
+            tma_load_2d_multicast(sa + xb * (Cl::kQRows * kBlockK * 2), &tmQ, &full_bar[stage], kb * kBlockK,
+                                  m_blk * kBlockM + xb * Cl::kQRows, qmask);
+          tma_load_2d_multicast(sa + kScanABytes + qa * (Cl::kXRows * kBlockK * 2), &tmX, &full_bar[stage], kb * kBlockK,
+                                n_blk * kScanBlockN + qa * Cl::kXRows, xmask);
           if (++stage == kScanStages) {
             stage = 0;
             phase ^= 1u;
@@ -184,9 +233,21 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       p_n0 = p_n1 = 0;
     };
 
+    // lane 0 of every consumer warp releases a slot on the empty barrier of each CTA of S(c)
+    uint32_t peers[Cl::kShare - 1];
+#pragma unroll
+    for (int j = 0; j < Cl::kShare - 1; ++j) peers[j] = Cl::peer_rank(rank, j);
+    auto release = [&](uint32_t s) {
+      if (lane == 0) {
+        mbar_arrive(&empty_bar[s]);
+#pragma unroll
+        for (int j = 0; j < Cl::kShare - 1; ++j) mbar_arrive_remote(&empty_bar[s], peers[j]);
+      }
+    };
+
     for (int tile = static_cast<int>(cluster_id_x()); tile < num_tiles; tile += static_cast<int>(cluster_count_x())) {
-      const int m_blk = (tile % pairs) * 2 + static_cast<int>(rank);
-      const int n_blk = tile / pairs;
+      const int m_blk = (tile % qgroups) * CQ + qa;
+      const int n_blk = (tile / qgroups) * CX + xb;
       const int row0 = m_blk * kBlockM + frow, row1 = row0 + 8;
       const float inf = __int_as_float(0x7f800000);
       const float t0 = row0 < nq ? thr[row0] : inf, t1 = row1 < nq ? thr[row1] : inf;
@@ -208,10 +269,7 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         wgmma_commit();
         if (kb > 0) {
           wgmma_wait<1>();
-          if (lane == 0) {
-            mbar_arrive(&empty_bar[prev_stage]);
-            mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
-          }
+          release(prev_stage);
         }
         prev_stage = stage;
         if (++stage == kScanStages) {
@@ -221,15 +279,12 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       }
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
-      if (num_k > 0 && lane == 0) {
-        mbar_arrive(&empty_bar[prev_stage]);
-        mbar_arrive_remote(&empty_bar[prev_stage], rank ^ 1u);
-      }
+      if (num_k > 0) release(prev_stage);
 
       // ------------------------------ filter on the fragments ------------------------------
       drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
       const int col0 = n_blk * kScanBlockN;
-      const int lim = n_cols - col0;
+      const int lim = n_cols - col0;  // <= 0: the whole corpus tile lies past n_cols and every column is masked
       unsigned long long* sb = stash + buf * (2 * kScanStash * kScanConsumers) + et;
       const int k0 = scan_filter_row<0>(acc, t0, row0, lim, q4, col0, sb, cand, count, overflow, C, row_base);
       const int k1 = scan_filter_row<1>(acc, t1, row1, lim, q4, col0, sb + kScanStash * kScanConsumers, cand, count,
@@ -262,47 +317,95 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
   cluster_sync_all();  // the peer may still be signalling this CTA's barriers or writing into its ring
 }
 
-// Host launcher.  Q: [nq, K] fp16 queries, row pitch ldq elements; X: [n_cols, K] fp16 corpus rows, row pitch ldx.
-// Survivors (score > thr[q]) are appended to cand[q * C ...] as make_key(score, row_base + column); a list that
-// would grow beyond C sets *overflow.  Returns cudaSuccess / a CUDA error; tensor-map failures map to
-// cudaErrorInvalidValue, and cudaErrorNotSupported means that no 2-CTA cluster of the kernel fits on the device.
+// Clusters of the CQ x CX scan that are co-resident on the device (cached per shape, one device per process); 0 when
+// none fits.  The persistent schedule wants every cluster co-resident (a second wave would double the run time).
+template <int CQ, int CX>
+static inline cudaError_t scan_wide_max_clusters(int num_sms, int* out) {
+  static int max_clusters = -1;
+  if (max_clusters < 0) {
+    constexpr int kSize = ScanCluster<CQ, CX>::kSize;
+    cudaError_t e =
+        cudaFuncSetAttribute(scan_wide_kernel<CQ, CX>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmemBytes);
+    if (e != cudaSuccess) return e;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(kSize * (num_sms / kSize));
+    cfg.blockDim = dim3(kGemmProducerThreads + kScanConsumers);
+    cfg.dynamicSmemBytes = kScanSmemBytes;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim = {static_cast<unsigned>(kSize), 1, 1};
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    int n = 0;
+    e = cudaOccupancyMaxActiveClusters(&n, scan_wide_kernel<CQ, CX>, &cfg);
+    if (e != cudaSuccess) return e;
+    max_clusters = n < num_sms / kSize ? n : num_sms / kSize;
+  }
+  *out = max_clusters;
+  return cudaSuccess;
+}
+
+template <int CQ, int CX>
 static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const __half* X, int64_t ldx, int nq, int n_cols,
                                            int K, const float* thr, unsigned long long* cand, int* count, int* overflow,
                                            int C, uint32_t row_base, int num_sms, cudaStream_t stream) {
-  if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
+  using Cl = ScanCluster<CQ, CX>;
   CUtensorMap tmQ, tmX;
-  if (make_tmap_bf16_2d(&tmQ, Q, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq * 2, kBlockK, kBlockM) != 0)
+  if (make_tmap_bf16_2d(&tmQ, Q, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq * 2, kBlockK, Cl::kQRows) != 0)
     return cudaErrorInvalidValue;
-  if (make_tmap_bf16_2d(&tmX, X, (uint64_t)K, (uint64_t)n_cols, (uint64_t)ldx * 2, kBlockK, kScanBlockN / 2) != 0)
+  if (make_tmap_bf16_2d(&tmX, X, (uint64_t)K, (uint64_t)n_cols, (uint64_t)ldx * 2, kBlockK, Cl::kXRows) != 0)
     return cudaErrorInvalidValue;
+  int max_clusters = 0;
+  cudaError_t e = scan_wide_max_clusters<CQ, CX>(num_sms, &max_clusters);
+  if (e != cudaSuccess) return e;
+  if (max_clusters < 1) return cudaErrorNotSupported;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(kGemmProducerThreads + kScanConsumers);
   cfg.dynamicSmemBytes = kScanSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
+  attr[0].val.clusterDim = {static_cast<unsigned>(Cl::kSize), 1, 1};
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  // the persistent schedule wants every cluster co-resident (a second wave of clusters would double the run time)
-  static int max_clusters = 0;
-  if (!max_clusters) {
-    cudaError_t e = cudaFuncSetAttribute(scan_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmemBytes);
-    if (e != cudaSuccess) return e;
-    cfg.gridDim = dim3(2 * (num_sms / 2));
-    int n = 0;
-    e = cudaOccupancyMaxActiveClusters(&n, scan_wide_kernel, &cfg);
-    if (e != cudaSuccess) return e;
-    if (n < 1) return cudaErrorNotSupported;
-    max_clusters = n < num_sms / 2 ? n : num_sms / 2;
-  }
-  const int pairs = (nq + 2 * kBlockM - 1) / (2 * kBlockM);
-  const int64_t num_tiles = static_cast<int64_t>(pairs) * ((n_cols + kScanBlockN - 1) / kScanBlockN);
+  const int qgroups = (nq + CQ * kBlockM - 1) / (CQ * kBlockM);
+  const int64_t num_tiles = static_cast<int64_t>(qgroups) * ((n_cols + CX * kScanBlockN - 1) / (CX * kScanBlockN));
   const int clusters = num_tiles < max_clusters ? static_cast<int>(num_tiles) : max_clusters;
-  cfg.gridDim = dim3(2 * clusters);
-  return cudaLaunchKernelEx(&cfg, scan_wide_kernel, tmQ, tmX, K, thr, cand, count, overflow, nq, n_cols, C, row_base);
+  cfg.gridDim = dim3(Cl::kSize * clusters);
+  return cudaLaunchKernelEx(&cfg, scan_wide_kernel<CQ, CX>, tmQ, tmX, K, thr, cand, count, overflow, nq, n_cols, C,
+                            row_base);
+}
+
+// Host launcher of the wide scan on cq x cx clusters (cq in {2, 4}, cx in {1, 2}).  Q: [nq, K] fp16 queries, row pitch
+// ldq elements; X: [n_cols, K] fp16 corpus rows, row pitch ldx.  Survivors (score > thr[q]) are appended to
+// cand[q * C ...] as make_key(score, row_base + column); a list that would grow beyond C sets *overflow.  Every shape
+// computes each score with the same wgmma sequence, so the candidate lists hold the same keys whatever the shape.
+// Returns cudaSuccess / a CUDA error; tensor-map failures and other shapes map to cudaErrorInvalidValue, and
+// cudaErrorNotSupported means that no cluster of the shape fits on the device.
+static inline cudaError_t launch_scan_cluster(int cq, int cx, const __half* Q, int64_t ldq, const __half* X, int64_t ldx,
+                                              int nq, int n_cols, int K, const float* thr, unsigned long long* cand,
+                                              int* count, int* overflow, int C, uint32_t row_base, int num_sms,
+                                              cudaStream_t stream) {
+  if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
+  if (cq == 2 && cx == 1)
+    return launch_scan_wide<2, 1>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
+  if (cq == 4 && cx == 1)
+    return launch_scan_wide<4, 1>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
+  if (cq == 2 && cx == 2)
+    return launch_scan_wide<2, 2>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
+  if (cq == 4 && cx == 2)
+    return launch_scan_wide<4, 2>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
+  return cudaErrorInvalidValue;
+}
+
+// Co-resident clusters of the cq x cx scan on this device (0 when none fits, -1 for another shape).
+static inline cudaError_t scan_cluster_capacity(int cq, int cx, int num_sms, int* out) {
+  *out = -1;
+  if (cq == 2 && cx == 1) return scan_wide_max_clusters<2, 1>(num_sms, out);
+  if (cq == 4 && cx == 1) return scan_wide_max_clusters<4, 1>(num_sms, out);
+  if (cq == 2 && cx == 2) return scan_wide_max_clusters<2, 2>(num_sms, out);
+  if (cq == 4 && cx == 2) return scan_wide_max_clusters<4, 2>(num_sms, out);
+  return cudaSuccess;
 }
 
 }  // namespace om

@@ -586,6 +586,7 @@ struct om_index {
   int64_t rescore_slack = -1;
   int force_safe = 0;
   int pair_scan = 1;      // > 128 queries: rounds after the first on the wide scan (scan_gemm.cuh); 0 = single-CTA tiles
+  int scan_cq = 0, scan_cx = 0;  // cluster shape of the wide scan (CQ CTAs along the queries x CX along the corpus); 0 = auto
   int growth = 0;         // each round scans (growth - 1) x the rows seen so far; 0 = auto: 2 for query batches (fewest
                           // filter survivors), 8 for <= 256 queries (HBM-bound streaming regime: 5 instead of 13
                           // dependent scan + select launch pairs over 8.8 M rows)
@@ -594,6 +595,7 @@ struct om_index {
   int stage_scores = 0;   // 1: emit candidate-stage scores instead of fp32 re-scores (measuring the error model)
   int64_t st_rounds = 0, st_retries = 0, st_capacity = 0, st_launches = 0;
   int64_t st_flagged = 0, st_flagged_wide = 0, st_exact = 0;
+  int64_t st_scan_cluster = 0, st_scan_clusters = 0;  // last wide scan: 10 CQ + CX and its co-resident clusters (0: none ran)
   // optional per-phase device timing (CUDA events on the launching stream), enabled by set_param("profile", 1)
   int profile = 0;
   double st_scan_us = 0, st_select_us = 0, st_final_us = 0, st_other_us = 0;
@@ -746,6 +748,12 @@ int om_index_set_param(om_index* ix, const char* name, int64_t value) {
     ix->growth = static_cast<int>(value);
   } else if (!strcmp(name, "pair_scan")) {
     ix->pair_scan = value != 0;
+  } else if (!strcmp(name, "scan_cluster_q")) {
+    if (value != 0 && value != 2 && value != 4) return fail(OM_EINVAL, "scan_cluster_q must be 0 (auto), 2 or 4");
+    ix->scan_cq = static_cast<int>(value);
+  } else if (!strcmp(name, "scan_cluster_x")) {
+    if (value != 0 && value != 1 && value != 2) return fail(OM_EINVAL, "scan_cluster_x must be 0 (auto), 1 or 2");
+    ix->scan_cx = static_cast<int>(value);
   } else if (!strcmp(name, "profile")) {
     ix->profile = static_cast<int>(value);
   } else if (!strcmp(name, "certify")) {
@@ -769,6 +777,8 @@ int64_t om_index_get_stat(const om_index* ix, const char* name) {
   if (!strcmp(name, "uncertified")) return ix->st_flagged;
   if (!strcmp(name, "uncertified_wide")) return ix->st_flagged_wide;
   if (!strcmp(name, "exact_queries")) return ix->st_exact;
+  if (!strcmp(name, "scan_cluster")) return ix->st_scan_cluster;
+  if (!strcmp(name, "scan_max_clusters")) return ix->st_scan_clusters;
   if (!strcmp(name, "scan_ns")) return static_cast<int64_t>(ix->st_scan_us * 1e3);
   if (!strcmp(name, "select_ns")) return static_cast<int64_t>(ix->st_select_us * 1e3);
   if (!strcmp(name, "finalize_ns")) return static_cast<int64_t>(ix->st_final_us * 1e3);
@@ -948,7 +958,7 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
         cudaError_t e;
         const int ncols = static_cast<int>(step);
-        // a 2-CTA cluster owns 2 x 128 query rows per tile: with <= 128 queries the peer's half would be padding (and the sweep is
+        // a cluster owns at least 2 x 128 query rows per tile: with <= 128 queries the peers' boxes would be padding (and the sweep is
         // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
         // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
         const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
@@ -956,8 +966,16 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
           EpiScan<true> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         } else if (pair) {
-          e = launch_scan_wide(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C,
-                               static_cast<uint32_t>(pos), sms, st);
+          // cluster shape CQ x CX: the index parameters, else 2 x 1.  The wider shapes cut L2 -> SM traffic by 25 - 50 %, but
+          // only 30 clusters of 4 and 15 of 8 CTAs fit an H100 SXM (120 SMs, against 66 pairs on all 132), and the whole
+          // search measured no faster on any of them beyond run-to-run noise at C2 and slower at C5 (DESIGN §7)
+          const int cq = ix->scan_cq ? ix->scan_cq : 2, cx = ix->scan_cx ? ix->scan_cx : 1;
+          int clusters = 0;
+          e = launch_scan_cluster(cq, cx, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
+                                  overflow, C, static_cast<uint32_t>(pos), sms, st);
+          if (e == cudaSuccess) e = scan_cluster_capacity(cq, cx, sms, &clusters);
+          ix->st_scan_cluster = 10 * cq + cx;
+          ix->st_scan_clusters = clusters;
         } else {
           EpiScan<false> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
@@ -1129,6 +1147,7 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   const int world = comm ? comm->world : 1;
   ix->st_rounds = ix->st_retries = ix->st_launches = 0;
   ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
+  ix->st_scan_cluster = ix->st_scan_clusters = 0;
   ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
   ix->ev_used = 0;
   // whole-search staging: queries (if they arrive from the host), results (if they leave to the host), flag list
