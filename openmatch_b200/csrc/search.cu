@@ -1038,7 +1038,12 @@ int merge_parts(const float* Dp, const int64_t* Ip, int64_t stride_d, int64_t st
     OM_CUDA(cudaGetLastError());
     return 0;
   }
-  // groups of g parts -> intermediate lists of width k_mid, then recurse on the groups
+  // groups of g parts -> intermediate lists of width k_mid, then recurse on the groups.  Each level shrinks only if a
+  // group of g >= 2 parts fits one merge (k_in <= 4096) and the groups' lists stay that narrow (k_out <= 4096); otherwise
+  // the part count never drops and the recursion would not end.
+  if (k_in > 4096 || k_out > 4096)
+    return fail(OM_EINVAL, "om_topk_merge_n: %d parts x %d entries exceed one merge of 8192 and need k_in, k_out <= 4096 "
+                "(got k_in = %d, k_out = %d)", nparts, k_in, k_in, k_out);
   const int g = std::max(2, 8192 / k_in);
   const int ngroups = (nparts + g - 1) / g;
   const int k_mid = static_cast<int>(std::min<int64_t>(k_out, static_cast<int64_t>(g) * k_in));
