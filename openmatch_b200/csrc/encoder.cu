@@ -451,7 +451,7 @@ __device__ __forceinline__ void norm_row(float4 (&v)[kMaxVec], int nvec, int H, 
 }
 
 __device__ __forceinline__ void affine_store(const float4 (&v)[kMaxVec], int nvec, int lane, const float* gamma,
-                                             const float* beta, float* out_f32, __nv_bfloat16* out_bf16) {
+                                             const float* beta, float* out) {
 #pragma unroll
   for (int j = 0; j < kMaxVec; ++j)
     if (j < nvec) {
@@ -462,43 +462,24 @@ __device__ __forceinline__ void affine_store(const float4 (&v)[kMaxVec], int nve
         const float4 b = *reinterpret_cast<const float4*>(beta + c);
         y.x += b.x, y.y += b.y, y.z += b.z, y.w += b.w;
       }
-      if (out_f32) *reinterpret_cast<float4*>(out_f32 + c) = y;
-      if (out_bf16) *reinterpret_cast<uint2*>(out_bf16 + c) = make_uint2(pack_bf16x2(y.x, y.y), pack_bf16x2(y.z, y.w));
+      *reinterpret_cast<float4*>(out + c) = y;
     }
 }
 
-// sum = h (+ add); y = Norm(sum) * gamma (+ beta).  Writes sum back to h when STORE_SUM (T5's pre-norm residual
-// stream), y as fp32 (nullable, may alias h: BERT's post-LN stream / T5's final norm) and as bf16 (nullable: the
-// next GEMM's A operand).  `add` is the bf16 output of the preceding O-proj / FFN2 GEMM: doing the residual add
-// here keeps those GEMM epilogues store-only — with the fp32 residual read in the epilogue they were bound by
-// exposed DRAM latency (tensor pipe 20 % on O-proj) — and this kernel streams at HBM speed anyway.
-template <bool RMS, bool STORE_SUM>
-__global__ void __launch_bounds__(128) norm_kernel(float* h, const __nv_bfloat16* __restrict__ add, const float* gamma,
-                                                   const float* beta, float eps, int T, int H, float* out_f32,
-                                                   __nv_bfloat16* out_bf16) {
+// out = Norm(h) * gamma (+ beta), fp32; out may alias h.
+template <bool RMS>
+__global__ void __launch_bounds__(128) norm_kernel(const float* h, const float* gamma, const float* beta, float eps,
+                                                   int T, int H, float* out) {
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= T) return;
   const int nvec = H >> 7;
   float4 v[kMaxVec];
-  float* src = h + static_cast<int64_t>(row) * H;
+  const float* src = h + static_cast<int64_t>(row) * H;
 #pragma unroll
   for (int j = 0; j < kMaxVec; ++j)
     if (j < nvec) v[j] = *reinterpret_cast<const float4*>(src + (j * 32 + lane) * 4);
-  if (add) {
-    const __nv_bfloat16* a = add + static_cast<int64_t>(row) * H;
-#pragma unroll
-    for (int j = 0; j < kMaxVec; ++j)
-      if (j < nvec) {
-        const uint2 raw = *reinterpret_cast<const uint2*>(a + (j * 32 + lane) * 4);
-        const float2 lo = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.x));
-        const float2 hi = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.y));
-        v[j].x += lo.x, v[j].y += lo.y, v[j].z += hi.x, v[j].w += hi.y;
-        if (STORE_SUM) *reinterpret_cast<float4*>(src + (j * 32 + lane) * 4) = v[j];
-      }
-  }
   norm_row<RMS>(v, nvec, H, eps);
-  affine_store(v, nvec, lane, gamma, beta, out_f32 ? out_f32 + static_cast<int64_t>(row) * H : nullptr,
-               out_bf16 ? out_bf16 + static_cast<int64_t>(row) * H : nullptr);
+  affine_store(v, nvec, lane, gamma, beta, out + static_cast<int64_t>(row) * H);
 }
 
 // Row statistics of a freshly embedded row: slot 0 of the row's kStatParts partials holds (sum, sum of squares), the
@@ -1544,10 +1525,10 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   // the one normalisation that runs as a kernel: last_hidden_state = LN_out(s) (BERT: last layer's output.LayerNorm,
   // T5: final_layer_norm), in place in e->h, for pooling and the optional out_hidden copy
   if (bert)
-    norm_kernel<false, false><<<rows4, 128, 0, st>>>(e->h, nullptr, e->layers[d.layers - 1].ln2_g,
-                                                     e->layers[d.layers - 1].ln2_b, d.ln_eps, T, H, e->h, nullptr);
+    norm_kernel<false><<<rows4, 128, 0, st>>>(e->h, e->layers[d.layers - 1].ln2_g, e->layers[d.layers - 1].ln2_b,
+                                              d.ln_eps, T, H, e->h);
   else
-    norm_kernel<true, false><<<rows4, 128, 0, st>>>(e->h, nullptr, e->final_g, nullptr, d.ln_eps, T, H, e->h, nullptr);
+    norm_kernel<true><<<rows4, 128, 0, st>>>(e->h, e->final_g, nullptr, d.ln_eps, T, H, e->h);
   OM_CUDA(cudaGetLastError());
   if (out_hidden)
     OM_CUDA(cudaMemcpyAsync(out_hidden, e->h, static_cast<size_t>(T) * H * 4, cudaMemcpyDeviceToDevice, st));

@@ -1,7 +1,9 @@
 // Persistent, warp-specialised wgmma GEMM core for sm_90a:   C[m, n] = sum_k A[m, k] * B[n, k]
-// (both operands K-major bf16 — or IEEE half with F16 — fp32 accumulation).  This one mainloop serves the three hot
-// steps: encoder linear layers (A = activations [T, H], B = nn.Linear weight [out, in]), brute-force search (A = queries
-// [nq, d], B = corpus rows [N, d]) and contrastive logits (Q * P^T).
+// (both operands K-major bf16 — or IEEE half with F16 — fp32 accumulation).  It runs the encoder linear layers
+// (A = activations [T, H], B = nn.Linear weight [out, in]) and the search scan rounds that the wide scan of
+// scan_gemm.cuh does not take: the first round, query chunks of <= 128 queries and every round with pair_scan off
+// (A = queries [nq, d], B = corpus rows [N, d]).  Its ring protocol (ring.cuh) is shared with the wide scan and the
+// fused loss.
 //
 //   warp 0 (one lane)       TMA producer : global -> STAGES-deep smem ring (128B-swizzled boxes)
 //   warps 1..3              idle (they pad the producer role to a whole warpgroup, so the consumers start at warp 4)
@@ -10,13 +12,13 @@
 //                           padded fp32 tile in shared memory and run the epilogue functor on it with the row-per-thread
 //                           mapping of the functor contract below (thread <-> accumulator row, 32-column chunks)
 //
-// Pipelines: smem full/empty (TMA <-> consumers, released per k block one wgmma group late); the staged accumulator
+// Pipelines: the STAGES-slot ring of ring.cuh (TMA <-> consumers, released one wgmma group late); the staged accumulator
 // tile is handed over with two named barriers per tile.  Tile schedule: static (tile = blockIdx.x + i * gridDim.x) or
 // dynamic (claimed from a global counter by the producer, published through a 4-deep smem ring).
 #pragma once
 #include <type_traits>
 
-#include "ptx.cuh"
+#include "ring.cuh"
 #include "tmap.cuh"
 
 namespace om {
@@ -94,14 +96,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     tma_prefetch_desc(&tmB);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], kGemmEpiWarps);  // every consumer warp
-    }
-    for (int i = 0; i < kSched; ++i) {
-      mbar_init(&sfull_bar[i], 1);
-      mbar_init(&sempty_bar[i], kGemmEpiWarps);  // one lane per consumer warp
-    }
+    ring_init(full_bar, empty_bar, STAGES, kGemmEpiWarps);  // every consumer warp
+    ring_init(sfull_bar, sempty_bar, kSched, kGemmEpiWarps);  // one lane per consumer warp
     fence_barrier_init();
   }
   __syncthreads();
@@ -116,7 +112,8 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
   if (warp == 0) {
     if (lane == 0) {
       // ------------------------------ TMA producer ------------------------------
-      uint32_t stage = 0, phase = 0, sslot = 0, sphase = 0;
+      Ring<STAGES> ring;
+      Ring<kSched> sched;
       int tile = first_tile;
       if (dyn) {
         tile = atomicAdd(tile_counter, 1);
@@ -124,13 +121,10 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       }
       while (true) {
         if (dyn) {  // publish (also the -1 sentinel) to the consumer warps
-          mbar_wait(&sempty_bar[sslot], sphase ^ 1u, 5);
-          tile_ring[sslot] = tile;
-          mbar_arrive(&sfull_bar[sslot]);
-          if (++sslot == kSched) {
-            sslot = 0;
-            sphase ^= 1u;
-          }
+          ring_wait_free(sempty_bar, sched, 5);
+          tile_ring[sched.stage] = tile;
+          mbar_arrive(&sfull_bar[sched.stage]);
+          sched.advance();
           if (tile < 0) break;
         } else if (tile >= num_tiles) {
           break;
@@ -140,15 +134,11 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
         const int m_blk = M_FASTEST ? tile % num_m : tile / num_n;
         const int n_blk = M_FASTEST ? tile / num_m : tile % num_n;
         for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u, 1);
-          uint8_t* sa = smem + stage * Cfg::kStageBytes;
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::kStageBytes);
-          tma_load_2d(sa, &tmA, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
-          tma_load_2d(sa + Cfg::kABytes, &tmB, &full_bar[stage], kb * kBlockK, n_blk * BN);
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          uint64_t* bar = ring_acquire_tx(full_bar, empty_bar, ring, Cfg::kStageBytes, 1);
+          uint8_t* sa = smem + ring.stage * Cfg::kStageBytes;
+          tma_load_2d(sa, &tmA, bar, kb * kBlockK, m_blk * kBlockM);
+          tma_load_2d(sa + Cfg::kABytes, &tmB, bar, kb * kBlockK, n_blk * BN);
+          ring.advance();
         }
         tile = (dyn && next >= num_tiles) ? -1 : next;
       }
@@ -162,19 +152,17 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
     constexpr int kChunks = BN / 32 / 2;
     typename Epi::State st;  // lives across tiles: functors may keep work in flight from one tile to the next
     if constexpr (Epi::smem_bytes(kGemmEpiWarps) > 0) epi.bind(st, epi_smem, et);
-    uint32_t stage = 0, phase = 0, sslot = 0, sphase = 0;
+    Ring<kSched> sched;
+    Ring<STAGES> ring;
     // staging coordinates of this thread's accumulator fragment
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2), fcol = 2 * (lane & 3);
     for (int tile = first_tile;; tile += tile_step) {
       if (dyn) {
-        mbar_wait_warp(&sfull_bar[sslot], sphase, 7);
-        tile = tile_ring[sslot];
+        mbar_wait_warp(&sfull_bar[sched.stage], sched.phase, 7);
+        tile = tile_ring[sched.stage];
         __syncwarp();
-        if (lane == 0) mbar_arrive(&sempty_bar[sslot]);
-        if (++sslot == kSched) {
-          sslot = 0;
-          sphase ^= 1u;
-        }
+        if (lane == 0) mbar_arrive(&sempty_bar[sched.stage]);
+        sched.advance();
         if (tile < 0) break;
       } else if (tile >= num_tiles) {
         break;
@@ -185,34 +173,23 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       epi.begin(st, row, m_blk, n_blk);
       if constexpr (Epi::kPrefetch) epi.prefetch(st, row, n_blk * BN + half * kChunks * 32);
 
-      // mainloop: one wgmma group per k block in flight; a stage is released once the group after it was issued
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      uint32_t prev_stage = 0;
-      for (int kb = 0; kb < num_k; ++kb) {
-        mbar_wait_warp(&full_bar[stage], phase, 3);
-        const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes) + wg * (64 * 128);
-        const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
-        wgmma_fence();
+      ring_consume(
+          full_bar, ring, 0, num_k, 3,
+          [&](uint32_t stage, uint32_t accumulate) {
+            const uint32_t a_addr = smem_u32(smem + stage * Cfg::kStageBytes) + wg * (64 * 128);
+            const uint32_t b_addr = smem_u32(smem + stage * Cfg::kStageBytes + Cfg::kABytes);
 #pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
-          wgmma_tile_k16<BN, F16>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
-                                  wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        if (kb > 0) {
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
-        }
-        prev_stage = stage;
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      wgmma_wait<0>();
+            for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+              wgmma_tile_k16<BN, F16>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
+                                      wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (accumulate | k) != 0 ? 1u : 0u);
+          },
+          [&](uint32_t stage) {
+            if (lane == 0) mbar_arrive(&empty_bar[stage]);
+          });
       wgmma_fence_regs(acc);
-      if (num_k > 0 && lane == 0) mbar_arrive(&empty_bar[prev_stage]);
 
       // stage the accumulators: every epilogue thread has finished reading the previous tile
       named_bar_sync(2, 32 * kGemmEpiWarps);
@@ -304,70 +281,5 @@ static inline cudaError_t launch_gemm(const void* A, int64_t lda, const void* B,
   kern<<<grid, threads, smem_bytes, stream>>>(tmA, tmB, M, N, K, epi, counter);
   return cudaGetLastError();
 }
-
-// --------------------------------------------------------------------------------------------------
-// Generic store epilogues
-// --------------------------------------------------------------------------------------------------
-struct EpiStoreF32 {  // C fp32 = acc (+ bias[n]) (+ resid[m, n])
-  float* C;
-  int64_t ldc;
-  const float* bias;   // nullable, [N]
-  const float* resid;  // nullable, [M, ldr]; may alias C (in-place residual add)
-  int64_t ldr;
-  int M, N;
-  static constexpr int kPasses = 1;
-  static constexpr bool kPrefetch = true;
-  __host__ __device__ static constexpr int smem_bytes(int) { return 0; }
-  struct State {
-    float4 pre[8];  // residual of the chunk about to be processed
-  };
-  __device__ __forceinline__ void begin(State&, int, int, int) const {}
-  __device__ __forceinline__ void end(State&, int) const {}
-  __device__ __forceinline__ bool fast(int row, int col0) const {
-    return row < M && col0 + 32 <= N && (((ldc | ldr) & 3) == 0);
-  }
-  __device__ __forceinline__ void prefetch(State& s, int row, int col0) const {
-    if (resid && col0 >= 0 && fast(row, col0)) {
-      const float4* r = reinterpret_cast<const float4*>(resid + (int64_t)row * ldr + col0);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s.pre[j] = r[j];
-    }
-  }
-  __device__ __forceinline__ void chunk(State& s, int row, int col0, const float (&v)[32], int next_col0) const {
-    if (row >= M || col0 >= N) return;
-    float* out = C + (int64_t)row * ldc + col0;
-    if (fast(row, col0)) {
-      float4 cur[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) cur[j] = resid ? s.pre[j] : make_float4(0.f, 0.f, 0.f, 0.f);
-      // all loads of the NEXT chunk are issued before any store of this one: with resid aliasing C the
-      // compiler must otherwise order every load behind the previous store (one HBM round trip each)
-      prefetch(s, row, next_col0);
-      float4 b[8];
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        b[j] = bias ? __ldg(reinterpret_cast<const float4*>(bias + col0) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        float4 o;
-        o.x = v[4 * j] + b[j].x + cur[j].x;
-        o.y = v[4 * j + 1] + b[j].y + cur[j].y;
-        o.z = v[4 * j + 2] + b[j].z + cur[j].z;
-        o.w = v[4 * j + 3] + b[j].w + cur[j].w;
-        reinterpret_cast<float4*>(out)[j] = o;
-      }
-    } else {
-#pragma unroll
-      for (int i = 0; i < 32; ++i)
-        if (col0 + i < N) {
-          float o = v[i];
-          if (bias) o += bias[col0 + i];
-          if (resid) o += resid[(int64_t)row * ldr + col0 + i];
-          out[i] = o;
-        }
-      prefetch(s, row, next_col0);
-    }
-  }
-};
 
 }  // namespace om

@@ -4,8 +4,8 @@
 // and their autograd backward (~8 PyTorch launches forward, as many backward).
 //
 // loss_fused_kernel: cooperative grid (<= 1 CTA per SM), phases separated by grid barriers; every GEMM runs on the
-// pipeline of gemm.cuh's design (TMA -> 4-stage smem ring -> one consumer warpgroup issuing wgmma 2 x (64x128x16), fp32
-// accumulators in registers -> stores), with the pipeline state carried from phase to phase:
+// ring of ring.cuh (TMA -> 4-stage smem ring -> one consumer warpgroup issuing wgmma 2 x (64x128x16), fp32
+// accumulators in registers -> stores), with the ring position carried from phase to phase:
 //   PREP    fp32 (or unaligned) inputs only: Q, P -> bf16 row-major copies.  Aligned bf16 inputs are read in place.
 //   LOGITS  S = Q P^T, fp32 [nq, np]                      (A = Q, B = P, both K-major)
 //   SOFTMAX one warp per query row, the row in registers: log-sum-exp (fp32), loss_i = lse_i - s_i,t_i,
@@ -24,10 +24,7 @@
 
 namespace om {
 
-#ifndef OM_LOSS_STAGES
-#define OM_LOSS_STAGES 4
-#endif
-constexpr int kLossBN = 128, kLossStages = OM_LOSS_STAGES, kLossThreads = 256;
+constexpr int kLossBN = 128, kLossStages = 4, kLossThreads = 256;
 struct LossCfg {
   static constexpr int kABytes = kBlockM * kBlockK * 2;
   static constexpr int kStageBytes = kABytes + kLossBN * kBlockK * 2;
@@ -104,9 +101,7 @@ struct LossSmem {
   uint8_t* ring;
   uint64_t *full_bar, *empty_bar;
 };
-struct Pipe {  // per-thread pipeline position, carried across the GEMM phases (producer and consumers advance identically)
-  uint32_t stage = 0, phase = 0;
-};
+using LossRing = Ring<kLossStages>;  // per-thread ring position, carried across the GEMM phases
 
 // MN-major operand tile in shared memory: two TMA boxes {64 mn, 64 k} back to back.  Inside a box the 64 mn elements
 // of one k are a 128-byte row, 8 such rows form a 1024-byte swizzle atom (stride between 8-k groups, SBO = 1024 B);
@@ -145,7 +140,7 @@ struct GemmDesc {
 // stores its partial tile to part[s], and the slice that arrives last at the tile's counter (per epilogue warp:
 // 32 rows) adds the S partials in the fixed order s = 0 .. S-1 into C, so the result does not depend on which slice
 // finished last.
-__device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const LossSmem& sm, Pipe& pipe, int warp,
+__device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const LossSmem& sm, LossRing& ring, int warp,
                                            int lane) {
   const int M = g.M, N = g.N, S = g.S, ldc = g.ldc;
   const int num_n = (N + kLossBN - 1) / kLossBN;
@@ -164,11 +159,9 @@ __device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const Los
         const int kb_end = min(num_k, (ks + 1) * kper);
         OM_TRACE(tslot);
         for (int kb = ks * kper; kb < kb_end; ++kb) {
-          mbar_wait(&sm.empty_bar[pipe.stage], pipe.phase ^ 1u, 1);
-          uint8_t* sa = sm.ring + pipe.stage * LossCfg::kStageBytes;
+          uint64_t* bar = ring_acquire_tx(sm.full_bar, sm.empty_bar, ring, LossCfg::kStageBytes, 1);
+          uint8_t* sa = sm.ring + ring.stage * LossCfg::kStageBytes;
           uint8_t* sb = sa + LossCfg::kABytes;
-          uint64_t* bar = &sm.full_bar[pipe.stage];
-          mbar_arrive_expect_tx(bar, LossCfg::kStageBytes);
           if (!g.a_mn) {
             tma_load_2d(sa, g.tmA, bar, kb * kBlockK, m0);
           } else {
@@ -181,10 +174,7 @@ __device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const Los
             tma_load_2d(sb, g.tmB, bar, n0, kb * kBlockK);
             tma_load_2d(sb + kMnBoxBytes, g.tmB, bar, n0 + 64, kb * kBlockK);
           }
-          if (++pipe.stage == kLossStages) {
-            pipe.stage = 0;
-            pipe.phase ^= 1u;
-          }
+          ring.advance();
         }
       }
     }
@@ -197,42 +187,32 @@ __device__ __forceinline__ void gemm_phase(const GemmDesc& g, int rot, const Los
       const int kb_begin = ks * kper, kb_end = min(num_k, kb_begin + kper);
       float* Cw = S > 1 ? g.part + static_cast<int64_t>(ks) * M * ldc : g.C;
       float acc[2][64];
-      uint32_t prev_stage = 0;
-      for (int kb = kb_begin; kb < kb_end; ++kb) {
-        mbar_wait_warp(&sm.full_bar[pipe.stage], pipe.phase, 3);
-        if (kb == kb_begin) OM_TRACE(tslot + 1);
-        const uint32_t a_addr = smem_u32(sm.ring + pipe.stage * LossCfg::kStageBytes);
-        const uint32_t b_addr = a_addr + LossCfg::kABytes;
-        // operand majors are immediates of the instruction: one fully unrolled k block per layout
-        auto issue = [&](auto a_mn, auto b_mn) {
+      ring_consume(
+          sm.full_bar, ring, kb_begin, kb_end, 3,
+          [&](uint32_t stage, uint32_t accumulate) {
+            if (!accumulate) OM_TRACE(tslot + 1);
+            const uint32_t a_addr = smem_u32(sm.ring + stage * LossCfg::kStageBytes);
+            const uint32_t b_addr = a_addr + LossCfg::kABytes;
+            // operand majors are immediates of the instruction: one fully unrolled k block per layout
+            auto mma = [&](auto a_mn, auto b_mn) {
 #pragma unroll
-          for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
-            const uint32_t accum = ((kb - kb_begin) | k) != 0 ? 1u : 0u;
+              for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
 #pragma unroll
-            for (int h = 0; h < 2; ++h)
-              loss_mma_k16<decltype(a_mn)::value, decltype(b_mn)::value>(acc[h], a_addr, b_addr, h, k, accum);
-          }
-        };
-        wgmma_fence();
-        if (!g.a_mn && !g.b_mn) issue(std::false_type{}, std::false_type{});
-        else if (!g.a_mn) issue(std::false_type{}, std::true_type{});
-        else if (g.b_mn) issue(std::true_type{}, std::true_type{});
-        else issue(std::true_type{}, std::false_type{});
-        wgmma_commit();
-        if (kb > kb_begin) {
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&sm.empty_bar[prev_stage]);
-        }
-        prev_stage = pipe.stage;
-        if (++pipe.stage == kLossStages) {
-          pipe.stage = 0;
-          pipe.phase ^= 1u;
-        }
-      }
-      wgmma_wait<0>();
+                for (int h = 0; h < 2; ++h)
+                  loss_mma_k16<decltype(a_mn)::value, decltype(b_mn)::value>(acc[h], a_addr, b_addr, h, k,
+                                                                             (accumulate | k) != 0 ? 1u : 0u);
+              }
+            };
+            if (!g.a_mn && !g.b_mn) mma(std::false_type{}, std::false_type{});
+            else if (!g.a_mn) mma(std::false_type{}, std::true_type{});
+            else if (g.b_mn) mma(std::true_type{}, std::true_type{});
+            else mma(std::true_type{}, std::false_type{});
+          },
+          [&](uint32_t stage) {
+            if (lane == 0) mbar_arrive(&sm.empty_bar[stage]);
+          });
       wgmma_fence_regs(acc[0]);
       wgmma_fence_regs(acc[1]);
-      if (lane == 0) mbar_arrive(&sm.empty_bar[prev_stage]);
       OM_TRACE(tslot + 3);
       // fragments -> global: every quad of lanes writes 32 consecutive bytes of a row (whole sectors)
       const bool vec = (ldc & 1) == 0 && (reinterpret_cast<uintptr_t>(Cw) & 7) == 0;
@@ -379,14 +359,11 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
     }
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kLossStages; ++i) {
-      mbar_init(&sm.full_bar[i], 1);
-      mbar_init(&sm.empty_bar[i], 4);  // one arrive per consumer warp
-    }
+    ring_init(sm.full_bar, sm.empty_bar, kLossStages, 4);  // one arrive per consumer warp
     fence_barrier_init();
   }
   __syncthreads();
-  Pipe pipe;
+  LossRing ring;
 
   // ------------------------------ PREP ------------------------------
   if (blockIdx.x == 0 && threadIdx.x == 0) {
@@ -411,7 +388,7 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
   // ------------------------------ LOGITS ------------------------------
   {
     const GemmDesc g{&maps.a[0], &maps.b[0], a.nq, a.np, a.d, a.S, a.np, false, false, 1, nullptr, nullptr, -1000};
-    gemm_phase(g, 0, sm, pipe, warp, lane);
+    gemm_phase(g, 0, sm, ring, warp, lane);
   }
   grid_sync(a.grid_bar);
   if (blockIdx.x == 0 && threadIdx.x == 0) a.ts[2] = global_timer_ns();
@@ -529,12 +506,12 @@ loss_fused_kernel(const __grid_constant__ LossMaps maps, const __grid_constant__
   int rot = 0;
   if (a.dQ) {  // first: the slice reduction of its last arrivers overlaps the dP tiles of everybody else
     const GemmDesc g{&maps.a[1], &maps.b[1], a.nq, a.d, a.np, a.dQ, a.d, false, true, a.dq_split, a.dq_part, a.dq_sem, 0};
-    gemm_phase(g, rot, sm, pipe, warp, lane);
+    gemm_phase(g, rot, sm, ring, warp, lane);
     rot = ((a.nq + kBlockM - 1) / kBlockM) * ((a.d + kLossBN - 1) / kLossBN) * a.dq_split;
   }
   if (a.dP) {
     const GemmDesc g{&maps.a[2], &maps.b[2], a.np, a.d, a.nq, a.dP, a.d, true, true, 1, nullptr, nullptr, 16};
-    gemm_phase(g, rot, sm, pipe, warp, lane);
+    gemm_phase(g, rot, sm, ring, warp, lane);
   }
   if (warp >= 4 && lane == 0) atomicMax(&a.ts[4], global_timer_ns());
   if (warp == 4 && lane == 0) OM_TRACE(61);

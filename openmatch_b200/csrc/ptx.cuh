@@ -24,20 +24,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
 
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31u; }
-
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred = 0;
-  asm volatile(
-      "{\n\t"
-      ".reg .pred P;\n\t"
-      "elect.sync _|P, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, P;\n\t"
-      "}\n"
-      : "=r"(pred));
-  return pred != 0;
-}
-
 // ----------------------------------------------------------------------------------------------
 // mbarrier
 // ----------------------------------------------------------------------------------------------
@@ -47,7 +33,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// Make generic-proxy writes to shared memory visible to the async proxy (TMA / UMMA reads).
+// Make generic-proxy writes to shared memory visible to the async proxy (TMA loads, wgmma operand reads).
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -83,9 +69,6 @@ static __device__ __noinline__ void mbar_wait_slow(uint64_t* bar, uint32_t parit
   const long long t0 = clock64();
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-#if defined(OM_SPIN_SLEEP_NS) && OM_SPIN_SLEEP_NS > 0
-    __nanosleep(OM_SPIN_SLEEP_NS);
-#endif
     if ((++spins & 1023u) != 0) continue;
     if (*reinterpret_cast<volatile unsigned int*>(&om_dev_fault) != 0u) return;
     if (clock64() - t0 > OM_WAIT_TIMEOUT_CYCLES) {
@@ -104,21 +87,12 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
 // warp parks at __syncwarp.  Hundreds of threads spinning on try_wait compete with the TMA/MMA threads for
 // the barrier unit.
 __device__ __forceinline__ void mbar_wait_warp(uint64_t* bar, uint32_t parity, uint32_t site) {
-#ifdef OM_EPI_ALL_LANES_WAIT
-  if (!mbar_try_wait(bar, parity)) {
-    while (!mbar_try_wait(bar, parity)) __nanosleep(OM_EPI_ALL_LANES_WAIT);
-  }
-  return;
-#endif
   if ((threadIdx.x & 31u) == 0) {
     if (!mbar_try_wait(bar, parity)) {
       const long long t0 = clock64();
       uint32_t spins = 0;
       while (!mbar_try_wait(bar, parity)) {
-#ifndef OM_EPI_POLL_SLEEP_NS
-#define OM_EPI_POLL_SLEEP_NS 64
-#endif
-        __nanosleep(OM_EPI_POLL_SLEEP_NS);
+        __nanosleep(64);
         if ((++spins & 1023u) != 0) continue;
         if (*reinterpret_cast<volatile unsigned int*>(&om_dev_fault) != 0u) break;
         if (clock64() - t0 > OM_WAIT_TIMEOUT_CYCLES) {
@@ -153,15 +127,6 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const void* tmap, ui
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d_hint(void* smem_dst, const void* tmap, uint64_t* bar, int32_t c0,
-                                                 int32_t c1, uint64_t policy) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.L2::cache_hint"
-      " [%0], [%1, {%3, %4}], [%2], %5;"
-      ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1),
-      "l"(policy)
-      : "memory");
-}
 // L2 prefetch of one box (no shared-memory destination, no completion tracking)
 __device__ __forceinline__ void tma_prefetch_l2_2d(const void* tmap, int32_t c0, int32_t c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
@@ -179,18 +144,6 @@ __device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bul
 // all of this thread's bulk groups have finished READING their shared-memory sources
 __device__ __forceinline__ void bulk_wait_group_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_group0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-__device__ __forceinline__ uint64_t l2_policy_evict_last() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
-
 
 // TMA load of one box into the same shared-memory offset of every CTA in `cta_mask` (cluster multicast); the
 // transaction bytes complete on the mbarrier at the same offset in each destination CTA.
@@ -327,7 +280,6 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 // fp32 pairs, element-wise (two FFMA each)
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
-__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
 __device__ __forceinline__ float2 splat2(float x) { return make_float2(x, x); }
 
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {

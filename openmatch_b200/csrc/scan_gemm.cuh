@@ -168,10 +168,8 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     tma_prefetch_desc(&tmX);
   }
   if (warp == 1 && lane == 0) {
-    for (int i = 0; i < kScanStages; ++i) {
-      mbar_init(&full_bar[i], 1);  // the own producer's expect_tx; the bytes come from every producer of S(c)
-      mbar_init(&empty_bar[i], Cl::kEmptyArrivals);
-    }
+    // full: the own producer's expect_tx, the bytes come from every producer of S(c)
+    ring_init(full_bar, empty_bar, kScanStages, Cl::kEmptyArrivals);
     fence_barrier_init();
   }
   cluster_sync_all();  // every peer's barriers exist before any multicast or remote arrive
@@ -185,25 +183,21 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (warp == 0 && lane == 0) {
       // ------------------------------ TMA producer ------------------------------
       const uint16_t qmask = Cl::q_mask(rank), xmask = Cl::x_mask(rank);
-      uint32_t stage = 0, phase = 0;
+      Ring<kScanStages> ring;
       for (int tile = static_cast<int>(cluster_id_x()); tile < num_tiles; tile += static_cast<int>(cluster_count_x())) {
         const int m_blk = (tile % qgroups) * CQ + qa;
         const int n_blk = (tile / qgroups) * CX + xb;
         for (int kb = 0; kb < num_k; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1u, 30);
-          uint8_t* sa = smem + stage * kScanStageBytes;
-          mbar_arrive_expect_tx(&full_bar[stage], kScanStageBytes);
+          uint64_t* bar = ring_acquire_tx(full_bar, empty_bar, ring, kScanStageBytes, 30);
+          uint8_t* sa = smem + ring.stage * kScanStageBytes;
           if constexpr (CX == 1)
-            tma_load_2d(sa, &tmQ, &full_bar[stage], kb * kBlockK, m_blk * kBlockM);
+            tma_load_2d(sa, &tmQ, bar, kb * kBlockK, m_blk * kBlockM);
           else
-            tma_load_2d_multicast(sa + xb * (Cl::kQRows * kBlockK * 2), &tmQ, &full_bar[stage], kb * kBlockK,
+            tma_load_2d_multicast(sa + xb * (Cl::kQRows * kBlockK * 2), &tmQ, bar, kb * kBlockK,
                                   m_blk * kBlockM + xb * Cl::kQRows, qmask);
-          tma_load_2d_multicast(sa + kScanABytes + qa * (Cl::kXRows * kBlockK * 2), &tmX, &full_bar[stage], kb * kBlockK,
+          tma_load_2d_multicast(sa + kScanABytes + qa * (Cl::kXRows * kBlockK * 2), &tmX, bar, kb * kBlockK,
                                 n_blk * kScanBlockN + qa * Cl::kXRows, xmask);
-          if (++stage == kScanStages) {
-            stage = 0;
-            phase ^= 1u;
-          }
+          ring.advance();
         }
       }
     }
@@ -214,7 +208,7 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const int wg = et >> 7;                                               // queries [64 wg, +64) of the CTA's 128
     const int q4 = lane & 3;
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
-    uint32_t stage = 0, phase = 0;
+    Ring<kScanStages> ring;
     int buf = 0;
     // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
     int p_n0 = 0, p_n1 = 0, p_excl0 = 0, p_excl1 = 0, p_pos0 = 0, p_pos1 = 0, p_row = 0, p_buf = 0;
@@ -252,34 +246,21 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const float inf = __int_as_float(0x7f800000);
       const float t0 = row0 < nq ? thr[row0] : inf, t1 = row1 < nq ? thr[row1] : inf;
 
-      // mainloop: one wgmma group per k block in flight; a stage is released once the group after it was issued
       float acc[128];
 #pragma unroll
       for (int i = 0; i < 128; ++i) acc[i] = 0.f;
-      uint32_t prev_stage = 0;
-      for (int kb = 0; kb < num_k; ++kb) {
-        mbar_wait_warp(&full_bar[stage], phase, 31);
-        const uint32_t a_addr = smem_u32(smem + stage * kScanStageBytes) + wg * (64 * 128);
-        const uint32_t b_addr = smem_u32(smem + stage * kScanStageBytes + kScanABytes);
-        wgmma_fence();
+      ring_consume(
+          full_bar, ring, 0, num_k, 31,
+          [&](uint32_t stage, uint32_t accumulate) {
+            const uint32_t a_addr = smem_u32(smem + stage * kScanStageBytes) + wg * (64 * 128);
+            const uint32_t b_addr = smem_u32(smem + stage * kScanStageBytes + kScanABytes);
 #pragma unroll
-        for (int k = 0; k < kBlockK / kWgmmaK; ++k)
-          wgmma_m64n256k16_f16<0, 0>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
-                                     wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        if (kb > 0) {
-          wgmma_wait<1>();
-          release(prev_stage);
-        }
-        prev_stage = stage;
-        if (++stage == kScanStages) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-      wgmma_wait<0>();
+            for (int k = 0; k < kBlockK / kWgmmaK; ++k)
+              wgmma_m64n256k16_f16<0, 0>(acc, wgmma_desc(a_addr + k * 32, kDescKMajorSW128),
+                                         wgmma_desc(b_addr + k * 32, kDescKMajorSW128), (accumulate | k) != 0 ? 1u : 0u);
+          },
+          release);
       wgmma_fence_regs(acc);
-      if (num_k > 0) release(prev_stage);
 
       // ------------------------------ filter on the fragments ------------------------------
       drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
