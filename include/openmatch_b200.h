@@ -19,6 +19,14 @@
  * NULL = legacy default stream); the library owns only its opaque handles.  One process drives one GPU;
  * a handle is not thread-safe, distinct handles are.  There is no CPU fallback: every compute entry
  * point fails with OM_ENODEVICE when no sm_90 device is present.
+ *
+ * Streams.  `stream` may be any stream, including a non-blocking one that does not wait for the legacy
+ * stream; the library issues the work of a call on that stream only.  The calls without a stream order
+ * themselves: om_encoder_set_weight runs after all work already issued on the device and has finished
+ * reading the caller's data on return; om_index_reserve synchronises the device when it grows the shard;
+ * om_index_reset touches no device memory (the error-norm maxima are zeroed on the stream of the next
+ * commit or search).  One handle must not be used from two streams at once.  The loss workspace is
+ * process-global: loss calls must not overlap across streams.
  */
 #ifndef OPENMATCH_B200_H_
 #define OPENMATCH_B200_H_
@@ -169,7 +177,7 @@ int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtype dtype, in
                                 const int64_t* target, int reduction, float loss_scale, float* loss_out,
                                 float* dQ, float* dP, float* scores_out, void* stream);
 /* Diagnostics: device time (ns, %globaltimer) the most recent loss call spent in its four phases
- * {PREP, LOGITS, SOFTMAX, GRADS}.  Synchronous. */
+ * {PREP, LOGITS, SOFTMAX, GRADS}.  Synchronises the device first, so it reads the last call on any stream. */
 int om_debug_loss_phase_ns(uint64_t out[4]);
 
 #ifdef __cplusplus

@@ -1038,7 +1038,7 @@ namespace {
 template <typename T>
 int dev_alloc(om_encoder* e, T** p, size_t count) {
   void* q = nullptr;
-  OM_CUDA(cudaMalloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
+  OM_CUDA(dev_malloc(&q, std::max<size_t>(count, 1) * sizeof(T)));
   e->allocs.push_back(q);
   *p = static_cast<T*>(q);
   return 0;
@@ -1055,8 +1055,12 @@ int mark(om_encoder* e, const std::string& name) {
   return 1;
 }
 
-// copies a fp32 [rows, cols] block (host or device) into dst (+ optional bf16 conversion)
+// copies a fp32 [rows, cols] block (host or device) into dst (+ optional bf16 conversion).  om_encoder_set_weight has no
+// stream: device data may still be in flight on any of the caller's streams (e.g. an optimizer step on a non-blocking
+// stream), so the copy runs after all work issued so far, and it has finished on return, when the caller may free or
+// overwrite the source.
 int upload(const void* data, om_memkind kind, size_t count, float* dst_f32, __nv_bfloat16* dst_bf16) {
+  if (kind == OM_DEVICE) OM_CUDA(cudaDeviceSynchronize());
   float* staged = dst_f32;
   float* tmp = nullptr;
   if (!staged) {
@@ -1069,8 +1073,8 @@ int upload(const void* data, om_memkind kind, size_t count, float* dst_f32, __nv
     f32_to_bf16_kernel<<<static_cast<int>(std::min<size_t>((count + 255) / 256, 4096)), 256>>>(staged, dst_bf16,
                                                                                               (int64_t)count);
     err = cudaGetLastError();
-    if (err == cudaSuccess) err = cudaDeviceSynchronize();
   }
+  if (err == cudaSuccess) err = cudaDeviceSynchronize();
   if (tmp) cudaFree(tmp);
   if (err != cudaSuccess) return fail(OM_ECUDA, "weight upload failed: %s", cudaGetErrorString(err));
   return 0;

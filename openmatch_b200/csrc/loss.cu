@@ -597,18 +597,20 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
   const size_t o_part = carve(dq_split > 1 ? (size_t)dq_split * nq * d * 4 : 0);
   if (off > ws.bytes) {
     if (ws.p) {
-      OM_CUDA(cudaStreamSynchronize(st));
+      // the workspace is process-global: the call that last used it may have run on another stream
+      OM_CUDA(cudaDeviceSynchronize());
       cudaFree(ws.p);
     }
     ws.p = nullptr;
     ws.bytes = 0;
     ws.maps_base = nullptr;
-    OM_CUDA(cudaMalloc(&ws.p, off));
+    OM_CUDA(dev_malloc(&ws.p, off));
     ws.bytes = off;
   }
   if (!ws.grid_bar) {
     OM_CUDA(cudaMalloc(&ws.grid_bar, kLossBarBytes));
-    OM_CUDA(cudaMemset(ws.grid_bar, 0, kLossBarBytes));
+    // on `st`, ahead of the launch below: a legacy-stream memset is not ordered before a launch on a non-blocking stream
+    OM_CUDA(cudaMemsetAsync(ws.grid_bar, 0, kLossBarBytes, st));
   }
   uint8_t* base = static_cast<uint8_t*>(ws.p);
   LossArgs a;
@@ -690,6 +692,7 @@ extern "C" int om_debug_loss_phase_ns(uint64_t out[4]) {
   if (!out) return fail(OM_EINVAL, "om_debug_loss_phase_ns: null output");
   if (!g_loss_ws.grid_bar) return fail(OM_ESTATE, "om_debug_loss_phase_ns: no loss call yet");
   unsigned long long ts[5];
+  OM_CUDA(cudaDeviceSynchronize());  // the last loss call may have run on any stream
   OM_CUDA(cudaMemcpy(ts, reinterpret_cast<uint8_t*>(g_loss_ws.grid_bar) + kLossBarBytes - 64, sizeof(ts), cudaMemcpyDeviceToHost));
   for (int i = 0; i < 4; ++i) out[i] = ts[i + 1] - ts[i];
   return 0;

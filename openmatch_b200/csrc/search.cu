@@ -550,7 +550,7 @@ struct DevBuf {  // grow-only device scratch
     if (p) cudaFree(p);
     p = nullptr;
     bytes = 0;
-    OM_CUDA(cudaMalloc(&p, need));
+    OM_CUDA(dev_malloc(&p, need));
     bytes = need;
     return 0;
   }
@@ -583,6 +583,7 @@ struct om_index {
   float* xf = nullptr;
   __half* xh = nullptr;
   float* gstats = nullptr;  // device [2]: max ||x||, max ||x - x_h|| over the committed rows (float bit patterns)
+  bool gstats_stale = false;  // set by om_index_reset: gstats is zeroed on the stream of the next commit / search
   int64_t rescore_slack = -1;
   int force_safe = 0;
   int pair_scan = 1;      // > 128 queries: rounds after the first on the wide scan (scan_gemm.cuh); 0 = single-CTA tiles
@@ -614,8 +615,8 @@ static int index_grow(om_index* ix, int64_t need) {
   __half* nxh = nullptr;
   // rows may still be in flight on the caller's stream(s) (encoder writing reserved rows, a pending commit)
   OM_CUDA(cudaDeviceSynchronize());
-  OM_CUDA(cudaMalloc(&nxf, static_cast<size_t>(ncap) * ix->d * sizeof(float)));
-  cudaError_t e = cudaMalloc(&nxh, static_cast<size_t>(ncap) * ix->dpad * sizeof(__half));
+  OM_CUDA(dev_malloc(&nxf, static_cast<size_t>(ncap) * ix->d * sizeof(float)));
+  cudaError_t e = dev_malloc(&nxh, static_cast<size_t>(ncap) * ix->dpad * sizeof(__half));
   if (e != cudaSuccess) {
     cudaFree(nxf);
     cudaGetLastError();
@@ -637,6 +638,16 @@ static int index_grow(om_index* ix, int64_t need) {
 static inline int grid_for(int64_t n, int threads) {
   int64_t g = (n + threads - 1) / threads;
   return static_cast<int>(std::min<int64_t>(std::max<int64_t>(g, 1), 132 * 16));
+}
+
+// Zeroes the error-norm maxima a reset left stale, on the stream of the commit or search that reads them next.  A reset
+// cannot zero them itself: a memset on any stream other than the caller's next one may land after that call's atomicMax
+// and leave maxima of 0, with which the certificate would prove wrong candidate lists exact.
+static int settle_reset(om_index* ix, cudaStream_t st) {
+  if (!ix->gstats_stale) return 0;
+  OM_CUDA(cudaMemsetAsync(ix->gstats, 0, 2 * sizeof(float), st));
+  ix->gstats_stale = false;
+  return 0;
 }
 
 extern "C" {
@@ -678,7 +689,7 @@ int om_index_dim(const om_index* ix) { return ix ? ix->d : 0; }
 int om_index_reset(om_index* ix) {
   if (!ix) return fail(OM_EINVAL, "om_index_reset: null index");
   ix->n = 0;
-  OM_CUDA(cudaMemset(ix->gstats, 0, 2 * sizeof(float)));
+  ix->gstats_stale = true;  // host only: see settle_reset
   return 0;
 }
 
@@ -694,6 +705,7 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   if (!ix || n < 0 || ix->n + n > ix->cap) return fail(OM_EINVAL, "om_index_commit: more rows than reserved");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  OM_TRY(settle_reset(ix, st));
   rows_to_f16_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xf + static_cast<size_t>(ix->n) * ix->d,
                                                      ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d, ix->dpad,
                                                      nullptr, nullptr, ix->gstats);
@@ -1264,6 +1276,7 @@ extern "C" int om_index_search(om_index* ix, const void* q, om_memkind q_kind, i
     return fail(OM_EINVAL, "om_index_search: bad arguments (nq=%d k=%d)", nq, k);
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
+  OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
   return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, static_cast<cudaStream_t>(stream));
 }
 
@@ -1310,6 +1323,7 @@ extern "C" int om_index_search_sharded(om_index* ix, om_comm* comm, const void* 
     return fail(OM_EINVAL, "om_index_search_sharded: bad arguments (nq=%d k=%d)", nq, k);
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
+  OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
   return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, static_cast<cudaStream_t>(stream));
 }
 
