@@ -89,8 +89,9 @@ int om_encoder_set_weight(om_encoder* enc, const char* name, const void* data, o
 int om_encoder_finalize(om_encoder* enc);
 /* input_ids / attention_mask / token_type_ids (nullable => zeros; ignored for T5): int64 [B, L] device,
  * row-major, exactly what DRInferenceCollator / QPCollator hand to the model; L <= 128.
- * out_reps: device [B, rep_dim] fp32 or bf16 with row pitch out_row_stride (elements) — may point into an
- * index shard obtained from om_index_reserve().  out_hidden: nullable device fp32 [B, L, hidden]
+ * out_reps: device [B, rep_dim] fp32, bf16 or fp16 with row pitch out_row_stride (elements) — may point into an
+ * index shard obtained from om_index_reserve() / om_index_reserve_rows().  fp16 output is the round-to-nearest-even
+ * of the fp32 output of the same call (values beyond the half range become inf).  out_hidden: nullable device fp32 [B, L, hidden]
  * (last_hidden_state).  Asynchronous on `stream`. */
 int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attention_mask,
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
@@ -100,12 +101,26 @@ void om_encoder_destroy(om_encoder* enc);
 
 /* ---- index: replaces faiss.IndexFlatIP (exact inner-product top-k) -------------------------------- */
 int om_index_create(int d, om_index** out); /* faiss.IndexFlatIP(d); lives on the current device */
-/* index.add(x): x [n, d] row-major, fp32 (host or device).  Rows get ids ntotal .. ntotal+n-1. */
+/* Index with a chosen row storage.  OM_F32 (= om_index_create): fp32 master rows + an fp16 scan copy, 6 bytes per
+ * element.  OM_F16: the fp16 rows [n, dpad] (dpad = d rounded up to 8) only, 2 bytes per element; they are the scan
+ * operand and the row store.  Search on an fp16 index is exact with respect to the STORED values: the exact top-k by
+ * fp32 inner product of the fp32 query with the fp16 rows, in the summation order of the fp32 re-score, ties by
+ * ascending id — bitwise what an fp32 index of the fp16-rounded rows returns.  Input fp16 cannot hold is refused:
+ * om_index_add of a NaN or of a value that rounds to +-inf in fp16 (|x| >= 65520) returns OM_EINVAL and adds nothing;
+ * rows written in place and committed with such values make every search return OM_EINVAL until om_index_reset (stat
+ * "nonfinite_rows").  OM_BF16 storage returns OM_EINVAL.  Every shard of a sharded search has the same storage. */
+int om_index_create_typed(int d, om_dtype storage, om_index** out);
+int om_index_storage(const om_index* idx); /* the om_dtype given at creation */
+/* index.add(x): x [n, d] row-major, fp32, bf16 or fp16 (host or device).  Rows get ids ntotal .. ntotal+n-1.
+ * fp16 storage: converted to fp16 with round-to-nearest-even; synchronises `stream`. */
 int om_index_add(om_index* idx, const void* x, om_memkind kind, om_dtype dtype, int64_t n, void* stream);
 /* Zero-copy ingest: reserve room for n more rows and get the device address of the fp32 row block
  * (row pitch = d floats) so the encoder can write embeddings in place; om_index_commit(n) publishes
  * them (builds the fp16 scan copy and updates the error-norm maxima the exactness certificate uses).  */
-int om_index_reserve(om_index* idx, int64_t n, float** dev_rows);
+int om_index_reserve(om_index* idx, int64_t n, float** dev_rows); /* fp32 storage only (OM_ESTATE otherwise) */
+/* Either storage: the device address of the next n rows, fp32 at pitch d or fp16 at pitch dpad (elements).  For fp16
+ * rows om_index_commit updates the error-norm maxima and counts rows with a non-finite element. */
+int om_index_reserve_rows(om_index* idx, int64_t n, void** dev_rows, int64_t* row_pitch_elems);
 int om_index_commit(om_index* idx, int64_t n, void* stream);
 int64_t om_index_ntotal(const om_index* idx);
 int om_index_dim(const om_index* idx);
@@ -154,6 +169,7 @@ int om_index_set_param(om_index* idx, const char* name, int64_t value);
 /* Statistics of the last search: "rounds", "overflow_retries", "candidates" (per query capacity),
  * "launches" (kernels launched), "uncertified" (queries the first level could not prove exact),
  * "uncertified_wide" (still unproven with 4096 candidates), "exact_queries" (answered by the exact fp32 scan),
+ * "nonfinite_rows" (fp16 storage: committed rows holding inf or NaN, as the last search read it; 0 after a reset),
  * and with "profile" on: "scan_ns", "select_ns",
  * "finalize_ns", "other_ns" (device time summed over the launches of each kind; other = exchange + merge + certify). */
 int64_t om_index_get_stat(const om_index* idx, const char* name);

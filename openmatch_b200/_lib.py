@@ -39,6 +39,9 @@ SIGNATURES = {
     "om_encoder_rep_dim": (c_int, [c_void_p]),
     "om_encoder_destroy": (None, [c_void_p]),
     "om_index_create": (c_int, [c_int, POINTER(c_void_p)]),
+    "om_index_create_typed": (c_int, [c_int, c_int, POINTER(c_void_p)]),
+    "om_index_storage": (c_int, [c_void_p]),
+    "om_index_reserve_rows": (c_int, [c_void_p, c_int64, POINTER(c_void_p), POINTER(c_int64)]),
     "om_index_add": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p]),
     "om_index_reserve": (c_int, [c_void_p, c_int64, POINTER(c_void_p)]),
     "om_index_commit": (c_int, [c_void_p, c_int64, c_void_p]),

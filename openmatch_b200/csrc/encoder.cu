@@ -955,7 +955,8 @@ __global__ void __launch_bounds__(256) head_kernel(const float* in, const float*
   }
 }
 
-// F.normalize(x, dim=1) = x / max(||x||_2, 1e-12) (optional) and store as fp32 / bf16 with a row pitch
+// F.normalize(x, dim=1) = x / max(||x||_2, 1e-12) (optional) and store as fp32 / bf16 / fp16 (round to nearest even from
+// the fp32 value, so an fp16 output is bitwise the rounding of the fp32 output of the same call) with a row pitch
 template <typename OutT>
 __global__ void finish_reps_kernel(const float* in, int B, int D, int normalize, OutT* out, int64_t pitch) {
   const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
@@ -1424,7 +1425,8 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   if (d.arch == OM_ARCH_BERT && L > d.max_pos) return fail(OM_EINVAL, "om_encode: L=%d exceeds max_position_embeddings", L);
   const int64_t T64 = static_cast<int64_t>(B) * L;
   if (T64 > e->Tmax) return fail(OM_EINVAL, "om_encode: B*L=%lld exceeds max_batch_tokens=%d", (long long)T64, e->Tmax);
-  if (out_dtype != OM_F32 && out_dtype != OM_BF16) return fail(OM_EINVAL, "om_encode: out dtype must be f32 or bf16");
+  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
+    return fail(OM_EINVAL, "om_encode: out dtype must be f32, bf16 or f16");
   const int rep_dim = om_encoder_rep_dim(e);
   if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode: out_row_stride < rep_dim");
   const int sms = device_sm_count();
@@ -1548,9 +1550,12 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   if (out_dtype == OM_F32)
     finish_reps_kernel<float><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<float*>(out_reps),
                                                           out_row_stride);
-  else
+  else if (out_dtype == OM_BF16)
     finish_reps_kernel<__nv_bfloat16><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize,
                                                                   static_cast<__nv_bfloat16*>(out_reps), out_row_stride);
+  else
+    finish_reps_kernel<__half><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<__half*>(out_reps),
+                                                           out_row_stride);
   OM_CUDA(cudaGetLastError());
   return 0;
 }

@@ -6,6 +6,10 @@
 // Storage per index shard: fp32 master rows [n, d] (what index.add received; used for exact re-scoring)
 // plus an fp16 scan copy [n, dpad] (tensor-core operand; IEEE half keeps 3 more significand bits than bf16 at the
 // same tensor-core rate, which is what makes the exactness certificate below affordable).
+// An index created with fp16 storage (om_index_create_typed) keeps only the fp16 rows [n, dpad]: they are the scan
+// operand and the row store at once, FINAL and the exact scan read them, and every "fp32 score" below is the fp32
+// inner product of the fp32 query with the STORED fp16 row (same summation order).  The corpus error term of the
+// certificate is then exactly 0.
 //
 // search(q, k):
 //   1. SCAN    fp16 Q * X^T on wgmma with the top-k filter fused into the epilogue (query batches: scan_gemm.cuh, 2-CTA
@@ -186,11 +190,42 @@ __global__ void __launch_bounds__(256) select_kernel(unsigned long long* cand, i
   }
 }
 
-// FINAL: one CTA per query: exact fp32 re-score of the candidates against the master rows,
-// sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row gathers are HBM-bound and
-// want every warp resident.
+// Row elements as fp32 for the re-score and the exact scan: group i of 4 consecutive elements (a float4, or one 8-byte
+// load of 4 halves; the row pitch keeps the groups aligned), and element i.  fp16 -> fp32 is exact, so a row stored in
+// fp16 scores bit for bit like the same values held as fp32.
+template <typename RowT>
+struct RowQuad;  // the type of one load of 4 row elements
+template <>
+struct RowQuad<float> {
+  using T = float4;
+};
+template <>
+struct RowQuad<__half> {
+  using T = uint2;
+};
+__device__ __forceinline__ float4 quad_f32(float4 v) { return v; }
+__device__ __forceinline__ float4 quad_f32(uint2 u) {
+  const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+  const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+  return make_float4(lo.x, lo.y, hi.x, hi.y);
+}
+__device__ __forceinline__ float elem_f32(float v) { return v; }
+__device__ __forceinline__ float elem_f32(__half v) { return __half2float(v); }
+// row pitch in elements: fp32 master rows [n, d], fp16 rows [n, dpad] with dpad = d rounded up to 8 (om_index_create)
+template <typename RowT>
+__device__ __forceinline__ int row_pitch(int d) { return sizeof(RowT) == 4 ? d : (d + 7) & ~7; }
+// the 4-element groups of row r (d % 4 == 0)
+template <typename RowT>
+__device__ __forceinline__ const typename RowQuad<RowT>::T* row_quads(const RowT* xs, size_t r, int d) {
+  return reinterpret_cast<const typename RowQuad<RowT>::T*>(xs) + r * (row_pitch<RowT>(d) >> 2);
+}
+
+// FINAL: one CTA per query: exact fp32 re-score of the candidates against the stored rows (fp32 master rows or fp16
+// rows), sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row
+// gathers are HBM-bound and want every warp resident.
+template <typename RowT>
 __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long long* cand, const int* count, int C,
-                                                          const float* __restrict__ qf, const float* __restrict__ xf,
+                                                          const float* __restrict__ qf, const RowT* __restrict__ xs,
                                                           int d, float* D, int64_t* I, int64_t id_offset, int k_out,
                                                           int stage_scores) {
   extern __shared__ unsigned long long fsm[];
@@ -209,18 +244,18 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
     const uint32_t row = key_row(mine[j]);
     float acc = 0.f;
     if ((d & 3) == 0) {
-      const float4* x4 = reinterpret_cast<const float4*>(xf) + static_cast<size_t>(row) * (d >> 2);
+      const auto* x4 = row_quads(xs, row, d);
       const float4* q4 = reinterpret_cast<const float4*>(sq);
       for (int i = lane; i < (d >> 2); i += 32) {
-        const float4 a = __ldg(x4 + i), b = q4[i];
+        const float4 a = quad_f32(__ldg(x4 + i)), b = q4[i];
         acc = fmaf(a.x, b.x, acc);
         acc = fmaf(a.y, b.y, acc);
         acc = fmaf(a.z, b.z, acc);
         acc = fmaf(a.w, b.w, acc);
       }
     } else {
-      const float* x = xf + static_cast<size_t>(row) * d;
-      for (int i = lane; i < d; i += 32) acc = fmaf(__ldg(x + i), sq[i], acc);
+      const RowT* x = xs + static_cast<size_t>(row) * row_pitch<RowT>(d);
+      for (int i = lane; i < d; i += 32) acc = fmaf(elem_f32(__ldg(x + i)), sq[i], acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -288,6 +323,53 @@ __global__ void __launch_bounds__(256) rows_to_f16_kernel(const float* __restric
     atomicMax(reinterpret_cast<int*>(gstats) + 1, __float_as_int(me != me ? __int_as_float(0x7fc00000) : me));
   }
 }
+
+// fp16 storage, add: src [n, d] (fp32 / bf16 / fp16) -> dst fp16 [n, dpad], round to nearest even.  Elements that become
+// ±inf or NaN in fp16 (NaN, |x| >= 65520) are counted in *bad: the caller then refuses the whole add.
+template <typename T>
+__global__ void to_f16_rows_kernel(const T* __restrict__ src, int64_t n, int d, __half* __restrict__ dst, int dpad, int* bad) {
+  int nb = 0;
+  for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n * d;
+       i += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    const int64_t r = i / d;
+    const __half h = __float2half_rn(static_cast<float>(src[i]));
+    dst[r * dpad + (i - r * d)] = h;
+    nb += (__hisinf(h) || __hisnan(h)) ? 1 : 0;
+  }
+  if (nb) atomicAdd(bad, nb);
+}
+
+// fp16 storage, commit: the stored rows x [n, dpad] are read in place.  Running maxima of ||x|| (gstats[0], summed in the
+// order of rows_to_f16_kernel, so an fp32 index of the same values gets the same bits); ||x - x_h|| is 0 and gstats[1]
+// stays as it is.  Rows holding a non-finite element are counted in *nonfinite: searches refuse the index until a reset.
+__global__ void __launch_bounds__(256) commit_f16_rows_kernel(const __half* __restrict__ x, int64_t n, int d, int dpad,
+                                                              float* gstats, int* nonfinite) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
+  float mx = 0.f;
+  int nbad = 0;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
+    const __half* y = x + r * dpad;
+    float sx = 0.f;
+    bool finite = true;
+    for (int c = 2 * lane; c < d; c += 64) {  // c + 1 < dpad (dpad is a multiple of 8): the pair load stays in the row
+      const float2 v = __half22float2(*reinterpret_cast<const __half2*>(y + c));
+      const float a = v.x, b = c + 1 < d ? v.y : 0.f;
+      finite = finite && isfinite(a) && isfinite(b);
+      sx = fmaf(a, a, fmaf(b, b, sx));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, o);
+    const float nx = sqrtf(sx);
+    mx = (nx > mx || nx != nx) ? nx : mx;
+    if (!__all_sync(0xffffffffu, finite) && lane == 0) ++nbad;
+  }
+  if (lane == 0) {
+    atomicMax(reinterpret_cast<int*>(gstats), __float_as_int(mx != mx ? __int_as_float(0x7fc00000) : mx));
+    if (nbad) atomicAdd(nonfinite, nbad);
+  }
+}
+
 template <typename T>
 __global__ void to_f32(const T* __restrict__ src, float* __restrict__ dst, int64_t n) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
@@ -406,12 +488,14 @@ __global__ void __launch_bounds__(1024) compact_flags_kernel(const int* __restri
 }
 
 // EXACT fp32 scan on the CUDA cores (the certificate's last resort and the "exact_only" test mode): one warp per
-// row group, queries of the tile in shared memory.  Per (query, row) the summation order is EXACTLY the one of
-// finalize_kernel (lane-strided float4 FMA chain, then the xor-butterfly), so both produce bit-identical scores.
+// row group, queries of the tile in shared memory, rows of type RowT (as finalize_kernel reads them).
+// Per (query, row) the summation order is EXACTLY the one of finalize_kernel (lane-strided 4-element FMA chain, then the
+// xor-butterfly), so both produce bit-identical scores.
 // Survivors (score > the query's strict threshold) are appended to the same candidate lists the tensor-core scan
 // uses; dense = 1: first round, every score stored at position = column.
-template <int NQT, int ROWS>
-__global__ void __launch_bounds__(256) exact_scan_kernel(const float* __restrict__ xf, int64_t n_rows, uint32_t row_base,
+template <int NQT, int ROWS, typename RowT>
+__global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict__ xs, int64_t n_rows,
+                                                         uint32_t row_base,
                                                          const float* __restrict__ qf, int nq, int d, int nqt,
                                                          const float* __restrict__ thr, unsigned long long* cand,
                                                          int* count, int* overflow, int C, int dense) {
@@ -420,7 +504,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const float* __restrict
   const int nact = min(nqt, nq - q0);
   for (int i = threadIdx.x; i < nact * d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q0) * d + i];
   __syncthreads();
-  const int lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31, pitch = row_pitch<RowT>(d);
   float t = __int_as_float(0x7f800000);
   if (lane < nact && !dense) t = thr[q0 + lane];
   const int64_t wg = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5), nw = static_cast<int64_t>(gridDim.x) * 8;
@@ -436,8 +520,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const float* __restrict
         float4 a[ROWS];
 #pragma unroll
         for (int rr = 0; rr < ROWS; ++rr)
-          a[rr] = r0 + rr < n_rows ? __ldg(reinterpret_cast<const float4*>(xf + static_cast<size_t>(r0 + rr) * d) + i)
-                                   : make_float4(0.f, 0.f, 0.f, 0.f);
+          a[rr] = r0 + rr < n_rows ? quad_f32(__ldg(row_quads(xs, r0 + rr, d) + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int j = 0; j < NQT; ++j) {
           if (j < nact) {
@@ -458,7 +541,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const float* __restrict
       for (int i = lane; i < d; i += 32) {
         float a[ROWS];
 #pragma unroll
-        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? __ldg(xf + static_cast<size_t>(r0 + rr) * d + i) : 0.f;
+        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? elem_f32(__ldg(xs + static_cast<size_t>(r0 + rr) * pitch + i)) : 0.f;
 #pragma unroll
         for (int j = 0; j < NQT; ++j)
           if (j < nact) {
@@ -579,11 +662,16 @@ struct Level {
 
 struct om_index {
   int d = 0, dpad = 0;
+  int storage = OM_F32;  // OM_F32: fp32 master rows xf + fp16 scan copy xh; OM_F16: xh only (xf stays null)
   int64_t n = 0, cap = 0;
   float* xf = nullptr;
   __half* xh = nullptr;
-  float* gstats = nullptr;  // device [2]: max ||x||, max ||x - x_h|| over the committed rows (float bit patterns)
-  bool gstats_stale = false;  // set by om_index_reset: gstats is zeroed on the stream of the next commit / search
+  // device [4]: [0] max ||x||, [1] max ||x - x_h|| over the committed rows (float bit patterns); fp16 storage: [2] rows
+  // with a non-finite element committed since the last reset (int), [3] scratch (int: rejected elements of an add,
+  // the all-reduced [2] of a sharded search)
+  float* gstats = nullptr;
+  bool gstats_stale = false;  // set by om_index_reset: gstats[0..2] are zeroed on the stream of the next commit / search
+  int64_t st_nonfinite = 0;   // gstats[2] as the last search read it
   int64_t rescore_slack = -1;
   int force_safe = 0;
   int pair_scan = 1;      // > 128 queries: rounds after the first on the wide scan (scan_gemm.cuh); 0 = single-CTA tiles
@@ -613,17 +701,19 @@ static int index_grow(om_index* ix, int64_t need) {
   ncap = round_up(std::max<int64_t>(ncap, 1024), 256);
   float* nxf = nullptr;
   __half* nxh = nullptr;
+  const bool master = ix->storage == OM_F32;
   // rows may still be in flight on the caller's stream(s) (encoder writing reserved rows, a pending commit)
   OM_CUDA(cudaDeviceSynchronize());
-  OM_CUDA(dev_malloc(&nxf, static_cast<size_t>(ncap) * ix->d * sizeof(float)));
+  if (master) OM_CUDA(dev_malloc(&nxf, static_cast<size_t>(ncap) * ix->d * sizeof(float)));
   cudaError_t e = dev_malloc(&nxh, static_cast<size_t>(ncap) * ix->dpad * sizeof(__half));
   if (e != cudaSuccess) {
     cudaFree(nxf);
     cudaGetLastError();
-    return fail(OM_ENOMEM, "index: cannot allocate the fp16 scan copy for %lld rows", (long long)ncap);
+    return fail(OM_ENOMEM, "index: cannot allocate the fp16 rows for %lld rows", (long long)ncap);
   }
   if (ix->n > 0) {
-    OM_CUDA(cudaMemcpy(nxf, ix->xf, static_cast<size_t>(ix->n) * ix->d * sizeof(float), cudaMemcpyDeviceToDevice));
+    if (master)
+      OM_CUDA(cudaMemcpy(nxf, ix->xf, static_cast<size_t>(ix->n) * ix->d * sizeof(float), cudaMemcpyDeviceToDevice));
     OM_CUDA(cudaMemcpy(nxh, ix->xh, static_cast<size_t>(ix->n) * ix->dpad * sizeof(__half), cudaMemcpyDeviceToDevice));
   }
   OM_CUDA(cudaDeviceSynchronize());
@@ -645,21 +735,26 @@ static inline int grid_for(int64_t n, int threads) {
 // and leave maxima of 0, with which the certificate would prove wrong candidate lists exact.
 static int settle_reset(om_index* ix, cudaStream_t st) {
   if (!ix->gstats_stale) return 0;
-  OM_CUDA(cudaMemsetAsync(ix->gstats, 0, 2 * sizeof(float), st));
+  OM_CUDA(cudaMemsetAsync(ix->gstats, 0, 3 * sizeof(float), st));
   ix->gstats_stale = false;
   return 0;
 }
 
 extern "C" {
 
-int om_index_create(int d, om_index** out) {
+int om_index_create(int d, om_index** out) { return om_index_create_typed(d, OM_F32, out); }
+
+int om_index_create_typed(int d, om_dtype storage, om_index** out) {
   if (!out || d <= 0) return fail(OM_EINVAL, "om_index_create: d must be positive");
+  if (storage != OM_F32 && storage != OM_F16)
+    return fail(OM_EINVAL, "om_index_create_typed: storage must be OM_F32 or OM_F16 (the scan operand is fp16)");
   OM_TRY(device_sm_count());
   om_index* ix = new (std::nothrow) om_index();
   if (!ix) return fail(OM_ENOMEM, "om_index_create: out of host memory");
   ix->d = d;
   ix->dpad = static_cast<int>(round_up(d, 8));  // 16-byte row pitch for TMA
-  if (cudaMalloc(&ix->gstats, 2 * sizeof(float)) != cudaSuccess || cudaMemset(ix->gstats, 0, 2 * sizeof(float)) != cudaSuccess ||
+  ix->storage = storage;
+  if (cudaMalloc(&ix->gstats, 4 * sizeof(float)) != cudaSuccess || cudaMemset(ix->gstats, 0, 4 * sizeof(float)) != cudaSuccess ||
       cudaHostAlloc(&ix->h_status, 8 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
     cudaGetLastError();
     cudaFree(ix->gstats);
@@ -685,19 +780,37 @@ void om_index_destroy(om_index* ix) {
 
 int64_t om_index_ntotal(const om_index* ix) { return ix ? ix->n : 0; }
 int om_index_dim(const om_index* ix) { return ix ? ix->d : 0; }
+int om_index_storage(const om_index* ix) { return ix ? ix->storage : fail(OM_EINVAL, "om_index_storage: null index"); }
 
 int om_index_reset(om_index* ix) {
   if (!ix) return fail(OM_EINVAL, "om_index_reset: null index");
   ix->n = 0;
   ix->gstats_stale = true;  // host only: see settle_reset
+  ix->st_nonfinite = 0;
+  return 0;
+}
+
+int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row_pitch_elems) {
+  if (!ix || n < 0 || !dev_rows || !row_pitch_elems) return fail(OM_EINVAL, "om_index_reserve_rows: bad arguments");
+  if (ix->n + n > 0xfffffff0ll) return fail(OM_EINVAL, "index shard limited to 2^32-16 rows; shard the corpus");
+  OM_TRY(index_grow(ix, ix->n + n));
+  if (ix->storage == OM_F16) {
+    *dev_rows = ix->xh + static_cast<size_t>(ix->n) * ix->dpad;
+    *row_pitch_elems = ix->dpad;
+  } else {
+    *dev_rows = ix->xf + static_cast<size_t>(ix->n) * ix->d;
+    *row_pitch_elems = ix->d;
+  }
   return 0;
 }
 
 int om_index_reserve(om_index* ix, int64_t n, float** dev_rows) {
   if (!ix || n < 0 || !dev_rows) return fail(OM_EINVAL, "om_index_reserve: bad arguments");
-  if (ix->n + n > 0xfffffff0ll) return fail(OM_EINVAL, "index shard limited to 2^32-16 rows; shard the corpus");
-  OM_TRY(index_grow(ix, ix->n + n));
-  *dev_rows = ix->xf + static_cast<size_t>(ix->n) * ix->d;
+  if (ix->storage != OM_F32) return fail(OM_ESTATE, "om_index_reserve: the index stores fp16 rows; use om_index_reserve_rows");
+  void* rows = nullptr;
+  int64_t pitch = 0;
+  OM_TRY(om_index_reserve_rows(ix, n, &rows, &pitch));
+  *dev_rows = static_cast<float*>(rows);
   return 0;
 }
 
@@ -706,18 +819,65 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   OM_TRY(settle_reset(ix, st));
-  rows_to_f16_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xf + static_cast<size_t>(ix->n) * ix->d,
-                                                     ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d, ix->dpad,
-                                                     nullptr, nullptr, ix->gstats);
+  if (ix->storage == OM_F16)
+    commit_f16_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d,
+                                                           ix->dpad, ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
+  else
+    rows_to_f16_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xf + static_cast<size_t>(ix->n) * ix->d,
+                                                       ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d, ix->dpad,
+                                                       nullptr, nullptr, ix->gstats);
   OM_CUDA(cudaGetLastError());
   ix->n += n;
   return 0;
+}
+
+// om_index_add on fp16 storage: convert into the reserved rows, count what fp16 cannot hold, and commit only if nothing
+// was out of range (the converted rows stay beyond ntotal otherwise).  Synchronises `st` to read the count.
+static int add_f16(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, cudaStream_t st) {
+  void* rows = nullptr;
+  int64_t pitch = 0;
+  OM_TRY(om_index_reserve_rows(ix, n, &rows, &pitch));
+  __half* dst = static_cast<__half*>(rows);
+  const size_t elems = static_cast<size_t>(n) * ix->d;
+  const size_t esize = dtype == OM_F32 ? 4 : 2;
+  const void* src = x;
+  void* tmp = nullptr;
+  if (kind == OM_HOST) {
+    OM_CUDA(cudaMalloc(&tmp, elems * esize));
+    OM_CUDA(cudaMemcpyAsync(tmp, x, elems * esize, cudaMemcpyHostToDevice, st));
+    src = tmp;
+  }
+  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
+  cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(int), st);
+  const int grid = grid_for(static_cast<int64_t>(elems), 256);
+  if (e == cudaSuccess) {
+    if (dtype == OM_F32)
+      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const float*>(src), n, ix->d, dst, ix->dpad, bad);
+    else if (dtype == OM_BF16)
+      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(src), n, ix->d, dst, ix->dpad, bad);
+    else
+      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const __half*>(src), n, ix->d, dst, ix->dpad, bad);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  if (tmp) cudaFree(tmp);
+  OM_CUDA(e);
+  if (ix->h_status[4] > 0)
+    return fail(OM_EINVAL, "om_index_add: %d elements are NaN or round to +-inf in fp16 (|x| >= 65520); fp16 storage cannot "
+                "hold them and no row was added", ix->h_status[4]);
+  return om_index_commit(ix, n, st);
 }
 
 int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, void* stream) {
   if (!ix || (!x && n > 0) || n < 0) return fail(OM_EINVAL, "om_index_add: bad arguments");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (ix->storage == OM_F16) {
+    if (dtype != OM_F32 && dtype != OM_BF16 && dtype != OM_F16)
+      return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
+    return add_f16(ix, x, kind, dtype, n, st);
+  }
   float* dst = nullptr;
   OM_TRY(om_index_reserve(ix, n, &dst));
   const size_t elems = static_cast<size_t>(n) * ix->d;
@@ -789,6 +949,7 @@ int64_t om_index_get_stat(const om_index* ix, const char* name) {
   if (!strcmp(name, "uncertified")) return ix->st_flagged;
   if (!strcmp(name, "uncertified_wide")) return ix->st_flagged_wide;
   if (!strcmp(name, "exact_queries")) return ix->st_exact;
+  if (!strcmp(name, "nonfinite_rows")) return ix->st_nonfinite;
   if (!strcmp(name, "scan_cluster")) return ix->st_scan_cluster;
   if (!strcmp(name, "scan_max_clusters")) return ix->st_scan_clusters;
   if (!strcmp(name, "scan_ns")) return static_cast<int64_t>(ix->st_scan_us * 1e3);
@@ -848,9 +1009,11 @@ int once_attrs() {
   static bool done = false;  // one device per process (enforced by device_sm_count)
   if (done) return 0;
   OM_CUDA(cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
-  OM_CUDA(cudaFuncSetAttribute(finalize_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
+  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
+  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
   OM_CUDA(cudaFuncSetAttribute(merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16));
-  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   done = true;
   return 0;
 }
@@ -997,9 +1160,15 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         const int nqt = std::max(1, std::min(8, (96 * 1024) / (ix->d * 4)));
         dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
                   static_cast<unsigned>((nqc + nqt - 1) / nqt));
-        exact_scan_kernel<8, 2><<<grid, 256, static_cast<size_t>(nqt) * ix->d * 4, st>>>(
-            ix->xf + static_cast<size_t>(pos) * ix->d, step, static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
-            L.count, overflow, C, first ? 1 : 0);
+        const size_t smem = static_cast<size_t>(nqt) * ix->d * 4;
+        if (ix->storage == OM_F16)
+          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xh + static_cast<size_t>(pos) * ix->dpad, step,
+                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
+                                                           L.count, overflow, C, first ? 1 : 0);
+        else
+          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xf + static_cast<size_t>(pos) * ix->d, step,
+                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
+                                                           L.count, overflow, C, first ? 1 : 0);
         OM_CUDA(cudaGetLastError());
       }
     }
@@ -1023,8 +1192,13 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
   const size_t fin_smem = static_cast<size_t>(P2) * 8 + static_cast<size_t>(ix->d) * 4;
   {
     Timed t(ix, st, 2);
-    finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, L.qf + static_cast<size_t>(q0) * ix->d, ix->xf, ix->d,
-                                                D, I, id_offset, k_out, ix->stage_scores);
+    const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
+    if (ix->storage == OM_F16)
+      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xh, ix->d, D, I, id_offset, k_out,
+                                                  ix->stage_scores);
+    else
+      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xf, ix->d, D, I, id_offset, k_out,
+                                                  ix->stage_scores);
   }
   OM_CUDA(cudaGetLastError());
   ix->st_launches += 1;
@@ -1155,6 +1329,24 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
   return fail(OM_EFAULT, "search level did not converge (bug)");
 }
 
+// fp16 storage: rows written in place may hold values fp16 cannot represent (inf from an overflowing encoder output, NaN),
+// and there is no fp32 copy to answer from, so the search is refused until om_index_reset.  Sharded: the shards' counts are
+// summed so that every rank takes the same decision.  One host synchronisation; fp32 indices skip the check.
+int check_finite_rows(om_index* ix, om_comm* comm, cudaStream_t st) {
+  if (ix->storage != OM_F16) return 0;
+  int* cnt = reinterpret_cast<int*>(ix->gstats) + 2;
+  const bool sharded = comm && comm->world > 1;
+  if (sharded) OM_NCCL(nccl_api().AllReduce(cnt, cnt + 1, 1, kNcclInt32, kNcclSum, comm->nccl, st));
+  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  ix->st_nonfinite = ix->h_status[4];
+  const int total = sharded ? ix->h_status[5] : ix->h_status[4];
+  if (total > 0)
+    return fail(OM_EINVAL, "search: %d committed fp16 rows hold inf or NaN (%d on this shard); fp16 storage cannot answer "
+                "exactly over them: reset the index", total, ix->h_status[4]);
+  return 0;
+}
+
 // The whole search: level 0 (all queries, k + slack candidates) -> level 1 (uncertified queries, widest list) ->
 // level 2 (still uncertified: exact fp32 scan).  comm == nullptr / world 1: single shard.
 int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
@@ -1167,6 +1359,7 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   ix->st_scan_cluster = ix->st_scan_clusters = 0;
   ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
   ix->ev_used = 0;
+  OM_TRY(check_finite_rows(ix, comm, st));
   // whole-search staging: queries (if they arrive from the host), results (if they leave to the host), flag list
   size_t off = 0;
   auto carve = [&](size_t bytes) {

@@ -13,6 +13,8 @@ import torch
 
 from . import _lib
 
+_OUT_DTYPES = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16}
+
 _BERT_KEYS = ("num_hidden_layers", "hidden_size", "num_attention_heads", "intermediate_size", "vocab_size",
               "max_position_embeddings", "type_vocab_size", "layer_norm_eps")
 
@@ -97,7 +99,9 @@ class CudaEncoder:
     def encode(self, input_ids: torch.Tensor, attention_mask: torch.Tensor,
                token_type_ids: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None,
                out_dtype: torch.dtype = torch.float32, return_hidden: bool = False):
-        """int64 [B, L] CUDA tensors in -> reps [B, rep_dim] (and last_hidden_state fp32 [B, L, H])."""
+        """int64 [B, L] CUDA tensors in -> reps [B, rep_dim] (and last_hidden_state fp32 [B, L, H]).  ``out`` / ``out_dtype``:
+        fp32, bf16 or fp16 (fp16 and bf16 are the round-to-nearest-even of the fp32 reps of the same call); ``out`` may
+        have any row stride (e.g. the rows ``FlatIPIndex.reserve_rows`` hands out)."""
         if not input_ids.is_cuda:
             raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
         B, L = input_ids.shape
@@ -106,11 +110,11 @@ class CudaEncoder:
         tt = token_type_ids.to(torch.int64).contiguous() if token_type_ids is not None else None
         if out is None:
             out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=ids.device)
-        if out.dtype not in (torch.float32, torch.bfloat16) or out.stride(1) != 1:
-            raise ValueError("out must be a row-major fp32 / bf16 CUDA tensor")
+        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
+            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
         hidden = torch.empty((B, L, self.hidden), dtype=torch.float32, device=ids.device) if return_hidden else None
         _lib.check(self._lib.om_encode(
             self._h, ids.data_ptr(), mask.data_ptr(), tt.data_ptr() if tt is not None else None, B, L,
-            out.data_ptr(), _lib.OM_F32 if out.dtype == torch.float32 else _lib.OM_BF16, out.stride(0),
+            out.data_ptr(), _OUT_DTYPES[out.dtype], out.stride(0),
             hidden.data_ptr() if hidden is not None else None, _lib.current_stream_ptr()))
         return (hidden, out) if return_hidden else out

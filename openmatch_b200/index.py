@@ -20,16 +20,30 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
+_STORAGE = {torch.float32: _lib.OM_F32, torch.float16: _lib.OM_F16}
+
+
 class FlatIPIndex:
     """``faiss.IndexFlatIP`` duck type (``d``, ``ntotal``, ``add``, ``search``, ``reset``) living on the
-    current CUDA device."""
+    current CUDA device.
 
-    def __init__(self, d: int):
+    ``dtype`` is the row storage.  ``torch.float32`` (default): fp32 master rows plus an fp16 scan copy (6 bytes per
+    element); search is exact over the rows as added.  ``torch.float16``: the fp16 rows only (2 bytes per element);
+    added rows are rounded to fp16 (nearest even) and search is exact with respect to the STORED values: the exact
+    top-k by fp32 inner product of the fp32 query with the fp16 rows, ties by ascending id, bitwise what a float32
+    index of the fp16-rounded rows returns.  fp16 storage refuses what it cannot hold: ``add`` of a NaN or of a value
+    that rounds to +-inf in fp16 (|x| >= 65520) raises and adds nothing; rows written in place through ``reserve_rows``
+    and committed with such values make ``search`` raise until ``reset`` (``stat("nonfinite_rows")``)."""
+
+    def __init__(self, d: int, dtype: torch.dtype = torch.float32):
+        if dtype not in _STORAGE:
+            raise ValueError("index storage must be torch.float32 or torch.float16, got %s" % dtype)
         self._lib = _lib.load()
         h = ctypes.c_void_p()
-        _lib.check(self._lib.om_index_create(int(d), ctypes.byref(h)))
+        _lib.check(self._lib.om_index_create_typed(int(d), _STORAGE[dtype], ctypes.byref(h)))
         self._h = h
         self.d = int(d)
+        self.dtype = dtype
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
@@ -42,18 +56,24 @@ class FlatIPIndex:
         return int(self._lib.om_index_ntotal(self._h))
 
     def add(self, x) -> None:
-        """x: float32 [n, d]; numpy (host) or torch tensor (host or CUDA)."""
-        if isinstance(x, torch.Tensor) and x.is_cuda:
-            x = x.contiguous()
-            if x.dtype not in (torch.float32, torch.bfloat16, torch.float16):
+        """x: [n, d]; numpy (host) or torch tensor (host or CUDA); float32, bfloat16 or float16 tensors are passed as they
+        are, anything else as float32."""
+        if isinstance(x, torch.Tensor) and (x.is_cuda or (self.dtype == torch.float16 and x.dtype in _ADD_DTYPES)):
+            x = x.detach().contiguous()
+            if x.dtype not in _ADD_DTYPES:
                 x = x.float()
-            dt = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16}[x.dtype]
+            kind = _lib.OM_DEVICE if x.is_cuda else _lib.OM_HOST
             self._check_shape(x.shape)
-            _lib.check(self._lib.om_index_add(self._h, x.data_ptr(), _lib.OM_DEVICE, dt, x.shape[0], _stream()))
+            _lib.check(self._lib.om_index_add(self._h, x.data_ptr(), kind, _ADD_DTYPES[x.dtype], x.shape[0], _stream()))
             torch.cuda.current_stream().synchronize()  # the caller's tensor may be freed right after
             return
         if isinstance(x, torch.Tensor):
             x = x.detach().cpu().numpy()
+        if self.dtype == torch.float16 and isinstance(x, np.ndarray) and x.dtype == np.float16:
+            x = np.ascontiguousarray(x)
+            self._check_shape(x.shape)
+            _lib.check(self._lib.om_index_add(self._h, x.ctypes.data, _lib.OM_HOST, _lib.OM_F16, x.shape[0], _stream()))
+            return
         x = np.ascontiguousarray(x, dtype=np.float32)
         self._check_shape(x.shape)
         _lib.check(self._lib.om_index_add(self._h, x.ctypes.data, _lib.OM_HOST, _lib.OM_F32, x.shape[0], _stream()))
@@ -126,21 +146,27 @@ class FlatIPIndex:
         _lib.check(self._lib.om_index_search(self._h, q_host.data_ptr(), _lib.OM_HOST, nq, int(k), D_host.data_ptr(),
                                              I_host.data_ptr(), _lib.OM_HOST, int(id_offset), _stream()))
 
+    def _rows_at(self, n: int):
+        """(device address, row pitch in elements) of the shard's rows after reserving room for n more"""
+        p, pitch = ctypes.c_void_p(), ctypes.c_int64()
+        _lib.check(self._lib.om_index_reserve_rows(self._h, int(n), ctypes.byref(p), ctypes.byref(pitch)))
+        return p.value, pitch.value
+
     def reserve_rows(self, n: int) -> torch.Tensor:
-        """Zero-copy ingest: a float32 CUDA tensor view [n, d] of the next n rows of the shard; fill it
-        (e.g. as the encoder's output buffer) and call ``commit_rows(n)``."""
-        p = ctypes.c_void_p()
-        _lib.check(self._lib.om_index_reserve(self._h, int(n), ctypes.byref(p)))
-        return _wrap_device_f32(p.value, (int(n), self.d))
+        """Zero-copy ingest: a CUDA tensor view [n, d] of the next n rows of the shard in the index's dtype (float16
+        rows have row stride dpad = d rounded up to 8); fill it (e.g. as the encoder's output buffer) and call
+        ``commit_rows(n)``."""
+        p, pitch = self._rows_at(n)
+        return _wrap_device(p, (int(n), self.d), pitch, self.dtype)
 
     def master_rows(self) -> torch.Tensor:
-        """float32 CUDA view [ntotal, d] of the shard's master rows (no copy)."""
+        """CUDA view [ntotal, d] of the shard's stored rows in the index's dtype (no copy).  Exported embedding files
+        upcast it to float32, so an fp16 index writes its fp16-rounded values."""
         n = self.ntotal
-        p = ctypes.c_void_p()
-        _lib.check(self._lib.om_index_reserve(self._h, 0, ctypes.byref(p)))  # address one past the last row
+        p, pitch = self._rows_at(0)  # address one past the last row
         if n == 0:
-            return torch.empty((0, self.d), dtype=torch.float32, device="cuda")
-        return _wrap_device_f32(p.value - n * self.d * 4, (n, self.d))
+            return torch.empty((0, self.d), dtype=self.dtype, device="cuda")
+        return _wrap_device(p - n * pitch * self.dtype.itemsize, (n, self.d), pitch, self.dtype)
 
     def commit_rows(self, n: int) -> None:
         _lib.check(self._lib.om_index_commit(self._h, int(n), _stream()))
@@ -156,14 +182,19 @@ class FlatIPIndex:
             raise ValueError("expected a [n, %d] matrix, got %s" % (self.d, tuple(shape)))
 
 
+_ADD_DTYPES = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16}
+
+
 class _CudaArrayView:
-    def __init__(self, ptr, shape):
-        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": "<f4", "data": (int(ptr), False),
-                                         "version": 3, "strides": None}
+    def __init__(self, ptr, shape, typestr, strides):
+        self.__cuda_array_interface__ = {"shape": tuple(shape), "typestr": typestr, "data": (int(ptr), False),
+                                         "version": 3, "strides": strides}
 
 
-def _wrap_device_f32(ptr: int, shape) -> torch.Tensor:
-    return torch.as_tensor(_CudaArrayView(ptr, shape), device="cuda")
+def _wrap_device(ptr: int, shape, pitch: int, dtype: torch.dtype) -> torch.Tensor:
+    size = dtype.itemsize
+    strides = None if pitch == shape[1] else (pitch * size, size)
+    return torch.as_tensor(_CudaArrayView(ptr, shape, "<f%d" % size, strides), device="cuda")
 
 
 class Comm:
@@ -243,13 +274,13 @@ class ShardedFlatIPIndex:
     HBM.  ``search`` = replicate queries -> local fused scan/top-k with global ids -> all-gather of the
     per-shard [nq, k] (score, id) lists over NCCL/NVLink -> merge (score desc, id asc) on every rank."""
 
-    def __init__(self, d: int, group=None):
+    def __init__(self, d: int, group=None, dtype: torch.dtype = torch.float32):
         import torch.distributed as dist
         self.dist = dist
         self.group = group
         self.world = dist.get_world_size(group) if dist.is_initialized() else 1
         self.rank = dist.get_rank(group) if dist.is_initialized() else 0
-        self.local = FlatIPIndex(d)
+        self.local = FlatIPIndex(d, dtype)  # every rank must pass the same dtype
         self.d = d
         self.offset = 0
         self._ntotal = 0

@@ -170,7 +170,7 @@ class DRModel(nn.Module):
 
     @torch.no_grad()
     def encode_into(self, items, out: Tensor, is_query: bool = False) -> Tensor:
-        """Inference only: representations of ``items`` written IN PLACE into ``out`` (fp32 / bf16 ``[B, rep_dim]``
+        """Inference only: representations of ``items`` written IN PLACE into ``out`` (fp32 / bf16 / fp16 ``[B, rep_dim]``
         CUDA tensor with unit column stride — e.g. the rows ``FlatIPIndex.reserve_rows`` handed out), no
         intermediate ``[B, d]`` tensor and no copy.  Same arithmetic as ``encode`` (:133-155)."""
         model, head = (self.lm_q, self.head_q) if is_query else (self.lm_p, self.head_p)

@@ -50,6 +50,13 @@ def _results_dict(query_ids: List[str], doc_lookup: np.ndarray, D: np.ndarray, I
     return out
 
 
+def _index_dtype(args) -> torch.dtype:
+    name = getattr(args, "index_dtype", "float32")
+    if name not in ("float32", "float16"):
+        raise ValueError("--index_dtype must be 'float32' or 'float16', got %r" % name)
+    return torch.float32 if name == "float32" else torch.float16
+
+
 class RankArrays:
     """Search output kept as arrays (``Retriever.search(..., as_arrays=True)``): row ``i`` of ``I`` / ``D`` holds the
     ranked rows of ``doc_names`` / scores for ``query_ids[i]``; ``to_dict()`` gives the reference's dict-of-dicts."""
@@ -90,8 +97,9 @@ class Retriever:
 
     # ------------------------------------------------------------------ index plumbing
     def _initialize_faiss_index(self, dim: int):
-        """Name kept from the reference (:38-41); the index is the HBM-resident flat IP index."""
-        self.index = FlatIPIndex(dim)
+        """Name kept from the reference (:38-41); the index is the HBM-resident flat IP index with the row storage
+        ``--index_dtype`` names (float32 or float16)."""
+        self.index = FlatIPIndex(dim, dtype=_index_dtype(self.args))
 
     def _move_index_to_gpu(self):
         """The reference clones a CPU faiss index to all GPUs here (:43-58).  Ours is born in HBM, one row
@@ -196,7 +204,7 @@ class Retriever:
     def _index_rows_to_host(self) -> np.ndarray:
         if self.index is None or self.index.ntotal == 0:
             return np.zeros((0, 0), dtype=np.float32)
-        return self.index.master_rows().cpu().numpy()  # one D2H copy per corpus shard
+        return self.index.master_rows().float().cpu().numpy()  # one D2H copy per corpus shard
 
     def init_index_and_add(self, partition: str = None):
         logger.info("Initializing index from pre-computed document embeddings")
