@@ -96,6 +96,18 @@ int om_encoder_finalize(om_encoder* enc);
 int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attention_mask,
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
               int64_t out_row_stride, float* out_hidden, void* stream);
+/* Variable-length batch, no padding.  tokens / token_type_ids (nullable => zeros; ignored for T5): int64 [T] device, the
+ * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 512 (BERT: <= max_position_embeddings; and
+ * <= max_batch_tokens), T = sum(seqlens).  Result: what om_encode returns for the same sequences padded to any L with
+ * attention_mask = 1 on their tokens, up to the order of floating-point sums in attention and pooling.  out_reps as in
+ * om_encode (row i = sequence i).  out_hidden: nullable fp32 [T, hidden], packed like tokens.  seqlens may be reused on
+ * return; no device synchronisation; asynchronous on `stream`.
+ * Layout: sequences of <= 128 tokens are bin-packed whole into 128-row attention tiles (first-fit decreasing, ties by
+ * input index: a deterministic function of seqlens); a longer one starts on a tile boundary and takes ceil(l / 128)
+ * tiles.  A layout of more than max_batch_tokens rows is encoded as consecutive groups of tiles on `stream`.
+ * Invalid input (a null pointer, B < 0, a length outside the range above) returns OM_EINVAL and writes nothing. */
+int om_encode_packed(om_encoder* enc, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens,
+                     int B, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream);
 int om_encoder_rep_dim(const om_encoder* enc);
 void om_encoder_destroy(om_encoder* enc);
 

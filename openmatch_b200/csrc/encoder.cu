@@ -24,7 +24,9 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <new>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -511,23 +513,76 @@ __device__ __forceinline__ void raw_store(const float4 (&v)[kMaxVec], int nvec, 
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// packed (variable-length) layout, om_encode_packed: sequences of <= 128 tokens are bin-packed whole into 128-row tiles,
+// longer ones start on a tile boundary and take ceil(l / 128) tiles; the rows in between are padding.
+// ---------------------------------------------------------------------------------------------------
+struct PackedSeq {  // one sequence of a packed call, in layout order (ascending row0)
+  int row0;         // first layout row, relative to the row group being encoded
+  int len;          // tokens
+  int out;          // output row of its representation (relative to the call's chunk of sequences)
+  int pad_;
+  int64_t tok0;     // offset of its first token in the caller's packed token array
+};
+
+// rowmap[r] = (slot of the sequence that holds layout row r, position inside it), (-1, -1) for a padding row; kmask[r] =
+// 0 for a real row, -inf for padding (padding rows are never attended to).  One thread per row: binary search of the
+// (row0-sorted) sequence table.
+__global__ void packed_rowmap_kernel(const PackedSeq* seqs, int nseq, int T, int2* rowmap, float* kmask) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= T) return;
+  int lo = 0, hi = nseq;  // the last sequence with row0 <= r lies in [lo, hi)
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (seqs[mid].row0 <= r) lo = mid;
+    else hi = mid;
+  }
+  const int pos = r - seqs[lo].row0;
+  const bool real = pos >= 0 && pos < seqs[lo].len;
+  rowmap[r] = real ? make_int2(lo, pos) : make_int2(-1, -1);
+  kmask[r] = real ? 0.f : __int_as_float(0xff800000);
+}
+
+// padding row of the packed layout: zeros (fp32, bf16) and zero statistics, so that everything computed from it stays
+// finite (a NaN there would reach real rows through P V, where masked keys are multiplied by 0)
+__device__ __forceinline__ void zero_row(int nvec, int lane, float* out_f32, __nv_bfloat16* out_bf16, float* stats_row) {
+  float4 v[kMaxVec];
+#pragma unroll
+  for (int j = 0; j < kMaxVec; ++j) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+  raw_store(v, nvec, lane, out_f32, out_bf16);
+  if (lane < kStatParts) reinterpret_cast<float2*>(stats_row)[lane] = make_float2(0.f, 0.f);
+}
+
 // BERT embeddings (modeling_bert.py:53-112): s = word[id] + type[tt] + pos[l], UN-normalised (fp32 + bf16) with its row
 // statistics; the embedding LayerNorm is applied by the first layer's QKV / O-proj epilogues like every other LayerNorm.
 // s is stored minus its row mean: only the embedding LayerNorm reads it, which is shift-invariant.  A common offset in
 // the embedding tables otherwise leaves rows whose mean is tens of times their standard deviation, and the bf16 copy that
 // the QKV GEMM reads (and the folded weights' rounding residue, scaled by mean / std) would bury the row's information.
+// rowmap != nullptr (packed layout): token and position come from the row map, padding rows are zeroed; a real token's
+// row is bitwise the row the padded layout gives it.
 __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, const int64_t* tts, const float* word,
                                                          const float* type, const float* pos, int T, int L, int H, int vocab,
                                                          int type_vocab, float* out_f32, __nv_bfloat16* out_bf16,
-                                                         float* stats) {
+                                                         float* stats, const int2* rowmap, const PackedSeq* seqs) {
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= T) return;
   const int nvec = H >> 7;
-  int64_t id = ids[row];
+  int64_t tok = row;
+  int l = row % L;
+  if (rowmap) {
+    const int2 m = rowmap[row];
+    if (m.x < 0) {
+      zero_row(nvec, lane, out_f32 + static_cast<int64_t>(row) * H, out_bf16 + static_cast<int64_t>(row) * H,
+               stats + static_cast<int64_t>(row) * (2 * kStatParts));
+      return;
+    }
+    tok = seqs[m.x].tok0 + m.y;
+    l = m.y;
+  }
+  int64_t id = ids[tok];
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
-  int64_t tt = tts ? tts[row] : 0;
+  int64_t tt = tts ? tts[tok] : 0;
   tt = tt < 0 ? 0 : (tt >= type_vocab ? type_vocab - 1 : tt);
-  const int l = row % L;
   float4 v[kMaxVec];
 #pragma unroll
   for (int j = 0; j < kMaxVec; ++j)
@@ -553,12 +608,24 @@ __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, con
 }
 
 // T5: h = embed_tokens[id] (no position embedding, no scaling; modeling_t5.py:682,734), fp32 + bf16 + row statistics
+// (rowmap: packed layout, as in bert_embed_kernel)
 __global__ void __launch_bounds__(128) t5_embed_kernel(const int64_t* ids, const float* emb, int T, int H, int vocab,
-                                                       float* out_f32, __nv_bfloat16* out_bf16, float* stats) {
+                                                       float* out_f32, __nv_bfloat16* out_bf16, float* stats,
+                                                       const int2* rowmap, const PackedSeq* seqs) {
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= T) return;
   const int nvec = H >> 7;
-  int64_t id = ids[row];
+  int64_t tok = row;
+  if (rowmap) {
+    const int2 m = rowmap[row];
+    if (m.x < 0) {
+      zero_row(nvec, lane, out_f32 + static_cast<int64_t>(row) * H, out_bf16 + static_cast<int64_t>(row) * H,
+               stats + static_cast<int64_t>(row) * (2 * kStatParts));
+      return;
+    }
+    tok = seqs[m.x].tok0 + m.y;
+  }
+  int64_t id = ids[tok];
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   float4 v[kMaxVec];
 #pragma unroll
@@ -612,6 +679,11 @@ struct AttnParams {
   const float* kmask;             // [T] 0 / -inf
   const float* relbias_log2;      // nullable [heads, 2*kMaxL-1], already multiplied by log2(e)
   __nv_bfloat16* ctx;             // [T, I]
+  // packed layout (om_encode_packed; nullptr for om_encode): a row's sequence and position come from rowmap [T], its
+  // length from seqs; attn_kernel starts at tile tile0 (the long sequences' tiles come first)
+  const int2* rowmap;
+  const PackedSeq* seqs;
+  int tile0;
 };
 
 // Q, K and V^T of a tile in shared memory (48 KB, TMA, 128B-swizzled); S, P and O never leave registers.
@@ -694,7 +766,8 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
   uint32_t par = 0;
 #pragma unroll 1
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, par ^= 1u) {
-    const int tile = item / n_heads, head = item - tile * n_heads;
+    const int t = item / n_heads, head = item - t * n_heads;
+    const int tile = p.tile0 + t;
     const int row0 = tile * p.Tvalid_rows;  // first token of this tile
     if (tid == 0) {  // shared memory of the previous item is free (trailing barrier): loads go out first
       mbar_arrive_expect_tx(&bars[0], 3 * 16384);
@@ -728,8 +801,14 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
         rr[u] = h * 64 + 16 * warp + (lane >> 2) + 8 * u;
         valid[u] = rr[u] < p.Tvalid_rows && row0 + rr[u] < p.T;
         // this row may attend key c iff the key is valid AND belongs to the row's own sequence [c_lo, c_hi)
-        c_lo[u] = valid[u] ? (rr[u] / p.L) * p.L : 0;
-        c_hi[u] = valid[u] ? c_lo[u] + p.L : 0;
+        if (p.rowmap) {  // packed: the sequence of the row map (contiguous inside the tile); a padding row attends none
+          const int2 mp = valid[u] ? p.rowmap[row0 + rr[u]] : make_int2(-1, -1);
+          c_lo[u] = mp.x >= 0 ? rr[u] - mp.y : 0;
+          c_hi[u] = mp.x >= 0 ? c_lo[u] + p.seqs[mp.x].len : 0;
+        } else {
+          c_lo[u] = valid[u] ? (rr[u] / p.L) * p.L : 0;
+          c_hi[u] = valid[u] ? c_lo[u] + p.L : 0;
+        }
       }
       float m[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
 #pragma unroll
@@ -797,10 +876,18 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, head = blockIdx.y;
-  const int nk = p.L / 128;                 // key tiles per sequence
   const int row0 = qt * 128;                // first token of this query tile
-  const int kt0 = (qt / nk) * nk;           // first tile of the sequence this query tile belongs to
-  const int qpos0 = (qt - kt0) * 128;       // position of the tile's first query inside its sequence
+  int nk = p.L / 128;                       // key tiles per sequence
+  int kt0 = (qt / nk) * nk;                 // first tile of the sequence this query tile belongs to
+  int qpos0 = (qt - kt0) * 128;             // position of the tile's first query inside its sequence
+  if (p.rowmap) {
+    // packed: the sequence starts on a tile boundary and the tile's first row is one of its tokens; the padding rows
+    // after its last token attend like its tokens (finite values nobody reads), its padding keys are masked by kmask
+    const int2 mp = p.rowmap[row0];
+    nk = (p.seqs[mp.x].len + 127) / 128;
+    qpos0 = mp.y;
+    kt0 = qt - mp.y / 128;
+  }
 
   if (tid == 0) {
     tma_prefetch_desc(&tmQK);
@@ -930,6 +1017,35 @@ __global__ void pool_kernel(const float* hidden, const int64_t* mask, int L, int
   }
 }
 
+// packed layout: pooled[out, :] = hidden[row0, :]  or  the mean of the sequence's len rows.  One block per sequence.
+__global__ void pool_packed_kernel(const float* hidden, const PackedSeq* seqs, int H, int mean, float* pooled) {
+  const PackedSeq s = seqs[blockIdx.x];
+  const float* src = hidden + static_cast<int64_t>(s.row0) * H;
+  float* dst = pooled + static_cast<int64_t>(s.out) * H;
+  if (!mean) {
+    for (int c = threadIdx.x; c < H; c += blockDim.x) dst[c] = src[c];
+    return;
+  }
+  const float denom = static_cast<float>(s.len);
+  for (int c = threadIdx.x; c < H; c += blockDim.x) {
+    float acc = 0.f;
+    for (int l = 0; l < s.len; ++l) acc += src[static_cast<int64_t>(l) * H + c];
+    dst[c] = acc / denom;
+  }
+}
+
+// packed layout: out[tok0 + pos, :] = hidden[row, :] for every real row (padding rows are dropped).  One warp per row.
+__global__ void __launch_bounds__(128) gather_packed_rows_kernel(const float* hidden, const int2* rowmap,
+                                                                 const PackedSeq* seqs, int T, int H, float* out) {
+  const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= T) return;
+  const int2 m = rowmap[row];
+  if (m.x < 0) return;
+  const float* src = hidden + static_cast<int64_t>(row) * H;
+  float* dst = out + (seqs[m.x].tok0 + m.y) * H;  // the caller's buffer: 4-byte alignment is all it promises
+  for (int c = lane; c < H; c += 32) dst[c] = src[c];
+}
+
 // out[b, o] = sum_i in[b, i] * W[o, i]  (bias-free LinearHead).  One warp per (o, group of 8 rows).
 __global__ void __launch_bounds__(256) head_kernel(const float* in, const float* W, int B, int Hin, int Hout, float* out) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -1031,6 +1147,11 @@ struct om_encoder {
   float *h = nullptr, *kmask = nullptr, *pooled = nullptr, *headed = nullptr;
   __nv_bfloat16 *xb = nullptr, *qk = nullptr, *vt = nullptr, *ctx = nullptr, *inter = nullptr;
   float* stats[2] = {nullptr, nullptr};  // [Tmax, kStatParts, 2] row statistics of the residual stream (ping-pong)
+  // packed calls: the sequence table of one chunk (device, and its pinned staging copy) and the row map of one row group
+  PackedSeq* pk_seqs = nullptr;     // [Tmax]
+  PackedSeq* pk_host = nullptr;     // [Tmax], pinned host memory
+  cudaEvent_t pk_copied = nullptr;  // recorded after the last upload from pk_host
+  int2* rowmap = nullptr;           // [Tmax]
   std::vector<void*> allocs;
 };
 
@@ -1087,6 +1208,187 @@ bool shape_is(const int64_t* shape, int ndim, int64_t a, int64_t b = -1) {
 }
 
 int bad_shape(const char* name) { return fail(OM_EINVAL, "om_encoder_set_weight: unexpected shape for '%s'", name); }
+
+// The layers and the final normalisation over T token rows whose embedding (e->h, e->xb, e->stats[0]) and key mask
+// (e->kmask) are in place.  Attention: tiles [0, n_long) run attn_long_kernel with ap_long, the next n_short tiles
+// attn_kernel with ap_short (tile0 = n_long); ap_short.Tvalid_rows is the tile-local V^T layout of EpiQKV.
+int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, const AttnParams& ap_short, int n_short,
+                  int sms, cudaStream_t st) {
+  const om_encoder_desc& d = e->d;
+  const int H = d.hidden, I = e->I, F = d.ffn;
+  const bool bert = d.arch == OM_ARCH_BERT;
+  const int rows4 = (T + 3) / 4;
+  const int n_tiles = n_long + n_short;
+  CUtensorMap tmQK, tmVt;
+  if (make_tmap_bf16_2d(&tmQK, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 128) != 0 ||
+      make_tmap_bf16_2d(&tmVt, e->vt, (uint64_t)n_tiles * 128, (uint64_t)I, (uint64_t)e->Tld * 2, 64, 64) != 0)
+    return fail(OM_ECUDA, "om_encode: tensor map creation failed");
+
+  // TMA-store tensor maps of the bf16 GEMM outputs (box = 64 columns x 32 rows = one epilogue warp's chunk pair) and the
+  // residual stream's maps (fp32 load + store, bf16 store; box = 32 columns x 32 rows = one chunk)
+  CUtensorMap tmQKout, tmInter, tmS, tmXb;
+  if (make_tmap_bf16_2d(&tmQKout, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 32) != 0 ||
+      make_tmap_bf16_2d(&tmInter, e->inter, (uint64_t)F, (uint64_t)T, (uint64_t)F * 2, 64, 32) != 0 ||
+      make_tmap_2d(&tmS, e->h, 4, (uint64_t)H, (uint64_t)T, (uint64_t)H * 4, 32, 32, 128) != 0 ||
+      make_tmap_2d(&tmXb, e->xb, 2, (uint64_t)H, (uint64_t)T, (uint64_t)H * 2, 32, 32, 64) != 0)
+    return fail(OM_ECUDA, "om_encode: output tensor map creation failed");
+  const float inv_h = 1.0f / static_cast<float>(H);
+  const int rms = bert ? 0 : 1;
+  const RowNorm normA{e->stats[0], inv_h, d.ln_eps, rms}, normB{e->stats[1], inv_h, d.ln_eps, rms};
+  const RowNorm ident{nullptr, inv_h, d.ln_eps, rms};
+  // 128 x 128 tiles, 3-stage ring: the staged fp32 accumulator tile (66 KB) and the functors' shared memory leave room for
+  // three 32 KB stages within the 227 KB an H100 block may use.  8 epilogue warps = 2 column groups per tile ->
+  // (H / 128) * 2 <= kStatParts statistics slots for the residual GEMMs.
+  auto wide_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, int M, int N, const auto& epi) -> cudaError_t {
+    return launch_gemm<128, 3, false>(A, K, W, K, M, N, K, epi, sms, st);
+  };
+  auto resid_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, const EpiResidNorm& epi) -> cudaError_t {
+    return launch_gemm<128, 3, false>(A, K, W, K, T, H, K, epi, sms, st);
+  };
+  if (((H + 127) / 128) * 2 > kStatParts)
+    return fail(OM_EINVAL, "om_encode: hidden=%d needs more statistics slots than kStatParts", H);
+  for (int li = 0; li < d.layers; ++li) {
+    const LayerW& w = e->layers[li];
+    NvtxRange nvtx_layer("om.encode.layer");
+    // LayerNorm that produced this layer's input (BERT; applied on the fly wherever the input is consumed)
+    const float* g_in = bert ? (li == 0 ? e->emb_g : e->layers[li - 1].ln2_g) : nullptr;
+    const float* b_in = bert ? (li == 0 ? e->emb_b : e->layers[li - 1].ln2_b) : nullptr;
+    {
+      EpiQKV epi{tmQKout, e->qk, e->vt, e->Tld, bert ? w.bqkv_fold : nullptr, T, 2 * I, ap_short.Tvalid_rows, normA};
+      cudaError_t err = wide_gemm(e->xb, H, w.wqkv, T, 3 * I, epi);
+      if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
+    }
+    if (n_long > 0) attn_long_kernel<<<dim3(n_long, d.heads), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
+    if (n_short > 0)
+      attn_kernel<<<std::min(n_short * d.heads, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short,
+                                                                                                n_short, d.heads);
+    OM_CUDA(cudaGetLastError());
+    {
+      // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
+      EpiResidNorm epi{tmS, tmXb, bert ? w.bo : nullptr, bert ? normA : ident, g_in, b_in, e->stats[1], 2, T, H, 128};
+      cudaError_t err = resid_gemm(e->ctx, I, w.wo, epi);
+      if (err != cudaSuccess) return fail(OM_ECUDA, "O-proj GEMM launch failed: %s", cudaGetErrorString(err));
+    }
+    {
+      cudaError_t err;
+      if (bert) {
+        EpiBiasActBf16<ACT_GELU> epi{tmInter, e->inter, F, w.b1_fold, T, F, normB};
+        err = wide_gemm(e->xb, H, w.w1, T, F, epi);
+      } else {
+        EpiBiasActBf16<ACT_RELU> epi{tmInter, e->inter, F, nullptr, T, F, normB};
+        err = wide_gemm(e->xb, H, w.w1, T, F, epi);
+      }
+      if (err != cudaSuccess) return fail(OM_ECUDA, "FFN1 GEMM launch failed: %s", cudaGetErrorString(err));
+    }
+    {
+      // s <- inter W2^T + b2 + LN_attn(s) (BERT) / + s (T5); statistics -> stats[0] (the next layer's input)
+      EpiResidNorm epi{tmS, tmXb, bert ? w.b2 : nullptr, bert ? normB : ident, w.ln1_g, w.ln1_b, e->stats[0], 2, T, H, 128};
+      cudaError_t err = resid_gemm(e->inter, F, w.w2, epi);
+      if (err != cudaSuccess) return fail(OM_ECUDA, "FFN2 GEMM launch failed: %s", cudaGetErrorString(err));
+    }
+  }
+  // the one normalisation that runs as a kernel: last_hidden_state = LN_out(s) (BERT: last layer's output.LayerNorm,
+  // T5: final_layer_norm), in place in e->h, for pooling and the optional out_hidden copy
+  if (bert)
+    norm_kernel<false><<<rows4, 128, 0, st>>>(e->h, e->layers[d.layers - 1].ln2_g, e->layers[d.layers - 1].ln2_b,
+                                              d.ln_eps, T, H, e->h);
+  else
+    norm_kernel<true><<<rows4, 128, 0, st>>>(e->h, e->final_g, nullptr, d.ln_eps, T, H, e->h);
+  OM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// pooled [B, hidden] (e->pooled) -> optional head -> optional normalise -> out_reps rows [B, rep_dim] at out_row_stride
+int finish_reps(om_encoder* e, int B, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, cudaStream_t st) {
+  const om_encoder_desc& d = e->d;
+  const int H = d.hidden, rep_dim = om_encoder_rep_dim(e);
+  const float* reps = e->pooled;
+  if (d.has_head) {
+    const int warps = d.head_out * ((B + 7) / 8);
+    head_kernel<<<(warps * 32 + 255) / 256, 256, 0, st>>>(e->pooled, e->head_w, B, H, d.head_out, e->headed);
+    reps = e->headed;
+  }
+  if (out_dtype == OM_F32)
+    finish_reps_kernel<float><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<float*>(out_reps),
+                                                          out_row_stride);
+  else if (out_dtype == OM_BF16)
+    finish_reps_kernel<__nv_bfloat16><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize,
+                                                                  static_cast<__nv_bfloat16*>(out_reps), out_row_stride);
+  else
+    finish_reps_kernel<__half><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<__half*>(out_reps),
+                                                           out_row_stride);
+  OM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Placement of the n sequences of one packed chunk (lengths len[0..n), token offsets tok0[0..n), each length <= Tmax):
+//   * a sequence of more than 128 tokens starts on a tile boundary and takes ceil(l / 128) tiles, in input order;
+//   * the others are bin-packed whole into tiles of min(128, Tmax) rows, first-fit decreasing (ties by input index:
+//     placement is a deterministic function of the lengths), each bin's sequences back to back in insertion order;
+//   * layout = the long sequences' tiles, then the bins; cut into row groups of at most Tmax rows at unit (sequence /
+//     bin) boundaries, each group encoded on its own (its long tiles come first).  The last unit of a group is counted
+//     up to its last token.
+// seqs receives the table in layout order (row0 relative to its group, out = index in the chunk).
+struct PackedGroup {
+  int k0, k1;     // sequences [k0, k1) of the table
+  int T;          // layout rows of the group
+  int n_long;     // tiles of long sequences (the first tiles of the group)
+  int n_tiles;
+};
+
+void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std::vector<PackedSeq>& seqs,
+                  std::vector<PackedGroup>& groups) {
+  seqs.clear();
+  groups.clear();
+  const int cap = std::min(kMaxL, Tmax);
+  std::vector<int> longs, shorts;
+  for (int i = 0; i < n; ++i) (len[i] > kMaxL ? longs : shorts).push_back(i);
+  std::stable_sort(shorts.begin(), shorts.end(), [&](int a, int b) { return len[a] > len[b]; });
+  std::vector<std::vector<int>> bins;
+  std::vector<int> fill;
+  std::vector<std::set<int>> by_room(cap + 1);  // open bins by free rows
+  for (int i : shorts) {
+    int best = -1;  // first fit: the lowest-numbered bin with room
+    for (int r = len[i]; r <= cap; ++r)
+      if (!by_room[r].empty() && (best < 0 || *by_room[r].begin() < best)) best = *by_room[r].begin();
+    if (best < 0) {
+      best = static_cast<int>(bins.size());
+      bins.emplace_back();
+      fill.push_back(0);
+    } else {
+      by_room[cap - fill[best]].erase(best);
+    }
+    bins[best].push_back(i);
+    fill[best] += len[i];
+    by_room[cap - fill[best]].insert(best);
+  }
+  PackedGroup g{0, 0, 0, 0, 0};
+  int row = 0;  // group-local first row of the next unit (a tile boundary)
+  auto unit = [&](const std::vector<int>& members, int tiles, int used, bool is_long) {
+    if (row > 0 && row + (tiles - 1) * 128 + used > Tmax) {
+      g.k1 = static_cast<int>(seqs.size());
+      groups.push_back(g);
+      g = PackedGroup{g.k1, g.k1, 0, 0, 0};
+      row = 0;
+    }
+    int off = 0;
+    for (int i : members) {
+      seqs.push_back(PackedSeq{row + off, len[i], i, 0, tok0[i]});
+      off += len[i];
+    }
+    g.T = row + (tiles - 1) * 128 + used;
+    g.n_long += is_long ? tiles : 0;
+    g.n_tiles += tiles;
+    row += tiles * 128;
+  };
+  for (int i : longs) {
+    const int tiles = (len[i] + 127) / 128;
+    unit(std::vector<int>{i}, tiles, len[i] - (tiles - 1) * 128, true);
+  }
+  for (size_t b = 0; b < bins.size(); ++b) unit(bins[b], 1, fill[b], false);
+  g.k1 = static_cast<int>(seqs.size());
+  if (g.k1 > g.k0) groups.push_back(g);
+}
 
 }  // namespace
 
@@ -1198,6 +1500,13 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   A(&e->stats[1], T * 2 * kStatParts);
   A(&e->pooled, T * H);  // at most Tmax sequences (L >= 1)
   A(&e->headed, (size_t)e->Tmax * std::max(d.head_out, 1));
+  A(&e->pk_seqs, T);
+  A(&e->rowmap, T);
+  if (rc == 0 && (cudaHostAlloc(&e->pk_host, T * sizeof(PackedSeq), cudaHostAllocDefault) != cudaSuccess ||
+                  cudaEventCreateWithFlags(&e->pk_copied, cudaEventDisableTiming) != cudaSuccess)) {
+    cudaGetLastError();
+    rc = fail(OM_ENOMEM, "om_encoder_create: out of pinned host memory");
+  }
   if (rc != 0) {
     om_encoder_destroy(e);
     return rc;
@@ -1220,6 +1529,8 @@ void om_encoder_destroy(om_encoder* e) {
     cudaFree(w.wqkv_f32);
     cudaFree(w.w1_f32);
   }
+  if (e->pk_host) cudaFreeHost(e->pk_host);
+  if (e->pk_copied) cudaEventDestroy(e->pk_copied);
   delete e;
 }
 
@@ -1432,7 +1743,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int T = static_cast<int>(T64), H = d.hidden, I = e->I, F = d.ffn;
+  const int T = static_cast<int>(T64), H = d.hidden, I = e->I;
   const bool bert = d.arch == OM_ARCH_BERT;
   const int rows4 = (T + 3) / 4;
 
@@ -1442,9 +1753,9 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   // e->stats[0] (input of a layer: from the embedding or the previous FFN2) / e->stats[1] (after the attention block)
   if (bert)
     bert_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
-                                             std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0]);
+                                             std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr);
   else
-    t5_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0]);
+    t5_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], nullptr, nullptr);
   OM_CUDA(cudaGetLastError());
 
   // attention geometry
@@ -1459,104 +1770,95 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   ap.kmask = e->kmask;
   ap.relbias_log2 = bert ? nullptr : (long_seq ? e->relbias_long_log2 : e->relbias_log2);
   ap.ctx = e->ctx;
+  ap.rowmap = nullptr;
+  ap.seqs = nullptr;
+  ap.tile0 = 0;
   const int n_tiles = long_seq ? T / 128 : (B + spt - 1) / spt;
-  CUtensorMap tmQK, tmVt;
-  if (make_tmap_bf16_2d(&tmQK, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 128) != 0 ||
-      make_tmap_bf16_2d(&tmVt, e->vt, (uint64_t)n_tiles * 128, (uint64_t)I, (uint64_t)e->Tld * 2, 64, 64) != 0)
-    return fail(OM_ECUDA, "om_encode: tensor map creation failed");
-
-  // TMA-store tensor maps of the bf16 GEMM outputs (box = 64 columns x 32 rows = one epilogue warp's chunk pair) and the
-  // residual stream's maps (fp32 load + store, bf16 store; box = 32 columns x 32 rows = one chunk)
-  CUtensorMap tmQKout, tmInter, tmS, tmXb;
-  if (make_tmap_bf16_2d(&tmQKout, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 32) != 0 ||
-      make_tmap_bf16_2d(&tmInter, e->inter, (uint64_t)F, (uint64_t)T, (uint64_t)F * 2, 64, 32) != 0 ||
-      make_tmap_2d(&tmS, e->h, 4, (uint64_t)H, (uint64_t)T, (uint64_t)H * 4, 32, 32, 128) != 0 ||
-      make_tmap_2d(&tmXb, e->xb, 2, (uint64_t)H, (uint64_t)T, (uint64_t)H * 2, 32, 32, 64) != 0)
-    return fail(OM_ECUDA, "om_encode: output tensor map creation failed");
-  const float inv_h = 1.0f / static_cast<float>(H);
-  const int rms = bert ? 0 : 1;
-  const RowNorm normA{e->stats[0], inv_h, d.ln_eps, rms}, normB{e->stats[1], inv_h, d.ln_eps, rms};
-  const RowNorm ident{nullptr, inv_h, d.ln_eps, rms};
-  // 128 x 128 tiles, 3-stage ring: the staged fp32 accumulator tile (66 KB) and the functors' shared memory leave room for
-  // three 32 KB stages within the 227 KB an H100 block may use.  8 epilogue warps = 2 column groups per tile ->
-  // (H / 128) * 2 <= kStatParts statistics slots for the residual GEMMs.
-  auto wide_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, int M, int N, const auto& epi) -> cudaError_t {
-    return launch_gemm<128, 3, false>(A, K, W, K, M, N, K, epi, sms, st);
-  };
-  auto resid_gemm = [&](const __nv_bfloat16* A, int K, const __nv_bfloat16* W, const EpiResidNorm& epi) -> cudaError_t {
-    return launch_gemm<128, 3, false>(A, K, W, K, T, H, K, epi, sms, st);
-  };
-  if (((H + 127) / 128) * 2 > kStatParts)
-    return fail(OM_EINVAL, "om_encode: hidden=%d needs more statistics slots than kStatParts", H);
-  for (int li = 0; li < d.layers; ++li) {
-    const LayerW& w = e->layers[li];
-    NvtxRange nvtx_layer("om.encode.layer");
-    // LayerNorm that produced this layer's input (BERT; applied on the fly wherever the input is consumed)
-    const float* g_in = bert ? (li == 0 ? e->emb_g : e->layers[li - 1].ln2_g) : nullptr;
-    const float* b_in = bert ? (li == 0 ? e->emb_b : e->layers[li - 1].ln2_b) : nullptr;
-    {
-      EpiQKV epi{tmQKout, e->qk, e->vt, e->Tld, bert ? w.bqkv_fold : nullptr, T, 2 * I, ap.Tvalid_rows, normA};
-      cudaError_t err = wide_gemm(e->xb, H, w.wqkv, T, 3 * I, epi);
-      if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
-    }
-    if (long_seq)
-      attn_long_kernel<<<dim3(n_tiles, d.heads), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap);
-    else
-      attn_kernel<<<std::min(n_tiles * d.heads, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap, n_tiles, d.heads);
-    OM_CUDA(cudaGetLastError());
-    {
-      // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
-      EpiResidNorm epi{tmS, tmXb, bert ? w.bo : nullptr, bert ? normA : ident, g_in, b_in, e->stats[1], 2, T, H, 128};
-      cudaError_t err = resid_gemm(e->ctx, I, w.wo, epi);
-      if (err != cudaSuccess) return fail(OM_ECUDA, "O-proj GEMM launch failed: %s", cudaGetErrorString(err));
-    }
-    {
-      cudaError_t err;
-      if (bert) {
-        EpiBiasActBf16<ACT_GELU> epi{tmInter, e->inter, F, w.b1_fold, T, F, normB};
-        err = wide_gemm(e->xb, H, w.w1, T, F, epi);
-      } else {
-        EpiBiasActBf16<ACT_RELU> epi{tmInter, e->inter, F, nullptr, T, F, normB};
-        err = wide_gemm(e->xb, H, w.w1, T, F, epi);
-      }
-      if (err != cudaSuccess) return fail(OM_ECUDA, "FFN1 GEMM launch failed: %s", cudaGetErrorString(err));
-    }
-    {
-      // s <- inter W2^T + b2 + LN_attn(s) (BERT) / + s (T5); statistics -> stats[0] (the next layer's input)
-      EpiResidNorm epi{tmS, tmXb, bert ? w.b2 : nullptr, bert ? normB : ident, w.ln1_g, w.ln1_b, e->stats[0], 2, T, H, 128};
-      cudaError_t err = resid_gemm(e->inter, F, w.w2, epi);
-      if (err != cudaSuccess) return fail(OM_ECUDA, "FFN2 GEMM launch failed: %s", cudaGetErrorString(err));
-    }
-  }
-  // the one normalisation that runs as a kernel: last_hidden_state = LN_out(s) (BERT: last layer's output.LayerNorm,
-  // T5: final_layer_norm), in place in e->h, for pooling and the optional out_hidden copy
-  if (bert)
-    norm_kernel<false><<<rows4, 128, 0, st>>>(e->h, e->layers[d.layers - 1].ln2_g, e->layers[d.layers - 1].ln2_b,
-                                              d.ln_eps, T, H, e->h);
-  else
-    norm_kernel<true><<<rows4, 128, 0, st>>>(e->h, e->final_g, nullptr, d.ln_eps, T, H, e->h);
-  OM_CUDA(cudaGetLastError());
+  OM_TRY(encode_layers(e, T, ap, long_seq ? n_tiles : 0, ap, long_seq ? 0 : n_tiles, sms, st));
   if (out_hidden)
     OM_CUDA(cudaMemcpyAsync(out_hidden, e->h, static_cast<size_t>(T) * H * 4, cudaMemcpyDeviceToDevice, st));
 
   NvtxRange nvtx_pool("om.encode.pool_head_normalize");
   pool_kernel<<<B, 256, 0, st>>>(e->h, attention_mask, L, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
-  const float* reps = e->pooled;
-  if (d.has_head) {
-    const int warps = d.head_out * ((B + 7) / 8);
-    head_kernel<<<(warps * 32 + 255) / 256, 256, 0, st>>>(e->pooled, e->head_w, B, H, d.head_out, e->headed);
-    reps = e->headed;
+  return finish_reps(e, B, out_reps, out_dtype, out_row_stride, st);
+}
+
+int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens, int B,
+                     void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream) {
+  if (!e || !tokens || !seqlens || !out_reps) return fail(OM_EINVAL, "om_encode_packed: null argument");
+  if (!e->finalized) return fail(OM_ESTATE, "om_encode_packed: call om_encoder_finalize first");
+  if (B < 0) return fail(OM_EINVAL, "om_encode_packed: B=%d is negative", B);
+  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
+    return fail(OM_EINVAL, "om_encode_packed: out dtype must be f32, bf16 or f16");
+  const int rep_dim = om_encoder_rep_dim(e);
+  if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_packed: out_row_stride < rep_dim");
+  const om_encoder_desc& d = e->d;
+  const bool bert = d.arch == OM_ARCH_BERT;
+  const int max_len = std::min(kMaxLongL, std::min(bert ? d.max_pos : kMaxLongL, e->Tmax));
+  std::vector<int64_t> tok0(static_cast<size_t>(B));
+  int64_t total = 0;
+  for (int i = 0; i < B; ++i) {
+    const int l = seqlens[i];
+    if (l < 1 || l > max_len)
+      return fail(OM_EINVAL, "om_encode_packed: seqlens[%d]=%d outside [1, %d] (512 tokens%s, max_batch_tokens=%d)", i, l,
+                  max_len, bert ? ", max_position_embeddings" : "", e->Tmax);
+    tok0[i] = total;
+    total += l;
   }
-  if (out_dtype == OM_F32)
-    finish_reps_kernel<float><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<float*>(out_reps),
-                                                          out_row_stride);
-  else if (out_dtype == OM_BF16)
-    finish_reps_kernel<__nv_bfloat16><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize,
-                                                                  static_cast<__nv_bfloat16*>(out_reps), out_row_stride);
-  else
-    finish_reps_kernel<__half><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<__half*>(out_reps),
-                                                           out_row_stride);
-  OM_CUDA(cudaGetLastError());
+  if (B == 0) return 0;
+  const int sms = device_sm_count();
+  if (sms < 0) return sms;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int H = d.hidden;
+  const size_t out_elem = out_dtype == OM_F32 ? 4 : 2;
+
+  NvtxRange nvtx("om.encode_packed");
+  AttnParams ap;
+  ap.L = 128;  // unused: every row's key range comes from the row map
+  ap.spt = 1;
+  ap.I = e->I;
+  ap.Tvalid_rows = 128;
+  ap.scale_log2 = (bert ? 0.125f : 1.0f) * kLog2e;
+  ap.kmask = e->kmask;
+  ap.ctx = e->ctx;
+  ap.rowmap = e->rowmap;
+  std::vector<PackedSeq> seqs;
+  std::vector<PackedGroup> groups;
+  // chunks of at most max_batch_tokens sequences (the pooled / head workspace rows); one chunk unless the batch holds
+  // more sequences than that
+  for (int c0 = 0; c0 < B; c0 += e->Tmax) {
+    const int n = std::min(B - c0, e->Tmax);
+    place_packed(seqlens + c0, tok0.data() + c0, n, e->Tmax, seqs, groups);
+    // upload the sequence table through the pinned staging buffer: wait (on the host) only until the previous upload
+    // from it has been read
+    OM_CUDA(cudaEventSynchronize(e->pk_copied));
+    memcpy(e->pk_host, seqs.data(), seqs.size() * sizeof(PackedSeq));
+    OM_CUDA(cudaMemcpyAsync(e->pk_seqs, e->pk_host, seqs.size() * sizeof(PackedSeq), cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaEventRecord(e->pk_copied, st));
+    for (const PackedGroup& g : groups) {
+      const PackedSeq* gs = e->pk_seqs + g.k0;
+      const int ns = g.k1 - g.k0, T = g.T, rows4 = (T + 3) / 4;
+      packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
+      if (bert)
+        bert_embed_kernel<<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H, d.vocab,
+                                                 std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], e->rowmap, gs);
+      else
+        t5_embed_kernel<<<rows4, 128, 0, st>>>(tokens, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], e->rowmap, gs);
+      OM_CUDA(cudaGetLastError());
+      ap.T = T;
+      ap.seqs = gs;
+      AttnParams ap_long = ap, ap_short = ap;
+      ap_long.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
+      ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
+      ap_short.tile0 = g.n_long;
+      OM_TRY(encode_layers(e, T, ap_long, g.n_long, ap_short, g.n_tiles - g.n_long, sms, st));
+      if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
+      pool_packed_kernel<<<ns, 256, 0, st>>>(e->h, gs, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
+      OM_CUDA(cudaGetLastError());
+    }
+    OM_TRY(finish_reps(e, n, static_cast<char*>(out_reps) + static_cast<size_t>(c0) * out_row_stride * out_elem, out_dtype,
+                       out_row_stride, st));
+  }
   return 0;
 }
 

@@ -24,6 +24,32 @@ def get_idx(obj) -> str:
     return str(example_id) if example_id is not None else None
 
 
+def _ragged_prefix(path: str):
+    """``<name>`` when ``path`` is ``<name>.tokens.npy`` next to ``<name>.offsets.npy`` (a ragged store), else None"""
+    if path.endswith(".tokens.npy") and os.path.exists(path[:-len(".tokens.npy")] + ".offsets.npy"):
+        return path[:-len(".tokens.npy")]
+    return None
+
+
+def write_ragged_store(prefix: str, ids_2d, names=None) -> str:
+    """Writes the rows of an int ``[n, L]`` id matrix (0 = padding, dropped) as a ragged store ``<prefix>.tokens.npy`` +
+    ``<prefix>.offsets.npy`` (+ ``<prefix>.ids.txt`` when ``names`` is given); returns the path to hand to
+    ``PretokenizedDataset`` (``data_args.corpus_path`` / ``query_path``).  Every row needs at least one token."""
+    ids_2d = np.asarray(ids_2d)
+    keep = ids_2d != 0
+    lens = keep.sum(1).astype(np.int64)
+    if ids_2d.shape[0] and lens.min() < 1:
+        raise ValueError("row %d holds no token" % int(np.argmin(lens)))
+    offsets = np.zeros(ids_2d.shape[0] + 1, dtype=np.int64)
+    np.cumsum(lens, out=offsets[1:])
+    np.save(prefix + ".tokens.npy", ids_2d[keep].astype(np.int32))
+    np.save(prefix + ".offsets.npy", offsets)
+    if names is not None:
+        with open(prefix + ".ids.txt", "w") as f:
+            f.write("\n".join(str(x) for x in names))
+    return prefix + ".tokens.npy"
+
+
 class InferenceDataset(IterableDataset):
     def __init__(self, tokenizer, data_args: DataArguments, is_query: bool = False, final: bool = True,
                  stream: bool = True, batch_size: int = 1, num_processes: int = 1, process_index: int = 0,
@@ -100,37 +126,73 @@ class PretokenizedDataset(InferenceDataset):
     Two ways out: the reference's per-example iterator (``__iter__`` -> DataLoader + DRInferenceCollator, same
     interleaving of ``batch_size`` blocks over the ranks, :99-115), and ``iter_batches()``, which hands whole
     ``[B, L]`` int32 slices of the memory map to ``Retriever`` (one memcpy into a pinned buffer per batch, no
-    per-row Python objects) — the ingest path that can feed the encoder at tens of thousands of passages/s."""
+    per-row Python objects) — the ingest path that can feed the encoder at tens of thousands of passages/s.
+
+    A ragged store (``write_ragged_store``) holds the same rows without padding: ``<name>.tokens.npy`` (int32, the rows
+    back to back) and ``<name>.offsets.npy`` (int64 ``[n + 1]``, row i = ``tokens[offsets[i]:offsets[i + 1]]``), with
+    the same optional ``<name>.ids.txt``; its path is ``<name>.tokens.npy``.  ``iter_batches()`` then yields
+    ``(text_ids, tokens int32 [sum(seqlens)], seqlens int32 [b])`` (rows truncated to ``max_len``) for
+    ``DRModel.encode_packed_into``, and ``__iter__`` yields padded examples as for the padded store."""
+
+    @property
+    def is_ragged(self) -> bool:
+        return _ragged_prefix(self.data_files[0]) is not None
 
     def _open(self):
-        ids = np.load(self.data_files[0], mmap_mode="r")
-        if ids.ndim != 2 or ids.dtype != np.int32:
-            raise ValueError("%s: expected an int32 [n, L] array, got %s %s" % (self.data_files[0], ids.dtype, ids.shape))
-        names_path = os.path.splitext(self.data_files[0])[0] + ".ids.txt"
+        prefix = _ragged_prefix(self.data_files[0])
+        if prefix is not None:
+            tokens = np.load(prefix + ".tokens.npy", mmap_mode="r")
+            offsets = np.load(prefix + ".offsets.npy")
+            if tokens.ndim != 1 or tokens.dtype != np.int32 or offsets.ndim != 1 or offsets.dtype != np.int64 \
+                    or offsets.shape[0] < 1 or offsets[0] != 0 or offsets[-1] != tokens.shape[0] \
+                    or (np.diff(offsets) < 0).any():
+                raise ValueError("%s: expected int32 tokens [T] and int64 offsets [n + 1] from 0 to T" % prefix)
+            rows, n, names_path = (tokens, offsets), offsets.shape[0] - 1, prefix + ".ids.txt"
+        else:
+            rows = np.load(self.data_files[0], mmap_mode="r")
+            if rows.ndim != 2 or rows.dtype != np.int32:
+                raise ValueError("%s: expected an int32 [n, L] array, got %s %s" % (self.data_files[0], rows.dtype,
+                                                                                   rows.shape))
+            n, names_path = rows.shape[0], os.path.splitext(self.data_files[0])[0] + ".ids.txt"
         names = None
         if os.path.exists(names_path):
             with open(names_path) as f:
                 names = f.read().split("\n")
-            if len(names) < ids.shape[0]:
-                raise ValueError("%s holds %d ids for %d rows" % (names_path, len(names), ids.shape[0]))
-        return ids, names
+            if len(names) < n:
+                raise ValueError("%s holds %d ids for %d rows" % (names_path, len(names), n))
+        return rows, names
+
+    def _num_rows(self) -> int:
+        prefix = _ragged_prefix(self.data_files[0])
+        if prefix is not None:
+            return np.load(prefix + ".offsets.npy", mmap_mode="r").shape[0] - 1
+        return np.load(self.data_files[0], mmap_mode="r").shape[0]
 
     def _records(self):
-        ids, names = self._open()
-        for i in range(ids.shape[0]):
-            yield {"id": names[i] if names else str(i), "row": ids[i]}
+        rows, names = self._open()
+        if isinstance(rows, tuple):
+            tokens, offsets = rows
+            for i in range(offsets.shape[0] - 1):
+                yield {"id": names[i] if names else str(i), "row": tokens[offsets[i]:offsets[i + 1]]}
+            return
+        for i in range(rows.shape[0]):
+            yield {"id": names[i] if names else str(i), "row": rows[i]}
 
     def num_local_rows(self) -> int:
         """rows this rank will see (blocks ``process_index, process_index + W, ...`` of ``batch_size`` rows)"""
-        n = np.load(self.data_files[0], mmap_mode="r").shape[0]
+        n = self._num_rows()
         bs, W, r = self.batch_size, self.num_processes, self.process_index
         full, rest = divmod(n, bs * W)
         return full * bs + max(0, min(bs, rest - r * bs))
 
     def iter_batches(self):
         """Yields ``(text_ids: list[str], ids: int32 [b, max_len] C-contiguous view or padded copy)`` for this rank's
-        blocks, in the order ``__iter__`` would produce the same examples."""
+        blocks, in the order ``__iter__`` would produce the same examples.  A ragged store yields
+        ``(text_ids, tokens, seqlens)`` instead (see the class docstring)."""
         ids, names = self._open()
+        if isinstance(ids, tuple):
+            yield from self._iter_ragged_batches(*ids, names)
+            return
         n, width = ids.shape
         bs, W, r = self.batch_size, self.num_processes, self.process_index
         for b0 in range(r * bs, n, W * bs):
@@ -141,6 +203,22 @@ class PretokenizedDataset(InferenceDataset):
                 padded[:, :width] = block
                 block = padded
             yield (names[b0:b1] if names else [str(i) for i in range(b0, b1)]), block
+
+    def _iter_ragged_batches(self, tokens, offsets, names):
+        n = offsets.shape[0] - 1
+        bs, W, r = self.batch_size, self.num_processes, self.process_index
+        for b0 in range(r * bs, n, W * bs):
+            b1 = min(n, b0 + bs)
+            starts = offsets[b0:b1]
+            lens = np.minimum(offsets[b0 + 1:b1 + 1] - starts, self.max_len)
+            if (lens < 1).any():
+                raise ValueError("%s: row %d is empty" % (self.data_files[0], b0 + int(np.argmin(lens))))
+            if (lens == offsets[b0 + 1:b1 + 1] - starts).all():  # nothing truncated: one contiguous slice
+                block = tokens[offsets[b0]:offsets[b1]]
+            else:
+                ends = np.cumsum(lens)
+                block = tokens[np.repeat(starts - (ends - lens), lens) + np.arange(int(ends[-1]))]
+            yield (names[b0:b1] if names else [str(i) for i in range(b0, b1)]), block, lens.astype(np.int32)
 
     def process_one(self, example):
         row = np.asarray(example["row"][: self.max_len], dtype=np.int64)

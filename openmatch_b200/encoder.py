@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes
 from typing import Dict, Optional
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -115,6 +116,37 @@ class CudaEncoder:
         hidden = torch.empty((B, L, self.hidden), dtype=torch.float32, device=ids.device) if return_hidden else None
         _lib.check(self._lib.om_encode(
             self._h, ids.data_ptr(), mask.data_ptr(), tt.data_ptr() if tt is not None else None, B, L,
+            out.data_ptr(), _OUT_DTYPES[out.dtype], out.stride(0),
+            hidden.data_ptr() if hidden is not None else None, _lib.current_stream_ptr()))
+        return (hidden, out) if return_hidden else out
+
+    @torch.no_grad()
+    def encode_packed(self, tokens: torch.Tensor, seqlens, token_type_ids: Optional[torch.Tensor] = None,
+                      out: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.float32,
+                      return_hidden: bool = False):
+        """Variable-length batch without padding: ``tokens`` int64 ``[T]`` CUDA tensor holding the sequences back to
+        back, ``seqlens`` their lengths (host int32 array / list / CPU tensor, each in [1, 512], sum = T) -> reps
+        ``[B, rep_dim]`` (and last_hidden_state fp32 ``[T, H]``, packed like ``tokens``).  The same representations
+        ``encode`` gives the sequences padded, up to the order of floating-point sums; ``out`` / ``out_dtype`` as there."""
+        if not tokens.is_cuda:
+            raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
+        if isinstance(seqlens, torch.Tensor):
+            seqlens = seqlens.detach().cpu().numpy()
+        lens = np.ascontiguousarray(np.asarray(seqlens).reshape(-1), dtype=np.int32)
+        B, T = int(lens.shape[0]), int(lens.sum(dtype=np.int64))
+        ids = tokens.reshape(-1).to(torch.int64).contiguous()
+        if ids.numel() != T:
+            raise ValueError("tokens holds %d ids, seqlens sum to %d" % (ids.numel(), T))
+        tt = token_type_ids.reshape(-1).to(torch.int64).contiguous() if token_type_ids is not None else None
+        if out is None:
+            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=ids.device)
+        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
+            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
+        if out.shape[0] != B or out.shape[1] != self.rep_dim:
+            raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
+        hidden = torch.empty((T, self.hidden), dtype=torch.float32, device=ids.device) if return_hidden else None
+        _lib.check(self._lib.om_encode_packed(
+            self._h, ids.data_ptr(), tt.data_ptr() if tt is not None else None, lens.ctypes.data, B,
             out.data_ptr(), _OUT_DTYPES[out.dtype], out.stride(0),
             hidden.data_ptr() if hidden is not None else None, _lib.current_stream_ptr()))
         return (hidden, out) if return_hidden else out

@@ -191,6 +191,21 @@ class DRModel(nn.Module):
             enc.encode(input_ids[sl], items["attention_mask"][sl], tt[sl] if tt is not None else None, out=out[sl])
         return out
 
+    @torch.no_grad()
+    def encode_packed_into(self, tokens: Tensor, seqlens, out: Tensor, is_query: bool = False) -> Tensor:
+        """Inference only, like ``encode_into``, for a variable-length batch without padding: ``tokens`` int CUDA tensor
+        ``[sum(seqlens)]`` (the sequences back to back), ``seqlens`` host lengths (each in [1, 512]); the representations
+        go IN PLACE into ``out`` ``[len(seqlens), rep_dim]``.  Equal to ``encode_into`` of the same sequences padded, up
+        to the order of floating-point sums."""
+        model, head = (self.lm_q, self.head_q) if is_query else (self.lm_p, self.head_p)
+        if "T5" in type(model).__name__ and not (self.model_args is not None and self.model_args.encoder_only):
+            raise NotImplementedError("encode_packed_into: encoder-decoder T5 pooling is not on the CUDA encoder; "
+                                      "use --encoder_only or pad the batch")
+        if not tokens.is_cuda:
+            raise RuntimeError("openmatch_b200 encodes on a CUDA device only (no CPU path): move the batch to GPU")
+        self._cuda_encoder(model, head).encode_packed(tokens, seqlens, out=out)
+        return out
+
     def rep_dim(self, is_query: bool = False) -> int:
         """width of the representations ``encode`` produces (head output, else the backbone's hidden size)"""
         head = self.head_q if is_query else self.head_p

@@ -151,6 +151,8 @@ class Retriever:
     def _encode_blocks(self, dataset, is_query: bool, into_index: bool):
         """Block ingest: memory-mapped int32 ``[b, L]`` slice -> pinned staging buffer (double-buffered) -> async H2D
         -> int64 ids + mask built on the device -> encoder (-> index rows in place)."""
+        if getattr(dataset, "is_ragged", False) and hasattr(self.model, "encode_packed_into"):
+            return self._encode_ragged_blocks(dataset, is_query, into_index)
         device = self.args.device
         ids: List[str] = []
         chunks: List[torch.Tensor] = []
@@ -179,6 +181,40 @@ class Retriever:
             else:
                 out = torch.empty((n, dim), dtype=torch.float32, device=device)
                 self.model.encode_into(batch, out, is_query)
+                chunks.append(out)
+        return ids, chunks
+
+    def _encode_ragged_blocks(self, dataset, is_query: bool, into_index: bool):
+        """Block ingest of a ragged store: the block's tokens without padding -> pinned staging buffer (double-buffered)
+        -> async H2D -> ``encode_packed_into`` (-> index rows in place, fp32 or fp16 storage alike)."""
+        device = self.args.device
+        ids: List[str] = []
+        chunks: List[torch.Tensor] = []
+        stage = [torch.empty((dataset.batch_size * dataset.max_len,), dtype=torch.int32).pin_memory() for _ in range(2)]
+        busy = [None, None]
+        if into_index:
+            if self.index is None:
+                self._initialize_faiss_index(self.model.rep_dim(is_query))
+            self.index.reserve_rows(dataset.num_local_rows())  # capacity only: no re-allocation while encoding
+        dim = self.model.rep_dim(is_query)
+        for bi, (names, tokens, seqlens) in enumerate(tqdm(dataset.iter_batches(),
+                                                           disable=self.args.local_process_index > 0)):
+            slot = bi & 1
+            if busy[slot] is not None:
+                busy[slot].synchronize()  # the H2D copy that last read this pinned buffer has finished
+            n, t = seqlens.shape[0], tokens.shape[0]
+            np.copyto(stage[slot][:t].numpy(), tokens)
+            d_tokens = stage[slot][:t].to(device, non_blocking=True)
+            busy[slot] = torch.cuda.Event()
+            busy[slot].record()
+            ids.extend(names)
+            if into_index:
+                rows = self.index.reserve_rows(n)
+                self.model.encode_packed_into(d_tokens, seqlens, rows, is_query)
+                self.index.commit_rows(n)
+            else:
+                out = torch.empty((n, dim), dtype=torch.float32, device=device)
+                self.model.encode_packed_into(d_tokens, seqlens, out, is_query)
                 chunks.append(out)
         return ids, chunks
 
