@@ -61,8 +61,10 @@ int om_device_sm_count(void);
 typedef struct om_encoder_desc {
   int32_t arch;             /* om_arch */
   int32_t layers;           /* num_hidden_layers / num_layers */
-  int32_t hidden;           /* hidden_size / d_model (multiple of 64) */
-  int32_t heads;            /* attention heads; head width is fixed at 64 (bert-base/large, t5-base) */
+  int32_t hidden;           /* hidden_size / d_model (multiple of 128, at most 1024) */
+  int32_t heads;            /* attention heads.  Head width: BERT hidden / heads, 64 (bert-base/large) or 32 (MiniLM,
+                               bge-small, e5-small, gte-small); T5 d_kv = 64.  heads * width: a multiple of 128, at
+                               most 2048.  Any other width returns OM_EINVAL */
   int32_t ffn;              /* intermediate_size / d_ff (multiple of 64) */
   int32_t vocab;            /* vocab_size */
   int32_t max_pos;          /* max_position_embeddings (BERT); ignored for T5 */

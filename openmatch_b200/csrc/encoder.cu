@@ -3,16 +3,17 @@
 // -> 'first' / 'mean' pooling (:145-150, src/openmatch/utils.py:233-235) -> bias-free LinearHead
 // (src/openmatch/modeling/linear.py:19,22-23) -> F.normalize (:153-154).
 //
-// Per layer (T = B*L tokens, H hidden, I = heads*64 attention width, F ffn).  LayerNorm / RMSNorm never runs as a
-// kernel of its own: the residual stream is kept UN-normalised (s, fp32 + a bf16 copy) together with per-row (sum,
-// sum of squares); the normalisation is folded algebraically into the GEMM that consumes it,
+// Per layer (T = B*L tokens, H hidden, I = heads * head width (64; BERT also 32) attention width, F ffn).  LayerNorm /
+// RMSNorm never runs as a kernel of its own: the residual stream is kept UN-normalised (s, fp32 + a bf16 copy) together
+// with per-row (sum, sum of squares); the normalisation is folded algebraically into the GEMM that consumes it,
 //        LN(s) W^T = rstd * (s Wf^T) + (W beta + b),   Wf = W diag(gamma) with every row centred (sum_i Wf[j, i] = 0,
 //        which makes the "- rstd * mean * rowsum" term vanish; RMSNorm has no mean, rows stay as they are),
 // and into the residual read of the GEMM that produces the next s:
 //   QKV    wgmma GEMM [T,H]x[3I,H]^T on bf16(s) and the folded weights; epilogue: rstd[row] * acc + folded bias
 //          -> bf16 Q|K [T,2I] and V transposed [I, T]
-//   ATTN   one CTA per (128-row tile, head), one warpgroup, 64 query rows at a time: S = Q K^T (wgmma, registers) ->
-//          masked softmax on the accumulator fragments -> P (bf16, registers) -> O = P V (wgmma) -> ctx bf16 [T,I]
+//   ATTN   one CTA per (128-row tile, 64 columns of Q|K = one 64-wide head or two 32-wide heads), one warpgroup, 64
+//          query rows and one head at a time: S = Q K^T (wgmma, registers) -> masked softmax on the accumulator
+//          fragments -> P (bf16, registers) -> O = P V (wgmma) -> ctx bf16 [T,I]
 //   OPROJ  wgmma GEMM [T,I]x[H,I]^T, epilogue (EpiResidNorm): s' = acc + bias + LN(s) (BERT) / + s (T5), written in
 //          place as fp32 (TMA load + TMA store of the residual tile) and as bf16, row statistics of s' accumulated
 //   FFN1   wgmma GEMM [T,H]x[F,H]^T on bf16(s') and folded weights; epilogue: rstd[row] * acc + folded bias, GELU(erf) /
@@ -35,7 +36,7 @@
 
 namespace om {
 
-constexpr int kHeadDim = 64;
+constexpr int kAttnCols = 64;    // columns of Q, K and V^T an attention work item loads: one 64-wide or two 32-wide heads
 constexpr int kMaxL = 128;       // one attention tile; sequences of at most kMaxL tokens take attn_kernel
 constexpr int kMaxLongL = 512;   // longer sequences (multiples of 128 tokens) take attn_long_kernel
 constexpr float kLog2e = 1.4426950408889634f;
@@ -698,11 +699,13 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// S = Q_h K^T for the 64 query rows [64 h, +64) of the tile: 4 wgmma m64n128k16 (K = head dim 64)
+// S = Q_h K^T for the 64 query rows [64 h, +64) of the tile: DH / 16 wgmma m64n128k16 (K = head width DH); qa / ka
+// address the head's first column inside the 64-column Q / K boxes (a 32-wide head takes k-steps 0-1 or 2-3 of them)
+template <int DH>
 __device__ __forceinline__ void attn_scores(float (&s)[64], uint32_t qa, uint32_t ka) {
   wgmma_fence();
 #pragma unroll
-  for (int k = 0; k < 4; ++k)
+  for (int k = 0; k < DH / 16; ++k)
     wgmma_m64n128k16_bf16<0, 0>(s, wgmma_desc(qa + k * 32, kDescKMajorSW128), wgmma_desc(ka + k * 32, kDescKMajorSW128),
                                 k != 0 ? 1u : 0u);
   wgmma_commit();
@@ -710,8 +713,10 @@ __device__ __forceinline__ void attn_scores(float (&s)[64], uint32_t qa, uint32_
   wgmma_fence_regs(s);
 }
 // O (+)= P V for the same 64 rows: P from registers (the probabilities in s, packed to bf16 as the A fragment of each
-// 16-key step), V^T [64 dims, 128 keys] as two K-major boxes of 64 keys
-__device__ __forceinline__ void attn_pv(float (&o)[32], const float (&s)[64], uint32_t va, uint32_t accumulate) {
+// 16-key step), V^T [DH dims, 128 keys] as two K-major boxes of 64 keys; va addresses the head's first row in the first
+// box (the second 32-wide head of a box starts 32 rows = 4 whole 1024-byte swizzle atoms in)
+template <int DH>
+__device__ __forceinline__ void attn_pv(float (&o)[DH / 2], const float (&s)[64], uint32_t va, uint32_t accumulate) {
   uint32_t a[8][4];
 #pragma unroll
   for (int kk = 0; kk < 8; ++kk) {
@@ -722,9 +727,13 @@ __device__ __forceinline__ void attn_pv(float (&o)[32], const float (&s)[64], ui
   }
   wgmma_fence();
 #pragma unroll
-  for (int kk = 0; kk < 8; ++kk)
-    wgmma_m64n64k16_bf16_rs(o, a[kk], wgmma_desc(va + (kk >> 2) * 8192 + (kk & 3) * 32, kDescKMajorSW128),
-                            (accumulate | kk) != 0 ? 1u : 0u);
+  for (int kk = 0; kk < 8; ++kk) {
+    const uint64_t vd = wgmma_desc(va + (kk >> 2) * 8192 + (kk & 3) * 32, kDescKMajorSW128);
+    if constexpr (DH == 64)
+      wgmma_m64n64k16_bf16_rs(o, a[kk], vd, (accumulate | kk) != 0 ? 1u : 0u);
+    else
+      wgmma_m64n32k16_bf16_rs(o, a[kk], vd, (accumulate | kk) != 0 ? 1u : 0u);
+  }
   wgmma_commit();
   wgmma_wait<0>();
   wgmma_fence_regs(o);
@@ -740,9 +749,14 @@ __device__ __forceinline__ float quad_sum(float v) {
 
 // Fragment coordinates (see ptx.cuh): element 4 j + e of a thread's accumulator is row rr[e >> 1], column 8 j + 2 (lane % 4)
 // + (e & 1) of the 64-row block.
+// DH = head width (64, or 32 for BERT).  A work item is a (tile, unit of kAttnCols columns) pair: the unit holds
+// 64 / DH whole heads, so the boxes, the shared-memory layout and the work per item are those of one 64-wide head.
+// The relative position bias (T5) exists for 64-wide heads only.
+template <int DH>
 __global__ void __launch_bounds__(128, kAttnCtasPerSm)
 attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p, int n_tiles,
-            int n_heads) {
+            int n_units) {
+  constexpr int NH = kAttnCols / DH;  // heads per unit
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint32_t* s_kb = reinterpret_cast<uint32_t*>(smem + kAttnSmemMisc);
@@ -758,23 +772,23 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
     fence_barrier_init();
   }
   __syncthreads();
-  // Persistent CTA: work items are (tile, head) pairs taken head-fastest, so that the CTAs running at the same time read
+  // Persistent CTA: work items are (tile, unit) pairs taken unit-fastest, so that the CTAs running at the same time read
   // the same token rows of qk (neighbouring 128-byte slices of one DRAM page instead of one slice from each of many pages).
-  const int n_items = n_tiles * n_heads;
-  const bool has_rel = p.relbias_log2 != nullptr;
+  const int n_items = n_tiles * n_units;
+  const bool has_rel = DH == 64 && p.relbias_log2 != nullptr;
   const uint32_t qa = smem_u32(smem + kAttnSmemQ), ka = smem_u32(smem + kAttnSmemK), va = smem_u32(smem + kAttnSmemV);
   uint32_t par = 0;
 #pragma unroll 1
   for (int item = blockIdx.x; item < n_items; item += gridDim.x, par ^= 1u) {
-    const int t = item / n_heads, head = item - t * n_heads;
+    const int t = item / n_units, unit = item - t * n_units;
     const int tile = p.tile0 + t;
     const int row0 = tile * p.Tvalid_rows;  // first token of this tile
     if (tid == 0) {  // shared memory of the previous item is free (trailing barrier): loads go out first
       mbar_arrive_expect_tx(&bars[0], 3 * 16384);
-      tma_load_2d(smem + kAttnSmemQ, &tmQK, &bars[0], head * kHeadDim, row0);
-      tma_load_2d(smem + kAttnSmemK, &tmQK, &bars[0], p.I + head * kHeadDim, row0);
-      tma_load_2d(smem + kAttnSmemV, &tmVt, &bars[0], tile * 128, head * kHeadDim);
-      tma_load_2d(smem + kAttnSmemV + 8192, &tmVt, &bars[0], tile * 128 + 64, head * kHeadDim);
+      tma_load_2d(smem + kAttnSmemQ, &tmQK, &bars[0], unit * kAttnCols, row0);
+      tma_load_2d(smem + kAttnSmemK, &tmQK, &bars[0], p.I + unit * kAttnCols, row0);
+      tma_load_2d(smem + kAttnSmemV, &tmVt, &bars[0], tile * 128, unit * kAttnCols);
+      tma_load_2d(smem + kAttnSmemV + 8192, &tmVt, &bars[0], tile * 128 + 64, unit * kAttnCols);
     }
     {
       const int tok = row0 + tid;
@@ -783,16 +797,17 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
       const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
       if (lane == 0) s_kb[warp] = bits;
       if (has_rel) {
-        for (int i = tid; i < 2 * kMaxL - 1; i += 128) s_rel[i] = p.relbias_log2[head * (2 * kMaxL - 1) + i];
+        for (int i = tid; i < 2 * kMaxL - 1; i += 128) s_rel[i] = p.relbias_log2[unit * (2 * kMaxL - 1) + i];
       }
     }
     __syncthreads();  // key bits / relative bias of this item are in place
     mbar_wait_warp(&bars[0], par, 10);
 
 #pragma unroll 1
-    for (int h = 0; h < 2; ++h) {
+    for (int hh = 0; hh < 2 * NH; ++hh) {
+      const int h = hh / NH, hd = hh % NH;  // 64-row half of the tile, head of the unit
       float sc[64];
-      attn_scores(sc, qa + h * 8192, ka);
+      attn_scores<DH>(sc, qa + h * 8192 + hd * DH * 2, ka + hd * DH * 2);
       // ---- softmax on the fragments: this thread holds columns 8 j + 2 (lane % 4) + {0, 1} of two query rows ----
       int rr[2], c_lo[2], c_hi[2];
       bool valid[2];
@@ -837,16 +852,17 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
           sc[4 * j + e] = pv;
           sum[e >> 1] += pv;
         }
-      float o[32];
-      attn_pv(o, sc, va, 0u);
+      float o[DH / 2];
+      attn_pv<DH>(o, sc, va + hd * DH * 128, 0u);
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         const float tot = quad_sum(sum[u]);
         const float inv = tot > 0.f ? 1.0f / tot : 0.f;
         if (valid[u]) {
-          __nv_bfloat16* dst = p.ctx + static_cast<int64_t>(row0 + rr[u]) * p.I + head * kHeadDim + 2 * (lane & 3);
+          __nv_bfloat16* dst =
+              p.ctx + static_cast<int64_t>(row0 + rr[u]) * p.I + unit * kAttnCols + hd * DH + 2 * (lane & 3);
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
+          for (int j = 0; j < DH / 8; ++j)
             *reinterpret_cast<uint32_t*>(dst + 8 * j) = pack_bf16x2(o[4 * j + 2 * u] * inv, o[4 * j + 2 * u + 1] * inv);
         }
       }
@@ -857,7 +873,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Sequences longer than one tile (L = 256 / 384 / 512, multiples of 128): one CTA per (128-row query tile, head)
+// Sequences longer than one tile (L = 256 / 384 / 512, multiples of 128): one CTA per (128-row query tile, unit)
 // loops over the sequence's 128-key tiles with an online softmax, 64 query rows at a time:  S_j = Q K_j^T (wgmma) ->
 // running max / sum per row on the fragments -> P_j (bf16, registers) -> O = O * alpha + P_j V_j (wgmma, accumulating in
 // registers).  Q stays in smem; K_j / V_j are re-loaded by TMA per iteration.
@@ -866,8 +882,11 @@ constexpr int kAttnLongSmemQ = 0, kAttnLongSmemK = 16384, kAttnLongSmemV = 32768
 constexpr int kAttnLongSmemMisc = 49152;  // rel[1024] f32, key bits [4 tiles x 4 words], barrier
 constexpr int kAttnLongSmemBytes = kAttnLongSmemMisc + 4096 + 64 + 64 + 1024;
 
+// DH and the (tile, unit) split of the heads as in attn_kernel: blockIdx.y is the unit.
+template <int DH>
 __global__ void __launch_bounds__(128, 2)
 attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p) {
+  constexpr int NH = kAttnCols / DH;  // heads per unit
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* s_rel = reinterpret_cast<float*>(smem + kAttnLongSmemMisc);
@@ -875,7 +894,7 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_kb + 16);  // [0] loads
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qt = blockIdx.x, head = blockIdx.y;
+  const int qt = blockIdx.x, unit = blockIdx.y;
   const int row0 = qt * 128;                // first token of this query tile
   int nk = p.L / 128;                       // key tiles per sequence
   int kt0 = (qt / nk) * nk;                 // first tile of the sequence this query tile belongs to
@@ -901,28 +920,34 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
     const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
     if (lane == 0) s_kb[j * 4 + warp] = bits;
   }
-  if (p.relbias_log2) {
-    for (int i = tid; i < 2 * kMaxLongL - 1; i += 128) s_rel[i] = p.relbias_log2[head * (2 * kMaxLongL - 1) + i];
+  if (DH == 64 && p.relbias_log2) {
+    for (int i = tid; i < 2 * kMaxLongL - 1; i += 128) s_rel[i] = p.relbias_log2[unit * (2 * kMaxLongL - 1) + i];
   }
   __syncthreads();
 
-  const bool has_rel = p.relbias_log2 != nullptr;
+  const bool has_rel = DH == 64 && p.relbias_log2 != nullptr;
   const uint32_t qa = smem_u32(smem + kAttnLongSmemQ), ka = smem_u32(smem + kAttnLongSmemK),
                  va = smem_u32(smem + kAttnLongSmemV);
+  // running state per (64-row half h, head hd of the unit) = index hh = h * NH + hd
   int rr[2][2];
   bool valid[2][2];
-  float m_run[2][2], sum[2][2], o[2][32];
+  float m_run[2 * NH][2], sum[2 * NH][2], o[2 * NH][DH / 2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
+  for (int h = 0; h < 2; ++h)
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
       rr[h][u] = h * 64 + 16 * warp + (lane >> 2) + 8 * u;
       valid[h][u] = row0 + rr[h][u] < p.T;
-      m_run[h][u] = __int_as_float(0xff800000);
-      sum[h][u] = 0.f;
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[h][i] = 0.f;
+  for (int hh = 0; hh < 2 * NH; ++hh) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      m_run[hh][u] = __int_as_float(0xff800000);
+      sum[hh][u] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) o[hh][i] = 0.f;
   }
 
 #pragma unroll 1
@@ -930,16 +955,17 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
     if (tid == 0) {
       // K / V of the previous iteration are dead: every warp passed the trailing barrier of that iteration
       mbar_arrive_expect_tx(&bars[0], (j == 0 ? 3 : 2) * 16384);
-      if (j == 0) tma_load_2d(smem + kAttnLongSmemQ, &tmQK, &bars[0], head * kHeadDim, row0);
-      tma_load_2d(smem + kAttnLongSmemK, &tmQK, &bars[0], p.I + head * kHeadDim, (kt0 + j) * 128);
-      tma_load_2d(smem + kAttnLongSmemV, &tmVt, &bars[0], (kt0 + j) * 128, head * kHeadDim);
-      tma_load_2d(smem + kAttnLongSmemV + 8192, &tmVt, &bars[0], (kt0 + j) * 128 + 64, head * kHeadDim);
+      if (j == 0) tma_load_2d(smem + kAttnLongSmemQ, &tmQK, &bars[0], unit * kAttnCols, row0);
+      tma_load_2d(smem + kAttnLongSmemK, &tmQK, &bars[0], p.I + unit * kAttnCols, (kt0 + j) * 128);
+      tma_load_2d(smem + kAttnLongSmemV, &tmVt, &bars[0], (kt0 + j) * 128, unit * kAttnCols);
+      tma_load_2d(smem + kAttnLongSmemV + 8192, &tmVt, &bars[0], (kt0 + j) * 128 + 64, unit * kAttnCols);
     }
     mbar_wait_warp(&bars[0], static_cast<uint32_t>(j & 1), 13);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
+    for (int hh = 0; hh < 2 * NH; ++hh) {
+      const int h = hh / NH, hd = hh % NH;
       float sc[64];
-      attn_scores(sc, qa + h * 8192, ka);
+      attn_scores<DH>(sc, qa + h * 8192 + hd * DH * 2, ka + hd * DH * 2);
       float m_j[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
@@ -956,11 +982,11 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
       float alpha[2], mm[2];
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
-        const float m_new = fmaxf(m_run[h][u], quad_max(m_j[u]));
+        const float m_new = fmaxf(m_run[hh][u], quad_max(m_j[u]));
         mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new : 0.f;  // no allowed key seen so far: all p = 0
-        alpha[u] = (m_run[h][u] > __int_as_float(0xff800000)) ? ex2_approx(m_run[h][u] - mm[u]) : 0.f;
-        m_run[h][u] = m_new;
-        sum[h][u] *= alpha[u];
+        alpha[u] = (m_run[hh][u] > __int_as_float(0xff800000)) ? ex2_approx(m_run[hh][u] - mm[u]) : 0.f;
+        m_run[hh][u] = m_new;
+        sum[hh][u] *= alpha[u];
       }
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
@@ -968,27 +994,29 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
         for (int e = 0; e < 4; ++e) {
           const float pv = ex2_approx(sc[4 * jj + e] - mm[e >> 1]);
           sc[4 * jj + e] = pv;
-          sum[h][e >> 1] += pv;
+          sum[hh][e >> 1] += pv;
         }
 #pragma unroll
-      for (int i = 0; i < 32; ++i) o[h][i] *= alpha[(i >> 1) & 1];
-      attn_pv(o[h], sc, va, 1u);
+      for (int i = 0; i < DH / 2; ++i) o[hh][i] *= alpha[(i >> 1) & 1];
+      attn_pv<DH>(o[hh], sc, va + hd * DH * 128, 1u);
     }
     __syncthreads();  // the next iteration's TMA loads overwrite K / V
   }
 
 #pragma unroll
-  for (int h = 0; h < 2; ++h)
+  for (int hh = 0; hh < 2 * NH; ++hh)
 #pragma unroll
     for (int u = 0; u < 2; ++u) {
-      const float tot = quad_sum(sum[h][u]);
+      const int h = hh / NH, hd = hh % NH;
+      const float tot = quad_sum(sum[hh][u]);
       const float inv = tot > 0.f ? 1.0f / tot : 0.f;
       if (valid[h][u]) {
-        __nv_bfloat16* dst = p.ctx + static_cast<int64_t>(row0 + rr[h][u]) * p.I + head * kHeadDim + 2 * (lane & 3);
+        __nv_bfloat16* dst =
+            p.ctx + static_cast<int64_t>(row0 + rr[h][u]) * p.I + unit * kAttnCols + hd * DH + 2 * (lane & 3);
 #pragma unroll
-        for (int jj = 0; jj < 8; ++jj)
+        for (int jj = 0; jj < DH / 8; ++jj)
           *reinterpret_cast<uint32_t*>(dst + 8 * jj) =
-              pack_bf16x2(o[h][4 * jj + 2 * u] * inv, o[h][4 * jj + 2 * u + 1] * inv);
+              pack_bf16x2(o[hh][4 * jj + 2 * u] * inv, o[hh][4 * jj + 2 * u + 1] * inv);
       }
     }
 }
@@ -1130,7 +1158,8 @@ struct LayerW {
 
 struct om_encoder {
   om_encoder_desc d;
-  int I = 0;  // heads * 64
+  int dh = 0;  // head width: 64, or 32 (BERT)
+  int I = 0;   // heads * dh
   std::vector<LayerW> layers;
   float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;  // BERT embeddings
   float* final_g = nullptr;                                                                    // T5 final RMSNorm
@@ -1258,10 +1287,20 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, c
       cudaError_t err = wide_gemm(e->xb, H, w.wqkv, T, 3 * I, epi);
       if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
     }
-    if (n_long > 0) attn_long_kernel<<<dim3(n_long, d.heads), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
-    if (n_short > 0)
-      attn_kernel<<<std::min(n_short * d.heads, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short,
-                                                                                                n_short, d.heads);
+    const int units = I / kAttnCols;  // work items per tile: one per 64-wide head or pair of 32-wide heads
+    if (n_long > 0) {
+      if (e->dh == 64)
+        attn_long_kernel<64><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
+      else
+        attn_long_kernel<32><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
+    }
+    if (n_short > 0) {
+      const int grid = std::min(n_short * units, sms * kAttnCtasPerSm);
+      if (e->dh == 64)
+        attn_kernel<64><<<grid, 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short, n_short, units);
+      else
+        attn_kernel<32><<<grid, 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short, n_short, units);
+    }
     OM_CUDA(cudaGetLastError());
     {
       // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
@@ -1296,6 +1335,13 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, c
     norm_kernel<true><<<rows4, 128, 0, st>>>(e->h, e->final_g, nullptr, d.ln_eps, T, H, e->h);
   OM_CUDA(cudaGetLastError());
   return 0;
+}
+
+// softmax scale * log2(e) of the attention logits: BERT divides them by sqrt(head width) (1/8 for 64, 1/sqrt(32) for 32,
+// applied to the fp32 scores), T5 does not scale them
+float attn_scale_log2(const om_encoder* e) {
+  const float scale = e->d.arch == OM_ARCH_BERT ? static_cast<float>(1.0 / sqrt(static_cast<double>(e->dh))) : 1.0f;
+  return scale * kLog2e;
 }
 
 // pooled [B, hidden] (e->pooled) -> optional head -> optional normalise -> out_reps rows [B, rep_dim] at out_row_stride
@@ -1401,10 +1447,17 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   if (d.arch != OM_ARCH_BERT && d.arch != OM_ARCH_T5ENC) return fail(OM_EINVAL, "unknown arch %d", d.arch);
   if (d.hidden <= 0 || d.hidden % 128 != 0 || d.hidden > 1024)
     return fail(OM_EINVAL, "hidden=%d unsupported (multiple of 128, <= 1024)", d.hidden);
-  if (d.heads <= 0 || d.heads * kHeadDim > 2048 || (d.heads * kHeadDim) % 128 != 0)
-    return fail(OM_EINVAL, "heads=%d unsupported (head width is 64; heads*64 must be a multiple of 128)", d.heads);
-  if (d.arch == OM_ARCH_BERT && d.heads * kHeadDim != d.hidden)
-    return fail(OM_EINVAL, "BERT requires hidden == heads * 64 (got hidden=%d heads=%d)", d.hidden, d.heads);
+  if (d.heads <= 0) return fail(OM_EINVAL, "heads=%d must be positive", d.heads);
+  // head width: BERT's is hidden / heads, 32 or 64; T5's (d_kv) is 64
+  if (d.arch == OM_ARCH_BERT && d.hidden % d.heads != 0)
+    return fail(OM_EINVAL, "BERT requires hidden to be a multiple of heads (got hidden=%d heads=%d)", d.hidden, d.heads);
+  const int dh = d.arch == OM_ARCH_BERT ? d.hidden / d.heads : 64;
+  if (dh != 32 && dh != 64)
+    return fail(OM_EINVAL, "BERT head width hidden/heads=%d unsupported (32 or 64; hidden=%d heads=%d)", dh, d.hidden,
+                d.heads);
+  if (d.heads * dh > 2048 || (d.heads * dh) % 128 != 0)
+    return fail(OM_EINVAL, "heads=%d unsupported (heads * head width %d must be a multiple of 128, at most 2048)", d.heads,
+                dh);
   if (d.ffn <= 0 || d.ffn % 64 != 0) return fail(OM_EINVAL, "ffn=%d must be a positive multiple of 64", d.ffn);
   if (d.layers <= 0 || d.vocab <= 0) return fail(OM_EINVAL, "layers/vocab must be positive");
   if (d.has_head && (d.head_out <= 0)) return fail(OM_EINVAL, "head_out must be positive when has_head=1");
@@ -1412,7 +1465,8 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   om_encoder* e = new (std::nothrow) om_encoder();
   if (!e) return fail(OM_ENOMEM, "out of host memory");
   e->d = d;
-  e->I = d.heads * kHeadDim;
+  e->dh = dh;
+  e->I = d.heads * dh;
   const int H = d.hidden, I = e->I, F = d.ffn;
   e->layers.resize(d.layers);
   int rc = 0;
@@ -1714,9 +1768,11 @@ int om_encoder_finalize(om_encoder* e) {
     }
   }
   static bool attr = false;
-  if (!attr) {
-    OM_CUDA(cudaFuncSetAttribute(attn_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
+  if (!attr) {  // every instantiation: handles of both head widths may live in one process
+    OM_CUDA(cudaFuncSetAttribute(attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
+    OM_CUDA(cudaFuncSetAttribute(attn_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
+    OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
+    OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
     attr = true;
   }
   e->finalized = true;
@@ -1766,7 +1822,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   ap.spt = spt;
   ap.I = I;
   ap.Tvalid_rows = long_seq ? 128 : spt * L;
-  ap.scale_log2 = (bert ? 0.125f : 1.0f) * kLog2e;
+  ap.scale_log2 = attn_scale_log2(e);
   ap.kmask = e->kmask;
   ap.relbias_log2 = bert ? nullptr : (long_seq ? e->relbias_long_log2 : e->relbias_log2);
   ap.ctx = e->ctx;
@@ -1818,7 +1874,7 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
   ap.spt = 1;
   ap.I = e->I;
   ap.Tvalid_rows = 128;
-  ap.scale_log2 = (bert ? 0.125f : 1.0f) * kLog2e;
+  ap.scale_log2 = attn_scale_log2(e);
   ap.kmask = e->kmask;
   ap.ctx = e->ctx;
   ap.rowmap = e->rowmap;

@@ -16,14 +16,23 @@ from . import _lib
 
 _OUT_DTYPES = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16}
 
+_HEAD_WIDTHS = (32, 64)  # BERT head widths hidden / heads the CUDA attention kernels implement (T5: d_kv 64)
+
 _BERT_KEYS = ("num_hidden_layers", "hidden_size", "num_attention_heads", "intermediate_size", "vocab_size",
               "max_position_embeddings", "type_vocab_size", "layer_norm_eps")
+
+
+def _check_bert_heads(hidden: int, heads: int):
+    if heads <= 0 or hidden % heads != 0 or hidden // heads not in _HEAD_WIDTHS:
+        raise ValueError("CUDA encoder needs 32- or 64-wide attention heads, got hidden_size=%d / num_attention_heads=%d"
+                         % (hidden, heads))
 
 
 def spec_from_hf_config(config) -> Dict:
     """Translate a HF ``BertConfig`` / ``T5Config`` into the plain dict ``CudaEncoder`` consumes."""
     mt = getattr(config, "model_type", "")
     if mt == "bert":
+        _check_bert_heads(config.hidden_size, config.num_attention_heads)
         if getattr(config, "hidden_act", "gelu") != "gelu":
             raise ValueError("CUDA encoder supports hidden_act='gelu' (erf) only, got %r" % config.hidden_act)
         if getattr(config, "position_embedding_type", "absolute") not in (None, "absolute"):
@@ -49,10 +58,10 @@ class CudaEncoder:
                  pooling: str = "first", normalize: bool = False, max_batch_tokens: int = 256 * 128):
         if pooling not in ("first", "mean"):
             raise ValueError("Unknown pooling type: {}".format(pooling))
+        if spec["arch"] == "bert":
+            _check_bert_heads(spec["hidden"], spec["heads"])
         self._lib = _lib.load()
         head_head_out = int(head_weight.shape[0]) if head_weight is not None else 0
-        if spec["heads"] * 64 != spec["hidden"] and spec["arch"] == "bert":
-            raise ValueError("CUDA encoder needs 64-wide attention heads")
         desc = _lib.EncoderDesc(
             arch=_lib.OM_ARCH_BERT if spec["arch"] == "bert" else _lib.OM_ARCH_T5ENC, layers=spec["layers"],
             hidden=spec["hidden"], heads=spec["heads"], ffn=spec["ffn"], vocab=spec["vocab"],
