@@ -110,6 +110,23 @@ int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attentio
  * Invalid input (a null pointer, B < 0, a length outside the range above) returns OM_EINVAL and writes nothing. */
 int om_encode_packed(om_encoder* enc, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens,
                      int B, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream);
+/* Cross-encoder pairs (re-ranking, OpenMatch's RRModel.encode on encode_pair's sequences).  Sequence i =
+ *   prefix ++ a_tokens[a_start_i : a_start_i + a_len_i] ++ b_tokens[b_start_i : b_start_i + b_len_i] ++ suffix,
+ * token types all 0.  a_tokens [a_total] / b_tokens [b_total]: int32 DEVICE token stores (e.g. the queries and the
+ * passages of a run, uploaded once); spans: int64 [B, 4] HOST (a_start, a_len, b_start, b_len); prefix / suffix: HOST,
+ * 0..4 ids each (NULL when empty).  The pair tokens are assembled on the device, straight into the packed layout.
+ * Result: bitwise what om_encode_packed returns for the same sequences given as an int64 token stream with
+ * token_type_ids = NULL (the layout is the same function of the lengths, the same kernels run on it); out_reps as there,
+ * no out_hidden.  A cross-encoder is an encoder with pooling first / mean, has_head = 1, head_out = 1 and normalize = 0:
+ * out_reps then holds one score per pair.  spans, prefix and suffix may be reused on return; no device synchronisation;
+ * asynchronous on `stream`.  Workspace for the assembled tokens (max_batch_tokens int64 + one span table) is allocated
+ * on a handle's first call.  Invalid input returns OM_EINVAL and writes nothing: a null pointer, B < 0, n_prefix or
+ * n_suffix outside [0, 4], a negative start or length, start + len beyond a_total / b_total, an assembled length
+ * n_prefix + a_len + b_len + n_suffix outside the om_encode_packed range.  a_len = 0 and b_len = 0 are legal; B = 0 does
+ * nothing. */
+int om_encode_pairs(om_encoder* enc, const int32_t* a_tokens, int64_t a_total, const int32_t* b_tokens, int64_t b_total,
+                    const int64_t* spans, int B, const int32_t* prefix, int n_prefix, const int32_t* suffix, int n_suffix,
+                    void* out_reps, om_dtype out_dtype, int64_t out_row_stride, void* stream);
 int om_encoder_rep_dim(const om_encoder* enc);
 void om_encoder_destroy(om_encoder* enc);
 

@@ -11,7 +11,8 @@ for _name in ("arguments", "utils", "loss", "modeling", "dataset", "trainer", "r
     _mod = importlib.import_module("openmatch_b200." + _name)
     sys.modules[__name__ + "." + _name] = _mod
     globals()[_name] = _mod
-for _sub in ("modeling.dense_retrieval_model", "modeling.linear", "retriever.dense_retriever", "trainer.dense_trainer",
-             "dataset.data_collator", "dataset.inference_dataset", "dataset.train_dataset", "driver.build_index",
-             "driver.retrieve", "driver.successive_retrieve", "driver.train_dr", "driver.build_hn"):
+for _sub in ("modeling.dense_retrieval_model", "modeling.linear", "modeling.reranking_model", "retriever.dense_retriever",
+             "retriever.reranker", "trainer.dense_trainer", "dataset.data_collator", "dataset.inference_dataset",
+             "dataset.train_dataset", "driver.build_index", "driver.retrieve", "driver.successive_retrieve",
+             "driver.train_dr", "driver.build_hn", "driver.rerank"):
     sys.modules[__name__ + "." + _sub] = importlib.import_module("openmatch_b200." + _sub)

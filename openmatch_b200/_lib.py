@@ -38,6 +38,8 @@ SIGNATURES = {
                           c_void_p]),
     "om_encode_packed": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_int, c_int64, c_void_p,
                                  c_void_p]),
+    "om_encode_pairs": (c_int, [c_void_p, c_void_p, c_int64, c_void_p, c_int64, c_void_p, c_int, c_void_p, c_int,
+                                c_void_p, c_int, c_void_p, c_int, c_int64, c_void_p]),
     "om_encoder_rep_dim": (c_int, [c_void_p]),
     "om_encoder_destroy": (None, [c_void_p]),
     "om_index_create": (c_int, [c_int, POINTER(c_void_p)]),

@@ -163,6 +163,8 @@ class InferenceArguments(RuntimeArguments):
     trec_run_path: str = field(default=None)
     id_key_name: str = field(default="id")
     retrieve_depth: int = field(default=100, metadata={"help": "top-k for driver.retrieve (reference hard-codes 100)"})
+    reranking_depth: int = field(default=None, metadata={"help": "driver.rerank: documents per query of the run to "
+                                                                   "re-rank (default: all)"})
     index_dtype: str = field(default="float32", metadata={
         "help": "row storage of the search index: 'float32' (fp32 rows + fp16 scan copy, 6 bytes per element) or "
                 "'float16' (fp16 rows only, 2 bytes per element; search is exact over the fp16-rounded rows)"})

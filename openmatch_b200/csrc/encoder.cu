@@ -1074,6 +1074,41 @@ __global__ void __launch_bounds__(128) gather_packed_rows_kernel(const float* hi
   for (int c = lane; c < H; c += 32) dst[c] = src[c];
 }
 
+// cross-encoder pairs (om_encode_pairs): the two token spans of one sequence, in the order of the sequence table
+struct PairSpan {
+  int64_t a0, b0;  // first token in the a / b store
+  int a_len, b_len;
+};
+struct PairSpecials {  // prefix / suffix ids, passed by value
+  int32_t prefix[4], suffix[4];
+  int n_prefix, n_suffix;
+};
+
+__device__ __forceinline__ int32_t special_id(const int32_t (&ids)[4], int k) {
+  int32_t id = 0;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) id = j == k ? ids[j] : id;  // no dynamic indexing: the array stays in registers
+  return id;
+}
+
+// tokens[s.row0 + pos] = (prefix ++ a[a0, a0 + a_len) ++ b[b0, b0 + b_len) ++ suffix)[pos] for every sequence s of one row
+// group: the group's token stream in layout order, read by the packed embedding kernels through tok0 = row0.  One block
+// per sequence.
+__global__ void pair_tokens_kernel(const int32_t* a, const int32_t* b, const PackedSeq* seqs, const PairSpan* spans,
+                                   PairSpecials sp, int64_t* tokens) {
+  const PackedSeq s = seqs[blockIdx.x];
+  const PairSpan p = spans[blockIdx.x];
+  for (int pos = threadIdx.x; pos < s.len; pos += blockDim.x) {
+    int k = pos;
+    int32_t id;
+    if (k < sp.n_prefix) id = special_id(sp.prefix, k);
+    else if ((k -= sp.n_prefix) < p.a_len) id = a[p.a0 + k];
+    else if ((k -= p.a_len) < p.b_len) id = b[p.b0 + k];
+    else id = special_id(sp.suffix, k - p.b_len);
+    tokens[s.row0 + pos] = id;
+  }
+}
+
 // out[b, o] = sum_i in[b, i] * W[o, i]  (bias-free LinearHead).  One warp per (o, group of 8 rows).
 __global__ void __launch_bounds__(256) head_kernel(const float* in, const float* W, int B, int Hin, int Hout, float* out) {
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
@@ -1181,6 +1216,11 @@ struct om_encoder {
   PackedSeq* pk_host = nullptr;     // [Tmax], pinned host memory
   cudaEvent_t pk_copied = nullptr;  // recorded after the last upload from pk_host
   int2* rowmap = nullptr;           // [Tmax]
+  // pair calls (om_encode_pairs), allocated on the first one: the span table of one chunk (device, and its pinned staging
+  // copy, uploaded under pk_copied) and the token stream of one row group
+  PairSpan* pr_spans = nullptr;  // [Tmax]
+  PairSpan* pr_host = nullptr;   // [Tmax], pinned host memory
+  int64_t* pr_tokens = nullptr;  // [Tmax]
   std::vector<void*> allocs;
 };
 
@@ -1436,6 +1476,77 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
   if (g.k1 > g.k0) groups.push_back(g);
 }
 
+// pair input of one packed chunk (om_encode_pairs): the two token stores, the chunk's spans in layout order (host) and
+// the special ids
+struct PairChunk {
+  const int32_t* a;
+  const int32_t* b;
+  const PairSpan* spans;
+  PairSpecials sp;
+};
+
+// Encodes one chunk of a packed call (its n sequences placed by place_packed into seqs / groups) into out rows [0, n):
+// uploads the sequence table, then per row group the row map, the embedding, the layers and the pooling; then the
+// output tail.  pairs != nullptr: each row group's token stream is first assembled from the pair stores into pr_tokens
+// (the table's tok0 = row0, tokens = token_type_ids = nullptr).
+int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* token_type_ids,
+                        const std::vector<PackedSeq>& seqs, const std::vector<PackedGroup>& groups, const PairChunk* pairs,
+                        int n, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, int sms,
+                        cudaStream_t st) {
+  const om_encoder_desc& d = e->d;
+  const bool bert = d.arch == OM_ARCH_BERT;
+  const int H = d.hidden;
+  // upload the tables through the pinned staging buffers: wait (on the host) only until the previous upload from them
+  // has been read
+  OM_CUDA(cudaEventSynchronize(e->pk_copied));
+  memcpy(e->pk_host, seqs.data(), seqs.size() * sizeof(PackedSeq));
+  OM_CUDA(cudaMemcpyAsync(e->pk_seqs, e->pk_host, seqs.size() * sizeof(PackedSeq), cudaMemcpyHostToDevice, st));
+  if (pairs) {
+    memcpy(e->pr_host, pairs->spans, seqs.size() * sizeof(PairSpan));
+    OM_CUDA(cudaMemcpyAsync(e->pr_spans, e->pr_host, seqs.size() * sizeof(PairSpan), cudaMemcpyHostToDevice, st));
+    tokens = e->pr_tokens;
+  }
+  OM_CUDA(cudaEventRecord(e->pk_copied, st));
+  AttnParams ap;
+  ap.L = 128;  // unused: every row's key range comes from the row map
+  ap.spt = 1;
+  ap.I = e->I;
+  ap.Tvalid_rows = 128;
+  ap.scale_log2 = attn_scale_log2(e);
+  ap.kmask = e->kmask;
+  ap.ctx = e->ctx;
+  ap.rowmap = e->rowmap;
+  for (const PackedGroup& g : groups) {
+    const PackedSeq* gs = e->pk_seqs + g.k0;
+    const int ns = g.k1 - g.k0, T = g.T, rows4 = (T + 3) / 4;
+    if (pairs)
+      pair_tokens_kernel<<<ns, 128, 0, st>>>(pairs->a, pairs->b, gs, e->pr_spans + g.k0, pairs->sp, e->pr_tokens);
+    packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
+    if (bert)
+      bert_embed_kernel<<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H, d.vocab,
+                                               std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], e->rowmap, gs);
+    else
+      t5_embed_kernel<<<rows4, 128, 0, st>>>(tokens, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], e->rowmap, gs);
+    OM_CUDA(cudaGetLastError());
+    ap.T = T;
+    ap.seqs = gs;
+    AttnParams ap_long = ap, ap_short = ap;
+    ap_long.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
+    ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
+    ap_short.tile0 = g.n_long;
+    OM_TRY(encode_layers(e, T, ap_long, g.n_long, ap_short, g.n_tiles - g.n_long, sms, st));
+    if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
+    pool_packed_kernel<<<ns, 256, 0, st>>>(e->h, gs, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
+    OM_CUDA(cudaGetLastError());
+  }
+  return finish_reps(e, n, out_reps, out_dtype, out_row_stride, st);
+}
+
+// the packed length limit: 512 tokens, max_position_embeddings (BERT) and max_batch_tokens
+int packed_max_len(const om_encoder* e) {
+  return std::min(kMaxLongL, std::min(e->d.arch == OM_ARCH_BERT ? e->d.max_pos : kMaxLongL, e->Tmax));
+}
+
 }  // namespace
 
 extern "C" {
@@ -1584,6 +1695,7 @@ void om_encoder_destroy(om_encoder* e) {
     cudaFree(w.w1_f32);
   }
   if (e->pk_host) cudaFreeHost(e->pk_host);
+  if (e->pr_host) cudaFreeHost(e->pr_host);
   if (e->pk_copied) cudaEventDestroy(e->pk_copied);
   delete e;
 }
@@ -1848,9 +1960,8 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
     return fail(OM_EINVAL, "om_encode_packed: out dtype must be f32, bf16 or f16");
   const int rep_dim = om_encoder_rep_dim(e);
   if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_packed: out_row_stride < rep_dim");
-  const om_encoder_desc& d = e->d;
-  const bool bert = d.arch == OM_ARCH_BERT;
-  const int max_len = std::min(kMaxLongL, std::min(bert ? d.max_pos : kMaxLongL, e->Tmax));
+  const bool bert = e->d.arch == OM_ARCH_BERT;
+  const int max_len = packed_max_len(e);
   std::vector<int64_t> tok0(static_cast<size_t>(B));
   int64_t total = 0;
   for (int i = 0; i < B; ++i) {
@@ -1865,19 +1976,9 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int H = d.hidden;
   const size_t out_elem = out_dtype == OM_F32 ? 4 : 2;
 
   NvtxRange nvtx("om.encode_packed");
-  AttnParams ap;
-  ap.L = 128;  // unused: every row's key range comes from the row map
-  ap.spt = 1;
-  ap.I = e->I;
-  ap.Tvalid_rows = 128;
-  ap.scale_log2 = attn_scale_log2(e);
-  ap.kmask = e->kmask;
-  ap.ctx = e->ctx;
-  ap.rowmap = e->rowmap;
   std::vector<PackedSeq> seqs;
   std::vector<PackedGroup> groups;
   // chunks of at most max_batch_tokens sequences (the pooled / head workspace rows); one chunk unless the batch holds
@@ -1885,35 +1986,92 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
   for (int c0 = 0; c0 < B; c0 += e->Tmax) {
     const int n = std::min(B - c0, e->Tmax);
     place_packed(seqlens + c0, tok0.data() + c0, n, e->Tmax, seqs, groups);
-    // upload the sequence table through the pinned staging buffer: wait (on the host) only until the previous upload
-    // from it has been read
-    OM_CUDA(cudaEventSynchronize(e->pk_copied));
-    memcpy(e->pk_host, seqs.data(), seqs.size() * sizeof(PackedSeq));
-    OM_CUDA(cudaMemcpyAsync(e->pk_seqs, e->pk_host, seqs.size() * sizeof(PackedSeq), cudaMemcpyHostToDevice, st));
-    OM_CUDA(cudaEventRecord(e->pk_copied, st));
-    for (const PackedGroup& g : groups) {
-      const PackedSeq* gs = e->pk_seqs + g.k0;
-      const int ns = g.k1 - g.k0, T = g.T, rows4 = (T + 3) / 4;
-      packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
-      if (bert)
-        bert_embed_kernel<<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H, d.vocab,
-                                                 std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], e->rowmap, gs);
-      else
-        t5_embed_kernel<<<rows4, 128, 0, st>>>(tokens, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], e->rowmap, gs);
-      OM_CUDA(cudaGetLastError());
-      ap.T = T;
-      ap.seqs = gs;
-      AttnParams ap_long = ap, ap_short = ap;
-      ap_long.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
-      ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
-      ap_short.tile0 = g.n_long;
-      OM_TRY(encode_layers(e, T, ap_long, g.n_long, ap_short, g.n_tiles - g.n_long, sms, st));
-      if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
-      pool_packed_kernel<<<ns, 256, 0, st>>>(e->h, gs, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
-      OM_CUDA(cudaGetLastError());
+    OM_TRY(encode_packed_chunk(e, tokens, token_type_ids, seqs, groups, nullptr, n,
+                               static_cast<char*>(out_reps) + static_cast<size_t>(c0) * out_row_stride * out_elem,
+                               out_dtype, out_row_stride, out_hidden, sms, st));
+  }
+  return 0;
+}
+
+int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, const int32_t* b_tokens, int64_t b_total,
+                    const int64_t* spans, int B, const int32_t* prefix, int n_prefix, const int32_t* suffix, int n_suffix,
+                    void* out_reps, om_dtype out_dtype, int64_t out_row_stride, void* stream) {
+  if (!e || !a_tokens || !b_tokens || !spans || !out_reps || (n_prefix > 0 && !prefix) || (n_suffix > 0 && !suffix))
+    return fail(OM_EINVAL, "om_encode_pairs: null argument");
+  if (!e->finalized) return fail(OM_ESTATE, "om_encode_pairs: call om_encoder_finalize first");
+  if (B < 0) return fail(OM_EINVAL, "om_encode_pairs: B=%d is negative", B);
+  if (a_total < 0 || b_total < 0)
+    return fail(OM_EINVAL, "om_encode_pairs: negative store size (a_total=%lld, b_total=%lld)", (long long)a_total,
+                (long long)b_total);
+  if (n_prefix < 0 || n_prefix > 4 || n_suffix < 0 || n_suffix > 4)
+    return fail(OM_EINVAL, "om_encode_pairs: n_prefix=%d / n_suffix=%d outside [0, 4]", n_prefix, n_suffix);
+  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
+    return fail(OM_EINVAL, "om_encode_pairs: out dtype must be f32, bf16 or f16");
+  const int rep_dim = om_encoder_rep_dim(e);
+  if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_pairs: out_row_stride < rep_dim");
+  const bool bert = e->d.arch == OM_ARCH_BERT;
+  const int max_len = packed_max_len(e);
+  std::vector<int32_t> lens(static_cast<size_t>(B));
+  for (int i = 0; i < B; ++i) {
+    const int64_t a0 = spans[4 * (size_t)i], al = spans[4 * (size_t)i + 1];
+    const int64_t b0 = spans[4 * (size_t)i + 2], bl = spans[4 * (size_t)i + 3];
+    if (a0 < 0 || al < 0 || b0 < 0 || bl < 0)
+      return fail(OM_EINVAL, "om_encode_pairs: pair %d has a negative start or length (%lld, %lld, %lld, %lld)", i,
+                  (long long)a0, (long long)al, (long long)b0, (long long)bl);
+    if (al > a_total - a0 || bl > b_total - b0)
+      return fail(OM_EINVAL, "om_encode_pairs: pair %d reads past a store (a %lld + %lld of %lld, b %lld + %lld of %lld)",
+                  i, (long long)a0, (long long)al, (long long)a_total, (long long)b0, (long long)bl, (long long)b_total);
+    const int64_t l = n_prefix + al + bl + n_suffix;
+    if (l < 1 || l > max_len)
+      return fail(OM_EINVAL, "om_encode_pairs: pair %d assembles %lld tokens, outside [1, %d] (512 tokens%s, "
+                  "max_batch_tokens=%d)", i, (long long)l, max_len, bert ? ", max_position_embeddings" : "", e->Tmax);
+    lens[i] = static_cast<int32_t>(l);
+  }
+  if (B == 0) return 0;
+  const int sms = device_sm_count();
+  if (sms < 0) return sms;
+  if (!e->pr_tokens) {  // first pair call on this handle
+    int rc = 0;
+    if (dev_alloc(e, &e->pr_spans, e->Tmax) != 0 || dev_alloc(e, &e->pr_tokens, e->Tmax) != 0) rc = OM_ECUDA;
+    if (rc == 0 && cudaHostAlloc(&e->pr_host, (size_t)e->Tmax * sizeof(PairSpan), cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      rc = fail(OM_ENOMEM, "om_encode_pairs: out of pinned host memory");
     }
-    OM_TRY(finish_reps(e, n, static_cast<char*>(out_reps) + static_cast<size_t>(c0) * out_row_stride * out_elem, out_dtype,
-                       out_row_stride, st));
+    if (rc != 0) {
+      e->pr_tokens = nullptr;  // retried on the next call; what was allocated is freed with the handle
+      return rc;
+    }
+  }
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t out_elem = out_dtype == OM_F32 ? 4 : 2;
+
+  NvtxRange nvtx("om.encode_pairs");
+  PairChunk pc;
+  pc.a = a_tokens;
+  pc.b = b_tokens;
+  pc.sp.n_prefix = n_prefix;
+  pc.sp.n_suffix = n_suffix;
+  for (int j = 0; j < 4; ++j) {
+    pc.sp.prefix[j] = j < n_prefix ? prefix[j] : 0;
+    pc.sp.suffix[j] = j < n_suffix ? suffix[j] : 0;
+  }
+  const std::vector<int64_t> no_tok0(static_cast<size_t>(B), 0);  // the token stream is assembled per row group
+  std::vector<PackedSeq> seqs;
+  std::vector<PackedGroup> groups;
+  std::vector<PairSpan> chunk_spans;
+  for (int c0 = 0; c0 < B; c0 += e->Tmax) {  // chunks as in om_encode_packed: the same layout, the same kernels
+    const int n = std::min(B - c0, e->Tmax);
+    place_packed(lens.data() + c0, no_tok0.data(), n, e->Tmax, seqs, groups);
+    chunk_spans.resize(seqs.size());
+    for (size_t k = 0; k < seqs.size(); ++k) {
+      const int64_t* s = spans + 4 * (static_cast<size_t>(c0) + seqs[k].out);
+      chunk_spans[k] = PairSpan{s[0], s[2], static_cast<int>(s[1]), static_cast<int>(s[3])};
+      seqs[k].tok0 = seqs[k].row0;
+    }
+    pc.spans = chunk_spans.data();
+    OM_TRY(encode_packed_chunk(e, nullptr, nullptr, seqs, groups, &pc, n,
+                               static_cast<char*>(out_reps) + static_cast<size_t>(c0) * out_row_stride * out_elem,
+                               out_dtype, out_row_stride, nullptr, sms, st));
   }
   return 0;
 }

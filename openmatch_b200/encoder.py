@@ -159,3 +159,36 @@ class CudaEncoder:
             out.data_ptr(), _OUT_DTYPES[out.dtype], out.stride(0),
             hidden.data_ptr() if hidden is not None else None, _lib.current_stream_ptr()))
         return (hidden, out) if return_hidden else out
+
+    @torch.no_grad()
+    def encode_pairs(self, a_tokens: torch.Tensor, b_tokens: torch.Tensor, spans, prefix=(), suffix=(),
+                     out: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.float32):
+        """Cross-encoder pairs assembled on the device: sequence i = ``prefix ++ a_tokens[a_start : a_start + a_len] ++
+        b_tokens[b_start : b_start + b_len] ++ suffix`` with ``spans[i] = (a_start, a_len, b_start, b_len)`` (host int64
+        ``[B, 4]``), token types 0; ``a_tokens`` / ``b_tokens``: int32 CUDA token stores; ``prefix`` / ``suffix``: up to
+        4 ids each.  -> reps ``[B, rep_dim]``, bitwise what ``encode_packed`` returns for the assembled sequences;
+        ``out`` / ``out_dtype`` as there."""
+        if not a_tokens.is_cuda or not b_tokens.is_cuda:
+            raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
+        if isinstance(spans, torch.Tensor):
+            spans = spans.detach().cpu().numpy()
+        sp = np.ascontiguousarray(np.asarray(spans, dtype=np.int64).reshape(-1, 4))
+        pre = np.ascontiguousarray(np.asarray(prefix, dtype=np.int32).reshape(-1))
+        suf = np.ascontiguousarray(np.asarray(suffix, dtype=np.int32).reshape(-1))
+        B = int(sp.shape[0])
+        a, b = (t.reshape(-1).to(torch.int32).contiguous() for t in (a_tokens, b_tokens))
+        na, nb = a.numel(), b.numel()
+        # an empty store has no address; any valid one does (every span of it is then empty)
+        a = a if na else torch.zeros(1, dtype=torch.int32, device=a.device)
+        b = b if nb else torch.zeros(1, dtype=torch.int32, device=b.device)
+        if out is None:
+            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=a.device)
+        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
+            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
+        if out.shape[0] != B or out.shape[1] != self.rep_dim:
+            raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
+        _lib.check(self._lib.om_encode_pairs(
+            self._h, a.data_ptr(), na, b.data_ptr(), nb, sp.ctypes.data, B, pre.ctypes.data if pre.size else None,
+            int(pre.size), suf.ctypes.data if suf.size else None, int(suf.size), out.data_ptr(), _OUT_DTYPES[out.dtype],
+            out.stride(0), _lib.current_stream_ptr()))
+        return out
