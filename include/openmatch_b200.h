@@ -43,7 +43,12 @@ enum { OM_OK = 0, OM_EINVAL = -1, OM_ECUDA = -2, OM_ENOMEM = -3, OM_ENODEVICE = 
 
 typedef enum { OM_F32 = 0, OM_BF16 = 1, OM_F16 = 2 } om_dtype;
 typedef enum { OM_HOST = 0, OM_DEVICE = 1 } om_memkind;
-typedef enum { OM_ARCH_BERT = 0, OM_ARCH_T5ENC = 1 } om_arch;
+/* OM_ARCH_ROBERTA: RoBERTa / XLM-RoBERTa / CamemBERT, BERT's encoder (same parameter names, optionally prefixed
+ * "roberta.") whose position ids come from the token ids, as HF's create_position_ids_from_input_ids computes them with
+ * padding_idx = pad_token_id = 1 (the value of every such config; fixed here): a token with id != 1 gets position
+ * 1 + (number of ids != 1 up to and including it in its sequence), a token with id 1 gets position 1, whatever the
+ * attention mask says.  Sequences are at most max_position_embeddings - 2 tokens long. */
+typedef enum { OM_ARCH_BERT = 0, OM_ARCH_T5ENC = 1, OM_ARCH_ROBERTA = 2 } om_arch;
 typedef enum { OM_POOL_FIRST = 0, OM_POOL_MEAN = 1 } om_pooling;
 typedef enum { OM_REDUCE_MEAN = 0, OM_REDUCE_SUM = 1 } om_reduction;
 
@@ -67,8 +72,9 @@ typedef struct om_encoder_desc {
                                most 2048.  Any other width returns OM_EINVAL */
   int32_t ffn;              /* intermediate_size / d_ff (multiple of 64) */
   int32_t vocab;            /* vocab_size */
-  int32_t max_pos;          /* max_position_embeddings (BERT); ignored for T5 */
-  int32_t type_vocab;       /* type_vocab_size (BERT); ignored for T5 */
+  int32_t max_pos;          /* max_position_embeddings (BERT; RoBERTa: including its offset of 2, e.g. 514, at least
+                               3); ignored for T5 */
+  int32_t type_vocab;       /* type_vocab_size (BERT; RoBERTa: normally 1); ignored for T5 */
   float ln_eps;             /* layer_norm_eps (1e-12 BERT) / layer_norm_epsilon (1e-6 T5) */
   int32_t pooling;          /* om_pooling: DRModel.pooling 'first' | 'mean' */
   int32_t has_head;         /* 1: bias-free LinearHead follows pooling */
@@ -90,7 +96,8 @@ int om_encoder_set_weight(om_encoder* enc, const char* name, const void* data, o
 /* Verifies that every required parameter was supplied and builds derived tables. */
 int om_encoder_finalize(om_encoder* enc);
 /* input_ids / attention_mask / token_type_ids (nullable => zeros; ignored for T5): int64 [B, L] device,
- * row-major, exactly what DRInferenceCollator / QPCollator hand to the model; L <= 128.
+ * row-major, exactly what DRInferenceCollator / QPCollator hand to the model; L <= 128 or 256 / 384 / 512, and
+ * L <= max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa).
  * out_reps: device [B, rep_dim] fp32, bf16 or fp16 with row pitch out_row_stride (elements) — may point into an
  * index shard obtained from om_index_reserve() / om_index_reserve_rows().  fp16 output is the round-to-nearest-even
  * of the fp32 output of the same call (values beyond the half range become inf).  out_hidden: nullable device fp32 [B, L, hidden]
@@ -99,7 +106,8 @@ int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attentio
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
               int64_t out_row_stride, float* out_hidden, void* stream);
 /* Variable-length batch, no padding.  tokens / token_type_ids (nullable => zeros; ignored for T5): int64 [T] device, the
- * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 512 (BERT: <= max_position_embeddings; and
+ * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 512 (BERT: <= max_position_embeddings; RoBERTa:
+ * <= max_position_embeddings - 2, positions computed from each sequence's own ids; and
  * <= max_batch_tokens), T = sum(seqlens).  Result: what om_encode returns for the same sequences padded to any L with
  * attention_mask = 1 on their tokens, up to the order of floating-point sums in attention and pooling.  out_reps as in
  * om_encode (row i = sequence i).  out_hidden: nullable fp32 [T, hidden], packed like tokens.  seqlens may be reused on

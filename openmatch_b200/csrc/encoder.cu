@@ -554,17 +554,55 @@ __device__ __forceinline__ void zero_row(int nvec, int lane, float* out_f32, __n
   if (lane < kStatParts) reinterpret_cast<float2*>(stats_row)[lane] = make_float2(0.f, 0.f);
 }
 
+// RoBERTa position ids (modeling_roberta.py create_position_ids_from_input_ids, padding_idx = kRobertaPad): a token with
+// id != 1 at index t of its sequence gets 1 + #{t' <= t : id[t'] != 1}, a token with id 1 gets position 1.  They come
+// from the ids alone, not from the attention mask, so a pad id inside a sequence's content takes position 1 and does not
+// advance the count.  pos_ids[layout row] for every token of the nseq sequences: seqs == nullptr, sequence b is the
+// padded row ids[b * L, (b + 1) * L) at layout rows b * L + t; else sequence k is ids[seqs[k].tok0 + t] at layout row
+// seqs[k].row0 + t, t < seqs[k].len.  One warp per sequence: an inclusive warp scan of (id != 1) per 32-token chunk and
+// a running carry.
+constexpr int kRobertaPad = 1;
+
+__global__ void __launch_bounds__(128) roberta_pos_kernel(const int64_t* ids, int nseq, int L, const PackedSeq* seqs,
+                                                          int32_t* pos_ids) {
+  const int s = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (s >= nseq) return;
+  int64_t tok0 = static_cast<int64_t>(s) * L, row0 = tok0;
+  int len = L;
+  if (seqs) {
+    tok0 = seqs[s].tok0;
+    row0 = seqs[s].row0;
+    len = seqs[s].len;
+  }
+  int carry = 0;
+  for (int c = 0; c < len; c += 32) {
+    const int t = c + lane;
+    const int real = t < len && ids[tok0 + t] != kRobertaPad ? 1 : 0;
+    int incl = real;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const int v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    if (t < len) pos_ids[row0 + t] = real ? kRobertaPad + carry + incl : kRobertaPad;
+    carry += __shfl_sync(0xffffffffu, incl, 31);
+  }
+}
+
 // BERT embeddings (modeling_bert.py:53-112): s = word[id] + type[tt] + pos[l], UN-normalised (fp32 + bf16) with its row
 // statistics; the embedding LayerNorm is applied by the first layer's QKV / O-proj epilogues like every other LayerNorm.
 // s is stored minus its row mean: only the embedding LayerNorm reads it, which is shift-invariant.  A common offset in
 // the embedding tables otherwise leaves rows whose mean is tens of times their standard deviation, and the bf16 copy that
 // the QKV GEMM reads (and the folded weights' rounding residue, scaled by mean / std) would bury the row's information.
 // rowmap != nullptr (packed layout): token and position come from the row map, padding rows are zeroed; a real token's
-// row is bitwise the row the padded layout gives it.
+// row is bitwise the row the padded layout gives it.  kPosIds (RoBERTa): the position is pos_ids[row] (roberta_pos_kernel)
+// instead of the token's index in its sequence; everything else is shared.
+template <bool kPosIds>
 __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, const int64_t* tts, const float* word,
                                                          const float* type, const float* pos, int T, int L, int H, int vocab,
                                                          int type_vocab, float* out_f32, __nv_bfloat16* out_bf16,
-                                                         float* stats, const int2* rowmap, const PackedSeq* seqs) {
+                                                         float* stats, const int2* rowmap, const PackedSeq* seqs,
+                                                         const int32_t* pos_ids) {
   const int row = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (row >= T) return;
   const int nvec = H >> 7;
@@ -580,6 +618,7 @@ __global__ void __launch_bounds__(128) bert_embed_kernel(const int64_t* ids, con
     tok = seqs[m.x].tok0 + m.y;
     l = m.y;
   }
+  if (kPosIds) l = pos_ids[row];
   int64_t id = ids[tok];
   id = id < 0 ? 0 : (id >= vocab ? vocab - 1 : id);
   int64_t tt = tts ? tts[tok] : 0;
@@ -1221,10 +1260,23 @@ struct om_encoder {
   PairSpan* pr_spans = nullptr;  // [Tmax]
   PairSpan* pr_host = nullptr;   // [Tmax], pinned host memory
   int64_t* pr_tokens = nullptr;  // [Tmax]
+  int32_t* pos_ids = nullptr;    // [Tmax] RoBERTa position id per layout row (roberta_pos_kernel); RoBERTa handles only
   std::vector<void*> allocs;
 };
 
 namespace {
+
+// RoBERTa is BERT's encoder with position ids computed from the token ids (roberta_pos_kernel)
+bool bert_like(int arch) { return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERTA; }
+
+// longest sequence the position table covers: max_position_embeddings (BERT), max_position_embeddings - 2 (RoBERTa:
+// positions start at padding_idx + 1 = 2)
+int max_pos_len(const om_encoder_desc& d) { return d.arch == OM_ARCH_ROBERTA ? d.max_pos - 2 : d.max_pos; }
+
+// that limit's name in the packed calls' error messages
+const char* pos_limit_name(int arch) {
+  return arch == OM_ARCH_ROBERTA ? ", max_position_embeddings - 2" : arch == OM_ARCH_BERT ? ", max_position_embeddings" : "";
+}
 
 template <typename T>
 int dev_alloc(om_encoder* e, T** p, size_t count) {
@@ -1285,7 +1337,7 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, c
                   int sms, cudaStream_t st) {
   const om_encoder_desc& d = e->d;
   const int H = d.hidden, I = e->I, F = d.ffn;
-  const bool bert = d.arch == OM_ARCH_BERT;
+  const bool bert = bert_like(d.arch);
   const int rows4 = (T + 3) / 4;
   const int n_tiles = n_long + n_short;
   CUtensorMap tmQK, tmVt;
@@ -1380,7 +1432,7 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, c
 // softmax scale * log2(e) of the attention logits: BERT divides them by sqrt(head width) (1/8 for 64, 1/sqrt(32) for 32,
 // applied to the fp32 scores), T5 does not scale them
 float attn_scale_log2(const om_encoder* e) {
-  const float scale = e->d.arch == OM_ARCH_BERT ? static_cast<float>(1.0 / sqrt(static_cast<double>(e->dh))) : 1.0f;
+  const float scale = bert_like(e->d.arch) ? static_cast<float>(1.0 / sqrt(static_cast<double>(e->dh))) : 1.0f;
   return scale * kLog2e;
 }
 
@@ -1494,7 +1546,7 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
                         int n, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, int sms,
                         cudaStream_t st) {
   const om_encoder_desc& d = e->d;
-  const bool bert = d.arch == OM_ARCH_BERT;
+  const bool bert = bert_like(d.arch), roberta = d.arch == OM_ARCH_ROBERTA;
   const int H = d.hidden;
   // upload the tables through the pinned staging buffers: wait (on the host) only until the previous upload from them
   // has been read
@@ -1522,9 +1574,15 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
     if (pairs)
       pair_tokens_kernel<<<ns, 128, 0, st>>>(pairs->a, pairs->b, gs, e->pr_spans + g.k0, pairs->sp, e->pr_tokens);
     packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
-    if (bert)
-      bert_embed_kernel<<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H, d.vocab,
-                                               std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], e->rowmap, gs);
+    if (roberta) {  // positions from the ids the embedding reads (for pairs: the stream pair_tokens_kernel assembled)
+      roberta_pos_kernel<<<(ns + 3) / 4, 128, 0, st>>>(tokens, ns, 0, gs, e->pos_ids);
+      bert_embed_kernel<true><<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H,
+                                                     d.vocab, std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0],
+                                                     e->rowmap, gs, e->pos_ids);
+    } else if (bert)
+      bert_embed_kernel<false><<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H,
+                                                      d.vocab, std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0],
+                                                      e->rowmap, gs, nullptr);
     else
       t5_embed_kernel<<<rows4, 128, 0, st>>>(tokens, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], e->rowmap, gs);
     OM_CUDA(cudaGetLastError());
@@ -1542,9 +1600,10 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
   return finish_reps(e, n, out_reps, out_dtype, out_row_stride, st);
 }
 
-// the packed length limit: 512 tokens, max_position_embeddings (BERT) and max_batch_tokens
+// the packed length limit: 512 tokens, max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa) and
+// max_batch_tokens
 int packed_max_len(const om_encoder* e) {
-  return std::min(kMaxLongL, std::min(e->d.arch == OM_ARCH_BERT ? e->d.max_pos : kMaxLongL, e->Tmax));
+  return std::min(kMaxLongL, std::min(bert_like(e->d.arch) ? max_pos_len(e->d) : kMaxLongL, e->Tmax));
 }
 
 }  // namespace
@@ -1555,14 +1614,16 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   if (!desc || !out) return fail(OM_EINVAL, "om_encoder_create: null argument");
   OM_TRY(device_sm_count());
   const om_encoder_desc& d = *desc;
-  if (d.arch != OM_ARCH_BERT && d.arch != OM_ARCH_T5ENC) return fail(OM_EINVAL, "unknown arch %d", d.arch);
+  if (!bert_like(d.arch) && d.arch != OM_ARCH_T5ENC) return fail(OM_EINVAL, "unknown arch %d", d.arch);
+  if (d.arch == OM_ARCH_ROBERTA && d.max_pos < 3)
+    return fail(OM_EINVAL, "RoBERTa max_position_embeddings=%d unsupported (at least 3: positions start at 2)", d.max_pos);
   if (d.hidden <= 0 || d.hidden % 128 != 0 || d.hidden > 1024)
     return fail(OM_EINVAL, "hidden=%d unsupported (multiple of 128, <= 1024)", d.hidden);
   if (d.heads <= 0) return fail(OM_EINVAL, "heads=%d must be positive", d.heads);
   // head width: BERT's is hidden / heads, 32 or 64; T5's (d_kv) is 64
-  if (d.arch == OM_ARCH_BERT && d.hidden % d.heads != 0)
+  if (bert_like(d.arch) && d.hidden % d.heads != 0)
     return fail(OM_EINVAL, "BERT requires hidden to be a multiple of heads (got hidden=%d heads=%d)", d.hidden, d.heads);
-  const int dh = d.arch == OM_ARCH_BERT ? d.hidden / d.heads : 64;
+  const int dh = bert_like(d.arch) ? d.hidden / d.heads : 64;
   if (dh != 32 && dh != 64)
     return fail(OM_EINVAL, "BERT head width hidden/heads=%d unsupported (32 or 64; hidden=%d heads=%d)", dh, d.hidden,
                 d.heads);
@@ -1584,9 +1645,10 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   auto A = [&](auto** p, size_t n) {
     if (rc == 0) rc = dev_alloc(e, p, n);
   };
-  if (d.arch == OM_ARCH_BERT) {
+  if (bert_like(d.arch)) {
     A(&e->word, (size_t)d.vocab * H);
     A(&e->pos, (size_t)d.max_pos * H);
+    if (d.arch == OM_ARCH_ROBERTA) A(&e->pos_ids, (size_t)d.max_batch_tokens);
     A(&e->type, (size_t)std::max(d.type_vocab, 1) * H);
     A(&e->emb_g, H);
     A(&e->emb_b, H);
@@ -1619,7 +1681,7 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
       rc = fail(OM_ENOMEM, "om_encoder_create: out of device memory (weight staging)");
     }
     char buf[160];
-    if (d.arch == OM_ARCH_BERT) {
+    if (bert_like(d.arch)) {
       A(&w.bqkv_fold, (size_t)3 * I);
       A(&w.b1_fold, F);
       A(&w.bqkv, (size_t)3 * I);
@@ -1707,6 +1769,7 @@ int om_encoder_set_weight(om_encoder* e, const char* name_c, const void* data, o
   if (!e || !name_c || !data || !shape) return fail(OM_EINVAL, "om_encoder_set_weight: null argument");
   std::string name(name_c);
   if (name.rfind("bert.", 0) == 0) name = name.substr(5);  // BertFor* checkpoints prefix the backbone
+  if (name.rfind("roberta.", 0) == 0) name = name.substr(8);  // and RobertaFor* / XLMRobertaFor* ones
   const om_encoder_desc& d = e->d;
   const int H = d.hidden, I = e->I, F = d.ffn;
   e->finalized = false;
@@ -1718,7 +1781,7 @@ int om_encoder_set_weight(om_encoder* e, const char* name_c, const void* data, o
     mark(e, "head.linear.weight");
     return 0;
   }
-  if (d.arch == OM_ARCH_BERT) {
+  if (bert_like(d.arch)) {
     if (name == "embeddings.word_embeddings.weight") {
       if (!shape_is(shape, ndim, d.vocab, H)) return bad_shape(name_c);
       OM_TRY(upload(data, kind, (size_t)d.vocab * H, e->word, nullptr));
@@ -1859,7 +1922,7 @@ int om_encoder_finalize(om_encoder* e) {
   // produced its input (embeddings.LayerNorm for l = 0, else layer l-1's output.LayerNorm) and W1 takes
   // attention.output.LayerNorm; T5 block l's QKV / wi take its own pre-norm RMS weights (no beta, no mean term).
   {
-    const bool bert = e->d.arch == OM_ARCH_BERT;
+    const bool bert = bert_like(e->d.arch);
     const int H = e->d.hidden, I = e->I, F = e->d.ffn;
     for (int li = 0; li < e->d.layers; ++li) {
       LayerW& w = e->layers[li];
@@ -1902,6 +1965,8 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
                 kMaxL);
   const om_encoder_desc& d = e->d;
   if (d.arch == OM_ARCH_BERT && L > d.max_pos) return fail(OM_EINVAL, "om_encode: L=%d exceeds max_position_embeddings", L);
+  if (d.arch == OM_ARCH_ROBERTA && L > max_pos_len(d))
+    return fail(OM_EINVAL, "om_encode: L=%d exceeds max_position_embeddings - 2 = %d (RoBERTa)", L, max_pos_len(d));
   const int64_t T64 = static_cast<int64_t>(B) * L;
   if (T64 > e->Tmax) return fail(OM_EINVAL, "om_encode: B*L=%lld exceeds max_batch_tokens=%d", (long long)T64, e->Tmax);
   if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
@@ -1912,16 +1977,22 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int T = static_cast<int>(T64), H = d.hidden, I = e->I;
-  const bool bert = d.arch == OM_ARCH_BERT;
+  const bool bert = bert_like(d.arch);
   const int rows4 = (T + 3) / 4;
 
   NvtxRange nvtx("om.encode");
   keymask_kernel<<<(T + 255) / 256, 256, 0, st>>>(attention_mask, e->kmask, T);
   // the residual stream s lives in e->h (fp32, un-normalised) with a bf16 copy in e->xb and row statistics in
   // e->stats[0] (input of a layer: from the embedding or the previous FFN2) / e->stats[1] (after the attention block)
-  if (bert)
-    bert_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
-                                             std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr);
+  if (d.arch == OM_ARCH_ROBERTA) {  // positions from the ids of each whole [L] row, as HF computes them
+    roberta_pos_kernel<<<(B + 3) / 4, 128, 0, st>>>(input_ids, B, L, nullptr, e->pos_ids);
+    bert_embed_kernel<true><<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
+                                                   std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr,
+                                                   e->pos_ids);
+  } else if (bert)
+    bert_embed_kernel<false><<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
+                                                    std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr,
+                                                    nullptr);
   else
     t5_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], nullptr, nullptr);
   OM_CUDA(cudaGetLastError());
@@ -1960,7 +2031,6 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
     return fail(OM_EINVAL, "om_encode_packed: out dtype must be f32, bf16 or f16");
   const int rep_dim = om_encoder_rep_dim(e);
   if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_packed: out_row_stride < rep_dim");
-  const bool bert = e->d.arch == OM_ARCH_BERT;
   const int max_len = packed_max_len(e);
   std::vector<int64_t> tok0(static_cast<size_t>(B));
   int64_t total = 0;
@@ -1968,7 +2038,7 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
     const int l = seqlens[i];
     if (l < 1 || l > max_len)
       return fail(OM_EINVAL, "om_encode_packed: seqlens[%d]=%d outside [1, %d] (512 tokens%s, max_batch_tokens=%d)", i, l,
-                  max_len, bert ? ", max_position_embeddings" : "", e->Tmax);
+                  max_len, pos_limit_name(e->d.arch), e->Tmax);
     tok0[i] = total;
     total += l;
   }
@@ -2009,7 +2079,6 @@ int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, con
     return fail(OM_EINVAL, "om_encode_pairs: out dtype must be f32, bf16 or f16");
   const int rep_dim = om_encoder_rep_dim(e);
   if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_pairs: out_row_stride < rep_dim");
-  const bool bert = e->d.arch == OM_ARCH_BERT;
   const int max_len = packed_max_len(e);
   std::vector<int32_t> lens(static_cast<size_t>(B));
   for (int i = 0; i < B; ++i) {
@@ -2024,7 +2093,7 @@ int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, con
     const int64_t l = n_prefix + al + bl + n_suffix;
     if (l < 1 || l > max_len)
       return fail(OM_EINVAL, "om_encode_pairs: pair %d assembles %lld tokens, outside [1, %d] (512 tokens%s, "
-                  "max_batch_tokens=%d)", i, (long long)l, max_len, bert ? ", max_position_embeddings" : "", e->Tmax);
+                  "max_batch_tokens=%d)", i, (long long)l, max_len, pos_limit_name(e->d.arch), e->Tmax);
     lens[i] = static_cast<int32_t>(l);
   }
   if (B == 0) return 0;

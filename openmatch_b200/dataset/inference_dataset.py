@@ -31,12 +31,13 @@ def _ragged_prefix(path: str):
     return None
 
 
-def write_ragged_store(prefix: str, ids_2d, names=None) -> str:
-    """Writes the rows of an int ``[n, L]`` id matrix (0 = padding, dropped) as a ragged store ``<prefix>.tokens.npy`` +
-    ``<prefix>.offsets.npy`` (+ ``<prefix>.ids.txt`` when ``names`` is given); returns the path to hand to
-    ``PretokenizedDataset`` (``data_args.corpus_path`` / ``query_path``).  Every row needs at least one token."""
+def write_ragged_store(prefix: str, ids_2d, names=None, pad_id: int = 0) -> str:
+    """Writes the rows of an int ``[n, L]`` id matrix (``pad_id`` = padding, dropped: the tokenizer's pad id, 1 for
+    RoBERTa) as a ragged store ``<prefix>.tokens.npy`` + ``<prefix>.offsets.npy`` (+ ``<prefix>.ids.txt`` when ``names``
+    is given); returns the path to hand to ``PretokenizedDataset`` (``data_args.corpus_path`` / ``query_path``).  Every
+    row needs at least one token."""
     ids_2d = np.asarray(ids_2d)
-    keep = ids_2d != 0
+    keep = ids_2d != pad_id
     lens = keep.sum(1).astype(np.int64)
     if ids_2d.shape[0] and lens.min() < 1:
         raise ValueError("row %d holds no token" % int(np.argmin(lens)))
@@ -120,8 +121,9 @@ class TsvDataset(InferenceDataset):
 
 
 class PretokenizedDataset(InferenceDataset):
-    """``<name>.npy``: int32 ``[n, L]`` token ids (0 = padding); optional ``<name>.ids.txt`` with one id per
-    row.  No tokenizer involved: rows are sliced to ``max_len`` and the mask is ``ids != 0``.
+    """``<name>.npy``: int32 ``[n, L]`` token ids, padded with the tokenizer's pad id (``pad_id``: 0 for BERT and T5, 1
+    for RoBERTa; 0 without a tokenizer); optional ``<name>.ids.txt`` with one id per row.  The tokenizer is not run:
+    rows are sliced to ``max_len``, padded with ``pad_id`` and the mask is ``ids != pad_id``.
 
     Two ways out: the reference's per-example iterator (``__iter__`` -> DataLoader + DRInferenceCollator, same
     interleaving of ``batch_size`` blocks over the ranks, :99-115), and ``iter_batches()``, which hands whole
@@ -133,6 +135,11 @@ class PretokenizedDataset(InferenceDataset):
     the same optional ``<name>.ids.txt``; its path is ``<name>.tokens.npy``.  ``iter_batches()`` then yields
     ``(text_ids, tokens int32 [sum(seqlens)], seqlens int32 [b])`` (rows truncated to ``max_len``) for
     ``DRModel.encode_packed_into``, and ``__iter__`` yields padded examples as for the padded store."""
+
+    @property
+    def pad_id(self) -> int:
+        pad = getattr(self.tokenizer, "pad_token_id", None) if self.tokenizer is not None else None
+        return int(pad) if pad is not None else 0
 
     @property
     def is_ragged(self) -> bool:
@@ -199,7 +206,7 @@ class PretokenizedDataset(InferenceDataset):
             b1 = min(n, b0 + bs)
             block = ids[b0:b1, : self.max_len]
             if width < self.max_len:  # stored narrower than the model's padded length: pad like the reference does
-                padded = np.zeros((b1 - b0, self.max_len), dtype=np.int32)
+                padded = np.full((b1 - b0, self.max_len), self.pad_id, dtype=np.int32)
                 padded[:, :width] = block
                 block = padded
             yield (names[b0:b1] if names else [str(i) for i in range(b0, b1)]), block
@@ -221,8 +228,9 @@ class PretokenizedDataset(InferenceDataset):
             yield (names[b0:b1] if names else [str(i) for i in range(b0, b1)]), block, lens.astype(np.int32)
 
     def process_one(self, example):
+        pad = self.pad_id
         row = np.asarray(example["row"][: self.max_len], dtype=np.int64)
         if row.shape[0] < self.max_len:
-            row = np.pad(row, (0, self.max_len - row.shape[0]))
-        return {"text_id": get_idx(example), "input_ids": row.tolist(), "attention_mask": (row != 0).astype(np.int64).tolist(),
+            row = np.pad(row, (0, self.max_len - row.shape[0]), constant_values=pad)
+        return {"text_id": get_idx(example), "input_ids": row.tolist(), "attention_mask": (row != pad).astype(np.int64).tolist(),
                 "token_type_ids": [0] * self.max_len}

@@ -28,9 +28,31 @@ def _check_bert_heads(hidden: int, heads: int):
                          % (hidden, heads))
 
 
+ROBERTA_PAD_ID = 1  # padding_idx of RoBERTa's position ids, fixed in the library (include/openmatch_b200.h)
+
+_ARCHS = {"bert": _lib.OM_ARCH_BERT, "t5": _lib.OM_ARCH_T5ENC, "roberta": _lib.OM_ARCH_ROBERTA}
+
+
 def spec_from_hf_config(config) -> Dict:
-    """Translate a HF ``BertConfig`` / ``T5Config`` into the plain dict ``CudaEncoder`` consumes."""
+    """Translate a HF ``BertConfig`` / ``RobertaConfig`` / ``XLMRobertaConfig`` / ``T5Config`` into the plain dict
+    ``CudaEncoder`` consumes."""
     mt = getattr(config, "model_type", "")
+    if mt in ("roberta", "xlm-roberta"):
+        _check_bert_heads(config.hidden_size, config.num_attention_heads)
+        if getattr(config, "hidden_act", "gelu") != "gelu":
+            raise ValueError("CUDA encoder supports hidden_act='gelu' (erf) only, got %r" % config.hidden_act)
+        if getattr(config, "position_embedding_type", "absolute") not in (None, "absolute"):
+            raise ValueError("CUDA encoder supports absolute position embeddings only")
+        if config.pad_token_id != ROBERTA_PAD_ID:
+            raise ValueError("CUDA encoder computes RoBERTa position ids with padding_idx %d, got pad_token_id=%r"
+                             % (ROBERTA_PAD_ID, config.pad_token_id))
+        if config.max_position_embeddings < 3:
+            raise ValueError("RoBERTa max_position_embeddings=%d leaves no position (positions start at 2)"
+                             % config.max_position_embeddings)
+        return dict(arch="roberta", layers=config.num_hidden_layers, hidden=config.hidden_size,
+                    heads=config.num_attention_heads, ffn=config.intermediate_size, vocab=config.vocab_size,
+                    max_pos=config.max_position_embeddings, type_vocab=config.type_vocab_size,
+                    ln_eps=config.layer_norm_eps)
     if mt == "bert":
         _check_bert_heads(config.hidden_size, config.num_attention_heads)
         if getattr(config, "hidden_act", "gelu") != "gelu":
@@ -50,7 +72,7 @@ def spec_from_hf_config(config) -> Dict:
                     ffn=config.d_ff, vocab=config.vocab_size, max_pos=0, type_vocab=0,
                     ln_eps=config.layer_norm_epsilon, rel_buckets=config.relative_attention_num_buckets,
                     rel_max_distance=getattr(config, "relative_attention_max_distance", 128))
-    raise ValueError("CUDA encoder supports BERT and T5-encoder backbones, got model_type=%r" % mt)
+    raise ValueError("CUDA encoder supports BERT, RoBERTa / XLM-RoBERTa and T5-encoder backbones, got model_type=%r" % mt)
 
 
 class CudaEncoder:
@@ -58,12 +80,14 @@ class CudaEncoder:
                  pooling: str = "first", normalize: bool = False, max_batch_tokens: int = 256 * 128):
         if pooling not in ("first", "mean"):
             raise ValueError("Unknown pooling type: {}".format(pooling))
-        if spec["arch"] == "bert":
+        if spec["arch"] not in _ARCHS:
+            raise ValueError("Unknown encoder arch %r" % spec["arch"])
+        if spec["arch"] in ("bert", "roberta"):
             _check_bert_heads(spec["hidden"], spec["heads"])
         self._lib = _lib.load()
         head_head_out = int(head_weight.shape[0]) if head_weight is not None else 0
         desc = _lib.EncoderDesc(
-            arch=_lib.OM_ARCH_BERT if spec["arch"] == "bert" else _lib.OM_ARCH_T5ENC, layers=spec["layers"],
+            arch=_ARCHS[spec["arch"]], layers=spec["layers"],
             hidden=spec["hidden"], heads=spec["heads"], ffn=spec["ffn"], vocab=spec["vocab"],
             max_pos=spec.get("max_pos", 0), type_vocab=spec.get("type_vocab", 0), ln_eps=float(spec["ln_eps"]),
             pooling=_lib.OM_POOL_MEAN if pooling == "mean" else _lib.OM_POOL_FIRST,

@@ -81,8 +81,12 @@ class RRModel(nn.Module):
 
     # ------------------------------------------------------------------ scoring
     def max_pair_len(self) -> int:
-        """longest assembled pair the model takes: 512, and max_position_embeddings for BERT"""
-        return min(512, getattr(self.lm.config, "max_position_embeddings", None) or 512)
+        """longest assembled pair the model takes: 512, and max_position_embeddings for BERT (minus RoBERTa's position
+        offset of 2)"""
+        max_pos = getattr(self.lm.config, "max_position_embeddings", None) or 512
+        if getattr(self.lm.config, "model_type", "") in ("roberta", "xlm-roberta"):
+            max_pos -= 2
+        return min(512, max_pos)
 
     def _cuda_encoder(self):
         from ..encoder import CudaEncoder

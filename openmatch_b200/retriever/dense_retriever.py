@@ -150,10 +150,11 @@ class Retriever:
 
     def _encode_blocks(self, dataset, is_query: bool, into_index: bool):
         """Block ingest: memory-mapped int32 ``[b, L]`` slice -> pinned staging buffer (double-buffered) -> async H2D
-        -> int64 ids + mask built on the device -> encoder (-> index rows in place)."""
+        -> int64 ids + mask (``ids != dataset.pad_id``) built on the device -> encoder (-> index rows in place)."""
         if getattr(dataset, "is_ragged", False) and hasattr(self.model, "encode_packed_into"):
             return self._encode_ragged_blocks(dataset, is_query, into_index)
         device = self.args.device
+        pad_id = getattr(dataset, "pad_id", 0)
         ids: List[str] = []
         chunks: List[torch.Tensor] = []
         bs, L = dataset.batch_size, dataset.max_len
@@ -174,7 +175,7 @@ class Retriever:
             d_ids = stage[slot][:n].to(device, non_blocking=True)
             busy[slot] = torch.cuda.Event()
             busy[slot].record()
-            batch = {"input_ids": d_ids.long(), "attention_mask": (d_ids != 0).long()}
+            batch = {"input_ids": d_ids.long(), "attention_mask": (d_ids != pad_id).long()}
             ids.extend(names)
             if into_index:
                 self._encode_rows_in_place(batch, is_query)

@@ -9,7 +9,7 @@ on the device until one copy at the end.
 
 Pair content (``DESIGN.md`` §6): the query / passage ids of ``InferenceDataset(final=False)``, i.e. the text rendered
 through its template and tokenised without special tokens, truncated to ``q_max_len`` / ``p_max_len``; a pretokenised
-row without its padding zeros and, when it starts with the tokenizer's prefix and ends with its suffix, without those.
+row without its padding (the tokenizer's pad id) and, when it starts with the tokenizer's prefix and ends with its suffix, without those.
 """
 from __future__ import annotations
 
@@ -54,10 +54,11 @@ def assemble_pairs(a_tokens: np.ndarray, b_tokens: np.ndarray, spans: np.ndarray
     return np.array([t for r in rows for t in r], dtype=np.int64), lens
 
 
-def _content(row: np.ndarray, prefix: Sequence[int], suffix: Sequence[int], max_len: int) -> np.ndarray:
-    """a pretokenised row's pair content: padding zeros dropped, a dense-retrieval row's special tokens stripped"""
+def _content(row: np.ndarray, prefix: Sequence[int], suffix: Sequence[int], max_len: int, pad_id: int = 0) -> np.ndarray:
+    """a pretokenised row's pair content: the padding (the tokenizer's pad id) dropped, a dense-retrieval row's special
+    tokens stripped"""
     row = np.asarray(row)
-    row = row[row != 0]
+    row = row[row != pad_id]
     npre, nsuf = len(prefix), len(suffix)
     if (npre or nsuf) and row.shape[0] >= npre + nsuf and list(row[:npre]) == list(prefix) \
             and list(row[row.shape[0] - nsuf:]) == list(suffix):
@@ -79,7 +80,7 @@ def token_store(dataset, ids: Sequence[str], prefix: Sequence[int], suffix: Sequ
             if i is None:
                 continue
             row = store[0][store[1][i]:store[1][i + 1]] if isinstance(store, tuple) else store[i]
-            rows[name] = _content(row, prefix, suffix, dataset.max_len)
+            rows[name] = _content(row, prefix, suffix, dataset.max_len, dataset.pad_id)
     else:  # text: tokenised once per id, as InferenceDataset(final=False) does
         for rec in dataset._records():
             name = get_idx(rec)
