@@ -47,7 +47,8 @@ typedef enum { OM_HOST = 0, OM_DEVICE = 1 } om_memkind;
  * "roberta.") whose position ids come from the token ids, as HF's create_position_ids_from_input_ids computes them with
  * padding_idx = pad_token_id = 1 (the value of every such config; fixed here): a token with id != 1 gets position
  * 1 + (number of ids != 1 up to and including it in its sequence), a token with id 1 gets position 1, whatever the
- * attention mask says.  Sequences are at most max_position_embeddings - 2 tokens long. */
+ * attention mask says.  Sequences are at most max_position_embeddings - 2 tokens long (8194 positions, as in
+ * XLM-RoBERTa-based bge-m3: 8192 tokens, the longest om_encode_packed takes). */
 typedef enum { OM_ARCH_BERT = 0, OM_ARCH_T5ENC = 1, OM_ARCH_ROBERTA = 2 } om_arch;
 typedef enum { OM_POOL_FIRST = 0, OM_POOL_MEAN = 1 } om_pooling;
 typedef enum { OM_REDUCE_MEAN = 0, OM_REDUCE_SUM = 1 } om_reduction;
@@ -106,15 +107,17 @@ int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attentio
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
               int64_t out_row_stride, float* out_hidden, void* stream);
 /* Variable-length batch, no padding.  tokens / token_type_ids (nullable => zeros; ignored for T5): int64 [T] device, the
- * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 512 (BERT: <= max_position_embeddings; RoBERTa:
- * <= max_position_embeddings - 2, positions computed from each sequence's own ids; and
- * <= max_batch_tokens), T = sum(seqlens).  Result: what om_encode returns for the same sequences padded to any L with
- * attention_mask = 1 on their tokens, up to the order of floating-point sums in attention and pooling.  out_reps as in
+ * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 8192 for BERT (and <= max_position_embeddings)
+ * and RoBERTa (and <= max_position_embeddings - 2, positions computed from each sequence's own ids), <= 512 for T5 (its
+ * relative-bias tables cover 512 tokens); and <= max_batch_tokens; T = sum(seqlens).  Result: what om_encode returns
+ * for the same sequences padded to any L it takes with attention_mask = 1 on their tokens, up to the order of
+ * floating-point sums in attention and pooling (longer sequences have no padded counterpart).  out_reps as in
  * om_encode (row i = sequence i).  out_hidden: nullable fp32 [T, hidden], packed like tokens.  seqlens may be reused on
  * return; no device synchronisation; asynchronous on `stream`.
  * Layout: sequences of <= 128 tokens are bin-packed whole into 128-row attention tiles (first-fit decreasing, ties by
  * input index: a deterministic function of seqlens); a longer one starts on a tile boundary and takes ceil(l / 128)
- * tiles.  A layout of more than max_batch_tokens rows is encoded as consecutive groups of tiles on `stream`.
+ * tiles, those of more than 512 tokens first (a pipelined attention kernel), then those of 129-512 tokens, then the
+ * bins.  A layout of more than max_batch_tokens rows is encoded as consecutive groups of tiles on `stream`.
  * Invalid input (a null pointer, B < 0, a length outside the range above) returns OM_EINVAL and writes nothing. */
 int om_encode_packed(om_encoder* enc, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens,
                      int B, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream);

@@ -38,7 +38,8 @@ namespace om {
 
 constexpr int kAttnCols = 64;    // columns of Q, K and V^T an attention work item loads: one 64-wide or two 32-wide heads
 constexpr int kMaxL = 128;       // one attention tile; sequences of at most kMaxL tokens take attn_kernel
-constexpr int kMaxLongL = 512;   // longer sequences (multiples of 128 tokens) take attn_long_kernel
+constexpr int kMaxLongL = 512;   // longer sequences (multiples of 128 tokens) take attn_long_kernel, longer packed
+                                 // ones attn_stream_kernel
 constexpr float kLog2e = 1.4426950408889634f;
 
 // ===================================================================================================
@@ -1060,6 +1061,184 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
     }
 }
 
+// ---------------------------------------------------------------------------------------------------
+// Sequences of kMaxLongL + 1 .. kMaxStreamL tokens (packed layout only): one CTA of three warpgroups per (128-row query
+// tile, unit), the online softmax of attn_long_kernel on a pipeline.  At these lengths attention is most of a layer
+// (4 L^2 I FLOP against 24 L H^2 for the GEMMs), and at head width 64 the exponentials take about as long as the MMAs,
+// so the loads must run ahead of the compute and the two halves of the query tile must not wait for each other:
+//   producer  warp 0: Q once, then the sequence's 128-key tiles (K, V^T: 32 KB, and the tile's key-validity bits,
+//             one ballot of kmask per 32 keys) into a ring of kAttnStreamStages slots with full / empty mbarriers
+//             (ring.cuh); warps 1-3 only hand their registers over (setmaxnreg)
+//   consumers warpgroups 1 and 2 own query rows [0, 64) and [64, 128) of the tile and walk the ring independently,
+//             S_j = Q K_j^T (wgmma) -> running max / sum -> P_j (bf16, registers) -> O = O alpha + P_j V_j (wgmma), and
+//             release a slot once both of its MMAs have completed; while one warpgroup is in its softmax the other's
+//             wgmma run.
+// The key-validity bits come per key tile, so the length is bounded by nothing the kernel sizes.  Keys of a tile that
+// are all valid (every tile but a sequence's last) skip the masking.  Padding rows after a sequence's last token attend
+// like its tokens (finite values nobody reads).
+// ---------------------------------------------------------------------------------------------------
+constexpr int kMaxStreamL = 8192;
+constexpr int kAttnStreamStages = 4;
+constexpr int kAttnStreamThreads = 384;
+constexpr int kAttnStreamStageBytes = 32768;  // K [128 keys, 64 cols] + V^T as two [64 cols, 64 keys] boxes
+constexpr int kAttnStreamSmemRing = 16384;    // after Q [128 rows, 64 cols]
+constexpr int kAttnStreamSmemMisc = kAttnStreamSmemRing + kAttnStreamStages * kAttnStreamStageBytes;
+// misc: key bits [stages][4] u32, full[stages], empty[stages], Q barrier
+constexpr int kAttnStreamSmemBytes = kAttnStreamSmemMisc + kAttnStreamStages * 16 + (2 * kAttnStreamStages + 1) * 8 + 1024;
+
+template <int DH>
+__global__ void __launch_bounds__(kAttnStreamThreads, 1)
+attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p) {
+  constexpr int NH = kAttnCols / DH;  // heads per unit
+  constexpr int S = kAttnStreamStages;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint32_t* s_kb = reinterpret_cast<uint32_t*>(smem + kAttnStreamSmemMisc);  // [S][4]: key bits of each slot
+  uint64_t* full = reinterpret_cast<uint64_t*>(s_kb + 4 * S);
+  uint64_t* empty = full + S;
+  uint64_t* qbar = empty + S;
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int qt = blockIdx.x, unit = blockIdx.y;
+  const int row0 = qt * 128;  // first row of this query tile
+  // the sequence starts on a tile boundary and the tile's first row is one of its tokens (place_packed)
+  const int2 mp = p.rowmap[row0];
+  const int nk = (p.seqs[mp.x].len + 127) / 128;  // key tiles of the sequence
+  const int kt0 = qt - mp.y / 128;                 // its first tile
+
+  if (tid == 0) {
+    tma_prefetch_desc(&tmQK);
+    tma_prefetch_desc(&tmVt);
+    ring_init(full, empty, S, 8);  // a slot is released by each of the 8 consumer warps
+    mbar_init(qbar, 1);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ------------------------------ producer warpgroup ------------------------------
+    setmaxnreg_dec<40>();
+    if (warp != 0) return;
+    if (lane == 0) {
+      mbar_arrive_expect_tx(qbar, 16384);
+      tma_load_2d(smem, &tmQK, qbar, unit * kAttnCols, row0);
+    }
+    Ring<S> ring;
+#pragma unroll 1
+    for (int j = 0; j < nk; ++j, ring.advance()) {
+      const int k0 = (kt0 + j) * 128;
+      unsigned bits[4];
+#pragma unroll
+      for (int w = 0; w < 4; ++w) {
+        const int tok = k0 + 32 * w + lane;
+        bits[w] = __ballot_sync(0xffffffffu, tok < p.T && p.kmask[tok] == 0.f);
+      }
+      if (lane == 0) {
+        ring_wait_free(empty, ring, 14);
+        uint32_t* kb = s_kb + 4 * ring.stage;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) kb[w] = bits[w];
+        // the arrive releases the bit stores above to every consumer that sees the slot's phase complete
+        mbar_arrive_expect_tx(&full[ring.stage], kAttnStreamStageBytes);
+        uint8_t* slot = smem + kAttnStreamSmemRing + ring.stage * kAttnStreamStageBytes;
+        tma_load_2d(slot, &tmQK, &full[ring.stage], p.I + unit * kAttnCols, k0);
+        tma_load_2d(slot + 16384, &tmVt, &full[ring.stage], k0, unit * kAttnCols);
+        tma_load_2d(slot + 16384 + 8192, &tmVt, &full[ring.stage], k0 + 64, unit * kAttnCols);
+      }
+      __syncwarp();
+    }
+    return;
+  }
+
+  // ------------------------------ consumer warpgroups ------------------------------
+  setmaxnreg_inc<232>();
+  const int wg = (warp >> 2) - 1;  // 64-row half of the tile
+  const uint32_t qa = smem_u32(smem) + wg * 8192, ring_a = smem_u32(smem + kAttnStreamSmemRing);
+  const float scale = p.scale_log2;
+  int rr[2];
+  float m_run[NH][2], sum[NH][2], o[NH][DH / 2];  // m_run: running maximum of the raw (unscaled) scores
+#pragma unroll
+  for (int u = 0; u < 2; ++u) rr[u] = wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * u;
+#pragma unroll
+  for (int hd = 0; hd < NH; ++hd) {
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      m_run[hd][u] = __int_as_float(0xff800000);
+      sum[hd][u] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < DH / 2; ++i) o[hd][i] = 0.f;
+  }
+  mbar_wait_warp(qbar, 0, 15);
+  Ring<S> ring;
+#pragma unroll 1
+  for (int j = 0; j < nk; ++j, ring.advance()) {
+    mbar_wait_warp(&full[ring.stage], ring.phase, 16);
+    const uint32_t ka = ring_a + ring.stage * kAttnStreamStageBytes, va = ka + 16384;
+    const uint32_t* kb = s_kb + 4 * ring.stage;
+    const bool all_keys = (kb[0] & kb[1] & kb[2] & kb[3]) == 0xffffffffu;
+#pragma unroll
+    for (int hd = 0; hd < NH; ++hd) {
+      float sc[64];
+      attn_scores<DH>(sc, qa + hd * DH * 2, ka + hd * DH * 2);
+      if (!all_keys) {
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
+            if (!((kb[c >> 5] >> (c & 31)) & 1u)) sc[4 * jj + e] = __int_as_float(0xff800000);
+          }
+      }
+      float m_j[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) m_j[e >> 1] = fmaxf(m_j[e >> 1], sc[4 * jj + e]);
+      // softmax in the log2 domain: p = 2^(s * scale - m * scale), one FFMA and one ex2 per score (scale > 0, so the
+      // maximum of the scaled scores is the scaled maximum)
+      float alpha[2], mm[2];
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const float m_new = fmaxf(m_run[hd][u], quad_max(m_j[u]));
+        mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new * scale : 0.f;  // no allowed key seen so far: all p = 0
+        alpha[u] = (m_run[hd][u] > __int_as_float(0xff800000)) ? ex2_approx(fmaf(m_run[hd][u], scale, -mm[u])) : 0.f;
+        m_run[hd][u] = m_new;
+        sum[hd][u] *= alpha[u];
+      }
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float pv = ex2_approx(fmaf(sc[4 * jj + e], scale, -mm[e >> 1]));  // ex2(-inf) = 0 for masked keys
+          sc[4 * jj + e] = pv;
+          sum[hd][e >> 1] += pv;
+        }
+#pragma unroll
+      for (int i = 0; i < DH / 2; ++i) o[hd][i] *= alpha[(i >> 1) & 1];
+      attn_pv<DH>(o[hd], sc, va + hd * DH * 128, 1u);
+    }
+    // both MMAs of every head have completed (attn_pv waits for its group): the slot may be refilled
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[ring.stage]);
+  }
+
+#pragma unroll
+  for (int hd = 0; hd < NH; ++hd)
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const float tot = quad_sum(sum[hd][u]);
+      const float inv = tot > 0.f ? 1.0f / tot : 0.f;
+      if (row0 + rr[u] < p.T) {
+        __nv_bfloat16* dst = p.ctx + static_cast<int64_t>(row0 + rr[u]) * p.I + unit * kAttnCols + hd * DH + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < DH / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jj) =
+              pack_bf16x2(o[hd][4 * jj + 2 * u] * inv, o[hd][4 * jj + 2 * u + 1] * inv);
+      }
+    }
+}
+
 // ===================================================================================================
 // pooling / head / normalise (fp32)
 // ===================================================================================================
@@ -1273,11 +1452,6 @@ bool bert_like(int arch) { return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERT
 // positions start at padding_idx + 1 = 2)
 int max_pos_len(const om_encoder_desc& d) { return d.arch == OM_ARCH_ROBERTA ? d.max_pos - 2 : d.max_pos; }
 
-// that limit's name in the packed calls' error messages
-const char* pos_limit_name(int arch) {
-  return arch == OM_ARCH_ROBERTA ? ", max_position_embeddings - 2" : arch == OM_ARCH_BERT ? ", max_position_embeddings" : "";
-}
-
 template <typename T>
 int dev_alloc(om_encoder* e, T** p, size_t count) {
   void* q = nullptr;
@@ -1331,19 +1505,36 @@ bool shape_is(const int64_t* shape, int ndim, int64_t a, int64_t b = -1) {
 int bad_shape(const char* name) { return fail(OM_EINVAL, "om_encoder_set_weight: unexpected shape for '%s'", name); }
 
 // The layers and the final normalisation over T token rows whose embedding (e->h, e->xb, e->stats[0]) and key mask
-// (e->kmask) are in place.  Attention: tiles [0, n_long) run attn_long_kernel with ap_long, the next n_short tiles
-// attn_kernel with ap_short (tile0 = n_long); ap_short.Tvalid_rows is the tile-local V^T layout of EpiQKV.
-int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, const AttnParams& ap_short, int n_short,
-                  int sms, cudaStream_t st) {
+// (e->kmask) are in place.  Attention: tiles [0, n_stream) run attn_stream_kernel with ap_long, the next n_long tiles
+// attn_long_kernel with ap_long seen from its first tile on, the next n_short tiles attn_kernel with ap_short
+// (tile0 = n_stream + n_long); ap_short.Tvalid_rows is the tile-local V^T layout of EpiQKV.
+int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_stream, int n_long, const AttnParams& ap_short,
+                  int n_short, int sms, cudaStream_t st) {
   const om_encoder_desc& d = e->d;
   const int H = d.hidden, I = e->I, F = d.ffn;
   const bool bert = bert_like(d.arch);
   const int rows4 = (T + 3) / 4;
-  const int n_tiles = n_long + n_short;
+  const int n_tiles = n_stream + n_long + n_short;
   CUtensorMap tmQK, tmVt;
   if (make_tmap_bf16_2d(&tmQK, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 128) != 0 ||
       make_tmap_bf16_2d(&tmVt, e->vt, (uint64_t)n_tiles * 128, (uint64_t)I, (uint64_t)e->Tld * 2, 64, 64) != 0)
     return fail(OM_ECUDA, "om_encode: tensor map creation failed");
+  // attn_long_kernel numbers its query tiles from the first row it sees: behind the stream tiles it gets tensor maps,
+  // row map, key mask and output that start at its first tile (the packed layout is position-independent)
+  CUtensorMap tmQKl = tmQK, tmVtl = tmVt;
+  AttnParams apl = ap_long;
+  if (n_stream > 0 && n_long > 0) {
+    const int off = n_stream * 128;
+    if (make_tmap_bf16_2d(&tmQKl, e->qk + (size_t)off * 2 * I, (uint64_t)2 * I, (uint64_t)(T - off), (uint64_t)2 * I * 2,
+                          64, 128) != 0 ||
+        make_tmap_bf16_2d(&tmVtl, e->vt + off, (uint64_t)(n_tiles - n_stream) * 128, (uint64_t)I, (uint64_t)e->Tld * 2,
+                          64, 64) != 0)
+      return fail(OM_ECUDA, "om_encode: tensor map creation failed");
+    apl.T = T - off;
+    apl.kmask += off;
+    apl.ctx += (size_t)off * I;
+    apl.rowmap += off;
+  }
 
   // TMA-store tensor maps of the bf16 GEMM outputs (box = 64 columns x 32 rows = one epilogue warp's chunk pair) and the
   // residual stream's maps (fp32 load + store, bf16 store; box = 32 columns x 32 rows = one chunk)
@@ -1380,11 +1571,18 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_long, c
       if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
     }
     const int units = I / kAttnCols;  // work items per tile: one per 64-wide head or pair of 32-wide heads
+    if (n_stream > 0) {
+      const dim3 grid(n_stream, units);
+      if (e->dh == 64)
+        attn_stream_kernel<64><<<grid, kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
+      else
+        attn_stream_kernel<32><<<grid, kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
+    }
     if (n_long > 0) {
       if (e->dh == 64)
-        attn_long_kernel<64><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
+        attn_long_kernel<64><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
       else
-        attn_long_kernel<32><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQK, tmVt, ap_long);
+        attn_long_kernel<32><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
     }
     if (n_short > 0) {
       const int grid = std::min(n_short * units, sms * kAttnCtasPerSm);
@@ -1463,14 +1661,16 @@ int finish_reps(om_encoder* e, int B, void* out_reps, om_dtype out_dtype, int64_
 //   * a sequence of more than 128 tokens starts on a tile boundary and takes ceil(l / 128) tiles, in input order;
 //   * the others are bin-packed whole into tiles of min(128, Tmax) rows, first-fit decreasing (ties by input index:
 //     placement is a deterministic function of the lengths), each bin's sequences back to back in insertion order;
-//   * layout = the long sequences' tiles, then the bins; cut into row groups of at most Tmax rows at unit (sequence /
-//     bin) boundaries, each group encoded on its own (its long tiles come first).  The last unit of a group is counted
-//     up to its last token.
+//   * layout = the tiles of the sequences of more than 512 tokens (attn_stream_kernel), then those of the other long
+//     sequences (attn_long_kernel), then the bins (attn_kernel); cut into row groups of at most Tmax rows at unit
+//     (sequence / bin) boundaries, each group encoded on its own (in the same order).  The last unit of a group is
+//     counted up to its last token.  Without a sequence of more than 512 tokens the first class is empty.
 // seqs receives the table in layout order (row0 relative to its group, out = index in the chunk).
 struct PackedGroup {
   int k0, k1;     // sequences [k0, k1) of the table
   int T;          // layout rows of the group
-  int n_long;     // tiles of long sequences (the first tiles of the group)
+  int n_stream;   // tiles of sequences of more than kMaxLongL tokens (the first tiles of the group)
+  int n_long;     // tiles of the other sequences of more than kMaxL tokens (the next ones)
   int n_tiles;
 };
 
@@ -1479,8 +1679,8 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
   seqs.clear();
   groups.clear();
   const int cap = std::min(kMaxL, Tmax);
-  std::vector<int> longs, shorts;
-  for (int i = 0; i < n; ++i) (len[i] > kMaxL ? longs : shorts).push_back(i);
+  std::vector<int> streams, longs, shorts;
+  for (int i = 0; i < n; ++i) (len[i] > kMaxLongL ? streams : len[i] > kMaxL ? longs : shorts).push_back(i);
   std::stable_sort(shorts.begin(), shorts.end(), [&](int a, int b) { return len[a] > len[b]; });
   std::vector<std::vector<int>> bins;
   std::vector<int> fill;
@@ -1500,13 +1700,14 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
     fill[best] += len[i];
     by_room[cap - fill[best]].insert(best);
   }
-  PackedGroup g{0, 0, 0, 0, 0};
+  PackedGroup g{0, 0, 0, 0, 0, 0};
   int row = 0;  // group-local first row of the next unit (a tile boundary)
-  auto unit = [&](const std::vector<int>& members, int tiles, int used, bool is_long) {
+  // kind: 2 = more than kMaxLongL tokens, 1 = more than kMaxL, 0 = a bin
+  auto unit = [&](const std::vector<int>& members, int tiles, int used, int kind) {
     if (row > 0 && row + (tiles - 1) * 128 + used > Tmax) {
       g.k1 = static_cast<int>(seqs.size());
       groups.push_back(g);
-      g = PackedGroup{g.k1, g.k1, 0, 0, 0};
+      g = PackedGroup{g.k1, g.k1, 0, 0, 0, 0};
       row = 0;
     }
     int off = 0;
@@ -1515,15 +1716,17 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
       off += len[i];
     }
     g.T = row + (tiles - 1) * 128 + used;
-    g.n_long += is_long ? tiles : 0;
+    g.n_stream += kind == 2 ? tiles : 0;
+    g.n_long += kind == 1 ? tiles : 0;
     g.n_tiles += tiles;
     row += tiles * 128;
   };
-  for (int i : longs) {
-    const int tiles = (len[i] + 127) / 128;
-    unit(std::vector<int>{i}, tiles, len[i] - (tiles - 1) * 128, true);
-  }
-  for (size_t b = 0; b < bins.size(); ++b) unit(bins[b], 1, fill[b], false);
+  for (int k = 2; k >= 1; --k)
+    for (int i : k == 2 ? streams : longs) {
+      const int tiles = (len[i] + 127) / 128;
+      unit(std::vector<int>{i}, tiles, len[i] - (tiles - 1) * 128, k);
+    }
+  for (size_t b = 0; b < bins.size(); ++b) unit(bins[b], 1, fill[b], 0);
   g.k1 = static_cast<int>(seqs.size());
   if (g.k1 > g.k0) groups.push_back(g);
 }
@@ -1591,8 +1794,8 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
     AttnParams ap_long = ap, ap_short = ap;
     ap_long.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
     ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
-    ap_short.tile0 = g.n_long;
-    OM_TRY(encode_layers(e, T, ap_long, g.n_long, ap_short, g.n_tiles - g.n_long, sms, st));
+    ap_short.tile0 = g.n_stream + g.n_long;
+    OM_TRY(encode_layers(e, T, ap_long, g.n_stream, g.n_long, ap_short, g.n_tiles - g.n_stream - g.n_long, sms, st));
     if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
     pool_packed_kernel<<<ns, 256, 0, st>>>(e->h, gs, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
     OM_CUDA(cudaGetLastError());
@@ -1600,10 +1803,17 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
   return finish_reps(e, n, out_reps, out_dtype, out_row_stride, st);
 }
 
-// the packed length limit: 512 tokens, max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa) and
-// max_batch_tokens
+// the packed length limit: 8192 tokens and max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa), 512
+// tokens (T5: its relative-bias tables cover 512), and max_batch_tokens
 int packed_max_len(const om_encoder* e) {
-  return std::min(kMaxLongL, std::min(bert_like(e->d.arch) ? max_pos_len(e->d) : kMaxLongL, e->Tmax));
+  return std::min(bert_like(e->d.arch) ? std::min(kMaxStreamL, max_pos_len(e->d)) : kMaxLongL, e->Tmax);
+}
+
+// the packed calls' error message: the limits behind packed_max_len
+const char* packed_limit_name(int arch) {
+  return arch == OM_ARCH_ROBERTA ? "8192 tokens, max_position_embeddings - 2"
+         : arch == OM_ARCH_BERT  ? "8192 tokens, max_position_embeddings"
+                                 : "512 tokens (T5)";
 }
 
 }  // namespace
@@ -1948,6 +2158,8 @@ int om_encoder_finalize(om_encoder* e) {
     OM_CUDA(cudaFuncSetAttribute(attn_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
     OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
     OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
+    OM_CUDA(cudaFuncSetAttribute(attn_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnStreamSmemBytes));
+    OM_CUDA(cudaFuncSetAttribute(attn_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnStreamSmemBytes));
     attr = true;
   }
   e->finalized = true;
@@ -2013,7 +2225,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   ap.seqs = nullptr;
   ap.tile0 = 0;
   const int n_tiles = long_seq ? T / 128 : (B + spt - 1) / spt;
-  OM_TRY(encode_layers(e, T, ap, long_seq ? n_tiles : 0, ap, long_seq ? 0 : n_tiles, sms, st));
+  OM_TRY(encode_layers(e, T, ap, 0, long_seq ? n_tiles : 0, ap, long_seq ? 0 : n_tiles, sms, st));
   if (out_hidden)
     OM_CUDA(cudaMemcpyAsync(out_hidden, e->h, static_cast<size_t>(T) * H * 4, cudaMemcpyDeviceToDevice, st));
 
@@ -2037,8 +2249,8 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
   for (int i = 0; i < B; ++i) {
     const int l = seqlens[i];
     if (l < 1 || l > max_len)
-      return fail(OM_EINVAL, "om_encode_packed: seqlens[%d]=%d outside [1, %d] (512 tokens%s, max_batch_tokens=%d)", i, l,
-                  max_len, pos_limit_name(e->d.arch), e->Tmax);
+      return fail(OM_EINVAL, "om_encode_packed: seqlens[%d]=%d outside [1, %d] (%s, max_batch_tokens=%d)", i, l,
+                  max_len, packed_limit_name(e->d.arch), e->Tmax);
     tok0[i] = total;
     total += l;
   }
@@ -2092,8 +2304,8 @@ int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, con
                   i, (long long)a0, (long long)al, (long long)a_total, (long long)b0, (long long)bl, (long long)b_total);
     const int64_t l = n_prefix + al + bl + n_suffix;
     if (l < 1 || l > max_len)
-      return fail(OM_EINVAL, "om_encode_pairs: pair %d assembles %lld tokens, outside [1, %d] (512 tokens%s, "
-                  "max_batch_tokens=%d)", i, (long long)l, max_len, pos_limit_name(e->d.arch), e->Tmax);
+      return fail(OM_EINVAL, "om_encode_pairs: pair %d assembles %lld tokens, outside [1, %d] (%s, "
+                  "max_batch_tokens=%d)", i, (long long)l, max_len, packed_limit_name(e->d.arch), e->Tmax);
     lens[i] = static_cast<int32_t>(l);
   }
   if (B == 0) return 0;

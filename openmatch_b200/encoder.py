@@ -75,6 +75,21 @@ def spec_from_hf_config(config) -> Dict:
     raise ValueError("CUDA encoder supports BERT, RoBERTa / XLM-RoBERTa and T5-encoder backbones, got model_type=%r" % mt)
 
 
+MAX_SEQ_LEN = 8192     # longest sequence of a packed call for BERT / RoBERTa (include/openmatch_b200.h)
+MAX_T5_SEQ_LEN = 512   # T5: its relative-bias tables cover 512 tokens
+
+
+def max_seq_len(spec: Dict, max_batch_tokens: int = 256 * 128) -> int:
+    """Longest sequence ``encode_packed`` / ``encode_pairs`` take for ``spec`` (a ``spec_from_hf_config`` dict) on a
+    handle of ``max_batch_tokens``: 8192 tokens and ``max_position_embeddings`` (BERT) / ``max_position_embeddings - 2``
+    (RoBERTa, whose positions start at 2); 512 tokens for T5; never more than ``max_batch_tokens``."""
+    if spec["arch"] == "t5":
+        limit = MAX_T5_SEQ_LEN
+    else:
+        limit = min(MAX_SEQ_LEN, spec["max_pos"] - (2 if spec["arch"] == "roberta" else 0))
+    return min(limit, int(max_batch_tokens))
+
+
 class CudaEncoder:
     def __init__(self, spec: Dict, state_dict: Dict[str, torch.Tensor], head_weight: Optional[torch.Tensor] = None,
                  pooling: str = "first", normalize: bool = False, max_batch_tokens: int = 256 * 128):
@@ -158,8 +173,9 @@ class CudaEncoder:
                       out: Optional[torch.Tensor] = None, out_dtype: torch.dtype = torch.float32,
                       return_hidden: bool = False):
         """Variable-length batch without padding: ``tokens`` int64 ``[T]`` CUDA tensor holding the sequences back to
-        back, ``seqlens`` their lengths (host int32 array / list / CPU tensor, each in [1, 512], sum = T) -> reps
-        ``[B, rep_dim]`` (and last_hidden_state fp32 ``[T, H]``, packed like ``tokens``).  The same representations
+        back, ``seqlens`` their lengths (host int32 array / list / CPU tensor, each in [1, ``max_seq_len(spec,
+        max_batch_tokens)``]: up to 8192 tokens for BERT / RoBERTa within the position table, 512 for T5; sum = T) ->
+        reps ``[B, rep_dim]`` (and last_hidden_state fp32 ``[T, H]``, packed like ``tokens``).  The same representations
         ``encode`` gives the sequences padded, up to the order of floating-point sums; ``out`` / ``out_dtype`` as there."""
         if not tokens.is_cuda:
             raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
@@ -190,8 +206,9 @@ class CudaEncoder:
         """Cross-encoder pairs assembled on the device: sequence i = ``prefix ++ a_tokens[a_start : a_start + a_len] ++
         b_tokens[b_start : b_start + b_len] ++ suffix`` with ``spans[i] = (a_start, a_len, b_start, b_len)`` (host int64
         ``[B, 4]``), token types 0; ``a_tokens`` / ``b_tokens``: int32 CUDA token stores; ``prefix`` / ``suffix``: up to
-        4 ids each.  -> reps ``[B, rep_dim]``, bitwise what ``encode_packed`` returns for the assembled sequences;
-        ``out`` / ``out_dtype`` as there."""
+        4 ids each; an assembled pair is at most ``max_seq_len(spec, max_batch_tokens)`` tokens long (as in
+        ``encode_packed``).  -> reps ``[B, rep_dim]``, bitwise what ``encode_packed`` returns for the assembled
+        sequences; ``out`` / ``out_dtype`` as there."""
         if not a_tokens.is_cuda or not b_tokens.is_cuda:
             raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
         if isinstance(spans, torch.Tensor):

@@ -33,6 +33,9 @@ from .linear import LinearHead
 
 logger = logging.getLogger(__name__)
 
+# widest padded batch om_encode takes (L <= 128, or 256 / 384 / 512); wider batches are encoded packed
+PADDED_MAX_LEN = 512
+
 
 @dataclass
 class DROutput:
@@ -140,6 +143,8 @@ class DRModel(nn.Module):
                 raise RuntimeError("openmatch_b200 encodes on a CUDA device only (no CPU path): move the batch to GPU")
             enc = self._cuda_encoder(model, head)
             B, L = input_ids.shape
+            if L > PADDED_MAX_LEN:
+                return self._encode_long(enc, items, need_hidden)
             max_b = max(1, enc.max_batch_tokens // L)
             hiddens, reps = [], []
             for lo in range(0, B, max_b):
@@ -168,6 +173,31 @@ class DRModel(nn.Module):
             reps = F.normalize(reps, dim=1)
         return hidden, reps
 
+    @staticmethod
+    def _encode_long(enc, items, need_hidden: bool, out: Tensor = None):
+        """A padded batch wider than ``PADDED_MAX_LEN`` tokens (each row up to ``encoder.max_seq_len``: 8192 for BERT /
+        RoBERTa) is encoded packed, without its padding.  The rows must be right-padded.  ``need_hidden``: the hidden
+        states come back ``[B, L, H]`` with the real tokens' rows filled and the padding rows zero (HF computes values
+        there that no pooling reads)."""
+        input_ids, mask = items["input_ids"], items["attention_mask"]
+        m = mask.bool()
+        lens = m.sum(1)
+        B, L = m.shape
+        if not torch.equal(m, torch.arange(L, device=m.device)[None, :] < lens[:, None]):
+            raise ValueError("DRModel.encode: attention_mask must be right padding (each row's tokens first)")
+        from ..encoder import max_seq_len
+        limit = max_seq_len(enc.spec, enc.max_batch_tokens)
+        if int(lens.max()) > limit:
+            raise ValueError("DRModel.encode: a row of %d tokens exceeds the model's %d" % (int(lens.max()), limit))
+        tt = items.get("token_type_ids", None)
+        r = enc.encode_packed(input_ids[m], lens.to(torch.int32).cpu(), token_type_ids=tt[m] if tt is not None else None,
+                              out=out, return_hidden=need_hidden)
+        if not need_hidden:
+            return None, r
+        hidden = torch.zeros((B, L, enc.hidden), dtype=torch.float32, device=input_ids.device)
+        hidden[m] = r[0]
+        return hidden, r[1]
+
     @torch.no_grad()
     def encode_into(self, items, out: Tensor, is_query: bool = False) -> Tensor:
         """Inference only: representations of ``items`` written IN PLACE into ``out`` (fp32 / bf16 / fp16 ``[B, rep_dim]``
@@ -184,6 +214,9 @@ class DRModel(nn.Module):
         B, L = input_ids.shape
         if out.shape[0] != B or out.shape[1] != enc.rep_dim:
             raise ValueError("out must be [%d, %d], got %s" % (B, enc.rep_dim, tuple(out.shape)))
+        if L > PADDED_MAX_LEN:
+            self._encode_long(enc, items, False, out=out)
+            return out
         max_b = max(1, enc.max_batch_tokens // L)
         tt = items.get("token_type_ids", None)
         for lo in range(0, B, max_b):
@@ -194,7 +227,8 @@ class DRModel(nn.Module):
     @torch.no_grad()
     def encode_packed_into(self, tokens: Tensor, seqlens, out: Tensor, is_query: bool = False) -> Tensor:
         """Inference only, like ``encode_into``, for a variable-length batch without padding: ``tokens`` int CUDA tensor
-        ``[sum(seqlens)]`` (the sequences back to back), ``seqlens`` host lengths (each in [1, 512]); the representations
+        ``[sum(seqlens)]`` (the sequences back to back), ``seqlens`` host lengths (each in [1, ``encoder.max_seq_len``]:
+        up to 8192 tokens for BERT / RoBERTa, 512 for T5); the representations
         go IN PLACE into ``out`` ``[len(seqlens), rep_dim]``.  Equal to ``encode_into`` of the same sequences padded, up
         to the order of floating-point sums."""
         model, head = (self.lm_q, self.head_q) if is_query else (self.lm_p, self.head_p)

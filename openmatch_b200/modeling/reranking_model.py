@@ -81,12 +81,11 @@ class RRModel(nn.Module):
 
     # ------------------------------------------------------------------ scoring
     def max_pair_len(self) -> int:
-        """longest assembled pair the model takes: 512, and max_position_embeddings for BERT (minus RoBERTa's position
-        offset of 2)"""
-        max_pos = getattr(self.lm.config, "max_position_embeddings", None) or 512
-        if getattr(self.lm.config, "model_type", "") in ("roberta", "xlm-roberta"):
-            max_pos -= 2
-        return min(512, max_pos)
+        """longest assembled pair the model takes (``encoder.max_seq_len``): 8192 tokens and max_position_embeddings for
+        BERT (minus RoBERTa's position offset of 2), 512 for T5, at most OPENMATCH_B200_MAX_BATCH_TOKENS"""
+        from ..encoder import max_seq_len, spec_from_hf_config
+        max_tokens = int(os.environ.get("OPENMATCH_B200_MAX_BATCH_TOKENS", 256 * 128))
+        return max_seq_len(spec_from_hf_config(self.lm.config), max_tokens)
 
     def _cuda_encoder(self):
         from ..encoder import CudaEncoder
@@ -99,8 +98,9 @@ class RRModel(nn.Module):
         return hit[1]
 
     def encode(self, items):
-        """Scores ``[B, 1]`` of padded pair batches (``input_ids`` / ``attention_mask`` / optional ``token_type_ids``,
-        ``[B, L]``, any ``L <= 512``), as the reference's ``RRModel.encode`` (:106-125)."""
+        """Scores ``[B, 1]`` of right-padded pair batches (``input_ids`` / ``attention_mask`` / optional
+        ``token_type_ids``, ``[B, L]``, each row's tokens at most ``max_pair_len()``: up to 8192 for BERT / RoBERTa),
+        as the reference's ``RRModel.encode`` (:106-125)."""
         if items is None:
             return None, None
         if self.feature != "last_hidden_state":
