@@ -91,7 +91,9 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out);
  * "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", or "head.linear.weight" for
  * the LinearHead).  Data is fp32, row-major, host or device; the library keeps its own packed copy, the
  * caller's tensor may be freed afterwards.  Unknown names (e.g. "pooler.*", which OpenMatch never uses)
- * are ignored and reported through the return value 1. */
+ * are ignored and reported through the return value 1.  Names are matched exactly.  Every parameter must be set
+ * before om_encoder_finalize: once it has folded the weights, om_encoder_set_weight returns OM_ESTATE and changes
+ * nothing (the handle stays finalized). */
 int om_encoder_set_weight(om_encoder* enc, const char* name, const void* data, om_memkind kind,
                           const int64_t* shape, int ndim);
 /* Verifies that every required parameter was supplied and builds derived tables. */

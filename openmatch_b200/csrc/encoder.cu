@@ -1409,6 +1409,17 @@ struct LayerW {
   float *bqkv_fold = nullptr, *b1_fold = nullptr;
 };
 
+// One parameter a handle takes (om_encoder_set_weight): its canonical HF name, its shape ([rows] when cols < 0), where
+// it lands (fp32 and / or bf16; bf16 only is converted through a temporary fp32 copy) and whether it has been set.
+struct Param {
+  std::string name;
+  int64_t rows, cols;
+  float* f32;
+  __nv_bfloat16* bf16;
+  bool set;
+  size_t count() const { return static_cast<size_t>(rows) * (cols < 0 ? 1 : cols); }
+};
+
 struct om_encoder {
   om_encoder_desc d;
   int dh = 0;  // head width: 64, or 32 (BERT)
@@ -1416,14 +1427,12 @@ struct om_encoder {
   std::vector<LayerW> layers;
   float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;  // BERT embeddings
   float* final_g = nullptr;                                                                    // T5 final RMSNorm
-  float* rel_w = nullptr;         // T5 [buckets, heads] (host copy kept in rel_host)
-  std::vector<float> rel_host;
+  float* rel_w = nullptr;         // T5 [buckets, heads]
   float* relbias_log2 = nullptr;  // [heads, 255]
   float* relbias_long_log2 = nullptr;  // [heads, 1023] (sequences longer than one tile)
   float* head_w = nullptr;        // [head_out, H]
-  std::vector<std::string> missing;
-  std::vector<std::pair<std::string, bool>> required;  // name -> set?
-  bool finalized = false;
+  std::vector<Param> params;      // in the order om_encoder_finalize lists missing ones: embeddings, layers, head
+  bool finalized = false;         // the weights are folded: no more om_encoder_set_weight
   // workspace
   int Tmax = 0, Tld = 0;
   float *h = nullptr, *kmask = nullptr, *pooled = nullptr, *headed = nullptr;
@@ -1448,9 +1457,19 @@ namespace {
 // RoBERTa is BERT's encoder with position ids computed from the token ids (roberta_pos_kernel)
 bool bert_like(int arch) { return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERTA; }
 
-// longest sequence the position table covers: max_position_embeddings (BERT), max_position_embeddings - 2 (RoBERTa:
-// positions start at padding_idx + 1 = 2)
-int max_pos_len(const om_encoder_desc& d) { return d.arch == OM_ARCH_ROBERTA ? d.max_pos - 2 : d.max_pos; }
+// The longest sequence the architecture and its position table allow: 8192 tokens and max_position_embeddings (BERT) /
+// max_position_embeddings - 2 (RoBERTa: positions start at padding_idx + 1 = 2); 512 tokens for T5 (its relative-bias
+// tables cover 512).  seq_limit_name names these limits for error messages.
+int max_seq_len(const om_encoder_desc& d) {
+  if (d.arch == OM_ARCH_T5ENC) return kMaxLongL;
+  return std::min(kMaxStreamL, d.arch == OM_ARCH_ROBERTA ? d.max_pos - 2 : d.max_pos);
+}
+
+const char* seq_limit_name(int arch) {
+  return arch == OM_ARCH_ROBERTA ? "8192 tokens, max_position_embeddings - 2"
+         : arch == OM_ARCH_BERT  ? "8192 tokens, max_position_embeddings"
+                                 : "512 tokens (T5)";
+}
 
 template <typename T>
 int dev_alloc(om_encoder* e, T** p, size_t count) {
@@ -1461,15 +1480,10 @@ int dev_alloc(om_encoder* e, T** p, size_t count) {
   return 0;
 }
 
-void require(om_encoder* e, const std::string& name) { e->required.emplace_back(name, false); }
-
-int mark(om_encoder* e, const std::string& name) {
-  for (auto& r : e->required)
-    if (r.first == name) {
-      r.second = true;
-      return 0;
-    }
-  return 1;
+// frees one of the handle's allocations before the handle itself
+void dev_free(om_encoder* e, void* p) {
+  e->allocs.erase(std::find(e->allocs.begin(), e->allocs.end(), p));
+  cudaFree(p);
 }
 
 // copies a fp32 [rows, cols] block (host or device) into dst (+ optional bf16 conversion).  om_encoder_set_weight has no
@@ -1497,12 +1511,29 @@ int upload(const void* data, om_memkind kind, size_t count, float* dst_f32, __nv
   return 0;
 }
 
-bool shape_is(const int64_t* shape, int ndim, int64_t a, int64_t b = -1) {
-  if (b < 0) return ndim == 1 && shape[0] == a;
-  return ndim == 2 && shape[0] == a && shape[1] == b;
+// The three attention kernels of one head width, each with the dynamic shared memory it runs with: attn_opt_in raises
+// their shared-memory limits, attn_launch runs one layer's attention over the tiles encode_layers describes (tmQKl /
+// tmVtl / apl: the tensor maps and parameters of the long-sequence tiles, seen from their first tile).
+template <int DH>
+cudaError_t attn_opt_in() {
+  const auto smem = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  cudaError_t err = cudaFuncSetAttribute(attn_stream_kernel<DH>, smem, kAttnStreamSmemBytes);
+  if (err == cudaSuccess) err = cudaFuncSetAttribute(attn_long_kernel<DH>, smem, kAttnLongSmemBytes);
+  if (err == cudaSuccess) err = cudaFuncSetAttribute(attn_kernel<DH>, smem, kAttnSmemBytes);
+  return err;
 }
 
-int bad_shape(const char* name) { return fail(OM_EINVAL, "om_encoder_set_weight: unexpected shape for '%s'", name); }
+template <int DH>
+void attn_launch(const CUtensorMap& tmQK, const CUtensorMap& tmVt, const AttnParams& ap_long, int n_stream,
+                 const CUtensorMap& tmQKl, const CUtensorMap& tmVtl, const AttnParams& apl, int n_long,
+                 const AttnParams& ap_short, int n_short, int units, int sms, cudaStream_t st) {
+  if (n_stream > 0)
+    attn_stream_kernel<DH><<<dim3(n_stream, units), kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
+  if (n_long > 0) attn_long_kernel<DH><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
+  if (n_short > 0)
+    attn_kernel<DH><<<std::min(n_short * units, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short,
+                                                                                                 n_short, units);
+}
 
 // The layers and the final normalisation over T token rows whose embedding (e->h, e->xb, e->stats[0]) and key mask
 // (e->kmask) are in place.  Attention: tiles [0, n_stream) run attn_stream_kernel with ap_long, the next n_long tiles
@@ -1571,26 +1602,8 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_stream,
       if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
     }
     const int units = I / kAttnCols;  // work items per tile: one per 64-wide head or pair of 32-wide heads
-    if (n_stream > 0) {
-      const dim3 grid(n_stream, units);
-      if (e->dh == 64)
-        attn_stream_kernel<64><<<grid, kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
-      else
-        attn_stream_kernel<32><<<grid, kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
-    }
-    if (n_long > 0) {
-      if (e->dh == 64)
-        attn_long_kernel<64><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
-      else
-        attn_long_kernel<32><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
-    }
-    if (n_short > 0) {
-      const int grid = std::min(n_short * units, sms * kAttnCtasPerSm);
-      if (e->dh == 64)
-        attn_kernel<64><<<grid, 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short, n_short, units);
-      else
-        attn_kernel<32><<<grid, 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short, n_short, units);
-    }
+    (e->dh == 64 ? attn_launch<64> : attn_launch<32>)(tmQK, tmVt, ap_long, n_stream, tmQKl, tmVtl, apl, n_long, ap_short,
+                                                      n_short, units, sms, st);
     OM_CUDA(cudaGetLastError());
     {
       // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
@@ -1624,6 +1637,39 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_stream,
   else
     norm_kernel<true><<<rows4, 128, 0, st>>>(e->h, e->final_g, nullptr, d.ln_eps, T, H, e->h);
   OM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Embeds T layout rows into e->h / e->xb / e->stats[0]: the padded rows of nseq sequences of L tokens (seqs == nullptr),
+// or the rows of a packed group (its sequence table seqs, L = 0, and the row map e->rowmap).  RoBERTa first computes the
+// position ids from the token ids, as HF does per sequence.
+int embed_rows(om_encoder* e, const int64_t* ids, const int64_t* tts, int T, int L, const PackedSeq* seqs, int nseq,
+               cudaStream_t st) {
+  const om_encoder_desc& d = e->d;
+  const int H = d.hidden, rows4 = (T + 3) / 4, type_vocab = std::max(d.type_vocab, 1);
+  const int2* rowmap = seqs ? e->rowmap : nullptr;
+  const int Lrow = seqs ? kMaxL : L;  // packed rows take their positions from the row map
+  if (d.arch == OM_ARCH_ROBERTA) {
+    roberta_pos_kernel<<<(nseq + 3) / 4, 128, 0, st>>>(ids, nseq, L, seqs, e->pos_ids);
+    bert_embed_kernel<true><<<rows4, 128, 0, st>>>(ids, tts, e->word, e->type, e->pos, T, Lrow, H, d.vocab, type_vocab,
+                                                   e->h, e->xb, e->stats[0], rowmap, seqs, e->pos_ids);
+  } else if (d.arch == OM_ARCH_BERT) {
+    bert_embed_kernel<false><<<rows4, 128, 0, st>>>(ids, tts, e->word, e->type, e->pos, T, Lrow, H, d.vocab, type_vocab,
+                                                    e->h, e->xb, e->stats[0], rowmap, seqs, nullptr);
+  } else {
+    t5_embed_kernel<<<rows4, 128, 0, st>>>(ids, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], rowmap, seqs);
+  }
+  OM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// the output arguments of the om_encode* entry points (who: the entry point, for the messages)
+int check_out(const om_encoder* e, const char* who, const void* out_reps, om_dtype out_dtype, int64_t out_row_stride) {
+  if (!out_reps) return fail(OM_EINVAL, "%s: null argument", who);
+  if (!e->finalized) return fail(OM_ESTATE, "%s: call om_encoder_finalize first", who);
+  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
+    return fail(OM_EINVAL, "%s: out dtype must be f32, bf16 or f16", who);
+  if (out_row_stride < om_encoder_rep_dim(e)) return fail(OM_EINVAL, "%s: out_row_stride < rep_dim", who);
   return 0;
 }
 
@@ -1749,7 +1795,7 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
                         int n, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, int sms,
                         cudaStream_t st) {
   const om_encoder_desc& d = e->d;
-  const bool bert = bert_like(d.arch), roberta = d.arch == OM_ARCH_ROBERTA;
+  const bool bert = bert_like(d.arch);
   const int H = d.hidden;
   // upload the tables through the pinned staging buffers: wait (on the host) only until the previous upload from them
   // has been read
@@ -1777,18 +1823,8 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
     if (pairs)
       pair_tokens_kernel<<<ns, 128, 0, st>>>(pairs->a, pairs->b, gs, e->pr_spans + g.k0, pairs->sp, e->pr_tokens);
     packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
-    if (roberta) {  // positions from the ids the embedding reads (for pairs: the stream pair_tokens_kernel assembled)
-      roberta_pos_kernel<<<(ns + 3) / 4, 128, 0, st>>>(tokens, ns, 0, gs, e->pos_ids);
-      bert_embed_kernel<true><<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H,
-                                                     d.vocab, std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0],
-                                                     e->rowmap, gs, e->pos_ids);
-    } else if (bert)
-      bert_embed_kernel<false><<<rows4, 128, 0, st>>>(tokens, token_type_ids, e->word, e->type, e->pos, T, kMaxL, H,
-                                                      d.vocab, std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0],
-                                                      e->rowmap, gs, nullptr);
-    else
-      t5_embed_kernel<<<rows4, 128, 0, st>>>(tokens, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], e->rowmap, gs);
-    OM_CUDA(cudaGetLastError());
+    // (for pairs, RoBERTa's positions come from the stream pair_tokens_kernel assembled)
+    OM_TRY(embed_rows(e, tokens, token_type_ids, T, 0, gs, ns, st));
     ap.T = T;
     ap.seqs = gs;
     AttnParams ap_long = ap, ap_short = ap;
@@ -1803,18 +1839,8 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
   return finish_reps(e, n, out_reps, out_dtype, out_row_stride, st);
 }
 
-// the packed length limit: 8192 tokens and max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa), 512
-// tokens (T5: its relative-bias tables cover 512), and max_batch_tokens
-int packed_max_len(const om_encoder* e) {
-  return std::min(bert_like(e->d.arch) ? std::min(kMaxStreamL, max_pos_len(e->d)) : kMaxLongL, e->Tmax);
-}
-
-// the packed calls' error message: the limits behind packed_max_len
-const char* packed_limit_name(int arch) {
-  return arch == OM_ARCH_ROBERTA ? "8192 tokens, max_position_embeddings - 2"
-         : arch == OM_ARCH_BERT  ? "8192 tokens, max_position_embeddings"
-                                 : "512 tokens (T5)";
-}
+// the packed length limit: max_seq_len and max_batch_tokens
+int packed_max_len(const om_encoder* e) { return std::min(max_seq_len(e->d), e->Tmax); }
 
 }  // namespace
 
@@ -1850,78 +1876,86 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   e->dh = dh;
   e->I = d.heads * dh;
   const int H = d.hidden, I = e->I, F = d.ffn;
+  const bool bert = bert_like(d.arch);
   e->layers.resize(d.layers);
   int rc = 0;
   auto A = [&](auto** p, size_t n) {
     if (rc == 0) rc = dev_alloc(e, p, n);
   };
-  if (bert_like(d.arch)) {
-    A(&e->word, (size_t)d.vocab * H);
-    A(&e->pos, (size_t)d.max_pos * H);
+  // a parameter of shape [rows] (cols < 0) or [rows, cols] landing in *f32 and / or *bf16, allocated here unless it
+  // already is: slot >= 0 makes it one of three q / k / v slices of its buffer
+  auto param = [&](std::string name, int64_t rows, int64_t cols, float** f32, __nv_bfloat16** bf16, int slot = -1) {
+    Param p{std::move(name), rows, cols, nullptr, nullptr, false};
+    const size_t n = p.count(), off = slot < 0 ? 0 : slot * n;
+    if (f32 && !*f32) A(f32, slot < 0 ? n : 3 * n);
+    if (bf16 && !*bf16) A(bf16, slot < 0 ? n : 3 * n);
+    if (rc != 0) return;
+    p.f32 = f32 ? *f32 + off : nullptr;
+    p.bf16 = bf16 ? *bf16 + off : nullptr;
+    e->params.push_back(std::move(p));
+  };
+  if (bert) {
+    A(&e->type, (size_t)std::max(d.type_vocab, 1) * H);  // at least one row: token types are clamped into the table
+    param("embeddings.word_embeddings.weight", d.vocab, H, &e->word, nullptr);
+    param("embeddings.position_embeddings.weight", d.max_pos, H, &e->pos, nullptr);
+    param("embeddings.token_type_embeddings.weight", d.type_vocab, H, &e->type, nullptr);
+    param("embeddings.LayerNorm.weight", H, -1, &e->emb_g, nullptr);
+    param("embeddings.LayerNorm.bias", H, -1, &e->emb_b, nullptr);
     if (d.arch == OM_ARCH_ROBERTA) A(&e->pos_ids, (size_t)d.max_batch_tokens);
-    A(&e->type, (size_t)std::max(d.type_vocab, 1) * H);
-    A(&e->emb_g, H);
-    A(&e->emb_b, H);
-    require(e, "embeddings.word_embeddings.weight");
-    require(e, "embeddings.position_embeddings.weight");
-    require(e, "embeddings.token_type_embeddings.weight");
-    require(e, "embeddings.LayerNorm.weight");
-    require(e, "embeddings.LayerNorm.bias");
   } else {
-    A(&e->word, (size_t)d.vocab * H);
-    A(&e->final_g, H);
-    A(&e->rel_w, (size_t)d.rel_buckets * d.heads);
+    param("shared.weight", d.vocab, H, &e->word, nullptr);
+    param("encoder.final_layer_norm.weight", H, -1, &e->final_g, nullptr);
+    param("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", d.rel_buckets, d.heads, &e->rel_w,
+          nullptr);
     A(&e->relbias_log2, (size_t)d.heads * (2 * kMaxL - 1));
     A(&e->relbias_long_log2, (size_t)d.heads * (2 * kMaxLongL - 1));
-    require(e, "shared.weight");
-    require(e, "encoder.final_layer_norm.weight");
-    require(e, "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight");
   }
+  // each layer's modules, named after "encoder.layer.<i>." (BERT) / "encoder.block.<i>." (T5): "<module>.weight" of
+  // shape [rows, cols] ([rows] for a norm) into f32 or bf16, and (BERT) "<module>.bias" of shape [rows].  The QKV and
+  // W1 weights land in fp32 staging buffers that om_encoder_finalize folds into wqkv / w1.
+  struct LayerModule {
+    const char* name;
+    int64_t rows, cols;
+    float* LayerW::*f32;
+    __nv_bfloat16* LayerW::*bf16;
+    float* LayerW::*bias;
+    int slot;
+  };
+  const std::vector<LayerModule> modules = bert ? std::vector<LayerModule>{
+      {"attention.self.query", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 0},
+      {"attention.self.key", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 1},
+      {"attention.self.value", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 2},
+      {"attention.output.dense", H, I, nullptr, &LayerW::wo, &LayerW::bo, -1},
+      {"attention.output.LayerNorm", H, -1, &LayerW::ln1_g, nullptr, &LayerW::ln1_b, -1},
+      {"intermediate.dense", F, H, &LayerW::w1_f32, nullptr, &LayerW::b1, -1},
+      {"output.dense", H, F, nullptr, &LayerW::w2, &LayerW::b2, -1},
+      {"output.LayerNorm", H, -1, &LayerW::ln2_g, nullptr, &LayerW::ln2_b, -1},
+  } : std::vector<LayerModule>{
+      {"layer.0.SelfAttention.q", I, H, &LayerW::wqkv_f32, nullptr, nullptr, 0},
+      {"layer.0.SelfAttention.k", I, H, &LayerW::wqkv_f32, nullptr, nullptr, 1},
+      {"layer.0.SelfAttention.v", I, H, &LayerW::wqkv_f32, nullptr, nullptr, 2},
+      {"layer.0.SelfAttention.o", H, I, nullptr, &LayerW::wo, nullptr, -1},
+      {"layer.0.layer_norm", H, -1, &LayerW::ln1_g, nullptr, nullptr, -1},
+      {"layer.1.DenseReluDense.wi", F, H, &LayerW::w1_f32, nullptr, nullptr, -1},
+      {"layer.1.DenseReluDense.wo", H, F, nullptr, &LayerW::w2, nullptr, -1},
+      {"layer.1.layer_norm", H, -1, &LayerW::ln2_g, nullptr, nullptr, -1},
+  };
   for (int i = 0; i < d.layers; ++i) {
     LayerW& w = e->layers[i];
     A(&w.wqkv, (size_t)3 * I * H);
-    A(&w.wo, (size_t)H * I);
     A(&w.w1, (size_t)F * H);
-    A(&w.w2, (size_t)H * F);
-    A(&w.ln1_g, H);
-    A(&w.ln2_g, H);
-    if (rc == 0 && (cudaMalloc(&w.wqkv_f32, (size_t)3 * I * H * 4) != cudaSuccess ||
-                    cudaMalloc(&w.w1_f32, (size_t)F * H * 4) != cudaSuccess)) {
-      cudaGetLastError();
-      rc = fail(OM_ENOMEM, "om_encoder_create: out of device memory (weight staging)");
-    }
-    char buf[160];
-    if (bert_like(d.arch)) {
+    if (bert) {
       A(&w.bqkv_fold, (size_t)3 * I);
       A(&w.b1_fold, F);
-      A(&w.bqkv, (size_t)3 * I);
-      A(&w.bo, H);
-      A(&w.b1, F);
-      A(&w.b2, H);
-      A(&w.ln1_b, H);
-      A(&w.ln2_b, H);
-      static const char* names[] = {"attention.self.query", "attention.self.key", "attention.self.value",
-                                    "attention.output.dense", "attention.output.LayerNorm", "intermediate.dense",
-                                    "output.dense", "output.LayerNorm"};
-      for (const char* n : names)
-        for (const char* suffix : {"weight", "bias"}) {
-          snprintf(buf, sizeof buf, "encoder.layer.%d.%s.%s", i, n, suffix);
-          require(e, buf);
-        }
-    } else {
-      static const char* names[] = {"layer.0.SelfAttention.q", "layer.0.SelfAttention.k", "layer.0.SelfAttention.v",
-                                    "layer.0.SelfAttention.o", "layer.0.layer_norm", "layer.1.DenseReluDense.wi",
-                                    "layer.1.DenseReluDense.wo", "layer.1.layer_norm"};
-      for (const char* n : names) {
-        snprintf(buf, sizeof buf, "encoder.block.%d.%s.weight", i, n);
-        require(e, buf);
-      }
+    }
+    const std::string prefix = (bert ? "encoder.layer." : "encoder.block.") + std::to_string(i) + ".";
+    for (const LayerModule& m : modules) {
+      param(prefix + m.name + ".weight", m.rows, m.cols, m.f32 ? &(w.*m.f32) : nullptr, m.bf16 ? &(w.*m.bf16) : nullptr,
+            m.slot);
+      if (m.bias) param(prefix + m.name + ".bias", m.rows, -1, &(w.*m.bias), nullptr, m.slot);
     }
   }
-  if (d.has_head) {
-    A(&e->head_w, (size_t)d.head_out * H);
-    require(e, "head.linear.weight");
-  }
+  if (d.has_head) param("head.linear.weight", d.head_out, H, &e->head_w, nullptr);
   // workspace
   e->Tmax = d.max_batch_tokens;
   e->Tld = static_cast<int>(round_up(2 * static_cast<int64_t>(e->Tmax) + 128, 8));  // V^T pitch: <= 128 columns per tile
@@ -1962,10 +1996,6 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
 void om_encoder_destroy(om_encoder* e) {
   if (!e) return;
   for (void* p : e->allocs) cudaFree(p);
-  for (LayerW& w : e->layers) {
-    cudaFree(w.wqkv_f32);
-    cudaFree(w.w1_f32);
-  }
   if (e->pk_host) cudaFreeHost(e->pk_host);
   if (e->pr_host) cudaFreeHost(e->pr_host);
   if (e->pk_copied) cudaEventDestroy(e->pk_copied);
@@ -1977,190 +2007,81 @@ int om_encoder_rep_dim(const om_encoder* e) { return e ? (e->d.has_head ? e->d.h
 int om_encoder_set_weight(om_encoder* e, const char* name_c, const void* data, om_memkind kind, const int64_t* shape,
                           int ndim) {
   if (!e || !name_c || !data || !shape) return fail(OM_EINVAL, "om_encoder_set_weight: null argument");
+  if (e->finalized) return fail(OM_ESTATE, "om_encoder_set_weight after om_encoder_finalize");
   std::string name(name_c);
   if (name.rfind("bert.", 0) == 0) name = name.substr(5);  // BertFor* checkpoints prefix the backbone
   if (name.rfind("roberta.", 0) == 0) name = name.substr(8);  // and RobertaFor* / XLMRobertaFor* ones
-  const om_encoder_desc& d = e->d;
-  const int H = d.hidden, I = e->I, F = d.ffn;
-  e->finalized = false;
-  if (name == "encoder.embed_tokens.weight") name = "shared.weight";
-  if (name == "head.linear.weight" || name == "linear.weight") {
-    if (!d.has_head) return 1;
-    if (!shape_is(shape, ndim, d.head_out, H)) return bad_shape(name_c);
-    OM_TRY(upload(data, kind, (size_t)d.head_out * H, e->head_w, nullptr));
-    mark(e, "head.linear.weight");
-    return 0;
-  }
-  if (bert_like(d.arch)) {
-    if (name == "embeddings.word_embeddings.weight") {
-      if (!shape_is(shape, ndim, d.vocab, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, (size_t)d.vocab * H, e->word, nullptr));
-    } else if (name == "embeddings.position_embeddings.weight") {
-      if (!shape_is(shape, ndim, d.max_pos, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, (size_t)d.max_pos * H, e->pos, nullptr));
-    } else if (name == "embeddings.token_type_embeddings.weight") {
-      if (!shape_is(shape, ndim, d.type_vocab, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, (size_t)d.type_vocab * H, e->type, nullptr));
-    } else if (name == "embeddings.LayerNorm.weight" || name == "embeddings.LayerNorm.bias") {
-      if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, H, name.back() == 't' ? e->emb_g : e->emb_b, nullptr));
-    } else if (name.rfind("encoder.layer.", 0) == 0) {
-      int li = -1, consumed = 0;
-      if (sscanf(name.c_str(), "encoder.layer.%d.%n", &li, &consumed) != 1 || li < 0 || li >= d.layers) return 1;
-      const std::string rest = name.substr(consumed);
-      LayerW& w = e->layers[li];
-      const bool is_w = rest.size() > 7 && rest.compare(rest.size() - 7, 7, ".weight") == 0;
-      const std::string mod = rest.substr(0, rest.rfind('.'));
-      int slot = mod == "attention.self.query" ? 0 : mod == "attention.self.key" ? 1 : mod == "attention.self.value" ? 2 : -1;
-      if (slot >= 0) {
-        if (is_w) {
-          if (!shape_is(shape, ndim, I, H)) return bad_shape(name_c);
-          if (!w.wqkv_f32) return fail(OM_ESTATE, "om_encoder_set_weight after om_encoder_finalize");
-          OM_TRY(upload(data, kind, (size_t)I * H, w.wqkv_f32 + (size_t)slot * I * H, nullptr));
-        } else {
-          if (!shape_is(shape, ndim, I)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, I, w.bqkv + (size_t)slot * I, nullptr));
-        }
-      } else if (mod == "attention.output.dense") {
-        if (is_w) {
-          if (!shape_is(shape, ndim, H, I)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, (size_t)H * I, nullptr, w.wo));
-        } else {
-          if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, H, w.bo, nullptr));
-        }
-      } else if (mod == "attention.output.LayerNorm" || mod == "output.LayerNorm") {
-        if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-        float* dst = mod[0] == 'a' ? (is_w ? w.ln1_g : w.ln1_b) : (is_w ? w.ln2_g : w.ln2_b);
-        OM_TRY(upload(data, kind, H, dst, nullptr));
-      } else if (mod == "intermediate.dense") {
-        if (is_w) {
-          if (!shape_is(shape, ndim, F, H)) return bad_shape(name_c);
-          if (!w.w1_f32) return fail(OM_ESTATE, "om_encoder_set_weight after om_encoder_finalize");
-          OM_TRY(upload(data, kind, (size_t)F * H, w.w1_f32, nullptr));
-        } else {
-          if (!shape_is(shape, ndim, F)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, F, w.b1, nullptr));
-        }
-      } else if (mod == "output.dense") {
-        if (is_w) {
-          if (!shape_is(shape, ndim, H, F)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, (size_t)H * F, nullptr, w.w2));
-        } else {
-          if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-          OM_TRY(upload(data, kind, H, w.b2, nullptr));
-        }
-      } else {
-        return 1;
-      }
-    } else {
-      return 1;  // e.g. pooler.*: computed by HF, never used by OpenMatch
-    }
-  } else {
-    if (name == "shared.weight") {
-      if (!shape_is(shape, ndim, d.vocab, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, (size_t)d.vocab * H, e->word, nullptr));
-    } else if (name == "encoder.final_layer_norm.weight") {
-      if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-      OM_TRY(upload(data, kind, H, e->final_g, nullptr));
-    } else if (name.rfind("encoder.block.", 0) == 0) {
-      int li = -1, consumed = 0;
-      if (sscanf(name.c_str(), "encoder.block.%d.%n", &li, &consumed) != 1 || li < 0 || li >= d.layers) return 1;
-      const std::string rest = name.substr(consumed);
-      LayerW& w = e->layers[li];
-      if (rest == "layer.0.SelfAttention.relative_attention_bias.weight") {
-        if (li != 0) return 1;
-        if (!shape_is(shape, ndim, d.rel_buckets, d.heads)) return bad_shape(name_c);
-        OM_TRY(upload(data, kind, (size_t)d.rel_buckets * d.heads, e->rel_w, nullptr));
-        e->rel_host.resize((size_t)d.rel_buckets * d.heads);
-        OM_CUDA(cudaMemcpy(e->rel_host.data(), e->rel_w, e->rel_host.size() * 4, cudaMemcpyDeviceToHost));
-      } else if (rest == "layer.0.SelfAttention.q.weight" || rest == "layer.0.SelfAttention.k.weight" ||
-                 rest == "layer.0.SelfAttention.v.weight") {
-        const int slot = rest[22] == 'q' ? 0 : rest[22] == 'k' ? 1 : 2;
-        if (!shape_is(shape, ndim, I, H)) return bad_shape(name_c);
-        if (!w.wqkv_f32) return fail(OM_ESTATE, "om_encoder_set_weight after om_encoder_finalize");
-        OM_TRY(upload(data, kind, (size_t)I * H, w.wqkv_f32 + (size_t)slot * I * H, nullptr));
-      } else if (rest == "layer.0.SelfAttention.o.weight") {
-        if (!shape_is(shape, ndim, H, I)) return bad_shape(name_c);
-        OM_TRY(upload(data, kind, (size_t)H * I, nullptr, w.wo));
-      } else if (rest == "layer.0.layer_norm.weight" || rest == "layer.1.layer_norm.weight") {
-        if (!shape_is(shape, ndim, H)) return bad_shape(name_c);
-        OM_TRY(upload(data, kind, H, rest[6] == '0' ? w.ln1_g : w.ln2_g, nullptr));
-      } else if (rest == "layer.1.DenseReluDense.wi.weight") {
-        if (!shape_is(shape, ndim, F, H)) return bad_shape(name_c);
-        if (!w.w1_f32) return fail(OM_ESTATE, "om_encoder_set_weight after om_encoder_finalize");
-        OM_TRY(upload(data, kind, (size_t)F * H, w.w1_f32, nullptr));
-      } else if (rest == "layer.1.DenseReluDense.wo.weight") {
-        if (!shape_is(shape, ndim, H, F)) return bad_shape(name_c);
-        OM_TRY(upload(data, kind, (size_t)H * F, nullptr, w.w2));
-      } else if (rest == "layer.1.DenseReluDense.wi_0.weight" || rest == "layer.1.DenseReluDense.wi_1.weight") {
-        return fail(OM_EINVAL, "gated-GELU T5 feed-forward (t5 v1.1) is not supported by this build");
-      } else {
-        return 1;
-      }
-    } else {
-      return 1;
-    }
-  }
-  return mark(e, name);
+  if (name == "encoder.embed_tokens.weight") name = "shared.weight";  // T5EncoderModel's name of the tied embedding
+  if (name == "linear.weight") name = "head.linear.weight";           // LinearHead's own state_dict
+  // the gated-GELU feed-forward (T5 v1.1, Flan-T5, mT5) has wi_0 / wi_1 where this one has wi: refused, not ignored
+  int li = -1, end = 0;
+  if (e->d.arch == OM_ARCH_T5ENC &&
+      sscanf(name.c_str(), "encoder.block.%d.layer.1.DenseReluDense.wi_%*1[01].weight%n", &li, &end) == 1 &&
+      end == static_cast<int>(name.size()) && li >= 0 && li < e->d.layers)
+    return fail(OM_EINVAL, "gated-GELU T5 feed-forward (t5 v1.1) is not supported by this build");
+  auto p = std::find_if(e->params.begin(), e->params.end(), [&](const Param& q) { return q.name == name; });
+  if (p == e->params.end()) return 1;  // e.g. pooler.*: computed by HF, never used by OpenMatch
+  const bool vec = p->cols < 0;
+  if (ndim != (vec ? 1 : 2) || shape[0] != p->rows || (!vec && shape[1] != p->cols))
+    return fail(OM_EINVAL, "om_encoder_set_weight: unexpected shape for '%s'", name_c);
+  OM_TRY(upload(data, kind, p->count(), p->f32, p->bf16));
+  p->set = true;
+  return 0;
 }
 
 int om_encoder_finalize(om_encoder* e) {
   if (!e) return fail(OM_EINVAL, "om_encoder_finalize: null encoder");
+  if (e->finalized) return fail(OM_ESTATE, "om_encoder_finalize called twice");
   std::string miss;
   int nmiss = 0;
-  for (auto& r : e->required)
-    if (!r.second) {
-      if (nmiss < 4) miss += (nmiss ? ", " : "") + r.first;
+  for (const Param& p : e->params)
+    if (!p.set) {
+      if (nmiss < 4) miss += (nmiss ? ", " : "") + p.name;
       ++nmiss;
     }
   if (nmiss) return fail(OM_ESTATE, "om_encoder_finalize: %d parameter(s) missing: %s%s", nmiss, miss.c_str(), nmiss > 4 ? ", ..." : "");
   if (e->d.arch == OM_ARCH_T5ENC) {
     const int nh = e->d.heads;
+    std::vector<float> bias((size_t)e->d.rel_buckets * nh);  // relative_attention_bias [buckets, heads]
+    OM_CUDA(cudaMemcpy(bias.data(), e->rel_w, bias.size() * 4, cudaMemcpyDeviceToHost));
     for (int pass = 0; pass < 2; ++pass) {  // one table per attention kernel
       const int maxl = pass == 0 ? kMaxL : kMaxLongL, W = 2 * maxl - 1;
       std::vector<float> table((size_t)nh * W);
       for (int rel = -(maxl - 1); rel <= maxl - 1; ++rel) {
         const int b = t5_bucket(rel, e->d.rel_buckets, e->d.rel_max_distance);
-        for (int h = 0; h < nh; ++h) table[(size_t)h * W + rel + maxl - 1] = e->rel_host[(size_t)b * nh + h] * kLog2e;
+        for (int h = 0; h < nh; ++h) table[(size_t)h * W + rel + maxl - 1] = bias[(size_t)b * nh + h] * kLog2e;
       }
       OM_CUDA(cudaMemcpy(pass == 0 ? e->relbias_log2 : e->relbias_long_log2, table.data(), table.size() * 4,
                          cudaMemcpyHostToDevice));
     }
   }
+  static bool attr = false;
+  if (!attr) {  // every instantiation: handles of both head widths may live in one process
+    OM_CUDA(attn_opt_in<64>());
+    OM_CUDA(attn_opt_in<32>());
+    attr = true;
+  }
   // fold every normalisation into the GEMM that consumes it (file header): BERT layer l's QKV takes the LayerNorm that
   // produced its input (embeddings.LayerNorm for l = 0, else layer l-1's output.LayerNorm) and W1 takes
   // attention.output.LayerNorm; T5 block l's QKV / wi take its own pre-norm RMS weights (no beta, no mean term).
-  {
-    const bool bert = bert_like(e->d.arch);
-    const int H = e->d.hidden, I = e->I, F = e->d.ffn;
-    for (int li = 0; li < e->d.layers; ++li) {
-      LayerW& w = e->layers[li];
-      if (!w.wqkv_f32 || !w.w1_f32) return fail(OM_ESTATE, "om_encoder_finalize called twice");
-      const float* g_in = bert ? (li == 0 ? e->emb_g : e->layers[li - 1].ln2_g) : w.ln1_g;
-      const float* b_in = bert ? (li == 0 ? e->emb_b : e->layers[li - 1].ln2_b) : nullptr;
-      fold_norm_kernel<<<(3 * I + 7) / 8, 256>>>(w.wqkv_f32, g_in, b_in, bert ? w.bqkv : nullptr, 3 * I, H, bert ? 1 : 0,
-                                                 w.wqkv, w.bqkv_fold);
-      fold_norm_kernel<<<(F + 7) / 8, 256>>>(w.w1_f32, bert ? w.ln1_g : w.ln2_g, bert ? w.ln1_b : nullptr,
-                                             bert ? w.b1 : nullptr, F, H, bert ? 1 : 0, w.w1, w.b1_fold);
-    }
-    OM_CUDA(cudaGetLastError());
-    OM_CUDA(cudaDeviceSynchronize());
-    for (LayerW& w : e->layers) {
-      cudaFree(w.wqkv_f32);
-      cudaFree(w.w1_f32);
-      w.wqkv_f32 = w.w1_f32 = nullptr;
-    }
+  // Nothing can fail once the fp32 staging copies are freed: from then on the handle is finalized.
+  const bool bert = bert_like(e->d.arch);
+  const int H = e->d.hidden, I = e->I, F = e->d.ffn;
+  for (int li = 0; li < e->d.layers; ++li) {
+    LayerW& w = e->layers[li];
+    const float* g_in = bert ? (li == 0 ? e->emb_g : e->layers[li - 1].ln2_g) : w.ln1_g;
+    const float* b_in = bert ? (li == 0 ? e->emb_b : e->layers[li - 1].ln2_b) : nullptr;
+    fold_norm_kernel<<<(3 * I + 7) / 8, 256>>>(w.wqkv_f32, g_in, b_in, bert ? w.bqkv : nullptr, 3 * I, H, bert ? 1 : 0,
+                                               w.wqkv, w.bqkv_fold);
+    fold_norm_kernel<<<(F + 7) / 8, 256>>>(w.w1_f32, bert ? w.ln1_g : w.ln2_g, bert ? w.ln1_b : nullptr,
+                                           bert ? w.b1 : nullptr, F, H, bert ? 1 : 0, w.w1, w.b1_fold);
   }
-  static bool attr = false;
-  if (!attr) {  // every instantiation: handles of both head widths may live in one process
-    OM_CUDA(cudaFuncSetAttribute(attn_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_long_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnLongSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_stream_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnStreamSmemBytes));
-    OM_CUDA(cudaFuncSetAttribute(attn_stream_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnStreamSmemBytes));
-    attr = true;
+  OM_CUDA(cudaGetLastError());
+  OM_CUDA(cudaDeviceSynchronize());
+  for (LayerW& w : e->layers) {
+    dev_free(e, w.wqkv_f32);
+    dev_free(e, w.w1_f32);
+    w.wqkv_f32 = w.w1_f32 = nullptr;
   }
   e->finalized = true;
   return 0;
@@ -2168,46 +2089,29 @@ int om_encoder_finalize(om_encoder* e) {
 
 int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_mask, const int64_t* token_type_ids,
               int B, int L, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream) {
-  if (!e || !input_ids || !attention_mask || !out_reps) return fail(OM_EINVAL, "om_encode: null argument");
-  if (!e->finalized) return fail(OM_ESTATE, "om_encode: call om_encoder_finalize first");
+  if (!e || !input_ids || !attention_mask) return fail(OM_EINVAL, "om_encode: null argument");
+  OM_TRY(check_out(e, "om_encode", out_reps, out_dtype, out_row_stride));
   if (B <= 0 || L <= 0) return fail(OM_EINVAL, "om_encode: B and L must be positive");
   const bool long_seq = L > kMaxL;
   if (long_seq && (L > kMaxLongL || L % 128 != 0))
     return fail(OM_EINVAL, "om_encode: L=%d unsupported (at most %d tokens, or 256 / 384 / 512: pad to a multiple of 128)", L,
                 kMaxL);
   const om_encoder_desc& d = e->d;
-  if (d.arch == OM_ARCH_BERT && L > d.max_pos) return fail(OM_EINVAL, "om_encode: L=%d exceeds max_position_embeddings", L);
-  if (d.arch == OM_ARCH_ROBERTA && L > max_pos_len(d))
-    return fail(OM_EINVAL, "om_encode: L=%d exceeds max_position_embeddings - 2 = %d (RoBERTa)", L, max_pos_len(d));
+  if (L > max_seq_len(d))
+    return fail(OM_EINVAL, "om_encode: L=%d exceeds %d (%s)", L, max_seq_len(d), seq_limit_name(d.arch));
   const int64_t T64 = static_cast<int64_t>(B) * L;
   if (T64 > e->Tmax) return fail(OM_EINVAL, "om_encode: B*L=%lld exceeds max_batch_tokens=%d", (long long)T64, e->Tmax);
-  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
-    return fail(OM_EINVAL, "om_encode: out dtype must be f32, bf16 or f16");
-  const int rep_dim = om_encoder_rep_dim(e);
-  if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode: out_row_stride < rep_dim");
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int T = static_cast<int>(T64), H = d.hidden, I = e->I;
   const bool bert = bert_like(d.arch);
-  const int rows4 = (T + 3) / 4;
 
   NvtxRange nvtx("om.encode");
   keymask_kernel<<<(T + 255) / 256, 256, 0, st>>>(attention_mask, e->kmask, T);
   // the residual stream s lives in e->h (fp32, un-normalised) with a bf16 copy in e->xb and row statistics in
   // e->stats[0] (input of a layer: from the embedding or the previous FFN2) / e->stats[1] (after the attention block)
-  if (d.arch == OM_ARCH_ROBERTA) {  // positions from the ids of each whole [L] row, as HF computes them
-    roberta_pos_kernel<<<(B + 3) / 4, 128, 0, st>>>(input_ids, B, L, nullptr, e->pos_ids);
-    bert_embed_kernel<true><<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
-                                                   std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr,
-                                                   e->pos_ids);
-  } else if (bert)
-    bert_embed_kernel<false><<<rows4, 128, 0, st>>>(input_ids, token_type_ids, e->word, e->type, e->pos, T, L, H, d.vocab,
-                                                    std::max(d.type_vocab, 1), e->h, e->xb, e->stats[0], nullptr, nullptr,
-                                                    nullptr);
-  else
-    t5_embed_kernel<<<rows4, 128, 0, st>>>(input_ids, e->word, T, H, d.vocab, e->h, e->xb, e->stats[0], nullptr, nullptr);
-  OM_CUDA(cudaGetLastError());
+  OM_TRY(embed_rows(e, input_ids, token_type_ids, T, L, nullptr, B, st));
 
   // attention geometry
   const int spt = L > 64 ? 1 : kMaxL / L;  // sequences per 128-row tile (long sequences: L / 128 tiles per sequence)
@@ -2236,13 +2140,9 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
 
 int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens, int B,
                      void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream) {
-  if (!e || !tokens || !seqlens || !out_reps) return fail(OM_EINVAL, "om_encode_packed: null argument");
-  if (!e->finalized) return fail(OM_ESTATE, "om_encode_packed: call om_encoder_finalize first");
+  if (!e || !tokens || !seqlens) return fail(OM_EINVAL, "om_encode_packed: null argument");
+  OM_TRY(check_out(e, "om_encode_packed", out_reps, out_dtype, out_row_stride));
   if (B < 0) return fail(OM_EINVAL, "om_encode_packed: B=%d is negative", B);
-  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
-    return fail(OM_EINVAL, "om_encode_packed: out dtype must be f32, bf16 or f16");
-  const int rep_dim = om_encoder_rep_dim(e);
-  if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_packed: out_row_stride < rep_dim");
   const int max_len = packed_max_len(e);
   std::vector<int64_t> tok0(static_cast<size_t>(B));
   int64_t total = 0;
@@ -2250,7 +2150,7 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
     const int l = seqlens[i];
     if (l < 1 || l > max_len)
       return fail(OM_EINVAL, "om_encode_packed: seqlens[%d]=%d outside [1, %d] (%s, max_batch_tokens=%d)", i, l,
-                  max_len, packed_limit_name(e->d.arch), e->Tmax);
+                  max_len, seq_limit_name(e->d.arch), e->Tmax);
     tok0[i] = total;
     total += l;
   }
@@ -2278,19 +2178,15 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
 int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, const int32_t* b_tokens, int64_t b_total,
                     const int64_t* spans, int B, const int32_t* prefix, int n_prefix, const int32_t* suffix, int n_suffix,
                     void* out_reps, om_dtype out_dtype, int64_t out_row_stride, void* stream) {
-  if (!e || !a_tokens || !b_tokens || !spans || !out_reps || (n_prefix > 0 && !prefix) || (n_suffix > 0 && !suffix))
+  if (!e || !a_tokens || !b_tokens || !spans || (n_prefix > 0 && !prefix) || (n_suffix > 0 && !suffix))
     return fail(OM_EINVAL, "om_encode_pairs: null argument");
-  if (!e->finalized) return fail(OM_ESTATE, "om_encode_pairs: call om_encoder_finalize first");
+  OM_TRY(check_out(e, "om_encode_pairs", out_reps, out_dtype, out_row_stride));
   if (B < 0) return fail(OM_EINVAL, "om_encode_pairs: B=%d is negative", B);
   if (a_total < 0 || b_total < 0)
     return fail(OM_EINVAL, "om_encode_pairs: negative store size (a_total=%lld, b_total=%lld)", (long long)a_total,
                 (long long)b_total);
   if (n_prefix < 0 || n_prefix > 4 || n_suffix < 0 || n_suffix > 4)
     return fail(OM_EINVAL, "om_encode_pairs: n_prefix=%d / n_suffix=%d outside [0, 4]", n_prefix, n_suffix);
-  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
-    return fail(OM_EINVAL, "om_encode_pairs: out dtype must be f32, bf16 or f16");
-  const int rep_dim = om_encoder_rep_dim(e);
-  if (out_row_stride < rep_dim) return fail(OM_EINVAL, "om_encode_pairs: out_row_stride < rep_dim");
   const int max_len = packed_max_len(e);
   std::vector<int32_t> lens(static_cast<size_t>(B));
   for (int i = 0; i < B; ++i) {
@@ -2305,7 +2201,7 @@ int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, con
     const int64_t l = n_prefix + al + bl + n_suffix;
     if (l < 1 || l > max_len)
       return fail(OM_EINVAL, "om_encode_pairs: pair %d assembles %lld tokens, outside [1, %d] (%s, "
-                  "max_batch_tokens=%d)", i, (long long)l, max_len, packed_limit_name(e->d.arch), e->Tmax);
+                  "max_batch_tokens=%d)", i, (long long)l, max_len, seq_limit_name(e->d.arch), e->Tmax);
     lens[i] = static_cast<int32_t>(l);
   }
   if (B == 0) return 0;

@@ -37,31 +37,22 @@ def spec_from_hf_config(config) -> Dict:
     """Translate a HF ``BertConfig`` / ``RobertaConfig`` / ``XLMRobertaConfig`` / ``T5Config`` into the plain dict
     ``CudaEncoder`` consumes."""
     mt = getattr(config, "model_type", "")
-    if mt in ("roberta", "xlm-roberta"):
+    if mt in ("bert", "roberta", "xlm-roberta"):
+        roberta = mt != "bert"
         _check_bert_heads(config.hidden_size, config.num_attention_heads)
         if getattr(config, "hidden_act", "gelu") != "gelu":
             raise ValueError("CUDA encoder supports hidden_act='gelu' (erf) only, got %r" % config.hidden_act)
         if getattr(config, "position_embedding_type", "absolute") not in (None, "absolute"):
             raise ValueError("CUDA encoder supports absolute position embeddings only")
-        if config.pad_token_id != ROBERTA_PAD_ID:
+        if roberta and config.pad_token_id != ROBERTA_PAD_ID:
             raise ValueError("CUDA encoder computes RoBERTa position ids with padding_idx %d, got pad_token_id=%r"
                              % (ROBERTA_PAD_ID, config.pad_token_id))
-        if config.max_position_embeddings < 3:
+        if roberta and config.max_position_embeddings < 3:
             raise ValueError("RoBERTa max_position_embeddings=%d leaves no position (positions start at 2)"
                              % config.max_position_embeddings)
-        return dict(arch="roberta", layers=config.num_hidden_layers, hidden=config.hidden_size,
-                    heads=config.num_attention_heads, ffn=config.intermediate_size, vocab=config.vocab_size,
-                    max_pos=config.max_position_embeddings, type_vocab=config.type_vocab_size,
-                    ln_eps=config.layer_norm_eps)
-    if mt == "bert":
-        _check_bert_heads(config.hidden_size, config.num_attention_heads)
-        if getattr(config, "hidden_act", "gelu") != "gelu":
-            raise ValueError("CUDA encoder supports hidden_act='gelu' (erf) only, got %r" % config.hidden_act)
-        if getattr(config, "position_embedding_type", "absolute") not in (None, "absolute"):
-            raise ValueError("CUDA encoder supports absolute position embeddings only")
-        return dict(arch="bert", layers=config.num_hidden_layers, hidden=config.hidden_size,
-                    heads=config.num_attention_heads, ffn=config.intermediate_size, vocab=config.vocab_size,
-                    max_pos=config.max_position_embeddings, type_vocab=config.type_vocab_size,
+        return dict(arch="roberta" if roberta else "bert", layers=config.num_hidden_layers,
+                    hidden=config.hidden_size, heads=config.num_attention_heads, ffn=config.intermediate_size,
+                    vocab=config.vocab_size, max_pos=config.max_position_embeddings, type_vocab=config.type_vocab_size,
                     ln_eps=config.layer_norm_eps)
     if mt == "t5":
         if config.d_kv != 64:
@@ -139,6 +130,16 @@ class CudaEncoder:
         if rc == 1:
             self.ignored.append(name)
 
+    def _out(self, out: Optional[torch.Tensor], out_dtype: torch.dtype, B: int, device):
+        """``out`` of the encode methods, checked, or a new ``[B, rep_dim]`` tensor of ``out_dtype``"""
+        if out is None:
+            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=device)
+        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
+            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
+        if out.shape[0] != B or out.shape[1] != self.rep_dim:
+            raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
+        return out
+
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None
         if h:
@@ -157,10 +158,7 @@ class CudaEncoder:
         ids = input_ids.to(torch.int64).contiguous()
         mask = attention_mask.to(torch.int64).contiguous()
         tt = token_type_ids.to(torch.int64).contiguous() if token_type_ids is not None else None
-        if out is None:
-            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=ids.device)
-        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
-            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
+        out = self._out(out, out_dtype, B, ids.device)
         hidden = torch.empty((B, L, self.hidden), dtype=torch.float32, device=ids.device) if return_hidden else None
         _lib.check(self._lib.om_encode(
             self._h, ids.data_ptr(), mask.data_ptr(), tt.data_ptr() if tt is not None else None, B, L,
@@ -187,12 +185,7 @@ class CudaEncoder:
         if ids.numel() != T:
             raise ValueError("tokens holds %d ids, seqlens sum to %d" % (ids.numel(), T))
         tt = token_type_ids.reshape(-1).to(torch.int64).contiguous() if token_type_ids is not None else None
-        if out is None:
-            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=ids.device)
-        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
-            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
-        if out.shape[0] != B or out.shape[1] != self.rep_dim:
-            raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
+        out = self._out(out, out_dtype, B, ids.device)
         hidden = torch.empty((T, self.hidden), dtype=torch.float32, device=ids.device) if return_hidden else None
         _lib.check(self._lib.om_encode_packed(
             self._h, ids.data_ptr(), tt.data_ptr() if tt is not None else None, lens.ctypes.data, B,
@@ -222,12 +215,7 @@ class CudaEncoder:
         # an empty store has no address; any valid one does (every span of it is then empty)
         a = a if na else torch.zeros(1, dtype=torch.int32, device=a.device)
         b = b if nb else torch.zeros(1, dtype=torch.int32, device=b.device)
-        if out is None:
-            out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=a.device)
-        if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
-            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
-        if out.shape[0] != B or out.shape[1] != self.rep_dim:
-            raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
+        out = self._out(out, out_dtype, B, a.device)
         _lib.check(self._lib.om_encode_pairs(
             self._h, a.data_ptr(), na, b.data_ptr(), nb, sp.ctypes.data, B, pre.ctypes.data if pre.size else None,
             int(pre.size), suf.ctypes.data if suf.size else None, int(suf.size), out.data_ptr(), _OUT_DTYPES[out.dtype],
