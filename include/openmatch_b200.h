@@ -117,9 +117,8 @@ int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attentio
  * om_encode (row i = sequence i).  out_hidden: nullable fp32 [T, hidden], packed like tokens.  seqlens may be reused on
  * return; no device synchronisation; asynchronous on `stream`.
  * Layout: sequences of <= 128 tokens are bin-packed whole into 128-row attention tiles (first-fit decreasing, ties by
- * input index: a deterministic function of seqlens); a longer one starts on a tile boundary and takes ceil(l / 128)
- * tiles, those of more than 512 tokens first (a pipelined attention kernel), then those of 129-512 tokens, then the
- * bins.  A layout of more than max_batch_tokens rows is encoded as consecutive groups of tiles on `stream`.
+ * input index: a deterministic function of seqlens); the longer ones come first, in input order, each starting on a
+ * tile boundary and taking ceil(l / 128) tiles (a pipelined attention kernel), then the bins.  A layout of more than max_batch_tokens rows is encoded as consecutive groups of tiles on `stream`.
  * Invalid input (a null pointer, B < 0, a length outside the range above) returns OM_EINVAL and writes nothing. */
 int om_encode_packed(om_encoder* enc, const int64_t* tokens, const int64_t* token_type_ids, const int32_t* seqlens,
                      int B, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, void* stream);

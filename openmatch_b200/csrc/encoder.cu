@@ -38,8 +38,8 @@ namespace om {
 
 constexpr int kAttnCols = 64;    // columns of Q, K and V^T an attention work item loads: one 64-wide or two 32-wide heads
 constexpr int kMaxL = 128;       // one attention tile; sequences of at most kMaxL tokens take attn_kernel
-constexpr int kMaxLongL = 512;   // longer sequences (multiples of 128 tokens) take attn_long_kernel, longer packed
-                                 // ones attn_stream_kernel
+constexpr int kMaxLongL = 512;   // longest padded om_encode sequence (a multiple of 128 tokens above kMaxL) and T5
+                                 // sequence; longer sequences take attn_stream_kernel
 constexpr float kLog2e = 1.4426950408889634f;
 
 // ===================================================================================================
@@ -718,7 +718,8 @@ struct AttnParams {
   int T, L, spt, I, Tvalid_rows;  // Tvalid_rows = spt * L: rows of the tile that belong to it
   float scale_log2;               // softmax scale * log2(e)
   const float* kmask;             // [T] 0 / -inf
-  const float* relbias_log2;      // nullable [heads, 2*kMaxL-1], already multiplied by log2(e)
+  const float* relbias_log2;      // nullable [heads, 2*kMaxL-1] (attn_kernel) / [heads, 2*kMaxLongL-1]
+                                  // (attn_stream_kernel), already multiplied by log2(e)
   __nv_bfloat16* ctx;             // [T, I]
   // packed layout (om_encode_packed; nullptr for om_encode): a row's sequence and position come from rowmap [T], its
   // length from seqs; attn_kernel starts at tile tile0 (the long sequences' tiles come first)
@@ -913,159 +914,11 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Sequences longer than one tile (L = 256 / 384 / 512, multiples of 128): one CTA per (128-row query tile, unit)
-// loops over the sequence's 128-key tiles with an online softmax, 64 query rows at a time:  S_j = Q K_j^T (wgmma) ->
-// running max / sum per row on the fragments -> P_j (bf16, registers) -> O = O * alpha + P_j V_j (wgmma, accumulating in
-// registers).  Q stays in smem; K_j / V_j are re-loaded by TMA per iteration.
-// ---------------------------------------------------------------------------------------------------
-constexpr int kAttnLongSmemQ = 0, kAttnLongSmemK = 16384, kAttnLongSmemV = 32768;
-constexpr int kAttnLongSmemMisc = 49152;  // rel[1024] f32, key bits [4 tiles x 4 words], barrier
-constexpr int kAttnLongSmemBytes = kAttnLongSmemMisc + 4096 + 64 + 64 + 1024;
-
-// DH and the (tile, unit) split of the heads as in attn_kernel: blockIdx.y is the unit.
-template <int DH>
-__global__ void __launch_bounds__(128, 2)
-attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p) {
-  constexpr int NH = kAttnCols / DH;  // heads per unit
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* s_rel = reinterpret_cast<float*>(smem + kAttnLongSmemMisc);
-  uint32_t* s_kb = reinterpret_cast<uint32_t*>(s_rel + 1024);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_kb + 16);  // [0] loads
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int qt = blockIdx.x, unit = blockIdx.y;
-  const int row0 = qt * 128;                // first token of this query tile
-  int nk = p.L / 128;                       // key tiles per sequence
-  int kt0 = (qt / nk) * nk;                 // first tile of the sequence this query tile belongs to
-  int qpos0 = (qt - kt0) * 128;             // position of the tile's first query inside its sequence
-  if (p.rowmap) {
-    // packed: the sequence starts on a tile boundary and the tile's first row is one of its tokens; the padding rows
-    // after its last token attend like its tokens (finite values nobody reads), its padding keys are masked by kmask
-    const int2 mp = p.rowmap[row0];
-    nk = (p.seqs[mp.x].len + 127) / 128;
-    qpos0 = mp.y;
-    kt0 = qt - mp.y / 128;
-  }
-
-  if (tid == 0) {
-    tma_prefetch_desc(&tmQK);
-    tma_prefetch_desc(&tmVt);
-    mbar_init(&bars[0], 1);
-    fence_barrier_init();
-  }
-  for (int j = 0; j < nk; ++j) {  // key validity of every key tile of the sequence: one ballot per warp and tile
-    const int tok = (kt0 + j) * 128 + tid;
-    const bool key_ok = tok < p.T && p.kmask[tok] == 0.f;
-    const unsigned bits = __ballot_sync(0xffffffffu, key_ok);
-    if (lane == 0) s_kb[j * 4 + warp] = bits;
-  }
-  if (DH == 64 && p.relbias_log2) {
-    for (int i = tid; i < 2 * kMaxLongL - 1; i += 128) s_rel[i] = p.relbias_log2[unit * (2 * kMaxLongL - 1) + i];
-  }
-  __syncthreads();
-
-  const bool has_rel = DH == 64 && p.relbias_log2 != nullptr;
-  const uint32_t qa = smem_u32(smem + kAttnLongSmemQ), ka = smem_u32(smem + kAttnLongSmemK),
-                 va = smem_u32(smem + kAttnLongSmemV);
-  // running state per (64-row half h, head hd of the unit) = index hh = h * NH + hd
-  int rr[2][2];
-  bool valid[2][2];
-  float m_run[2 * NH][2], sum[2 * NH][2], o[2 * NH][DH / 2];
-#pragma unroll
-  for (int h = 0; h < 2; ++h)
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      rr[h][u] = h * 64 + 16 * warp + (lane >> 2) + 8 * u;
-      valid[h][u] = row0 + rr[h][u] < p.T;
-    }
-#pragma unroll
-  for (int hh = 0; hh < 2 * NH; ++hh) {
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      m_run[hh][u] = __int_as_float(0xff800000);
-      sum[hh][u] = 0.f;
-    }
-#pragma unroll
-    for (int i = 0; i < DH / 2; ++i) o[hh][i] = 0.f;
-  }
-
-#pragma unroll 1
-  for (int j = 0; j < nk; ++j) {
-    if (tid == 0) {
-      // K / V of the previous iteration are dead: every warp passed the trailing barrier of that iteration
-      mbar_arrive_expect_tx(&bars[0], (j == 0 ? 3 : 2) * 16384);
-      if (j == 0) tma_load_2d(smem + kAttnLongSmemQ, &tmQK, &bars[0], unit * kAttnCols, row0);
-      tma_load_2d(smem + kAttnLongSmemK, &tmQK, &bars[0], p.I + unit * kAttnCols, (kt0 + j) * 128);
-      tma_load_2d(smem + kAttnLongSmemV, &tmVt, &bars[0], (kt0 + j) * 128, unit * kAttnCols);
-      tma_load_2d(smem + kAttnLongSmemV + 8192, &tmVt, &bars[0], (kt0 + j) * 128 + 64, unit * kAttnCols);
-    }
-    mbar_wait_warp(&bars[0], static_cast<uint32_t>(j & 1), 13);
-#pragma unroll
-    for (int hh = 0; hh < 2 * NH; ++hh) {
-      const int h = hh / NH, hd = hh % NH;
-      float sc[64];
-      attn_scores<DH>(sc, qa + h * 8192 + hd * DH * 2, ka + hd * DH * 2);
-      float m_j[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int u = e >> 1, c = 8 * jj + 2 * (lane & 3) + (e & 1);
-          float v = sc[4 * jj + e] * p.scale_log2;
-          if (has_rel) v += s_rel[(kMaxLongL - 1) - (qpos0 + rr[h][u]) + j * 128 + c];
-          const bool ok = valid[h][u] && ((s_kb[j * 4 + (c >> 5)] >> (c & 31)) & 1u);
-          v = ok ? v : __int_as_float(0xff800000);
-          sc[4 * jj + e] = v;
-          m_j[u] = fmaxf(m_j[u], v);
-        }
-      float alpha[2], mm[2];
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const float m_new = fmaxf(m_run[hh][u], quad_max(m_j[u]));
-        mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new : 0.f;  // no allowed key seen so far: all p = 0
-        alpha[u] = (m_run[hh][u] > __int_as_float(0xff800000)) ? ex2_approx(m_run[hh][u] - mm[u]) : 0.f;
-        m_run[hh][u] = m_new;
-        sum[hh][u] *= alpha[u];
-      }
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj)
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const float pv = ex2_approx(sc[4 * jj + e] - mm[e >> 1]);
-          sc[4 * jj + e] = pv;
-          sum[hh][e >> 1] += pv;
-        }
-#pragma unroll
-      for (int i = 0; i < DH / 2; ++i) o[hh][i] *= alpha[(i >> 1) & 1];
-      attn_pv<DH>(o[hh], sc, va + hd * DH * 128, 1u);
-    }
-    __syncthreads();  // the next iteration's TMA loads overwrite K / V
-  }
-
-#pragma unroll
-  for (int hh = 0; hh < 2 * NH; ++hh)
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      const int h = hh / NH, hd = hh % NH;
-      const float tot = quad_sum(sum[hh][u]);
-      const float inv = tot > 0.f ? 1.0f / tot : 0.f;
-      if (valid[h][u]) {
-        __nv_bfloat16* dst =
-            p.ctx + static_cast<int64_t>(row0 + rr[h][u]) * p.I + unit * kAttnCols + hd * DH + 2 * (lane & 3);
-#pragma unroll
-        for (int jj = 0; jj < DH / 8; ++jj)
-          *reinterpret_cast<uint32_t*>(dst + 8 * jj) =
-              pack_bf16x2(o[hh][4 * jj + 2 * u] * inv, o[hh][4 * jj + 2 * u + 1] * inv);
-      }
-    }
-}
-
-// ---------------------------------------------------------------------------------------------------
-// Sequences of kMaxLongL + 1 .. kMaxStreamL tokens (packed layout only): one CTA of three warpgroups per (128-row query
-// tile, unit), the online softmax of attn_long_kernel on a pipeline.  At these lengths attention is most of a layer
-// (4 L^2 I FLOP against 24 L H^2 for the GEMMs), and at head width 64 the exponentials take about as long as the MMAs,
-// so the loads must run ahead of the compute and the two halves of the query tile must not wait for each other:
+// Sequences of kMaxL + 1 .. kMaxStreamL tokens, padded (L = 256 / 384 / 512) or packed: one CTA of three warpgroups per
+// (128-row query tile, unit) loops over the sequence's 128-key tiles with an online softmax.  At these lengths attention
+// is a large share of a layer (4 L^2 I FLOP against 24 L H^2 for the GEMMs), and at head width 64 the exponentials take
+// about as long as the MMAs, so the loads must run ahead of the compute and the two halves of the query tile must not
+// wait for each other:
 //   producer  warp 0: Q once, then the sequence's 128-key tiles (K, V^T: 32 KB, and the tile's key-validity bits,
 //             one ballot of kmask per 32 keys) into a ring of kAttnStreamStages slots with full / empty mbarriers
 //             (ring.cuh); warps 1-3 only hand their registers over (setmaxnreg)
@@ -1075,7 +928,8 @@ attn_long_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant
 //             wgmma run.
 // The key-validity bits come per key tile, so the length is bounded by nothing the kernel sizes.  Keys of a tile that
 // are all valid (every tile but a sequence's last) skip the masking.  Padding rows after a sequence's last token attend
-// like its tokens (finite values nobody reads).
+// like its tokens (finite values nobody reads).  REL (T5, 64-wide heads, at most kMaxLongL tokens) adds the relative
+// position bias, a [2 kMaxLongL - 1] row per head held in shared memory.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kMaxStreamL = 8192;
 constexpr int kAttnStreamStages = 4;
@@ -1083,28 +937,38 @@ constexpr int kAttnStreamThreads = 384;
 constexpr int kAttnStreamStageBytes = 32768;  // K [128 keys, 64 cols] + V^T as two [64 cols, 64 keys] boxes
 constexpr int kAttnStreamSmemRing = 16384;    // after Q [128 rows, 64 cols]
 constexpr int kAttnStreamSmemMisc = kAttnStreamSmemRing + kAttnStreamStages * kAttnStreamStageBytes;
-// misc: key bits [stages][4] u32, full[stages], empty[stages], Q barrier
-constexpr int kAttnStreamSmemBytes = kAttnStreamSmemMisc + kAttnStreamStages * 16 + (2 * kAttnStreamStages + 1) * 8 + 1024;
+// misc: key bits [stages][4] u32, full[stages], empty[stages], Q barrier; then the relative bias row (REL)
+constexpr int kAttnStreamSmemRel = kAttnStreamSmemMisc + 256;
+static_assert(kAttnStreamStages * 16 + (2 * kAttnStreamStages + 1) * 8 <= 256, "stream kernel: misc overlaps rel");
+constexpr int kAttnStreamSmemBytes = kAttnStreamSmemRel + (2 * kMaxLongL - 1) * 4 + 1024;
 
-template <int DH>
+template <int DH, bool REL>
 __global__ void __launch_bounds__(kAttnStreamThreads, 1)
 attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p) {
   constexpr int NH = kAttnCols / DH;  // heads per unit
   constexpr int S = kAttnStreamStages;
+  static_assert(!REL || DH == 64, "the relative position bias exists for 64-wide heads only");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint32_t* s_kb = reinterpret_cast<uint32_t*>(smem + kAttnStreamSmemMisc);  // [S][4]: key bits of each slot
   uint64_t* full = reinterpret_cast<uint64_t*>(s_kb + 4 * S);
   uint64_t* empty = full + S;
   uint64_t* qbar = empty + S;
+  float* s_rel = reinterpret_cast<float*>(smem + kAttnStreamSmemRel);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int qt = blockIdx.x, unit = blockIdx.y;
   const int row0 = qt * 128;  // first row of this query tile
-  // the sequence starts on a tile boundary and the tile's first row is one of its tokens (place_packed)
-  const int2 mp = p.rowmap[row0];
-  const int nk = (p.seqs[mp.x].len + 127) / 128;  // key tiles of the sequence
-  const int kt0 = qt - mp.y / 128;                 // its first tile
+  // the sequence's length and the position of the tile's first query in it: padded, every sequence takes L / 128 tiles;
+  // packed, it starts on a tile boundary and the tile's first row is one of its tokens (place_packed)
+  int len = p.L, qpos0 = qt % (p.L / 128) * 128;
+  if (p.rowmap) {
+    const int2 mp = p.rowmap[row0];
+    len = p.seqs[mp.x].len;
+    qpos0 = mp.y;
+  }
+  const int nk = (len + 127) / 128;  // key tiles of the sequence
+  const int kt0 = qt - qpos0 / 128;  // its first tile
 
   if (tid == 0) {
     tma_prefetch_desc(&tmQK);
@@ -1112,6 +976,10 @@ attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_consta
     ring_init(full, empty, S, 8);  // a slot is released by each of the 8 consumer warps
     mbar_init(qbar, 1);
     fence_barrier_init();
+  }
+  if constexpr (REL) {
+    for (int i = tid; i < 2 * kMaxLongL - 1; i += kAttnStreamThreads)
+      s_rel[i] = p.relbias_log2[unit * (2 * kMaxLongL - 1) + i];
   }
   __syncthreads();
 
@@ -1155,8 +1023,11 @@ attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_consta
   const int wg = (warp >> 2) - 1;  // 64-row half of the tile
   const uint32_t qa = smem_u32(smem) + wg * 8192, ring_a = smem_u32(smem + kAttnStreamSmemRing);
   const float scale = p.scale_log2;
+  // m_run: running maximum of the raw (unscaled) scores, or under REL of the scaled and biased logits (the bias breaks
+  // "the maximum of the scaled scores is the scaled maximum"); ms scales m_run and the scores in the softmax below
+  const float ms = REL ? 1.f : scale;
   int rr[2];
-  float m_run[NH][2], sum[NH][2], o[NH][DH / 2];  // m_run: running maximum of the raw (unscaled) scores
+  float m_run[NH][2], sum[NH][2], o[NH][DH / 2];
 #pragma unroll
   for (int u = 0; u < 2; ++u) rr[u] = wg * 64 + 16 * (warp & 3) + (lane >> 2) + 8 * u;
 #pragma unroll
@@ -1190,19 +1061,28 @@ attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_consta
             if (!((kb[c >> 5] >> (c & 31)) & 1u)) sc[4 * jj + e] = __int_as_float(0xff800000);
           }
       }
+      if constexpr (REL) {  // scaled logit + bias of the relative position (key - query); a masked key stays -inf
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int c = 8 * jj + 2 * (lane & 3) + (e & 1);
+            sc[4 * jj + e] = fmaf(sc[4 * jj + e], scale, s_rel[(kMaxLongL - 1) - (qpos0 + rr[e >> 1]) + 128 * j + c]);
+          }
+      }
       float m_j[2] = {__int_as_float(0xff800000), __int_as_float(0xff800000)};
 #pragma unroll
       for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
         for (int e = 0; e < 4; ++e) m_j[e >> 1] = fmaxf(m_j[e >> 1], sc[4 * jj + e]);
       // softmax in the log2 domain: p = 2^(s * scale - m * scale), one FFMA and one ex2 per score (scale > 0, so the
-      // maximum of the scaled scores is the scaled maximum)
+      // maximum of the scaled scores is the scaled maximum); under REL p = 2^(v - m) on the biased logits v
       float alpha[2], mm[2];
 #pragma unroll
       for (int u = 0; u < 2; ++u) {
         const float m_new = fmaxf(m_run[hd][u], quad_max(m_j[u]));
-        mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new * scale : 0.f;  // no allowed key seen so far: all p = 0
-        alpha[u] = (m_run[hd][u] > __int_as_float(0xff800000)) ? ex2_approx(fmaf(m_run[hd][u], scale, -mm[u])) : 0.f;
+        mm[u] = (m_new > __int_as_float(0xff800000)) ? m_new * ms : 0.f;  // no allowed key seen so far: all p = 0
+        alpha[u] = (m_run[hd][u] > __int_as_float(0xff800000)) ? ex2_approx(fmaf(m_run[hd][u], ms, -mm[u])) : 0.f;
         m_run[hd][u] = m_new;
         sum[hd][u] *= alpha[u];
       }
@@ -1210,7 +1090,7 @@ attn_stream_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_consta
       for (int jj = 0; jj < 16; ++jj)
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
-          const float pv = ex2_approx(fmaf(sc[4 * jj + e], scale, -mm[e >> 1]));  // ex2(-inf) = 0 for masked keys
+          const float pv = ex2_approx(fmaf(sc[4 * jj + e], ms, -mm[e >> 1]));  // ex2(-inf) = 0 for masked keys
           sc[4 * jj + e] = pv;
           sum[hd][e >> 1] += pv;
         }
@@ -1511,61 +1391,42 @@ int upload(const void* data, om_memkind kind, size_t count, float* dst_f32, __nv
   return 0;
 }
 
-// The three attention kernels of one head width, each with the dynamic shared memory it runs with: attn_opt_in raises
-// their shared-memory limits, attn_launch runs one layer's attention over the tiles encode_layers describes (tmQKl /
-// tmVtl / apl: the tensor maps and parameters of the long-sequence tiles, seen from their first tile).
+// The attention kernels of one head width, each with the dynamic shared memory it runs with: attn_opt_in raises their
+// shared-memory limits, attn_launch runs one layer's attention over the tiles encode_layers describes.
 template <int DH>
 cudaError_t attn_opt_in() {
   const auto smem = cudaFuncAttributeMaxDynamicSharedMemorySize;
-  cudaError_t err = cudaFuncSetAttribute(attn_stream_kernel<DH>, smem, kAttnStreamSmemBytes);
-  if (err == cudaSuccess) err = cudaFuncSetAttribute(attn_long_kernel<DH>, smem, kAttnLongSmemBytes);
+  cudaError_t err = cudaFuncSetAttribute(attn_stream_kernel<DH, false>, smem, kAttnStreamSmemBytes);
+  if (DH == 64 && err == cudaSuccess) err = cudaFuncSetAttribute(attn_stream_kernel<64, true>, smem, kAttnStreamSmemBytes);
   if (err == cudaSuccess) err = cudaFuncSetAttribute(attn_kernel<DH>, smem, kAttnSmemBytes);
   return err;
 }
 
 template <int DH>
-void attn_launch(const CUtensorMap& tmQK, const CUtensorMap& tmVt, const AttnParams& ap_long, int n_stream,
-                 const CUtensorMap& tmQKl, const CUtensorMap& tmVtl, const AttnParams& apl, int n_long,
+void attn_launch(const CUtensorMap& tmQK, const CUtensorMap& tmVt, const AttnParams& ap_stream, int n_stream,
                  const AttnParams& ap_short, int n_short, int units, int sms, cudaStream_t st) {
   if (n_stream > 0)
-    attn_stream_kernel<DH><<<dim3(n_stream, units), kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_long);
-  if (n_long > 0) attn_long_kernel<DH><<<dim3(n_long, units), 128, kAttnLongSmemBytes, st>>>(tmQKl, tmVtl, apl);
+    (DH == 64 && ap_stream.relbias_log2 ? attn_stream_kernel<64, true> : attn_stream_kernel<DH, false>)
+        <<<dim3(n_stream, units), kAttnStreamThreads, kAttnStreamSmemBytes, st>>>(tmQK, tmVt, ap_stream);
   if (n_short > 0)
     attn_kernel<DH><<<std::min(n_short * units, sms * kAttnCtasPerSm), 128, kAttnSmemBytes, st>>>(tmQK, tmVt, ap_short,
                                                                                                  n_short, units);
 }
 
 // The layers and the final normalisation over T token rows whose embedding (e->h, e->xb, e->stats[0]) and key mask
-// (e->kmask) are in place.  Attention: tiles [0, n_stream) run attn_stream_kernel with ap_long, the next n_long tiles
-// attn_long_kernel with ap_long seen from its first tile on, the next n_short tiles attn_kernel with ap_short
-// (tile0 = n_stream + n_long); ap_short.Tvalid_rows is the tile-local V^T layout of EpiQKV.
-int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_stream, int n_long, const AttnParams& ap_short,
+// (e->kmask) are in place.  Attention: tiles [0, n_stream) run attn_stream_kernel with ap_stream, the next n_short
+// tiles attn_kernel with ap_short (tile0 = n_stream); ap_short.Tvalid_rows is the tile-local V^T layout of EpiQKV.
+int encode_layers(om_encoder* e, int T, const AttnParams& ap_stream, int n_stream, const AttnParams& ap_short,
                   int n_short, int sms, cudaStream_t st) {
   const om_encoder_desc& d = e->d;
   const int H = d.hidden, I = e->I, F = d.ffn;
   const bool bert = bert_like(d.arch);
   const int rows4 = (T + 3) / 4;
-  const int n_tiles = n_stream + n_long + n_short;
+  const int n_tiles = n_stream + n_short;
   CUtensorMap tmQK, tmVt;
   if (make_tmap_bf16_2d(&tmQK, e->qk, (uint64_t)2 * I, (uint64_t)T, (uint64_t)2 * I * 2, 64, 128) != 0 ||
       make_tmap_bf16_2d(&tmVt, e->vt, (uint64_t)n_tiles * 128, (uint64_t)I, (uint64_t)e->Tld * 2, 64, 64) != 0)
     return fail(OM_ECUDA, "om_encode: tensor map creation failed");
-  // attn_long_kernel numbers its query tiles from the first row it sees: behind the stream tiles it gets tensor maps,
-  // row map, key mask and output that start at its first tile (the packed layout is position-independent)
-  CUtensorMap tmQKl = tmQK, tmVtl = tmVt;
-  AttnParams apl = ap_long;
-  if (n_stream > 0 && n_long > 0) {
-    const int off = n_stream * 128;
-    if (make_tmap_bf16_2d(&tmQKl, e->qk + (size_t)off * 2 * I, (uint64_t)2 * I, (uint64_t)(T - off), (uint64_t)2 * I * 2,
-                          64, 128) != 0 ||
-        make_tmap_bf16_2d(&tmVtl, e->vt + off, (uint64_t)(n_tiles - n_stream) * 128, (uint64_t)I, (uint64_t)e->Tld * 2,
-                          64, 64) != 0)
-      return fail(OM_ECUDA, "om_encode: tensor map creation failed");
-    apl.T = T - off;
-    apl.kmask += off;
-    apl.ctx += (size_t)off * I;
-    apl.rowmap += off;
-  }
 
   // TMA-store tensor maps of the bf16 GEMM outputs (box = 64 columns x 32 rows = one epilogue warp's chunk pair) and the
   // residual stream's maps (fp32 load + store, bf16 store; box = 32 columns x 32 rows = one chunk)
@@ -1602,8 +1463,7 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_long, int n_stream,
       if (err != cudaSuccess) return fail(OM_ECUDA, "QKV GEMM launch failed: %s", cudaGetErrorString(err));
     }
     const int units = I / kAttnCols;  // work items per tile: one per 64-wide head or pair of 32-wide heads
-    (e->dh == 64 ? attn_launch<64> : attn_launch<32>)(tmQK, tmVt, ap_long, n_stream, tmQKl, tmVtl, apl, n_long, ap_short,
-                                                      n_short, units, sms, st);
+    (e->dh == 64 ? attn_launch<64> : attn_launch<32>)(tmQK, tmVt, ap_stream, n_stream, ap_short, n_short, units, sms, st);
     OM_CUDA(cudaGetLastError());
     {
       // s <- ctx Wo^T + bo + LN_in(s) (BERT) / + s (T5); statistics of the new s -> stats[1]
@@ -1707,16 +1567,14 @@ int finish_reps(om_encoder* e, int B, void* out_reps, om_dtype out_dtype, int64_
 //   * a sequence of more than 128 tokens starts on a tile boundary and takes ceil(l / 128) tiles, in input order;
 //   * the others are bin-packed whole into tiles of min(128, Tmax) rows, first-fit decreasing (ties by input index:
 //     placement is a deterministic function of the lengths), each bin's sequences back to back in insertion order;
-//   * layout = the tiles of the sequences of more than 512 tokens (attn_stream_kernel), then those of the other long
-//     sequences (attn_long_kernel), then the bins (attn_kernel); cut into row groups of at most Tmax rows at unit
-//     (sequence / bin) boundaries, each group encoded on its own (in the same order).  The last unit of a group is
-//     counted up to its last token.  Without a sequence of more than 512 tokens the first class is empty.
+//   * layout = the tiles of the sequences of more than 128 tokens (attn_stream_kernel), then the bins (attn_kernel);
+//     cut into row groups of at most Tmax rows at unit (sequence / bin) boundaries, each group encoded on its own (in
+//     the same order).  The last unit of a group is counted up to its last token.
 // seqs receives the table in layout order (row0 relative to its group, out = index in the chunk).
 struct PackedGroup {
   int k0, k1;     // sequences [k0, k1) of the table
   int T;          // layout rows of the group
-  int n_stream;   // tiles of sequences of more than kMaxLongL tokens (the first tiles of the group)
-  int n_long;     // tiles of the other sequences of more than kMaxL tokens (the next ones)
+  int n_stream;   // tiles of sequences of more than kMaxL tokens (the first tiles of the group)
   int n_tiles;
 };
 
@@ -1725,8 +1583,8 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
   seqs.clear();
   groups.clear();
   const int cap = std::min(kMaxL, Tmax);
-  std::vector<int> streams, longs, shorts;
-  for (int i = 0; i < n; ++i) (len[i] > kMaxLongL ? streams : len[i] > kMaxL ? longs : shorts).push_back(i);
+  std::vector<int> streams, shorts;
+  for (int i = 0; i < n; ++i) (len[i] > kMaxL ? streams : shorts).push_back(i);
   std::stable_sort(shorts.begin(), shorts.end(), [&](int a, int b) { return len[a] > len[b]; });
   std::vector<std::vector<int>> bins;
   std::vector<int> fill;
@@ -1746,14 +1604,13 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
     fill[best] += len[i];
     by_room[cap - fill[best]].insert(best);
   }
-  PackedGroup g{0, 0, 0, 0, 0, 0};
+  PackedGroup g{0, 0, 0, 0, 0};
   int row = 0;  // group-local first row of the next unit (a tile boundary)
-  // kind: 2 = more than kMaxLongL tokens, 1 = more than kMaxL, 0 = a bin
-  auto unit = [&](const std::vector<int>& members, int tiles, int used, int kind) {
+  auto unit = [&](const std::vector<int>& members, int tiles, int used, bool stream) {
     if (row > 0 && row + (tiles - 1) * 128 + used > Tmax) {
       g.k1 = static_cast<int>(seqs.size());
       groups.push_back(g);
-      g = PackedGroup{g.k1, g.k1, 0, 0, 0, 0};
+      g = PackedGroup{g.k1, g.k1, 0, 0, 0};
       row = 0;
     }
     int off = 0;
@@ -1762,17 +1619,15 @@ void place_packed(const int32_t* len, const int64_t* tok0, int n, int Tmax, std:
       off += len[i];
     }
     g.T = row + (tiles - 1) * 128 + used;
-    g.n_stream += kind == 2 ? tiles : 0;
-    g.n_long += kind == 1 ? tiles : 0;
+    g.n_stream += stream ? tiles : 0;
     g.n_tiles += tiles;
     row += tiles * 128;
   };
-  for (int k = 2; k >= 1; --k)
-    for (int i : k == 2 ? streams : longs) {
-      const int tiles = (len[i] + 127) / 128;
-      unit(std::vector<int>{i}, tiles, len[i] - (tiles - 1) * 128, k);
-    }
-  for (size_t b = 0; b < bins.size(); ++b) unit(bins[b], 1, fill[b], 0);
+  for (int i : streams) {
+    const int tiles = (len[i] + 127) / 128;
+    unit(std::vector<int>{i}, tiles, len[i] - (tiles - 1) * 128, true);
+  }
+  for (size_t b = 0; b < bins.size(); ++b) unit(bins[b], 1, fill[b], false);
   g.k1 = static_cast<int>(seqs.size());
   if (g.k1 > g.k0) groups.push_back(g);
 }
@@ -1827,11 +1682,11 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
     OM_TRY(embed_rows(e, tokens, token_type_ids, T, 0, gs, ns, st));
     ap.T = T;
     ap.seqs = gs;
-    AttnParams ap_long = ap, ap_short = ap;
-    ap_long.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
+    AttnParams ap_stream = ap, ap_short = ap;
+    ap_stream.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
     ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
-    ap_short.tile0 = g.n_stream + g.n_long;
-    OM_TRY(encode_layers(e, T, ap_long, g.n_stream, g.n_long, ap_short, g.n_tiles - g.n_stream - g.n_long, sms, st));
+    ap_short.tile0 = g.n_stream;
+    OM_TRY(encode_layers(e, T, ap_stream, g.n_stream, ap_short, g.n_tiles - g.n_stream, sms, st));
     if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
     pool_packed_kernel<<<ns, 256, 0, st>>>(e->h, gs, H, d.pooling == OM_POOL_MEAN ? 1 : 0, e->pooled);
     OM_CUDA(cudaGetLastError());
@@ -2129,7 +1984,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   ap.seqs = nullptr;
   ap.tile0 = 0;
   const int n_tiles = long_seq ? T / 128 : (B + spt - 1) / spt;
-  OM_TRY(encode_layers(e, T, ap, 0, long_seq ? n_tiles : 0, ap, long_seq ? 0 : n_tiles, sms, st));
+  OM_TRY(encode_layers(e, T, ap, long_seq ? n_tiles : 0, ap, long_seq ? 0 : n_tiles, sms, st));
   if (out_hidden)
     OM_CUDA(cudaMemcpyAsync(out_hidden, e->h, static_cast<size_t>(T) * H * 4, cudaMemcpyDeviceToDevice, st));
 

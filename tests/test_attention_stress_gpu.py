@@ -1,4 +1,4 @@
-"""GPU: every attention kernel (attn_kernel, attn_long_kernel, attn_stream_kernel, each at head width 64 and 32) at the
+"""GPU: every attention kernel (attn_kernel and attn_stream_kernel, each at head width 64 and 32) at the
 adversarial attention statistics of tests/attention_stress.py, judged sequence by sequence against the float64 oracle.
 
 Each sequence's reps and attended hidden rows, and the aggregate over the call, are held to the rule of _judge in
@@ -118,8 +118,7 @@ def test_magnets_padded(enc_mod, dh, L):
 
 
 # (length, magnets) of one packed call: a 4097-token sequence without a magnet (its last tile holds one key and 127
-# padding rows) and a 513-token one with magnets at its ends (attn_stream_kernel); 129 - 512-token sequences
-# (attn_long_kernel); bins whose sequences alternate with and without boundary magnets: [127 ends, 1 none],
+# padding rows) and a 513-token one with magnets at its ends; 129 - 512-token sequences (all attn_stream_kernel); bins whose sequences alternate with and without boundary magnets: [127 ends, 1 none],
 # [60 ends, 40 none, 23 ends, 5 none], [2 none, 1 ends] (first-fit decreasing), [128 none] first after the long units
 PACKED = [(4097, "none"), (513, "ends"), (511, "none"), (129, "ends"), (512, "none"), (60, "ends"), (128, "none"),
           (40, "none"), (127, "ends"), (23, "ends"), (1, "none"), (5, "none"), (2, "none"), (1, "ends"),
@@ -130,7 +129,7 @@ PACKED = [(4097, "none"), (513, "ends"), (511, "none"), (129, "ends"), (512, "no
 @pytest.mark.parametrize("dh", [64, 32])
 def test_magnets_packed(enc_mod, dh, layout):
     # "cut": without the 4097-token sequence and max_batch_tokens 700, so the call is cut into row groups between the
-    # stream unit, the long units and the bins
+    # the long units and the bins
     gen, spec, sd = _magnet_model(dh, 3100 + dh)
     cases = PACKED if layout == "one_group" else PACKED[1:]
     seqs = [st.with_magnets(gen, n, where) for n, where in cases]

@@ -1,7 +1,7 @@
 """GPU: sequences of 513 - 8192 tokens on the sm_90a encoder (attn_stream_kernel), BERT and RoBERTa, head widths 64 and 32.
 
-Every batch below mixes bins (<= 128 tokens, attn_kernel), 129 - 512-token sequences (attn_long_kernel) and longer ones
-(attn_stream_kernel), so all three attention kernels run in every layer.  Reps and attended hidden rows are held to the
+Every batch below mixes bins (<= 128 tokens, attn_kernel), 129 - 512-token sequences and longer ones (both
+attn_stream_kernel), so both attention kernels run in every layer.  Reps and attended hidden rows are held to the
 float64-oracle bound of tests/test_encoder_numerics_gpu.py (err_kernel <= 2 err_autocast + 2e-4, plus rel-L2 <= 1e-2 and
 cosine >= 0.9999), one sequence per oracle call; the online softmax at 8192 tokens with the row maxima in the first,
 the last and a moving key tile; bitwise batch invariance, pair assembly and the padded DRModel path; refusals before any
@@ -20,7 +20,7 @@ from test_encoder_numerics_gpu import F64, _judge, _Logits, _ospec, _tile_gap
 
 pytestmark = pytest.mark.gpu
 
-SHORT = [1, 77, 128, 129, 300, 512]  # one sequence of each attention kernel below 513 tokens
+SHORT = [1, 77, 128, 129, 300, 512]  # both sides of the one-tile limit of attn_kernel, up to 512 tokens
 
 
 @pytest.fixture(scope="module")

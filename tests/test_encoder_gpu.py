@@ -228,7 +228,7 @@ def test_t5_base_vs_oracle(enc_mod, L, B):
 
 @pytest.mark.parametrize("L,B", [(256, 3), (384, 2), (512, 2)])
 def test_bert_long_sequences_vs_oracle(enc_mod, L, B):
-    # sequences longer than one attention tile: online softmax over 128-key tiles (attn_long_kernel)
+    # sequences longer than one attention tile: online softmax over 128-key tiles (attn_stream_kernel)
     gen = torch.Generator().manual_seed(300 + L)
     layers, H, F, vocab = 2, 768, 3072, 2000
     sd = _rand_bert_sd(gen, layers, H, F, vocab, 512)

@@ -1,6 +1,6 @@
 """GPU: BERT encoders with 32-wide attention heads (all-MiniLM, bge-small, e5-small, gte-small: hidden 384, 12 heads).
 
-attn_kernel<32> / attn_long_kernel<32> take one work item per (tile, pair of heads).  Reps and attended hidden rows are
+attn_kernel<32> / attn_stream_kernel<32> take one work item per (tile, pair of heads).  Reps and attended hidden rows are
 held to the float64-oracle bound of tests/test_encoder_numerics_gpu.py (err_kernel <= 2 err_autocast + 2e-4, plus
 rel-L2 <= 1e-2 and cosine >= 0.9999) on the padded and the packed path; the reference's own golden vectors, the HF
 module, handles of both widths in one process, side streams, poisoned workspaces, refusals and the drivers end to end."""
@@ -51,7 +51,7 @@ def _other_dtype(enc, reps, ids, mask, tt, dtype):
 
 
 # (model, L, B, pooling, head, normalize, out dtype, query scale): every attn_kernel packing (L = 1 .. 128 -> 128 .. 1
-# sequences per tile) and attn_long_kernel at 2, 3 and 4 key tiles
+# sequences per tile) and attn_stream_kernel at 2, 3 and 4 key tiles
 PADDED = [("bge_small", 128, 6, "first", False, True, torch.float32, 1), ("bge_small", 512, 2, "mean", False, True,
                                                                           torch.bfloat16, 1),
           ("bge_small", 37, 9, "mean", True, False, torch.float16, 1),
@@ -172,7 +172,7 @@ def test_hf_parity_through_drmodel(enc_mod, pooling, normalize):
 # ------------------------------------------------------------------------------------------------------------------
 # handles of both widths in one process, side streams, poisoned workspaces
 # ------------------------------------------------------------------------------------------------------------------
-GEOMS = [(32, 11), (100, 7), (256, 3)]  # attn_kernel with 4 and 1 sequences per tile, attn_long_kernel
+GEOMS = [(32, 11), (100, 7), (256, 3)]  # attn_kernel with 4 and 1 sequences per tile, attn_stream_kernel
 
 
 def _inputs(gen):

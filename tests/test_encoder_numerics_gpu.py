@@ -174,7 +174,7 @@ def test_attention_isolated_per_token(enc_mod, L, B):
 
 
 # ------------------------------------------------------------------------------------------------------------------
-# online softmax across key tiles (attn_long_kernel) and saturated exponents (both attention kernels)
+# online softmax across key tiles (attn_stream_kernel) and saturated exponents (both attention kernels)
 # ------------------------------------------------------------------------------------------------------------------
 def _tile_gap(s, rows, q_tiles, early):
     """for every selected query row: (max logit of key tile 0 - max of later tiles) if early, else

@@ -202,17 +202,17 @@ def _free_port():
         return s.getsockname()[1]
 
 
-def _big_run_inputs(tmp_path):
-    """2 queries x 150 passages (more than the reference's top-100 merge keeps)"""
+def _big_run_inputs(tmp_path, write=True):
+    """2 queries x 150 passages (more than the reference's top-100 merge keeps).  Only the caller that passes
+    write=True writes the files: a rank that rewrote them could truncate the corpus while another rank reads it."""
     from transformers import BertTokenizer
     words = ["river", "bank", "money", "loan", "water", "fish", "tree", "green", "blue", "sky"]
-    (tmp_path / "vocab.txt").write_text("\n".join(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "[MASK]"] + words))
     rng = np.random.default_rng(11)
-    with open(tmp_path / "corpus.tsv", "w") as f:
-        for i in range(150):
-            f.write("d%d\t%s\t%s\n" % (i, words[i % 10], " ".join(rng.choice(words, 1 + i % 37))))
-    with open(tmp_path / "queries.tsv", "w") as f:
-        f.write("qa\triver bank\nqb\tgreen tree sky water\n")
+    corpus = "".join("d%d\t%s\t%s\n" % (i, words[i % 10], " ".join(rng.choice(words, 1 + i % 37))) for i in range(150))
+    if write:
+        (tmp_path / "vocab.txt").write_text("\n".join(["[PAD]", "[UNK]", "[CLS]", "[SEP]", "[MASK]"] + words))
+        (tmp_path / "corpus.tsv").write_text(corpus)
+        (tmp_path / "queries.tsv").write_text("qa\triver bank\nqb\tgreen tree sky water\n")
     run = {q: {"d%d" % i: float(-i) for i in rng.permutation(150)} for q in ("qa", "qb")}
     z = {"q_max_len": 8, "p_max_len": 32}
     tok = BertTokenizer(str(tmp_path / "vocab.txt"), do_lower_case=True)
@@ -225,7 +225,7 @@ def _worker(rank, world, port, tmp):
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
         from openmatch_b200.utils import save_as_trec
-        tok, (qds, cds), run = _big_run_inputs(pathlib.Path(tmp))
+        tok, (qds, cds), run = _big_run_inputs(pathlib.Path(tmp), write=False)
         result = _fake_reranker(tok, cds, world, rank).rerank(qds, run)
         if rank == 0:
             save_as_trec(result, os.path.join(tmp, "out", "rerank.trec"))

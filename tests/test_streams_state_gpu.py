@@ -521,7 +521,7 @@ def test_index_call_sequence_matches_fresh_index(om):
 # ---------------------------------------------------------------------------------------------------------------------
 # Filling device memory from outside and releasing it does not work: on the H100 the driver hands every cudaMalloc
 # zero-filled pages.  OPENMATCH_B200_POISON_ALLOC=1 makes the library fill its own fresh buffers with 0xFF bytes instead.
-POISON_GEOMS = [(32, 11), (100, 7), (256, 3)]  # attn_kernel with 4 and 1 sequences per tile, attn_long_kernel
+POISON_GEOMS = [(32, 11), (100, 7), (256, 3)]  # attn_kernel with 4 and 1 sequences per tile, attn_stream_kernel
 
 
 @pytest.fixture(scope="module")
