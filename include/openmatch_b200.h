@@ -48,8 +48,29 @@ typedef enum { OM_HOST = 0, OM_DEVICE = 1 } om_memkind;
  * padding_idx = pad_token_id = 1 (the value of every such config; fixed here): a token with id != 1 gets position
  * 1 + (number of ids != 1 up to and including it in its sequence), a token with id 1 gets position 1, whatever the
  * attention mask says.  Sequences are at most max_position_embeddings - 2 tokens long (8194 positions, as in
- * XLM-RoBERTa-based bge-m3: 8192 tokens, the longest om_encode_packed takes). */
-typedef enum { OM_ARCH_BERT = 0, OM_ARCH_T5ENC = 1, OM_ARCH_ROBERTA = 2 } om_arch;
+ * XLM-RoBERTa-based bge-m3: 8192 tokens, the longest om_encode_packed takes).
+ * OM_ARCH_MPNET: MPNet (all-mpnet-base-v2, multi-qa-mpnet), BERT's post-LN encoder with 64-wide heads only (any other
+ * width returns OM_EINVAL), no token-type embeddings (token_type_ids are ignored, as for T5), RoBERTa's position ids
+ * (padding_idx 1, whatever pad_token_id says) and a relative position bias shared by all layers, added to the scaled
+ * logits: T5's bidirectional bucket of (key index - query index) in the sequence, rel_buckets = 32 and
+ * rel_max_distance = 128 (both required, as MPNetEncoder.compute_position_bias fixes them).  Names, optionally prefixed
+ * "mpnet.": embeddings.{word_embeddings, position_embeddings, LayerNorm}, encoder.layer.<i>.attention.attn.{q, k, v, o},
+ * encoder.layer.<i>.attention.LayerNorm, encoder.layer.<i>.intermediate.dense, encoder.layer.<i>.output.{dense,
+ * LayerNorm}, encoder.relative_attention_bias.weight [32, heads].  Sequences are at most min(512,
+ * max_position_embeddings - 2) tokens long (the relative-bias tables cover 512).
+ * OM_ARCH_DISTILBERT: DistilBERT (TAS-B, msmarco-distilbert, multi-qa-distilbert), BERT's encoder and arithmetic with
+ * no token-type embeddings (token_type_ids are ignored) and positions 0 .. L-1; every LayerNorm eps is 1e-12 in HF, so
+ * pass ln_eps = 1e-12.  Names, optionally prefixed "distilbert.": embeddings.{word_embeddings, position_embeddings,
+ * LayerNorm}, transformer.layer.<i>.attention.{q_lin, k_lin, v_lin, out_lin}, transformer.layer.<i>.sa_layer_norm,
+ * transformer.layer.<i>.ffn.{lin1, lin2}, transformer.layer.<i>.output_layer_norm.  Sequences are at most min(8192,
+ * max_position_embeddings) tokens long, as for BERT. */
+typedef enum {
+  OM_ARCH_BERT = 0,
+  OM_ARCH_T5ENC = 1,
+  OM_ARCH_ROBERTA = 2,
+  OM_ARCH_MPNET = 3,
+  OM_ARCH_DISTILBERT = 4
+} om_arch;
 typedef enum { OM_POOL_FIRST = 0, OM_POOL_MEAN = 1 } om_pooling;
 typedef enum { OM_REDUCE_MEAN = 0, OM_REDUCE_SUM = 1 } om_reduction;
 
@@ -73,16 +94,16 @@ typedef struct om_encoder_desc {
                                most 2048.  Any other width returns OM_EINVAL */
   int32_t ffn;              /* intermediate_size / d_ff (multiple of 64) */
   int32_t vocab;            /* vocab_size */
-  int32_t max_pos;          /* max_position_embeddings (BERT; RoBERTa: including its offset of 2, e.g. 514, at least
-                               3); ignored for T5 */
-  int32_t type_vocab;       /* type_vocab_size (BERT; RoBERTa: normally 1); ignored for T5 */
+  int32_t max_pos;          /* max_position_embeddings (BERT; RoBERTa, MPNet: including their offset of 2, e.g. 514,
+                               at least 3); ignored for T5 */
+  int32_t type_vocab;       /* type_vocab_size (BERT; RoBERTa: normally 1); ignored for T5, MPNet and DistilBERT */
   float ln_eps;             /* layer_norm_eps (1e-12 BERT) / layer_norm_epsilon (1e-6 T5) */
   int32_t pooling;          /* om_pooling: DRModel.pooling 'first' | 'mean' */
   int32_t has_head;         /* 1: bias-free LinearHead follows pooling */
   int32_t head_out;         /* LinearHead output_dim (any positive width) */
   int32_t normalize;        /* 1: F.normalize(reps, dim=1) */
-  int32_t rel_buckets;      /* T5 relative_attention_num_buckets (32) */
-  int32_t rel_max_distance; /* T5 relative_attention_max_distance (128) */
+  int32_t rel_buckets;      /* T5 relative_attention_num_buckets (32); MPNet: must be 32 */
+  int32_t rel_max_distance; /* T5 relative_attention_max_distance (128); MPNet: must be 128 */
   int32_t max_batch_tokens; /* workspace sizing: max B*L per om_encode call (e.g. 256*128) */
 } om_encoder_desc;
 
@@ -98,9 +119,9 @@ int om_encoder_set_weight(om_encoder* enc, const char* name, const void* data, o
                           const int64_t* shape, int ndim);
 /* Verifies that every required parameter was supplied and builds derived tables. */
 int om_encoder_finalize(om_encoder* enc);
-/* input_ids / attention_mask / token_type_ids (nullable => zeros; ignored for T5): int64 [B, L] device,
- * row-major, exactly what DRInferenceCollator / QPCollator hand to the model; L <= 128 or 256 / 384 / 512, and
- * L <= max_position_embeddings (BERT) / max_position_embeddings - 2 (RoBERTa).
+/* input_ids / attention_mask / token_type_ids (nullable => zeros; ignored for T5, MPNet and DistilBERT): int64 [B, L]
+ * device, row-major, exactly what DRInferenceCollator / QPCollator hand to the model; L <= 128 or 256 / 384 / 512, and
+ * L <= max_position_embeddings (BERT, DistilBERT) / max_position_embeddings - 2 (RoBERTa, MPNet).
  * out_reps: device [B, rep_dim] fp32, bf16 or fp16 with row pitch out_row_stride (elements) — may point into an
  * index shard obtained from om_index_reserve() / om_index_reserve_rows().  fp16 output is the round-to-nearest-even
  * of the fp32 output of the same call (values beyond the half range become inf).  out_hidden: nullable device fp32 [B, L, hidden]
@@ -108,10 +129,11 @@ int om_encoder_finalize(om_encoder* enc);
 int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attention_mask,
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
               int64_t out_row_stride, float* out_hidden, void* stream);
-/* Variable-length batch, no padding.  tokens / token_type_ids (nullable => zeros; ignored for T5): int64 [T] device, the
- * B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 8192 for BERT (and <= max_position_embeddings)
- * and RoBERTa (and <= max_position_embeddings - 2, positions computed from each sequence's own ids), <= 512 for T5 (its
- * relative-bias tables cover 512 tokens); and <= max_batch_tokens; T = sum(seqlens).  Result: what om_encode returns
+/* Variable-length batch, no padding.  tokens / token_type_ids (nullable => zeros; ignored for T5, MPNet and DistilBERT):
+ * int64 [T] device, the B sequences back to back; seqlens: int32 [B] HOST, 1 <= seqlens[i] <= 8192 for BERT and
+ * DistilBERT (and <= max_position_embeddings) and RoBERTa (and <= max_position_embeddings - 2, positions computed from
+ * each sequence's own ids), <= 512 for T5 and MPNet (their relative-bias tables cover 512 tokens; MPNet also <=
+ * max_position_embeddings - 2); and <= max_batch_tokens; T = sum(seqlens).  Result: what om_encode returns
  * for the same sequences padded to any L it takes with attention_mask = 1 on their tokens, up to the order of
  * floating-point sums in attention and pooling (longer sequences have no padded counterpart).  out_reps as in
  * om_encode (row i = sequence i).  out_hidden: nullable fp32 [T, hidden], packed like tokens.  seqlens may be reused on

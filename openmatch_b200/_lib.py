@@ -14,7 +14,7 @@ LIB_PATH = os.environ.get("OPENMATCH_B200_LIB") or os.path.join(_HERE, "lib", "l
 
 OM_F32, OM_BF16, OM_F16 = 0, 1, 2
 OM_HOST, OM_DEVICE = 0, 1
-OM_ARCH_BERT, OM_ARCH_T5ENC, OM_ARCH_ROBERTA = 0, 1, 2
+OM_ARCH_BERT, OM_ARCH_T5ENC, OM_ARCH_ROBERTA, OM_ARCH_MPNET, OM_ARCH_DISTILBERT = 0, 1, 2, 3, 4
 OM_POOL_FIRST, OM_POOL_MEAN = 0, 1
 OM_REDUCE_MEAN, OM_REDUCE_SUM = 0, 1
 

@@ -792,7 +792,7 @@ __device__ __forceinline__ float quad_sum(float v) {
 // + (e & 1) of the 64-row block.
 // DH = head width (64, or 32 for BERT).  A work item is a (tile, unit of kAttnCols columns) pair: the unit holds
 // 64 / DH whole heads, so the boxes, the shared-memory layout and the work per item are those of one 64-wide head.
-// The relative position bias (T5) exists for 64-wide heads only.
+// The relative position bias (T5, MPNet) exists for 64-wide heads only.
 template <int DH>
 __global__ void __launch_bounds__(128, kAttnCtasPerSm)
 attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CUtensorMap tmVt, AttnParams p, int n_tiles,
@@ -928,7 +928,7 @@ attn_kernel(const __grid_constant__ CUtensorMap tmQK, const __grid_constant__ CU
 //             wgmma run.
 // The key-validity bits come per key tile, so the length is bounded by nothing the kernel sizes.  Keys of a tile that
 // are all valid (every tile but a sequence's last) skip the masking.  Padding rows after a sequence's last token attend
-// like its tokens (finite values nobody reads).  REL (T5, 64-wide heads, at most kMaxLongL tokens) adds the relative
+// like its tokens (finite values nobody reads).  REL (T5, MPNet: 64-wide heads, at most kMaxLongL tokens) adds the relative
 // position bias, a [2 kMaxLongL - 1] row per head held in shared memory.
 // ---------------------------------------------------------------------------------------------------
 constexpr int kMaxStreamL = 8192;
@@ -1307,7 +1307,7 @@ struct om_encoder {
   std::vector<LayerW> layers;
   float *word = nullptr, *pos = nullptr, *type = nullptr, *emb_g = nullptr, *emb_b = nullptr;  // BERT embeddings
   float* final_g = nullptr;                                                                    // T5 final RMSNorm
-  float* rel_w = nullptr;         // T5 [buckets, heads]
+  float* rel_w = nullptr;         // T5, MPNet [buckets, heads]
   float* relbias_log2 = nullptr;  // [heads, 255]
   float* relbias_long_log2 = nullptr;  // [heads, 1023] (sequences longer than one tile)
   float* head_w = nullptr;        // [head_out, H]
@@ -1328,27 +1328,38 @@ struct om_encoder {
   PairSpan* pr_spans = nullptr;  // [Tmax]
   PairSpan* pr_host = nullptr;   // [Tmax], pinned host memory
   int64_t* pr_tokens = nullptr;  // [Tmax]
-  int32_t* pos_ids = nullptr;    // [Tmax] RoBERTa position id per layout row (roberta_pos_kernel); RoBERTa handles only
+  int32_t* pos_ids = nullptr;    // [Tmax] RoBERTa / MPNet position id per layout row (roberta_pos_kernel); their handles only
   std::vector<void*> allocs;
 };
 
 namespace {
 
-// RoBERTa is BERT's encoder with position ids computed from the token ids (roberta_pos_kernel)
-bool bert_like(int arch) { return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERTA; }
+// BERT's post-LN encoder: RoBERTa with position ids computed from the token ids (roberta_pos_kernel), MPNet with those
+// position ids and a relative position bias, DistilBERT under other parameter names; MPNet and DistilBERT have no
+// token-type embeddings
+bool bert_like(int arch) {
+  return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERTA || arch == OM_ARCH_MPNET || arch == OM_ARCH_DISTILBERT;
+}
+bool has_token_types(int arch) { return arch == OM_ARCH_BERT || arch == OM_ARCH_ROBERTA; }
+bool ids_positions(int arch) { return arch == OM_ARCH_ROBERTA || arch == OM_ARCH_MPNET; }
+// a relative position bias shared by all layers, added to the scaled logits (relbias_log2 / relbias_long_log2)
+bool has_relbias(int arch) { return arch == OM_ARCH_T5ENC || arch == OM_ARCH_MPNET; }
 
-// The longest sequence the architecture and its position table allow: 8192 tokens and max_position_embeddings (BERT) /
-// max_position_embeddings - 2 (RoBERTa: positions start at padding_idx + 1 = 2); 512 tokens for T5 (its relative-bias
-// tables cover 512).  seq_limit_name names these limits for error messages.
+// The longest sequence the architecture and its position table allow: 8192 tokens and max_position_embeddings (BERT,
+// DistilBERT) / max_position_embeddings - 2 (RoBERTa: positions start at padding_idx + 1 = 2); 512 tokens for T5 and
+// MPNet (their relative-bias tables cover 512; MPNet also within max_position_embeddings - 2).  seq_limit_name names
+// these limits for error messages.
 int max_seq_len(const om_encoder_desc& d) {
   if (d.arch == OM_ARCH_T5ENC) return kMaxLongL;
+  if (d.arch == OM_ARCH_MPNET) return std::min(kMaxLongL, d.max_pos - 2);
   return std::min(kMaxStreamL, d.arch == OM_ARCH_ROBERTA ? d.max_pos - 2 : d.max_pos);
 }
 
 const char* seq_limit_name(int arch) {
-  return arch == OM_ARCH_ROBERTA ? "8192 tokens, max_position_embeddings - 2"
-         : arch == OM_ARCH_BERT  ? "8192 tokens, max_position_embeddings"
-                                 : "512 tokens (T5)";
+  return arch == OM_ARCH_ROBERTA                                ? "8192 tokens, max_position_embeddings - 2"
+         : arch == OM_ARCH_BERT || arch == OM_ARCH_DISTILBERT ? "8192 tokens, max_position_embeddings"
+         : arch == OM_ARCH_MPNET                                ? "512 tokens, max_position_embeddings - 2 (MPNet)"
+                                                                : "512 tokens (T5)";
 }
 
 template <typename T>
@@ -1501,19 +1512,22 @@ int encode_layers(om_encoder* e, int T, const AttnParams& ap_stream, int n_strea
 }
 
 // Embeds T layout rows into e->h / e->xb / e->stats[0]: the padded rows of nseq sequences of L tokens (seqs == nullptr),
-// or the rows of a packed group (its sequence table seqs, L = 0, and the row map e->rowmap).  RoBERTa first computes the
-// position ids from the token ids, as HF does per sequence.
+// or the rows of a packed group (its sequence table seqs, L = 0, and the row map e->rowmap).  RoBERTa and MPNet first
+// compute the position ids from the token ids, as HF does per sequence.  MPNet and DistilBERT ignore token_type_ids:
+// every row adds the zeroed single row of e->type.
 int embed_rows(om_encoder* e, const int64_t* ids, const int64_t* tts, int T, int L, const PackedSeq* seqs, int nseq,
                cudaStream_t st) {
   const om_encoder_desc& d = e->d;
-  const int H = d.hidden, rows4 = (T + 3) / 4, type_vocab = std::max(d.type_vocab, 1);
+  const bool types = has_token_types(d.arch);
+  const int H = d.hidden, rows4 = (T + 3) / 4, type_vocab = types ? std::max(d.type_vocab, 1) : 1;
+  if (!types) tts = nullptr;
   const int2* rowmap = seqs ? e->rowmap : nullptr;
   const int Lrow = seqs ? kMaxL : L;  // packed rows take their positions from the row map
-  if (d.arch == OM_ARCH_ROBERTA) {
+  if (ids_positions(d.arch)) {
     roberta_pos_kernel<<<(nseq + 3) / 4, 128, 0, st>>>(ids, nseq, L, seqs, e->pos_ids);
     bert_embed_kernel<true><<<rows4, 128, 0, st>>>(ids, tts, e->word, e->type, e->pos, T, Lrow, H, d.vocab, type_vocab,
                                                    e->h, e->xb, e->stats[0], rowmap, seqs, e->pos_ids);
-  } else if (d.arch == OM_ARCH_BERT) {
+  } else if (bert_like(d.arch)) {
     bert_embed_kernel<false><<<rows4, 128, 0, st>>>(ids, tts, e->word, e->type, e->pos, T, Lrow, H, d.vocab, type_vocab,
                                                     e->h, e->xb, e->stats[0], rowmap, seqs, nullptr);
   } else {
@@ -1650,7 +1664,7 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
                         int n, void* out_reps, om_dtype out_dtype, int64_t out_row_stride, float* out_hidden, int sms,
                         cudaStream_t st) {
   const om_encoder_desc& d = e->d;
-  const bool bert = bert_like(d.arch);
+  const bool rel = has_relbias(d.arch);
   const int H = d.hidden;
   // upload the tables through the pinned staging buffers: wait (on the host) only until the previous upload from them
   // has been read
@@ -1678,13 +1692,13 @@ int encode_packed_chunk(om_encoder* e, const int64_t* tokens, const int64_t* tok
     if (pairs)
       pair_tokens_kernel<<<ns, 128, 0, st>>>(pairs->a, pairs->b, gs, e->pr_spans + g.k0, pairs->sp, e->pr_tokens);
     packed_rowmap_kernel<<<(T + 255) / 256, 256, 0, st>>>(gs, ns, T, e->rowmap, e->kmask);
-    // (for pairs, RoBERTa's positions come from the stream pair_tokens_kernel assembled)
+    // (for pairs, RoBERTa's and MPNet's positions come from the stream pair_tokens_kernel assembled)
     OM_TRY(embed_rows(e, tokens, token_type_ids, T, 0, gs, ns, st));
     ap.T = T;
     ap.seqs = gs;
     AttnParams ap_stream = ap, ap_short = ap;
-    ap_stream.relbias_log2 = bert ? nullptr : e->relbias_long_log2;
-    ap_short.relbias_log2 = bert ? nullptr : e->relbias_log2;
+    ap_stream.relbias_log2 = rel ? e->relbias_long_log2 : nullptr;
+    ap_short.relbias_log2 = rel ? e->relbias_log2 : nullptr;
     ap_short.tile0 = g.n_stream;
     OM_TRY(encode_layers(e, T, ap_stream, g.n_stream, ap_short, g.n_tiles - g.n_stream, sms, st));
     if (out_hidden) gather_packed_rows_kernel<<<rows4, 128, 0, st>>>(e->h, e->rowmap, gs, T, H, out_hidden);
@@ -1706,8 +1720,9 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   OM_TRY(device_sm_count());
   const om_encoder_desc& d = *desc;
   if (!bert_like(d.arch) && d.arch != OM_ARCH_T5ENC) return fail(OM_EINVAL, "unknown arch %d", d.arch);
-  if (d.arch == OM_ARCH_ROBERTA && d.max_pos < 3)
-    return fail(OM_EINVAL, "RoBERTa max_position_embeddings=%d unsupported (at least 3: positions start at 2)", d.max_pos);
+  if (ids_positions(d.arch) && d.max_pos < 3)
+    return fail(OM_EINVAL, "%s max_position_embeddings=%d unsupported (at least 3: positions start at 2)",
+                d.arch == OM_ARCH_MPNET ? "MPNet" : "RoBERTa", d.max_pos);
   if (d.hidden <= 0 || d.hidden % 128 != 0 || d.hidden > 1024)
     return fail(OM_EINVAL, "hidden=%d unsupported (multiple of 128, <= 1024)", d.hidden);
   if (d.heads <= 0) return fail(OM_EINVAL, "heads=%d must be positive", d.heads);
@@ -1718,6 +1733,13 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   if (dh != 32 && dh != 64)
     return fail(OM_EINVAL, "BERT head width hidden/heads=%d unsupported (32 or 64; hidden=%d heads=%d)", dh, d.hidden,
                 d.heads);
+  // the relative position bias exists in the 64-wide attention instantiations only
+  if (d.arch == OM_ARCH_MPNET && dh != 64)
+    return fail(OM_EINVAL, "MPNet head width hidden/heads=%d unsupported (64 only; hidden=%d heads=%d)", dh, d.hidden,
+                d.heads);
+  if (d.arch == OM_ARCH_MPNET && (d.rel_buckets != 32 || d.rel_max_distance != 128))
+    return fail(OM_EINVAL, "MPNet needs rel_buckets=32 and rel_max_distance=128 (got %d, %d)", d.rel_buckets,
+                d.rel_max_distance);
   if (d.heads * dh > 2048 || (d.heads * dh) % 128 != 0)
     return fail(OM_EINVAL, "heads=%d unsupported (heads * head width %d must be a multiple of 128, at most 2048)", d.heads,
                 dh);
@@ -1750,24 +1772,29 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
     e->params.push_back(std::move(p));
   };
   if (bert) {
-    A(&e->type, (size_t)std::max(d.type_vocab, 1) * H);  // at least one row: token types are clamped into the table
+    // at least one row: token types are clamped into the table (without token types: one row, zeroed below)
+    A(&e->type, (size_t)(has_token_types(d.arch) ? std::max(d.type_vocab, 1) : 1) * H);
     param("embeddings.word_embeddings.weight", d.vocab, H, &e->word, nullptr);
     param("embeddings.position_embeddings.weight", d.max_pos, H, &e->pos, nullptr);
-    param("embeddings.token_type_embeddings.weight", d.type_vocab, H, &e->type, nullptr);
+    if (has_token_types(d.arch)) param("embeddings.token_type_embeddings.weight", d.type_vocab, H, &e->type, nullptr);
     param("embeddings.LayerNorm.weight", H, -1, &e->emb_g, nullptr);
     param("embeddings.LayerNorm.bias", H, -1, &e->emb_b, nullptr);
-    if (d.arch == OM_ARCH_ROBERTA) A(&e->pos_ids, (size_t)d.max_batch_tokens);
+    if (ids_positions(d.arch)) A(&e->pos_ids, (size_t)d.max_batch_tokens);
   } else {
     param("shared.weight", d.vocab, H, &e->word, nullptr);
     param("encoder.final_layer_norm.weight", H, -1, &e->final_g, nullptr);
-    param("encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight", d.rel_buckets, d.heads, &e->rel_w,
-          nullptr);
+  }
+  if (has_relbias(d.arch)) {
+    param(d.arch == OM_ARCH_MPNET ? "encoder.relative_attention_bias.weight"
+                                  : "encoder.block.0.layer.0.SelfAttention.relative_attention_bias.weight",
+          d.rel_buckets, d.heads, &e->rel_w, nullptr);
     A(&e->relbias_log2, (size_t)d.heads * (2 * kMaxL - 1));
     A(&e->relbias_long_log2, (size_t)d.heads * (2 * kMaxLongL - 1));
   }
-  // each layer's modules, named after "encoder.layer.<i>." (BERT) / "encoder.block.<i>." (T5): "<module>.weight" of
-  // shape [rows, cols] ([rows] for a norm) into f32 or bf16, and (BERT) "<module>.bias" of shape [rows].  The QKV and
-  // W1 weights land in fp32 staging buffers that om_encoder_finalize folds into wqkv / w1.
+  // each layer's modules, named after "encoder.layer.<i>." (BERT, MPNet) / "transformer.layer.<i>." (DistilBERT) /
+  // "encoder.block.<i>." (T5): "<module>.weight" of shape [rows, cols] ([rows] for a norm) into f32 or bf16, and (all
+  // but T5) "<module>.bias" of shape [rows].  The QKV and W1 weights land in fp32 staging buffers that
+  // om_encoder_finalize folds into wqkv / w1.
   struct LayerModule {
     const char* name;
     int64_t rows, cols;
@@ -1776,7 +1803,25 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
     float* LayerW::*bias;
     int slot;
   };
-  const std::vector<LayerModule> modules = bert ? std::vector<LayerModule>{
+  const std::vector<LayerModule> modules = d.arch == OM_ARCH_MPNET ? std::vector<LayerModule>{
+      {"attention.attn.q", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 0},
+      {"attention.attn.k", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 1},
+      {"attention.attn.v", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 2},
+      {"attention.attn.o", H, I, nullptr, &LayerW::wo, &LayerW::bo, -1},
+      {"attention.LayerNorm", H, -1, &LayerW::ln1_g, nullptr, &LayerW::ln1_b, -1},
+      {"intermediate.dense", F, H, &LayerW::w1_f32, nullptr, &LayerW::b1, -1},
+      {"output.dense", H, F, nullptr, &LayerW::w2, &LayerW::b2, -1},
+      {"output.LayerNorm", H, -1, &LayerW::ln2_g, nullptr, &LayerW::ln2_b, -1},
+  } : d.arch == OM_ARCH_DISTILBERT ? std::vector<LayerModule>{
+      {"attention.q_lin", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 0},
+      {"attention.k_lin", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 1},
+      {"attention.v_lin", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 2},
+      {"attention.out_lin", H, I, nullptr, &LayerW::wo, &LayerW::bo, -1},
+      {"sa_layer_norm", H, -1, &LayerW::ln1_g, nullptr, &LayerW::ln1_b, -1},
+      {"ffn.lin1", F, H, &LayerW::w1_f32, nullptr, &LayerW::b1, -1},
+      {"ffn.lin2", H, F, nullptr, &LayerW::w2, &LayerW::b2, -1},
+      {"output_layer_norm", H, -1, &LayerW::ln2_g, nullptr, &LayerW::ln2_b, -1},
+  } : bert ? std::vector<LayerModule>{
       {"attention.self.query", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 0},
       {"attention.self.key", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 1},
       {"attention.self.value", I, H, &LayerW::wqkv_f32, nullptr, &LayerW::bqkv, 2},
@@ -1803,7 +1848,10 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
       A(&w.bqkv_fold, (size_t)3 * I);
       A(&w.b1_fold, F);
     }
-    const std::string prefix = (bert ? "encoder.layer." : "encoder.block.") + std::to_string(i) + ".";
+    const std::string prefix = std::string(d.arch == OM_ARCH_DISTILBERT ? "transformer.layer."
+                                           : bert                         ? "encoder.layer."
+                                                                          : "encoder.block.") +
+                               std::to_string(i) + ".";
     for (const LayerModule& m : modules) {
       param(prefix + m.name + ".weight", m.rows, m.cols, m.f32 ? &(w.*m.f32) : nullptr, m.bf16 ? &(w.*m.bf16) : nullptr,
             m.slot);
@@ -1840,7 +1888,8 @@ int om_encoder_create(const om_encoder_desc* desc, om_encoder** out) {
   // statistics slots a GEMM configuration never writes must read as zero (see RowNorm)
   if (cudaMemset(e->stats[0], 0, T * 2 * kStatParts * 4) != cudaSuccess ||
       cudaMemset(e->stats[1], 0, T * 2 * kStatParts * 4) != cudaSuccess ||
-      cudaMemset(e->vt, 0, (size_t)I * e->Tld * 2) != cudaSuccess) {
+      cudaMemset(e->vt, 0, (size_t)I * e->Tld * 2) != cudaSuccess ||
+      (bert && !has_token_types(d.arch) && cudaMemset(e->type, 0, (size_t)H * 4) != cudaSuccess)) {
     om_encoder_destroy(e);
     return fail(OM_ECUDA, "workspace memset failed");
   }
@@ -1866,6 +1915,8 @@ int om_encoder_set_weight(om_encoder* e, const char* name_c, const void* data, o
   std::string name(name_c);
   if (name.rfind("bert.", 0) == 0) name = name.substr(5);  // BertFor* checkpoints prefix the backbone
   if (name.rfind("roberta.", 0) == 0) name = name.substr(8);  // and RobertaFor* / XLMRobertaFor* ones
+  if (name.rfind("mpnet.", 0) == 0) name = name.substr(6);    // MPNetFor*
+  if (name.rfind("distilbert.", 0) == 0) name = name.substr(11);  // DistilBertFor*
   if (name == "encoder.embed_tokens.weight") name = "shared.weight";  // T5EncoderModel's name of the tied embedding
   if (name == "linear.weight") name = "head.linear.weight";           // LinearHead's own state_dict
   // the gated-GELU feed-forward (T5 v1.1, Flan-T5, mT5) has wi_0 / wi_1 where this one has wi: refused, not ignored
@@ -1895,7 +1946,7 @@ int om_encoder_finalize(om_encoder* e) {
       ++nmiss;
     }
   if (nmiss) return fail(OM_ESTATE, "om_encoder_finalize: %d parameter(s) missing: %s%s", nmiss, miss.c_str(), nmiss > 4 ? ", ..." : "");
-  if (e->d.arch == OM_ARCH_T5ENC) {
+  if (has_relbias(e->d.arch)) {  // T5, MPNet: the bias of every relative position a kernel sees, log2 domain
     const int nh = e->d.heads;
     std::vector<float> bias((size_t)e->d.rel_buckets * nh);  // relative_attention_bias [buckets, heads]
     OM_CUDA(cudaMemcpy(bias.data(), e->rel_w, bias.size() * 4, cudaMemcpyDeviceToHost));
@@ -1960,7 +2011,6 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const int T = static_cast<int>(T64), H = d.hidden, I = e->I;
-  const bool bert = bert_like(d.arch);
 
   NvtxRange nvtx("om.encode");
   keymask_kernel<<<(T + 255) / 256, 256, 0, st>>>(attention_mask, e->kmask, T);
@@ -1978,7 +2028,7 @@ int om_encode(om_encoder* e, const int64_t* input_ids, const int64_t* attention_
   ap.Tvalid_rows = long_seq ? 128 : spt * L;
   ap.scale_log2 = attn_scale_log2(e);
   ap.kmask = e->kmask;
-  ap.relbias_log2 = bert ? nullptr : (long_seq ? e->relbias_long_log2 : e->relbias_log2);
+  ap.relbias_log2 = has_relbias(d.arch) ? (long_seq ? e->relbias_long_log2 : e->relbias_log2) : nullptr;
   ap.ctx = e->ctx;
   ap.rowmap = nullptr;
   ap.seqs = nullptr;

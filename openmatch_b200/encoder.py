@@ -28,14 +28,19 @@ def _check_bert_heads(hidden: int, heads: int):
                          % (hidden, heads))
 
 
-ROBERTA_PAD_ID = 1  # padding_idx of RoBERTa's position ids, fixed in the library (include/openmatch_b200.h)
+ROBERTA_PAD_ID = 1  # padding_idx of RoBERTa's and MPNet's position ids, fixed in the library (include/openmatch_b200.h)
 
-_ARCHS = {"bert": _lib.OM_ARCH_BERT, "t5": _lib.OM_ARCH_T5ENC, "roberta": _lib.OM_ARCH_ROBERTA}
+_ARCHS = {"bert": _lib.OM_ARCH_BERT, "t5": _lib.OM_ARCH_T5ENC, "roberta": _lib.OM_ARCH_ROBERTA,
+          "mpnet": _lib.OM_ARCH_MPNET, "distilbert": _lib.OM_ARCH_DISTILBERT}
+_BERT_LIKE = ("bert", "roberta", "mpnet", "distilbert")
+
+# MPNetEncoder.compute_position_bias buckets with num_buckets = 32 and max_distance = 128 whatever the config says
+MPNET_REL_BUCKETS, MPNET_REL_MAX_DISTANCE = 32, 128
 
 
 def spec_from_hf_config(config) -> Dict:
-    """Translate a HF ``BertConfig`` / ``RobertaConfig`` / ``XLMRobertaConfig`` / ``T5Config`` into the plain dict
-    ``CudaEncoder`` consumes."""
+    """Translate a HF ``BertConfig`` / ``RobertaConfig`` / ``XLMRobertaConfig`` / ``MPNetConfig`` /
+    ``DistilBertConfig`` / ``T5Config`` into the plain dict ``CudaEncoder`` consumes."""
     mt = getattr(config, "model_type", "")
     if mt in ("bert", "roberta", "xlm-roberta"):
         roberta = mt != "bert"
@@ -54,6 +59,29 @@ def spec_from_hf_config(config) -> Dict:
                     hidden=config.hidden_size, heads=config.num_attention_heads, ffn=config.intermediate_size,
                     vocab=config.vocab_size, max_pos=config.max_position_embeddings, type_vocab=config.type_vocab_size,
                     ln_eps=config.layer_norm_eps)
+    if mt == "mpnet":
+        if config.num_attention_heads <= 0 or config.hidden_size != 64 * config.num_attention_heads:
+            raise ValueError("CUDA encoder needs 64-wide MPNet attention heads, got hidden_size=%d / "
+                             "num_attention_heads=%d" % (config.hidden_size, config.num_attention_heads))
+        if getattr(config, "hidden_act", "gelu") != "gelu":
+            raise ValueError("CUDA encoder supports hidden_act='gelu' (erf) only, got %r" % config.hidden_act)
+        if config.relative_attention_num_buckets != MPNET_REL_BUCKETS:
+            raise ValueError("CUDA encoder needs MPNet relative_attention_num_buckets=%d (the buckets HF computes), got %r"
+                             % (MPNET_REL_BUCKETS, config.relative_attention_num_buckets))
+        if config.max_position_embeddings < 3:
+            raise ValueError("MPNet max_position_embeddings=%d leaves no position (positions start at 2)"
+                             % config.max_position_embeddings)
+        return dict(arch="mpnet", layers=config.num_hidden_layers, hidden=config.hidden_size,
+                    heads=config.num_attention_heads, ffn=config.intermediate_size, vocab=config.vocab_size,
+                    max_pos=config.max_position_embeddings, type_vocab=0, ln_eps=config.layer_norm_eps,
+                    rel_buckets=MPNET_REL_BUCKETS, rel_max_distance=MPNET_REL_MAX_DISTANCE)
+    if mt == "distilbert":
+        _check_bert_heads(config.dim, config.n_heads)
+        if getattr(config, "activation", "gelu") != "gelu":
+            raise ValueError("CUDA encoder supports activation='gelu' (erf) only, got %r" % config.activation)
+        return dict(arch="distilbert", layers=config.n_layers, hidden=config.dim, heads=config.n_heads,
+                    ffn=config.hidden_dim, vocab=config.vocab_size, max_pos=config.max_position_embeddings,
+                    type_vocab=0, ln_eps=1e-12)  # every DistilBERT LayerNorm has eps 1e-12 (modeling_distilbert.py)
     if mt == "t5":
         if config.d_kv != 64:
             raise ValueError("CUDA encoder supports d_kv == 64 only")
@@ -63,19 +91,23 @@ def spec_from_hf_config(config) -> Dict:
                     ffn=config.d_ff, vocab=config.vocab_size, max_pos=0, type_vocab=0,
                     ln_eps=config.layer_norm_epsilon, rel_buckets=config.relative_attention_num_buckets,
                     rel_max_distance=getattr(config, "relative_attention_max_distance", 128))
-    raise ValueError("CUDA encoder supports BERT, RoBERTa / XLM-RoBERTa and T5-encoder backbones, got model_type=%r" % mt)
+    raise ValueError("CUDA encoder supports BERT, RoBERTa / XLM-RoBERTa, MPNet, DistilBERT and T5-encoder backbones, "
+                     "got model_type=%r" % mt)
 
 
-MAX_SEQ_LEN = 8192     # longest sequence of a packed call for BERT / RoBERTa (include/openmatch_b200.h)
-MAX_T5_SEQ_LEN = 512   # T5: its relative-bias tables cover 512 tokens
+MAX_SEQ_LEN = 8192     # longest sequence of a packed call for BERT / RoBERTa / DistilBERT (include/openmatch_b200.h)
+MAX_T5_SEQ_LEN = 512   # T5 and MPNet: their relative-bias tables cover 512 tokens
 
 
 def max_seq_len(spec: Dict, max_batch_tokens: int = 256 * 128) -> int:
     """Longest sequence ``encode_packed`` / ``encode_pairs`` take for ``spec`` (a ``spec_from_hf_config`` dict) on a
-    handle of ``max_batch_tokens``: 8192 tokens and ``max_position_embeddings`` (BERT) / ``max_position_embeddings - 2``
-    (RoBERTa, whose positions start at 2); 512 tokens for T5; never more than ``max_batch_tokens``."""
+    handle of ``max_batch_tokens``: 8192 tokens and ``max_position_embeddings`` (BERT, DistilBERT) /
+    ``max_position_embeddings - 2`` (RoBERTa, whose positions start at 2); 512 tokens for T5, and for MPNet within
+    ``max_position_embeddings - 2``; never more than ``max_batch_tokens``."""
     if spec["arch"] == "t5":
         limit = MAX_T5_SEQ_LEN
+    elif spec["arch"] == "mpnet":
+        limit = min(MAX_T5_SEQ_LEN, spec["max_pos"] - 2)
     else:
         limit = min(MAX_SEQ_LEN, spec["max_pos"] - (2 if spec["arch"] == "roberta" else 0))
     return min(limit, int(max_batch_tokens))
@@ -88,7 +120,7 @@ class CudaEncoder:
             raise ValueError("Unknown pooling type: {}".format(pooling))
         if spec["arch"] not in _ARCHS:
             raise ValueError("Unknown encoder arch %r" % spec["arch"])
-        if spec["arch"] in ("bert", "roberta"):
+        if spec["arch"] in _BERT_LIKE:
             _check_bert_heads(spec["hidden"], spec["heads"])
         self._lib = _lib.load()
         head_head_out = int(head_weight.shape[0]) if head_weight is not None else 0

@@ -82,7 +82,8 @@ class RRModel(nn.Module):
     # ------------------------------------------------------------------ scoring
     def max_pair_len(self) -> int:
         """longest assembled pair the model takes (``encoder.max_seq_len``): 8192 tokens and max_position_embeddings for
-        BERT (minus RoBERTa's position offset of 2), 512 for T5, at most OPENMATCH_B200_MAX_BATCH_TOKENS"""
+        BERT / DistilBERT (minus RoBERTa's position offset of 2), 512 for T5 and MPNet, at most
+        OPENMATCH_B200_MAX_BATCH_TOKENS"""
         from ..encoder import max_seq_len, spec_from_hf_config
         max_tokens = int(os.environ.get("OPENMATCH_B200_MAX_BATCH_TOKENS", 256 * 128))
         return max_seq_len(spec_from_hf_config(self.lm.config), max_tokens)
