@@ -41,7 +41,7 @@ extern "C" {
 
 enum { OM_OK = 0, OM_EINVAL = -1, OM_ECUDA = -2, OM_ENOMEM = -3, OM_ENODEVICE = -4, OM_ESTATE = -5, OM_EFAULT = -6 };
 
-typedef enum { OM_F32 = 0, OM_BF16 = 1, OM_F16 = 2 } om_dtype;
+typedef enum { OM_F32 = 0, OM_BF16 = 1, OM_F16 = 2, OM_I8 = 3 } om_dtype;
 typedef enum { OM_HOST = 0, OM_DEVICE = 1 } om_memkind;
 /* OM_ARCH_ROBERTA: RoBERTa / XLM-RoBERTa / CamemBERT, BERT's encoder (same parameter names, optionally prefixed
  * "roberta.") whose position ids come from the token ids, as HF's create_position_ids_from_input_ids computes them with
@@ -124,7 +124,10 @@ int om_encoder_finalize(om_encoder* enc);
  * L <= max_position_embeddings (BERT, DistilBERT) / max_position_embeddings - 2 (RoBERTa, MPNet).
  * out_reps: device [B, rep_dim] fp32, bf16 or fp16 with row pitch out_row_stride (elements) — may point into an
  * index shard obtained from om_index_reserve() / om_index_reserve_rows().  fp16 output is the round-to-nearest-even
- * of the fp32 output of the same call (values beyond the half range become inf).  out_hidden: nullable device fp32 [B, L, hidden]
+ * of the fp32 output of the same call (values beyond the half range become inf).  OM_I8 output: rows of an int8 index
+ * (see om_index_create_typed), the fp32 output of the same call quantised by the index's rule: out_reps 4-byte aligned,
+ * out_row_stride (bytes) a multiple of 4 and at least dpad + 16 (dpad = rep_dim rounded up to 16); a row holding inf
+ * or NaN gets a NaN scale (om_index_commit counts it).  out_hidden: nullable device fp32 [B, L, hidden]
  * (last_hidden_state).  Asynchronous on `stream`. */
 int om_encode(om_encoder* enc, const int64_t* input_ids, const int64_t* attention_mask,
               const int64_t* token_type_ids, int B, int L, void* out_reps, om_dtype out_dtype,
@@ -173,18 +176,29 @@ int om_index_create(int d, om_index** out); /* faiss.IndexFlatIP(d); lives on th
  * ascending id — bitwise what an fp32 index of the fp16-rounded rows returns.  Input fp16 cannot hold is refused:
  * om_index_add of a NaN or of a value that rounds to +-inf in fp16 (|x| >= 65520) returns OM_EINVAL and adds nothing;
  * rows written in place and committed with such values make every search return OM_EINVAL until om_index_reset (stat
- * "nonfinite_rows").  OM_BF16 storage returns OM_EINVAL.  Every shard of a sharded search has the same storage. */
+ * "nonfinite_rows").
+ * OM_I8: one byte per element and a per-row fp32 scale, rows of dpad + 16 bytes (dpad = d rounded up to 16): the codes
+ * [0, d), zeros to dpad, the scale s at byte dpad, zeros to the end.  A row x (fp32; bf16 / fp16 converted exactly) is
+ * stored as s = amax / 127 (amax = max |x_j|, IEEE division) and c_j = clamp(rint(x_j / s), -127, 127) (IEEE division,
+ * half to even); a zero row gets s = 0 and codes 0; element j then holds fp32(s * c_j).  Search is exact with respect to
+ * those values, bitwise what an fp32 index of them returns (same summation order, ties by ascending id).  om_index_add of
+ * a row holding inf or NaN returns OM_EINVAL and adds nothing; rows written in place and committed with a non-finite
+ * scale make every search return OM_EINVAL until om_index_reset (stat "nonfinite_rows").  The scan runs on s8 tensor
+ * cores with a two-level int8 split of the query; "pair_scan" and "scan_cluster_*" do not apply.
+ * OM_BF16 storage returns OM_EINVAL.  Every shard of a sharded search has the same storage. */
 int om_index_create_typed(int d, om_dtype storage, om_index** out);
 int om_index_storage(const om_index* idx); /* the om_dtype given at creation */
 /* index.add(x): x [n, d] row-major, fp32, bf16 or fp16 (host or device).  Rows get ids ntotal .. ntotal+n-1.
- * fp16 storage: converted to fp16 with round-to-nearest-even; synchronises `stream`. */
+ * fp16 storage: converted to fp16 with round-to-nearest-even; int8 storage: quantised by the OM_I8 rule; both synchronise
+ * `stream`. */
 int om_index_add(om_index* idx, const void* x, om_memkind kind, om_dtype dtype, int64_t n, void* stream);
 /* Zero-copy ingest: reserve room for n more rows and get the device address of the fp32 row block
  * (row pitch = d floats) so the encoder can write embeddings in place; om_index_commit(n) publishes
  * them (builds the fp16 scan copy and updates the error-norm maxima the exactness certificate uses).  */
 int om_index_reserve(om_index* idx, int64_t n, float** dev_rows); /* fp32 storage only (OM_ESTATE otherwise) */
-/* Either storage: the device address of the next n rows, fp32 at pitch d or fp16 at pitch dpad (elements).  For fp16
- * rows om_index_commit updates the error-norm maxima and counts rows with a non-finite element. */
+/* Any storage: the device address of the next n rows, fp32 at pitch d, fp16 at pitch dpad (elements) or int8 rows at
+ * pitch dpad + 16 (bytes).  For fp16 / int8 rows om_index_commit updates the error-norm maxima and counts rows with a
+ * non-finite element (fp16) or scale (int8). */
 int om_index_reserve_rows(om_index* idx, int64_t n, void** dev_rows, int64_t* row_pitch_elems);
 int om_index_commit(om_index* idx, int64_t n, void* stream);
 int64_t om_index_ntotal(const om_index* idx);
@@ -234,7 +248,7 @@ int om_index_set_param(om_index* idx, const char* name, int64_t value);
 /* Statistics of the last search: "rounds", "overflow_retries", "candidates" (per query capacity),
  * "launches" (kernels launched), "uncertified" (queries the first level could not prove exact),
  * "uncertified_wide" (still unproven with 4096 candidates), "exact_queries" (answered by the exact fp32 scan),
- * "nonfinite_rows" (fp16 storage: committed rows holding inf or NaN, as the last search read it; 0 after a reset),
+ * "nonfinite_rows" (fp16 / int8 storage: committed rows holding inf or NaN, as the last search read it; 0 after a reset),
  * and with "profile" on: "scan_ns", "select_ns",
  * "finalize_ns", "other_ns" (device time summed over the launches of each kind; other = exchange + merge + certify). */
 int64_t om_index_get_stat(const om_index* idx, const char* name);
@@ -249,7 +263,7 @@ int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, in
                     int64_t* I, void* stream);
 
 /* ---- loss: replaces matmul + cross_entropy + autograd backward ------------------------------------ */
-/* Q [nq, d], P [np, d] device, fp32 or bf16 (both the same dtype), row-major.
+/* Q [nq, d], P [np, d] device, fp32 or bf16 (both the same dtype; any other returns OM_EINVAL), row-major.
  * target: nullable int64 [nq] device (NULL => i * (np / nq), loss.py:11-13).
  * loss_out: device fp32 scalar = loss_scale * reduce_i(logsumexp_j s_ij - s_i,target_i).
  * dQ [nq, d], dP [np, d]: nullable device fp32 gradients of loss_out.  scores_out: nullable device fp32

@@ -12,7 +12,7 @@ from ctypes import POINTER, c_char_p, c_float, c_int, c_int32, c_int64, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("OPENMATCH_B200_LIB") or os.path.join(_HERE, "lib", "libopenmatch_b200.so")
 
-OM_F32, OM_BF16, OM_F16 = 0, 1, 2
+OM_F32, OM_BF16, OM_F16, OM_I8 = 0, 1, 2, 3
 OM_HOST, OM_DEVICE = 0, 1
 OM_ARCH_BERT, OM_ARCH_T5ENC, OM_ARCH_ROBERTA, OM_ARCH_MPNET, OM_ARCH_DISTILBERT = 0, 1, 2, 3, 4
 OM_POOL_FIRST, OM_POOL_MEAN = 0, 1

@@ -166,5 +166,6 @@ class InferenceArguments(RuntimeArguments):
     reranking_depth: int = field(default=None, metadata={"help": "driver.rerank: documents per query of the run to "
                                                                    "re-rank (default: all)"})
     index_dtype: str = field(default="float32", metadata={
-        "help": "row storage of the search index: 'float32' (fp32 rows + fp16 scan copy, 6 bytes per element) or "
-                "'float16' (fp16 rows only, 2 bytes per element; search is exact over the fp16-rounded rows)"})
+        "help": "row storage of the search index: 'float32' (fp32 rows + fp16 scan copy, 6 bytes per element), "
+                "'float16' (fp16 rows only, 2 bytes per element; search is exact over the fp16-rounded rows) or 'int8' "
+                "(one byte per element + a per-row scale; search is exact over the dequantised rows)"})

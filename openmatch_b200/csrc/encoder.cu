@@ -33,6 +33,7 @@
 
 #include "common.h"
 #include "gemm.cuh"
+#include "quant_i8.cuh"
 
 namespace om {
 
@@ -1250,6 +1251,22 @@ __global__ void finish_reps_kernel(const float* in, int B, int D, int normalize,
   for (int i = lane; i < D; i += 32) out[static_cast<int64_t>(b) * pitch + i] = static_cast<OutT>(src[i] * scale);
 }
 
+// OM_I8 output: the values finish_reps_kernel<float> stores, quantised into int8 index rows (quant_i8.cuh), one warp per row
+__global__ void finish_reps_i8_kernel(const float* in, int B, int D, int normalize, int8_t* out, int64_t pitch) {
+  const int b = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (b >= B) return;
+  const float* src = in + static_cast<int64_t>(b) * D;
+  float scale = 1.f;
+  if (normalize) {
+    float q = 0.f;
+    for (int i = lane; i < D; i += 32) q = fmaf(src[i], src[i], q);
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) q += __shfl_xor_sync(0xffffffffu, q, s);
+    scale = 1.0f / fmaxf(sqrtf(q), 1e-12f);
+  }
+  quantize_row_i8([&](int i) { return __fmul_rn(src[i], scale); }, D, i8_dpad(D), out + static_cast<int64_t>(b) * pitch, lane);
+}
+
 __global__ void f32_to_bf16_kernel(const float* src, __nv_bfloat16* dst, int64_t n) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<int64_t>(gridDim.x) * blockDim.x)
@@ -1541,9 +1558,13 @@ int embed_rows(om_encoder* e, const int64_t* ids, const int64_t* tts, int T, int
 int check_out(const om_encoder* e, const char* who, const void* out_reps, om_dtype out_dtype, int64_t out_row_stride) {
   if (!out_reps) return fail(OM_EINVAL, "%s: null argument", who);
   if (!e->finalized) return fail(OM_ESTATE, "%s: call om_encoder_finalize first", who);
-  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16)
-    return fail(OM_EINVAL, "%s: out dtype must be f32, bf16 or f16", who);
+  if (out_dtype != OM_F32 && out_dtype != OM_BF16 && out_dtype != OM_F16 && out_dtype != OM_I8)
+    return fail(OM_EINVAL, "%s: out dtype must be f32, bf16, f16 or i8", who);
   if (out_row_stride < om_encoder_rep_dim(e)) return fail(OM_EINVAL, "%s: out_row_stride < rep_dim", who);
+  if (out_dtype == OM_I8 && (out_row_stride < i8_dpad(om_encoder_rep_dim(e)) + 16 || out_row_stride % 4 != 0 ||
+                             reinterpret_cast<uintptr_t>(out_reps) % 4 != 0))
+    return fail(OM_EINVAL, "%s: int8 rows need a 4-byte aligned out_reps and an out_row_stride that is a multiple of 4 and "
+                "at least %d bytes (rep_dim rounded up to 16, + 16 for the scale)", who, i8_dpad(om_encoder_rep_dim(e)) + 16);
   return 0;
 }
 
@@ -1567,6 +1588,9 @@ int finish_reps(om_encoder* e, int B, void* out_reps, om_dtype out_dtype, int64_
   if (out_dtype == OM_F32)
     finish_reps_kernel<float><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<float*>(out_reps),
                                                           out_row_stride);
+  else if (out_dtype == OM_I8)
+    finish_reps_i8_kernel<<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize, static_cast<int8_t*>(out_reps),
+                                                       out_row_stride);
   else if (out_dtype == OM_BF16)
     finish_reps_kernel<__nv_bfloat16><<<(B + 3) / 4, 128, 0, st>>>(reps, B, rep_dim, d.normalize,
                                                                   static_cast<__nv_bfloat16*>(out_reps), out_row_stride);
@@ -2063,7 +2087,7 @@ int om_encode_packed(om_encoder* e, const int64_t* tokens, const int64_t* token_
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t out_elem = out_dtype == OM_F32 ? 4 : 2;
+  const size_t out_elem = out_dtype == OM_F32 ? 4 : out_dtype == OM_I8 ? 1 : 2;
 
   NvtxRange nvtx("om.encode_packed");
   std::vector<PackedSeq> seqs;
@@ -2125,7 +2149,7 @@ int om_encode_pairs(om_encoder* e, const int32_t* a_tokens, int64_t a_total, con
     }
   }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const size_t out_elem = out_dtype == OM_F32 ? 4 : 2;
+  const size_t out_elem = out_dtype == OM_F32 ? 4 : out_dtype == OM_I8 ? 1 : 2;
 
   NvtxRange nvtx("om.encode_pairs");
   PairChunk pc;

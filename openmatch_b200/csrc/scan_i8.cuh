@@ -1,0 +1,285 @@
+// Search scan of an int8 index (quant_i8.cuh row layout): s8 x s8 wgmma with exact int32 accumulation, the top-k filter
+// applied to the combined fp32 score on the accumulator registers.  One kernel serves every round of an int8 index: the
+// dense first round (every score stored) and the threshold rounds, for any number of queries.  The fp16 scan kernels
+// (gemm.cuh, scan_gemm.cuh) and their options (pair_scan, scan_cluster_*) do not apply to int8 indices.
+//
+//   query      q ~ q_h = sig_hi * q_hi + sig_lo * q_lo: two int8 vectors, sig_hi = amax / 127, sig_lo = sig_hi / 254, so
+//              q_h carries ~15 bits and the certificate's query term ||q - q_h|| * max ||x^|| stays far below the rank gaps
+//   operands   per k block of 128 codes (one 128-byte SW128 row, the fp16 boxes' swizzle and descriptors; a k32 step
+//              advances 32 B): the tile's 128 query rows of q_hi and of q_lo and 128 corpus rows, 48 KB per ring slot
+//   tile       one CTA: 128 queries x 128 corpus rows; consumer warpgroup g owns queries [64 g, +64) and holds two
+//              m64n128 int32 accumulator sets A_hi, A_lo (128 registers, the fp16 wide scan's m64n256 budget).  Products
+//              and sums are exact: 127^2 * 16384 < 2^31
+//   score      fp32(s_r * fp32(sig_hi * A_hi + fp32(sig_lo * A_lo))), s_r the row's scale: a few roundings of 2^-24 that
+//              certify_kernel's bound covers (csrc/search.cu)
+//   schedule   persistent, static, queries fastest: every CTA works on neighbouring corpus tiles
+//   filter     as in scan_wide_kernel: a thread owns two query rows (fragment rows l/4, l/4 + 8) x 32 columns; one
+//              32-value max per row against the query's strict threshold, survivors through a bit mask into a
+//              double-buffered stash, one atomicAdd per quad and row whose result is consumed one tile later.  DENSE: every
+//              score stored at position = column
+#pragma once
+#include <stdint.h>
+
+#include "scan_epilogue.cuh"
+
+namespace om {
+
+constexpr int kI8BlockK = 128;                        // codes per k block
+constexpr int kI8BlockN = 128;                        // corpus rows per tile
+constexpr int kI8Stages = 4;
+constexpr int kI8BoxBytes = kBlockM * kI8BlockK;      // 16 KB: 128 rows of one operand
+constexpr int kI8StageBytes = 3 * kI8BoxBytes;        // q_hi, q_lo, corpus
+constexpr int kI8Consumers = 256;                     // two consumer warpgroups
+constexpr int kI8Stash = 4;                           // survivors a thread parks per row and tile
+constexpr int kI8StashOffset = kI8Stages * kI8StageBytes;
+constexpr int kI8StashBytes = 2 * 2 * kI8Stash * kI8Consumers * 8;  // [buffer][row half][slot][thread] keys
+constexpr int kI8BarOffset = kI8StashOffset + kI8StashBytes;
+constexpr int kI8SmemBytes = kI8BarOffset + 2 * kI8Stages * 8 + 1024;  // + slack for 1024-B alignment of the base
+static_assert(kI8SmemBytes <= 232448, "int8 scan ring + stash exceed the 227 KB of shared memory an H100 block may use");
+
+// Filter of one fragment row (v[i] = column 8 (i >> 1) + 2 q4 + (i & 1) of the tile): returns the number of survivors
+// parked in the stash (<= kI8Stash).  stash: this thread's slot 0 of (buffer, row); slot j is at stash[j * kI8Consumers].
+__device__ __forceinline__ int scan_i8_filter_row(const float (&v)[32], float t, int row, int lim, int q4, int col0,
+                                                  unsigned long long* stash, unsigned long long* cand, int* count,
+                                                  int* overflow, int C, uint32_t row_base) {
+  float mx = v[0];
+#pragma unroll
+  for (int i = 1; i < 32; ++i) mx = fmaxf(mx, v[i]);
+  if (!(mx > t)) return 0;  // common case
+  uint32_t mask = 0;
+#pragma unroll
+  for (int i = 0; i < 32; ++i) mask |= (v[i] > t ? 1u : 0u) << i;
+  if (lim < kI8BlockN) {  // last corpus tile: columns >= lim score 0 (zero scale), which can beat a negative threshold
+#pragma unroll 1
+    for (int i = 0; i < 32; ++i)
+      if (8 * (i >> 1) + 2 * q4 + (i & 1) >= lim) mask &= ~(1u << i);
+  }
+  const int n = __popc(mask);
+  int pos = 0;
+  if (n > kI8Stash) {  // more than the stash holds: reserve the excess synchronously
+    pos = atomicAdd(count + row, n - kI8Stash);
+    if (pos + (n - kI8Stash) > C) *overflow = 1;
+  }
+  unsigned long long* mine = cand + static_cast<size_t>(row) * C;
+  int idx = 0;
+#pragma unroll 1
+  while (mask) {
+    const int i = __ffs(mask) - 1;
+    mask &= mask - 1;
+    const unsigned long long key =
+        make_key(EpiScan<false>::pick32(v, i), row_base + static_cast<uint32_t>(col0 + 8 * (i >> 1) + 2 * q4 + (i & 1)));
+    if (idx < kI8Stash)
+      stash[idx * kI8Consumers] = key;
+    else if (pos + idx - kI8Stash < C)
+      mine[pos + idx - kI8Stash] = key;
+    ++idx;
+  }
+  return n < kI8Stash ? n : kI8Stash;
+}
+
+template <bool DENSE>
+__global__ void __launch_bounds__(kGemmProducerThreads + kI8Consumers, 1)
+scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
+               const __grid_constant__ CUtensorMap tmX, int K, const int8_t* __restrict__ xrows, int64_t pitch, int dpad,
+               const float2* __restrict__ qsig, const float* __restrict__ thr, unsigned long long* cand, int* count,
+               int* overflow, int nq, int n_cols, int C, uint32_t row_base) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  unsigned long long* stash = reinterpret_cast<unsigned long long*>(smem + kI8StashOffset);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kI8BarOffset);
+  uint64_t* empty_bar = full_bar + kI8Stages;
+  const int warp = __shfl_sync(0xffffffffu, static_cast<int>(threadIdx.x >> 5), 0);
+  const int lane = static_cast<int>(threadIdx.x & 31);
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmQh);
+    tma_prefetch_desc(&tmQl);
+    tma_prefetch_desc(&tmX);
+  }
+  if (warp == 1 && lane == 0) {
+    ring_init(full_bar, empty_bar, kI8Stages, kI8Consumers / 32);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  const int qgroups = (nq + kBlockM - 1) / kBlockM;
+  const int num_tiles = qgroups * ((n_cols + kI8BlockN - 1) / kI8BlockN);
+  const int num_k = (K + kI8BlockK - 1) / kI8BlockK;
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ------------------------------ TMA producer ------------------------------
+      Ring<kI8Stages> ring;
+      for (int tile = static_cast<int>(blockIdx.x); tile < num_tiles; tile += static_cast<int>(gridDim.x)) {
+        const int m_blk = tile % qgroups, n_blk = tile / qgroups;
+        for (int kb = 0; kb < num_k; ++kb) {
+          uint64_t* bar = ring_acquire_tx(full_bar, empty_bar, ring, kI8StageBytes, 40);
+          uint8_t* s = smem + ring.stage * kI8StageBytes;
+          tma_load_2d(s, &tmQh, bar, kb * kI8BlockK, m_blk * kBlockM);
+          tma_load_2d(s + kI8BoxBytes, &tmQl, bar, kb * kI8BlockK, m_blk * kBlockM);
+          tma_load_2d(s + 2 * kI8BoxBytes, &tmX, bar, kb * kI8BlockK, n_blk * kI8BlockN);
+          ring.advance();
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ------------------------------ consumers: wgmma + filter ------------------------------
+    const int et = static_cast<int>(threadIdx.x) - kGemmProducerThreads;  // 0 .. 255
+    const int wg = et >> 7;                                               // queries [64 wg, +64) of the tile's 128
+    const int q4 = lane & 3;
+    const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
+    Ring<kI8Stages> ring;
+    int buf = 0;
+    // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
+    int p_n0 = 0, p_n1 = 0, p_excl0 = 0, p_excl1 = 0, p_pos0 = 0, p_pos1 = 0, p_row = 0, p_buf = 0;
+    auto drain = [&]() {
+      if (!__any_sync(0xffffffffu, (p_n0 | p_n1) != 0)) return;
+      const int b0 = __shfl_sync(0xffffffffu, p_pos0, lane & ~3) + p_excl0;
+      const int b1 = __shfl_sync(0xffffffffu, p_pos1, lane & ~3) + p_excl1;
+      const unsigned long long* s = stash + p_buf * (2 * kI8Stash * kI8Consumers) + et;
+      unsigned long long* m0 = cand + static_cast<size_t>(p_row) * C;
+      unsigned long long* m1 = cand + static_cast<size_t>(p_row + 8) * C;
+      for (int j = 0; j < p_n0; ++j)
+        if (b0 + j < C) m0[b0 + j] = s[j * kI8Consumers];
+      for (int j = 0; j < p_n1; ++j)
+        if (b1 + j < C) m1[b1 + j] = s[(kI8Stash + j) * kI8Consumers];
+      if ((p_n0 > 0 && b0 + p_n0 > C) || (p_n1 > 0 && b1 + p_n1 > C)) *overflow = 1;
+      p_n0 = p_n1 = 0;
+    };
+    auto release = [&](uint32_t s) {
+      if (lane == 0) mbar_arrive(&empty_bar[s]);
+    };
+
+    for (int tile = static_cast<int>(blockIdx.x); tile < num_tiles; tile += static_cast<int>(gridDim.x)) {
+      const int m_blk = tile % qgroups, n_blk = tile / qgroups;
+      const int row0 = m_blk * kBlockM + frow, row1 = row0 + 8;
+      const int col0 = n_blk * kI8BlockN;
+      // issued before the mainloop, first read after it: the loads' latency hides behind the MMAs
+      const float inf = __int_as_float(0x7f800000);
+      const float2 g0 = row0 < nq ? qsig[row0] : make_float2(0.f, 0.f), g1 = row1 < nq ? qsig[row1] : make_float2(0.f, 0.f);
+      float t0 = inf, t1 = inf;
+      if constexpr (!DENSE) {
+        t0 = row0 < nq ? thr[row0] : inf;
+        t1 = row1 < nq ? thr[row1] : inf;
+      }
+      float sc[32];  // scales of this thread's columns col0 + 8 (i >> 1) + 2 q4 + (i & 1)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) {
+        const int c = col0 + 8 * (i >> 1) + 2 * q4 + (i & 1);
+        sc[i] = c < n_cols ? __ldg(reinterpret_cast<const float*>(xrows + static_cast<size_t>(c) * pitch + dpad)) : 0.f;
+      }
+
+      int32_t ah[64], al[64];
+#pragma unroll
+      for (int i = 0; i < 64; ++i) ah[i] = al[i] = 0;
+      ring_consume(
+          full_bar, ring, 0, num_k, 41,
+          [&](uint32_t stage, uint32_t accumulate) {
+            const uint32_t qh = smem_u32(smem + stage * kI8StageBytes) + wg * (64 * kI8BlockK);
+            const uint32_t ql = qh + kI8BoxBytes;
+            const uint32_t xb = smem_u32(smem + stage * kI8StageBytes + 2 * kI8BoxBytes);
+#pragma unroll
+            for (int k = 0; k < kI8BlockK / 32; ++k) {
+              const uint64_t db = wgmma_desc(xb + k * 32, kDescKMajorSW128);
+              const uint32_t acc = (accumulate | k) != 0 ? 1u : 0u;
+              wgmma_m64n128k32_s8(ah, wgmma_desc(qh + k * 32, kDescKMajorSW128), db, acc);
+              wgmma_m64n128k32_s8(al, wgmma_desc(ql + k * 32, kDescKMajorSW128), db, acc);
+            }
+          },
+          release);
+      wgmma_fence_regs(ah);
+      wgmma_fence_regs(al);
+
+      // combined scores of fragment rows frow (v0) and frow + 8 (v1): v_H[2 j + b] = accumulator [4 j + 2 H + b]
+      float v0[32], v1[32];
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int b = 0; b < 2; ++b) {
+          const int i = 2 * j + b;
+          v0[i] = __fmul_rn(sc[i], __fmaf_rn(g0.x, static_cast<float>(ah[4 * j + b]), __fmul_rn(g0.y, static_cast<float>(al[4 * j + b]))));
+          v1[i] = __fmul_rn(sc[i], __fmaf_rn(g1.x, static_cast<float>(ah[4 * j + 2 + b]), __fmul_rn(g1.y, static_cast<float>(al[4 * j + 2 + b]))));
+        }
+
+      if constexpr (DENSE) {  // first round: every score at position = column
+#pragma unroll 1
+        for (int h = 0; h < 2; ++h) {
+          const int row = h ? row1 : row0;
+          if (row >= nq) continue;
+          unsigned long long* mine = cand + static_cast<size_t>(row) * C;
+#pragma unroll
+          for (int i = 0; i < 32; ++i) {
+            const int c = col0 + 8 * (i >> 1) + 2 * q4 + (i & 1);
+            if (c < n_cols) mine[c] = make_key(h ? v1[i] : v0[i], row_base + static_cast<uint32_t>(c));
+          }
+        }
+        continue;
+      }
+
+      // ------------------------------ filter on the fragments ------------------------------
+      drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
+      const int lim = n_cols - col0;
+      unsigned long long* sb = stash + buf * (2 * kI8Stash * kI8Consumers) + et;
+      const int k0 = scan_i8_filter_row(v0, t0, row0, lim, q4, col0, sb, cand, count, overflow, C, row_base);
+      const int k1 = scan_i8_filter_row(v1, t1, row1, lim, q4, col0, sb + kI8Stash * kI8Consumers, cand, count, overflow,
+                                        C, row_base);
+      if (__any_sync(0xffffffffu, (k0 | k1) != 0)) {
+        // quad aggregation: lanes 4 i .. 4 i + 3 share both rows; exclusive prefix per lane, one atomic per quad and row
+        int x0 = k0, x1 = k1;
+        int y0 = __shfl_up_sync(0xffffffffu, x0, 1, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 1, 4);
+        if (q4 >= 1) x0 += y0, x1 += y1;
+        y0 = __shfl_up_sync(0xffffffffu, x0, 2, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 2, 4);
+        if (q4 >= 2) x0 += y0, x1 += y1;
+        const int n0 = __shfl_sync(0xffffffffu, x0, lane | 3), n1 = __shfl_sync(0xffffffffu, x1, lane | 3);
+        if (q4 == 0) {
+          if (n0 > 0) p_pos0 = atomicAdd(count + row0, n0);  // result first used by the next drain()
+          if (n1 > 0) p_pos1 = atomicAdd(count + row1, n1);
+        }
+        p_n0 = k0;
+        p_n1 = k1;
+        p_excl0 = x0 - k0;
+        p_excl1 = x1 - k1;
+        p_row = row0;
+        p_buf = buf;
+        buf ^= 1;
+      }
+    }
+    drain();
+  }
+
+  __syncthreads();
+}
+
+// Host launcher.  Qh, Ql: [nq, K] int8 query splits, row pitch ldq bytes; qsig [nq] (sig_hi, sig_lo); X: the corpus rows of
+// the round, [n_cols] rows of pitch `pitch` bytes with the scale at byte dpad.  DENSE: every score goes to
+// cand[q * C + column]; otherwise survivors (score > thr[q]) are appended as make_key(score, row_base + column) and a
+// list that would grow beyond C sets *overflow.  Returns cudaSuccess / a CUDA error (tensor-map failures:
+// cudaErrorInvalidValue).
+template <bool DENSE>
+static inline cudaError_t launch_scan_i8(const int8_t* Qh, const int8_t* Ql, int64_t ldq, const float2* qsig,
+                                         const int8_t* X, int64_t pitch, int dpad, int nq, int n_cols, int K,
+                                         const float* thr, unsigned long long* cand, int* count, int* overflow, int C,
+                                         uint32_t row_base, int num_sms, cudaStream_t stream) {
+  if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
+  CUtensorMap tmQh, tmQl, tmX;
+  if (make_tmap_2d(&tmQh, Qh, 1, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq, kI8BlockK, kBlockM, 128) != 0 ||
+      make_tmap_2d(&tmQl, Ql, 1, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq, kI8BlockK, kBlockM, 128) != 0 ||
+      make_tmap_2d(&tmX, X, 1, (uint64_t)K, (uint64_t)n_cols, (uint64_t)pitch, kI8BlockK, kI8BlockN, 128) != 0)
+    return cudaErrorInvalidValue;
+  static bool attr_set = false;  // per instantiation
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(scan_i8_kernel<DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kI8SmemBytes);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  const int64_t num_tiles =
+      static_cast<int64_t>((nq + kBlockM - 1) / kBlockM) * ((n_cols + kI8BlockN - 1) / kI8BlockN);
+  const int grid = static_cast<int>(num_tiles < num_sms ? num_tiles : num_sms);
+  scan_i8_kernel<DENSE><<<grid, kGemmProducerThreads + kI8Consumers, kI8SmemBytes, stream>>>(
+      tmQh, tmQl, tmX, K, X, pitch, dpad, qsig, thr, cand, count, overflow, nq, n_cols, C, row_base);
+  return cudaGetLastError();
+}
+
+}  // namespace om

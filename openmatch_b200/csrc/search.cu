@@ -10,6 +10,9 @@
 // operand and the row store at once, FINAL and the exact scan read them, and every "fp32 score" below is the fp32
 // inner product of the fp32 query with the STORED fp16 row (same summation order).  The corpus error term of the
 // certificate is then exactly 0.
+// An index created with int8 storage keeps rows of int8 codes and a per-row fp32 scale (quant_i8.cuh); every round scans
+// on scan_i8.cuh (s8 tensor cores, a two-level int8 split of the query), and FINAL, the exact scan and the certificate
+// treat fp32(s * c) as the stored row, with a corpus term of 0 as for fp16.
 //
 // search(q, k):
 //   1. SCAN    fp16 Q * X^T on wgmma with the top-k filter fused into the epilogue (query batches: scan_gemm.cuh, 2-CTA
@@ -44,8 +47,10 @@
 #include "common.h"
 #include "gemm.cuh"
 #include "nccl_dyn.h"
+#include "quant_i8.cuh"
 #include "scan_epilogue.cuh"
 #include "scan_gemm.cuh"
+#include "scan_i8.cuh"
 
 namespace om {
 
@@ -211,14 +216,46 @@ __device__ __forceinline__ float4 quad_f32(uint2 u) {
 }
 __device__ __forceinline__ float elem_f32(float v) { return v; }
 __device__ __forceinline__ float elem_f32(__half v) { return __half2float(v); }
-// row pitch in elements: fp32 master rows [n, d], fp16 rows [n, dpad] with dpad = d rounded up to 8 (om_index_create)
+// row pitch in elements: fp32 master rows [n, d], fp16 rows [n, dpad] with dpad = d rounded up to 8 (om_index_create),
+// int8 rows of i8_dpad(d) + 16 bytes (quant_i8.cuh)
 template <typename RowT>
 __device__ __forceinline__ int row_pitch(int d) { return sizeof(RowT) == 4 ? d : (d + 7) & ~7; }
-// the 4-element groups of row r (d % 4 == 0)
+template <>
+__device__ __forceinline__ int row_pitch<int8_t>(int d) { return i8_dpad(d) + 16; }
+// the 4-element groups of row r (d % 4 == 0), read with load_quad(group pointer, i)
 template <typename RowT>
 __device__ __forceinline__ const typename RowQuad<RowT>::T* row_quads(const RowT* xs, size_t r, int d) {
   return reinterpret_cast<const typename RowQuad<RowT>::T*>(xs) + r * (row_pitch<RowT>(d) >> 2);
 }
+// the elements of row r, read with load_elem(element pointer, i)
+template <typename RowT>
+__device__ __forceinline__ const RowT* row_elems(const RowT* xs, size_t r, int d) {
+  return xs + r * row_pitch<RowT>(d);
+}
+template <typename QuadT>
+__device__ __forceinline__ float4 load_quad(const QuadT* x4, int i) { return quad_f32(__ldg(x4 + i)); }
+template <typename RowT>
+__device__ __forceinline__ float load_elem(const RowT* x, int i) { return elem_f32(__ldg(x + i)); }
+// int8 rows: 4 codes per group, and the row's scale; element j reads as fp32(s * c_j), so a row stored in int8 scores bit
+// for bit like the same values held as fp32
+struct I8Row {
+  const int8_t* p;
+  float s;
+};
+__device__ __forceinline__ I8Row i8_row(const int8_t* xs, size_t r, int d) {
+  const int8_t* p = xs + r * row_pitch<int8_t>(d);
+  return {p, __ldg(reinterpret_cast<const float*>(p + i8_dpad(d)))};
+}
+__device__ __forceinline__ I8Row row_quads(const int8_t* xs, size_t r, int d) { return i8_row(xs, r, d); }
+__device__ __forceinline__ I8Row row_elems(const int8_t* xs, size_t r, int d) { return i8_row(xs, r, d); }
+__device__ __forceinline__ float4 load_quad(I8Row x, int i) {
+  const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(x.p) + i);
+  return make_float4(__fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u))),
+                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 8))),
+                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 16))),
+                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 24))));
+}
+__device__ __forceinline__ float load_elem(I8Row x, int i) { return __fmul_rn(x.s, static_cast<float>(__ldg(x.p + i))); }
 
 // FINAL: one CTA per query: exact fp32 re-score of the candidates against the stored rows (fp32 master rows or fp16
 // rows), sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row
@@ -244,18 +281,18 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
     const uint32_t row = key_row(mine[j]);
     float acc = 0.f;
     if ((d & 3) == 0) {
-      const auto* x4 = row_quads(xs, row, d);
+      const auto x4 = row_quads(xs, row, d);
       const float4* q4 = reinterpret_cast<const float4*>(sq);
       for (int i = lane; i < (d >> 2); i += 32) {
-        const float4 a = quad_f32(__ldg(x4 + i)), b = q4[i];
+        const float4 a = load_quad(x4, i), b = q4[i];
         acc = fmaf(a.x, b.x, acc);
         acc = fmaf(a.y, b.y, acc);
         acc = fmaf(a.z, b.z, acc);
         acc = fmaf(a.w, b.w, acc);
       }
     } else {
-      const RowT* x = xs + static_cast<size_t>(row) * row_pitch<RowT>(d);
-      for (int i = lane; i < d; i += 32) acc = fmaf(elem_f32(__ldg(x + i)), sq[i], acc);
+      const auto x = row_elems(xs, row, d);
+      for (int i = lane; i < d; i += 32) acc = fmaf(load_elem(x, i), sq[i], acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -367,6 +404,103 @@ __global__ void __launch_bounds__(256) commit_f16_rows_kernel(const __half* __re
   if (lane == 0) {
     atomicMax(reinterpret_cast<int*>(gstats), __float_as_int(mx != mx ? __int_as_float(0x7fc00000) : mx));
     if (nbad) atomicAdd(nonfinite, nbad);
+  }
+}
+
+// int8 storage, add: src [n, d] (fp32 / bf16 / fp16, converted exactly to fp32) -> rows of quant_i8.cuh, one warp per row.
+// Rows holding inf or NaN are counted in *bad: the caller then refuses the whole add.
+template <typename T>
+__global__ void __launch_bounds__(256) quantize_rows_i8_kernel(const T* __restrict__ src, int64_t n, int d, int8_t* __restrict__ dst,
+                                                               int64_t pitch, int* bad) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
+  int nb = 0;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
+    const T* x = src + r * d;
+    const bool finite = quantize_row_i8([&](int j) { return static_cast<float>(x[j]); }, d, i8_dpad(d), dst + r * pitch, lane);
+    nb += finite ? 0 : 1;
+  }
+  if (lane == 0 && nb) atomicAdd(bad, nb);
+}
+
+// int8 storage, commit: the stored rows are read in place.  Running maximum of ||x^|| over the rows, x^_j = fp32(s c_j)
+// (gstats[0], summed in the order of rows_to_f16_kernel, so an fp32 index of the same values gets the same bits);
+// gstats[1] stays 0 (the stored values are the rows).  Rows with a non-finite scale are counted in *nonfinite: searches
+// refuse the index until a reset.
+__global__ void __launch_bounds__(256) commit_i8_rows_kernel(const int8_t* __restrict__ x, int64_t n, int d, float* gstats,
+                                                             int* nonfinite) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
+  float mx = 0.f;
+  int nbad = 0;
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
+    const I8Row row = i8_row(x, r, d);
+    float sx = 0.f;
+    for (int c = 2 * lane; c < d; c += 64) {
+      const float a = __fmul_rn(row.s, static_cast<float>(row.p[c]));
+      const float b = c + 1 < d ? __fmul_rn(row.s, static_cast<float>(row.p[c + 1])) : 0.f;
+      sx = fmaf(a, a, fmaf(b, b, sx));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, o);
+    const float nx = sqrtf(sx);
+    mx = (nx > mx || nx != nx) ? nx : mx;
+    if (lane == 0 && !isfinite(row.s)) ++nbad;
+  }
+  if (lane == 0) {
+    atomicMax(reinterpret_cast<int*>(gstats), __float_as_int(mx != mx ? __int_as_float(0x7fc00000) : mx));
+    if (nbad) atomicAdd(nonfinite, nbad);
+  }
+}
+
+// Queries of an int8 index: fp32 [nq, d] -> the two-level split q ~ q_h = sig_hi q_hi + sig_lo q_lo of scan_i8.cuh
+// (sig_hi = amax / 127, sig_lo = sig_hi / 254, codes rounded half to even after an IEEE division; pad columns zero), one
+// warp per query.  Certificate inputs: hn = ||sig_hi q_hi|| + ||sig_lo q_lo|| (>= ||q_h||, bounds the magnitude of the
+// scan's two products) and en = ||q - q_h|| (each element's residual with two FMAs: both are exact up to one rounding of
+// a value far below the residual).  A non-finite query gets en = NaN: its certificate fails and the exact scan answers.
+__global__ void __launch_bounds__(256) queries_to_i8_kernel(const float* __restrict__ qf, int64_t nq, int d, int dpad,
+                                                            int8_t* __restrict__ qhi, int8_t* __restrict__ qlo,
+                                                            float2* __restrict__ sig, float* __restrict__ hn,
+                                                            float* __restrict__ en) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
+  for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < nq; r += nwarps) {
+    const float* x = qf + r * d;
+    float amax = 0.f;
+    bool finite = true;
+    for (int j = lane; j < d; j += 32) {
+      finite = finite && isfinite(x[j]);
+      amax = fmaxf(amax, fabsf(x[j]));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+    finite = __all_sync(0xffffffffu, finite);
+    const float sh = __fdiv_rn(amax, 127.f), sl = __fdiv_rn(sh, 254.f);
+    float nh = 0.f, nl = 0.f, ne = 0.f;
+    for (int j = lane; j < dpad; j += 32) {
+      const float v = j < d ? x[j] : 0.f;
+      const float ch = sh > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(v, sh)), -127.f), 127.f) : 0.f;
+      const float res = __fmaf_rn(-sh, ch, v);
+      const float cl = sl > 0.f ? fminf(fmaxf(rintf(__fdiv_rn(res, sl)), -127.f), 127.f) : 0.f;
+      const float e = __fmaf_rn(-sl, cl, res);
+      qhi[r * dpad + j] = static_cast<int8_t>(ch);
+      qlo[r * dpad + j] = static_cast<int8_t>(cl);
+      const float ph = sh * ch, pl = sl * cl;
+      nh = fmaf(ph, ph, nh);
+      nl = fmaf(pl, pl, nl);
+      ne = fmaf(e, e, ne);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      nh += __shfl_xor_sync(0xffffffffu, nh, o);
+      nl += __shfl_xor_sync(0xffffffffu, nl, o);
+      ne += __shfl_xor_sync(0xffffffffu, ne, o);
+    }
+    if (lane == 0) {
+      sig[r] = make_float2(sh, sl);
+      hn[r] = sqrtf(nh) + sqrtf(nl);
+      en[r] = finite ? sqrtf(ne) : __int_as_float(0x7fc00000);
+    }
   }
 }
 
@@ -504,7 +638,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
   const int nact = min(nqt, nq - q0);
   for (int i = threadIdx.x; i < nact * d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q0) * d + i];
   __syncthreads();
-  const int lane = threadIdx.x & 31, pitch = row_pitch<RowT>(d);
+  const int lane = threadIdx.x & 31;
   float t = __int_as_float(0x7f800000);
   if (lane < nact && !dense) t = thr[q0 + lane];
   const int64_t wg = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5), nw = static_cast<int64_t>(gridDim.x) * 8;
@@ -520,7 +654,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
         float4 a[ROWS];
 #pragma unroll
         for (int rr = 0; rr < ROWS; ++rr)
-          a[rr] = r0 + rr < n_rows ? quad_f32(__ldg(row_quads(xs, r0 + rr, d) + i)) : make_float4(0.f, 0.f, 0.f, 0.f);
+          a[rr] = r0 + rr < n_rows ? load_quad(row_quads(xs, r0 + rr, d), i) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int j = 0; j < NQT; ++j) {
           if (j < nact) {
@@ -541,7 +675,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
       for (int i = lane; i < d; i += 32) {
         float a[ROWS];
 #pragma unroll
-        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? elem_f32(__ldg(xs + static_cast<size_t>(r0 + rr) * pitch + i)) : 0.f;
+        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? load_elem(row_elems(xs, r0 + rr, d), i) : 0.f;
 #pragma unroll
         for (int j = 0; j < NQT; ++j)
           if (j < nact) {
@@ -649,8 +783,9 @@ struct DevBuf {  // grow-only device scratch
 struct Level {
   int nq = 0, k = 0, kp = 0, kp_target = 0, C = 0, growth = 2, mode = 0, world = 1, kc = 0, nqc_max = 0;
   const float* qf = nullptr;  // [nq, d] fp32 (not owned by the workspace)
-  __half* qh = nullptr;       // [nq, dpad] scan operand
-  float *hn = nullptr, *en = nullptr;  // per query ||q_h||, ||q - q_h||
+  __half* qh = nullptr;       // [nq, dpad] scan operand (int8 index: q_hi [nq, dpad] then q_lo [nq, dpad], int8)
+  float2* qsig = nullptr;     // int8 index: per query (sig_hi, sig_lo)
+  float *hn = nullptr, *en = nullptr;  // per query ||q_h|| (int8 index: ||sig_hi q_hi|| + ||sig_lo q_lo||), ||q - q_h||
   unsigned long long* cand = nullptr;
   int* count = nullptr;
   float* thr = nullptr;
@@ -662,13 +797,14 @@ struct Level {
 
 struct om_index {
   int d = 0, dpad = 0;
-  int storage = OM_F32;  // OM_F32: fp32 master rows xf + fp16 scan copy xh; OM_F16: xh only (xf stays null)
+  int storage = OM_F32;  // OM_F32: fp32 master rows xf + fp16 scan copy xh; OM_F16: xh only; OM_I8: xq only
   int64_t n = 0, cap = 0;
   float* xf = nullptr;
   __half* xh = nullptr;
-  // device [4]: [0] max ||x||, [1] max ||x - x_h|| over the committed rows (float bit patterns); fp16 storage: [2] rows
-  // with a non-finite element committed since the last reset (int), [3] scratch (int: rejected elements of an add,
-  // the all-reduced [2] of a sharded search)
+  int8_t* xq = nullptr;  // int8 rows of quant_i8.cuh, pitch dpad + 16 bytes (dpad = d rounded up to 16)
+  // device [4]: [0] max ||x||, [1] max ||x - x_h|| over the committed rows (float bit patterns); fp16 / int8 storage: [2]
+  // rows with a non-finite element (fp16) or scale (int8) committed since the last reset (int), [3] scratch (int: rejected
+  // elements or rows of an add, the all-reduced [2] of a sharded search)
   float* gstats = nullptr;
   bool gstats_stale = false;  // set by om_index_reset: gstats[0..2] are zeroed on the stream of the next commit / search
   int64_t st_nonfinite = 0;   // gstats[2] as the last search read it
@@ -695,10 +831,28 @@ struct om_index {
   int* h_status = nullptr;  // pinned host mirror of Level::status
 };
 
+static inline int64_t i8_pitch(const om_index* ix) { return static_cast<int64_t>(ix->dpad) + 16; }
+
+static int index_grow_i8(om_index* ix, int64_t ncap) {
+  int8_t* nxq = nullptr;
+  OM_CUDA(cudaDeviceSynchronize());  // rows may still be in flight on the caller's stream(s)
+  if (dev_malloc(&nxq, static_cast<size_t>(ncap) * i8_pitch(ix)) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(OM_ENOMEM, "index: cannot allocate the int8 rows for %lld rows", (long long)ncap);
+  }
+  if (ix->n > 0) OM_CUDA(cudaMemcpy(nxq, ix->xq, static_cast<size_t>(ix->n) * i8_pitch(ix), cudaMemcpyDeviceToDevice));
+  OM_CUDA(cudaDeviceSynchronize());
+  cudaFree(ix->xq);
+  ix->xq = nxq;
+  ix->cap = ncap;
+  return 0;
+}
+
 static int index_grow(om_index* ix, int64_t need) {
   if (need <= ix->cap) return 0;
   int64_t ncap = std::max<int64_t>(need, ix->cap + ix->cap / 2);
   ncap = round_up(std::max<int64_t>(ncap, 1024), 256);
+  if (ix->storage == OM_I8) return index_grow_i8(ix, ncap);
   float* nxf = nullptr;
   __half* nxh = nullptr;
   const bool master = ix->storage == OM_F32;
@@ -746,13 +900,13 @@ int om_index_create(int d, om_index** out) { return om_index_create_typed(d, OM_
 
 int om_index_create_typed(int d, om_dtype storage, om_index** out) {
   if (!out || d <= 0) return fail(OM_EINVAL, "om_index_create: d must be positive");
-  if (storage != OM_F32 && storage != OM_F16)
-    return fail(OM_EINVAL, "om_index_create_typed: storage must be OM_F32 or OM_F16 (the scan operand is fp16)");
+  if (storage != OM_F32 && storage != OM_F16 && storage != OM_I8)
+    return fail(OM_EINVAL, "om_index_create_typed: storage must be OM_F32, OM_F16 or OM_I8");
   OM_TRY(device_sm_count());
   om_index* ix = new (std::nothrow) om_index();
   if (!ix) return fail(OM_ENOMEM, "om_index_create: out of host memory");
   ix->d = d;
-  ix->dpad = static_cast<int>(round_up(d, 8));  // 16-byte row pitch for TMA
+  ix->dpad = storage == OM_I8 ? i8_dpad(d) : static_cast<int>(round_up(d, 8));  // 16-byte row pitch for TMA
   ix->storage = storage;
   if (cudaMalloc(&ix->gstats, 4 * sizeof(float)) != cudaSuccess || cudaMemset(ix->gstats, 0, 4 * sizeof(float)) != cudaSuccess ||
       cudaHostAlloc(&ix->h_status, 8 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
@@ -769,6 +923,7 @@ void om_index_destroy(om_index* ix) {
   if (!ix) return;
   cudaFree(ix->xf);
   cudaFree(ix->xh);
+  cudaFree(ix->xq);
   cudaFree(ix->gstats);
   if (ix->h_status) cudaFreeHost(ix->h_status);
   ix->ws.release();
@@ -797,6 +952,9 @@ int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row
   if (ix->storage == OM_F16) {
     *dev_rows = ix->xh + static_cast<size_t>(ix->n) * ix->dpad;
     *row_pitch_elems = ix->dpad;
+  } else if (ix->storage == OM_I8) {
+    *dev_rows = ix->xq + static_cast<size_t>(ix->n) * i8_pitch(ix);
+    *row_pitch_elems = i8_pitch(ix);
   } else {
     *dev_rows = ix->xf + static_cast<size_t>(ix->n) * ix->d;
     *row_pitch_elems = ix->d;
@@ -806,7 +964,9 @@ int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row
 
 int om_index_reserve(om_index* ix, int64_t n, float** dev_rows) {
   if (!ix || n < 0 || !dev_rows) return fail(OM_EINVAL, "om_index_reserve: bad arguments");
-  if (ix->storage != OM_F32) return fail(OM_ESTATE, "om_index_reserve: the index stores fp16 rows; use om_index_reserve_rows");
+  if (ix->storage != OM_F32)
+    return fail(OM_ESTATE, "om_index_reserve: the index stores %s rows; use om_index_reserve_rows",
+                ix->storage == OM_F16 ? "fp16" : "int8");
   void* rows = nullptr;
   int64_t pitch = 0;
   OM_TRY(om_index_reserve_rows(ix, n, &rows, &pitch));
@@ -819,7 +979,10 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   OM_TRY(settle_reset(ix, st));
-  if (ix->storage == OM_F16)
+  if (ix->storage == OM_I8)
+    commit_i8_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xq + static_cast<size_t>(ix->n) * i8_pitch(ix), n, ix->d,
+                                                          ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
+  else if (ix->storage == OM_F16)
     commit_f16_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d,
                                                            ix->dpad, ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
   else
@@ -831,13 +994,14 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   return 0;
 }
 
-// om_index_add on fp16 storage: convert into the reserved rows, count what fp16 cannot hold, and commit only if nothing
-// was out of range (the converted rows stay beyond ntotal otherwise).  Synchronises `st` to read the count.
-static int add_f16(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, cudaStream_t st) {
+// om_index_add on fp16 / int8 storage: convert into the reserved rows, count what the storage cannot hold, and commit only
+// if nothing was out of range (the converted rows stay beyond ntotal otherwise).  Synchronises `st` to read the count.
+static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, cudaStream_t st) {
   void* rows = nullptr;
   int64_t pitch = 0;
   OM_TRY(om_index_reserve_rows(ix, n, &rows, &pitch));
   __half* dst = static_cast<__half*>(rows);
+  int8_t* dq = static_cast<int8_t*>(rows);
   const size_t elems = static_cast<size_t>(n) * ix->d;
   const size_t esize = dtype == OM_F32 ? 4 : 2;
   const void* src = x;
@@ -849,8 +1013,16 @@ static int add_f16(om_index* ix, const void* x, om_memkind kind, om_dtype dtype,
   }
   int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
   cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(int), st);
-  const int grid = grid_for(static_cast<int64_t>(elems), 256);
-  if (e == cudaSuccess) {
+  const int grid = grid_for(static_cast<int64_t>(elems), 256), grid_rows = grid_for(n, 8);
+  if (e == cudaSuccess && ix->storage == OM_I8) {
+    if (dtype == OM_F32)
+      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const float*>(src), n, ix->d, dq, pitch, bad);
+    else if (dtype == OM_BF16)
+      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(src), n, ix->d, dq, pitch, bad);
+    else
+      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const __half*>(src), n, ix->d, dq, pitch, bad);
+    e = cudaGetLastError();
+  } else if (e == cudaSuccess) {
     if (dtype == OM_F32)
       to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const float*>(src), n, ix->d, dst, ix->dpad, bad);
     else if (dtype == OM_BF16)
@@ -863,6 +1035,9 @@ static int add_f16(om_index* ix, const void* x, om_memkind kind, om_dtype dtype,
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (tmp) cudaFree(tmp);
   OM_CUDA(e);
+  if (ix->h_status[4] > 0 && ix->storage == OM_I8)
+    return fail(OM_EINVAL, "om_index_add: %d rows hold inf or NaN; int8 storage cannot hold them and no row was added",
+                ix->h_status[4]);
   if (ix->h_status[4] > 0)
     return fail(OM_EINVAL, "om_index_add: %d elements are NaN or round to +-inf in fp16 (|x| >= 65520); fp16 storage cannot "
                 "hold them and no row was added", ix->h_status[4]);
@@ -873,10 +1048,10 @@ int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, i
   if (!ix || (!x && n > 0) || n < 0) return fail(OM_EINVAL, "om_index_add: bad arguments");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (ix->storage == OM_F16) {
+  if (ix->storage != OM_F32) {
     if (dtype != OM_F32 && dtype != OM_BF16 && dtype != OM_F16)
       return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
-    return add_f16(ix, x, kind, dtype, n, st);
+    return add_converted(ix, x, kind, dtype, n, st);
   }
   float* dst = nullptr;
   OM_TRY(om_index_reserve(ix, n, &dst));
@@ -1011,9 +1186,11 @@ int once_attrs() {
   OM_CUDA(cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
   OM_CUDA(cudaFuncSetAttribute(finalize_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
   OM_CUDA(cudaFuncSetAttribute(finalize_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
+  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
   OM_CUDA(cudaFuncSetAttribute(merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16));
   OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
   done = true;
   return 0;
 }
@@ -1075,7 +1252,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   const size_t nqc = L.nqc_max;
   const size_t o_qh = carve(static_cast<size_t>(nq) * dpad * 2), o_hn = carve(static_cast<size_t>(nq) * 4),
                o_en = carve(static_cast<size_t>(nq) * 4), o_cand = carve(nqc * L.C * 8), o_count = carve(nqc * 4),
-               o_thr = carve(nqc * 4), o_status = carve(256);
+               o_thr = carve(nqc * 4), o_status = carve(256), o_sig = carve(static_cast<size_t>(nq) * 8);
   size_t o_send = 0, o_recv = 0;
   if (world > 1) {
     const size_t blk = exchange_block_bytes(nqc, L.kc);
@@ -1085,6 +1262,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   OM_TRY(ix->ws.reserve(off));
   uint8_t* base = static_cast<uint8_t*>(ix->ws.p);
   L.qh = reinterpret_cast<__half*>(base + o_qh);
+  L.qsig = reinterpret_cast<float2*>(base + o_sig);
   L.hn = reinterpret_cast<float*>(base + o_hn);
   L.en = reinterpret_cast<float*>(base + o_en);
   L.cand = reinterpret_cast<unsigned long long*>(base + o_cand);
@@ -1093,7 +1271,13 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   L.status = reinterpret_cast<int*>(base + o_status);
   L.send = world > 1 ? base + o_send : nullptr;
   L.recv = world > 1 ? base + o_recv : nullptr;
-  if (mode == 0) {
+  if (mode == 0 && ix->storage == OM_I8) {
+    int8_t* q8 = reinterpret_cast<int8_t*>(L.qh);
+    queries_to_i8_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, nq, d, dpad, q8, q8 + static_cast<size_t>(nq) * dpad, L.qsig,
+                                                          L.hn, L.en);
+    OM_CUDA(cudaGetLastError());
+    ix->st_launches += 1;
+  } else if (mode == 0) {
     rows_to_f16_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, L.qh, nq, d, dpad, L.hn, L.en, nullptr);
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 1;
@@ -1102,7 +1286,8 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
 }
 
 // One sweep of the shard for queries [q0, q0 + nqc) of the level.  safe = false: doubling rounds; safe = true: fixed
-// rounds of C - kp rows, which cannot overflow.  mode 0: fp16 tensor-core scan, 1: exact fp32 scan.
+// rounds of C - kp rows, which cannot overflow.  mode 0: tensor-core scan (fp16; int8 index: scan_i8.cuh), 1: exact fp32
+// scan.
 int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sms, cudaStream_t st) {
   const int64_t growth = L.growth;
   const int64_t N = ix->n;
@@ -1129,7 +1314,22 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
       step = std::min<int64_t>(N - pos, (growth - 1) * pos);
     {
       Timed t(ix, st, 0);
-      if (L.mode == 0) {
+      if (L.mode == 0 && ix->storage == OM_I8) {
+        // every round on the int8 scan (pair_scan and the cluster shape do not apply)
+        const int8_t* q8 = reinterpret_cast<const int8_t*>(L.qh);
+        const int8_t* qhi = q8 + static_cast<size_t>(q0) * ix->dpad;
+        const int8_t* qlo = q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
+        const int8_t* xrows = ix->xq + static_cast<size_t>(pos) * i8_pitch(ix);
+        const int ncols = static_cast<int>(step);
+        cudaError_t e;
+        if (first)
+          e = launch_scan_i8<true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, i8_pitch(ix), ix->dpad, nqc, ncols, ix->d, L.thr,
+                                   L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
+        else
+          e = launch_scan_i8<false>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, i8_pitch(ix), ix->dpad, nqc, ncols, ix->d, L.thr,
+                                    L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
+        if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
+      } else if (L.mode == 0) {
         const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
         cudaError_t e;
         const int ncols = static_cast<int>(step);
@@ -1161,7 +1361,11 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
                   static_cast<unsigned>((nqc + nqt - 1) / nqt));
         const size_t smem = static_cast<size_t>(nqt) * ix->d * 4;
-        if (ix->storage == OM_F16)
+        if (ix->storage == OM_I8)
+          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xq + static_cast<size_t>(pos) * i8_pitch(ix), step,
+                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
+                                                           L.count, overflow, C, first ? 1 : 0);
+        else if (ix->storage == OM_F16)
           exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xh + static_cast<size_t>(pos) * ix->dpad, step,
                                                            static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
                                                            L.count, overflow, C, first ? 1 : 0);
@@ -1193,7 +1397,10 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
   {
     Timed t(ix, st, 2);
     const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
-    if (ix->storage == OM_F16)
+    if (ix->storage == OM_I8)
+      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xq, ix->d, D, I, id_offset, k_out,
+                                                  ix->stage_scores);
+    else if (ix->storage == OM_F16)
       finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xh, ix->d, D, I, id_offset, k_out,
                                                   ix->stage_scores);
     else
@@ -1329,11 +1536,12 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
   return fail(OM_EFAULT, "search level did not converge (bug)");
 }
 
-// fp16 storage: rows written in place may hold values fp16 cannot represent (inf from an overflowing encoder output, NaN),
-// and there is no fp32 copy to answer from, so the search is refused until om_index_reset.  Sharded: the shards' counts are
-// summed so that every rank takes the same decision.  One host synchronisation; fp32 indices skip the check.
+// fp16 / int8 storage: rows written in place may hold values the storage cannot represent (inf from an overflowing encoder
+// output, NaN; int8: a non-finite scale), and there is no fp32 copy to answer from, so the search is refused until
+// om_index_reset.  Sharded: the shards' counts are summed so that every rank takes the same decision.  One host
+// synchronisation; fp32 indices skip the check.
 int check_finite_rows(om_index* ix, om_comm* comm, cudaStream_t st) {
-  if (ix->storage != OM_F16) return 0;
+  if (ix->storage == OM_F32) return 0;
   int* cnt = reinterpret_cast<int*>(ix->gstats) + 2;
   const bool sharded = comm && comm->world > 1;
   if (sharded) OM_NCCL(nccl_api().AllReduce(cnt, cnt + 1, 1, kNcclInt32, kNcclSum, comm->nccl, st));
@@ -1342,8 +1550,8 @@ int check_finite_rows(om_index* ix, om_comm* comm, cudaStream_t st) {
   ix->st_nonfinite = ix->h_status[4];
   const int total = sharded ? ix->h_status[5] : ix->h_status[4];
   if (total > 0)
-    return fail(OM_EINVAL, "search: %d committed fp16 rows hold inf or NaN (%d on this shard); fp16 storage cannot answer "
-                "exactly over them: reset the index", total, ix->h_status[4]);
+    return fail(OM_EINVAL, "search: %d committed %s rows hold inf or NaN (%d on this shard); the storage cannot answer "
+                "exactly over them: reset the index", total, ix->storage == OM_I8 ? "int8" : "fp16", ix->h_status[4]);
   return 0;
 }
 

@@ -45,9 +45,10 @@ static inline int make_tmap_bf16_2d(CUtensorMap* out, const void* gptr, uint64_t
   return static_cast<int>(r);
 }
 
-// Generic 2-D row-major tiled map: `elem_bytes` 2 (bf16) or 4 (fp32); swizzle_bytes 128 or 64 (= the box's inner extent
-// in bytes).  Used by the residual epilogue: fp32 boxes {32 cols, 32 rows} with SWIZZLE_128B (TMA load + in-place TMA
-// store of the residual stream) and bf16 boxes {32 cols, 32 rows} with SWIZZLE_64B (one chunk of a bf16 output).
+// Generic 2-D row-major tiled map: `elem_bytes` 1 (int8), 2 (bf16) or 4 (fp32); swizzle_bytes 128 or 64 (= the box's
+// inner extent in bytes).  Used by the residual epilogue: fp32 boxes {32 cols, 32 rows} with SWIZZLE_128B (TMA load +
+// in-place TMA store of the residual stream) and bf16 boxes {32 cols, 32 rows} with SWIZZLE_64B (one chunk of a bf16
+// output); and by the int8 search scan: boxes {128 codes, 128 rows} with SWIZZLE_128B.
 static inline int make_tmap_2d(CUtensorMap* out, const void* gptr, int elem_bytes, uint64_t inner, uint64_t rows,
                                uint64_t row_stride_bytes, uint32_t box_inner, uint32_t box_rows, int swizzle_bytes) {
   PFN_tmapEncodeTiled fn = tmap_encode_fn();
@@ -56,7 +57,10 @@ static inline int make_tmap_2d(CUtensorMap* out, const void* gptr, int elem_byte
   cuuint64_t strides[1] = {row_stride_bytes};
   cuuint32_t box[2] = {box_inner, box_rows};
   cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+  const CUtensorMapDataType type = elem_bytes == 4   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                                     : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
+  CUresult r = fn(out, type, 2,
                   const_cast<void*>(gptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   swizzle_bytes == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);

@@ -14,7 +14,8 @@ import torch
 
 from . import _lib
 
-_OUT_DTYPES = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16}
+_OUT_DTYPES = {torch.float32: _lib.OM_F32, torch.bfloat16: _lib.OM_BF16, torch.float16: _lib.OM_F16,
+               torch.int8: _lib.OM_I8}
 
 _HEAD_WIDTHS = (32, 64)  # BERT head widths hidden / heads the CUDA attention kernels implement (T5: d_kv 64)
 
@@ -165,9 +166,11 @@ class CudaEncoder:
     def _out(self, out: Optional[torch.Tensor], out_dtype: torch.dtype, B: int, device):
         """``out`` of the encode methods, checked, or a new ``[B, rep_dim]`` tensor of ``out_dtype``"""
         if out is None:
+            if out_dtype == torch.int8:
+                raise ValueError("int8 output goes into the rows of an int8 index (FlatIPIndex.reserve_rows): pass out")
             out = torch.empty((B, self.rep_dim), dtype=out_dtype, device=device)
         if out.dtype not in _OUT_DTYPES or out.stride(1) != 1:
-            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor")
+            raise ValueError("out must be a row-major fp32 / bf16 / fp16 CUDA tensor or int8 index rows")
         if out.shape[0] != B or out.shape[1] != self.rep_dim:
             raise ValueError("out must be [%d, %d], got %s" % (B, self.rep_dim, tuple(out.shape)))
         return out
@@ -183,7 +186,8 @@ class CudaEncoder:
                out_dtype: torch.dtype = torch.float32, return_hidden: bool = False):
         """int64 [B, L] CUDA tensors in -> reps [B, rep_dim] (and last_hidden_state fp32 [B, L, H]).  ``out`` / ``out_dtype``:
         fp32, bf16 or fp16 (fp16 and bf16 are the round-to-nearest-even of the fp32 reps of the same call); ``out`` may
-        have any row stride (e.g. the rows ``FlatIPIndex.reserve_rows`` hands out)."""
+        have any row stride (e.g. the rows ``FlatIPIndex.reserve_rows`` hands out).  An int8 ``out`` must be the rows of
+        an int8 index: the fp32 reps of the same call are quantised by the index's rule, scales included."""
         if not input_ids.is_cuda:
             raise RuntimeError("openmatch_b200 encoder runs on CUDA tensors only (no CPU path)")
         B, L = input_ids.shape

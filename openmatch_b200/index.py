@@ -20,7 +20,7 @@ def _stream() -> int:
     return torch.cuda.current_stream().cuda_stream
 
 
-_STORAGE = {torch.float32: _lib.OM_F32, torch.float16: _lib.OM_F16}
+_STORAGE = {torch.float32: _lib.OM_F32, torch.float16: _lib.OM_F16, torch.int8: _lib.OM_I8}
 
 
 class FlatIPIndex:
@@ -33,11 +33,18 @@ class FlatIPIndex:
     top-k by fp32 inner product of the fp32 query with the fp16 rows, ties by ascending id, bitwise what a float32
     index of the fp16-rounded rows returns.  fp16 storage refuses what it cannot hold: ``add`` of a NaN or of a value
     that rounds to +-inf in fp16 (|x| >= 65520) raises and adds nothing; rows written in place through ``reserve_rows``
-    and committed with such values make ``search`` raise until ``reset`` (``stat("nonfinite_rows")``)."""
+    and committed with such values make ``search`` raise until ``reset`` (``stat("nonfinite_rows")``).
+
+    ``torch.int8``: one byte per element plus a per-row fp32 scale (rows of ``dpad + 16`` bytes, ``dpad`` = d rounded up
+    to 16; the scale sits at byte ``dpad``).  A row x is stored as ``s = max|x| / 127`` and ``c = clamp(rint(x / s),
+    -127, 127)`` (a zero row: s = 0); search is exact with respect to the dequantised values ``fp32(s * c)``, bitwise
+    what a float32 index of ``rows_f32()`` returns.  ``add`` of a row holding inf or NaN raises and adds nothing; rows
+    written in place (the encoder quantises into an int8 ``reserve_rows`` view) and committed with a non-finite scale
+    make ``search`` raise until ``reset``."""
 
     def __init__(self, d: int, dtype: torch.dtype = torch.float32):
         if dtype not in _STORAGE:
-            raise ValueError("index storage must be torch.float32 or torch.float16, got %s" % dtype)
+            raise ValueError("index storage must be torch.float32, torch.float16 or torch.int8, got %s" % dtype)
         self._lib = _lib.load()
         h = ctypes.c_void_p()
         _lib.check(self._lib.om_index_create_typed(int(d), _STORAGE[dtype], ctypes.byref(h)))
@@ -58,7 +65,7 @@ class FlatIPIndex:
     def add(self, x) -> None:
         """x: [n, d]; numpy (host) or torch tensor (host or CUDA); float32, bfloat16 or float16 tensors are passed as they
         are, anything else as float32."""
-        if isinstance(x, torch.Tensor) and (x.is_cuda or (self.dtype == torch.float16 and x.dtype in _ADD_DTYPES)):
+        if isinstance(x, torch.Tensor) and (x.is_cuda or (self.dtype != torch.float32 and x.dtype in _ADD_DTYPES)):
             x = x.detach().contiguous()
             if x.dtype not in _ADD_DTYPES:
                 x = x.float()
@@ -69,7 +76,7 @@ class FlatIPIndex:
             return
         if isinstance(x, torch.Tensor):
             x = x.detach().cpu().numpy()
-        if self.dtype == torch.float16 and isinstance(x, np.ndarray) and x.dtype == np.float16:
+        if self.dtype != torch.float32 and isinstance(x, np.ndarray) and x.dtype == np.float16:
             x = np.ascontiguousarray(x)
             self._check_shape(x.shape)
             _lib.check(self._lib.om_index_add(self._h, x.ctypes.data, _lib.OM_HOST, _lib.OM_F16, x.shape[0], _stream()))
@@ -154,8 +161,8 @@ class FlatIPIndex:
 
     def reserve_rows(self, n: int) -> torch.Tensor:
         """Zero-copy ingest: a CUDA tensor view [n, d] of the next n rows of the shard in the index's dtype (float16
-        rows have row stride dpad = d rounded up to 8); fill it (e.g. as the encoder's output buffer) and call
-        ``commit_rows(n)``."""
+        rows have row stride dpad = d rounded up to 8, int8 rows dpad + 16 with dpad = d rounded up to 16 and the row's
+        scale beyond the view); fill it (e.g. as the encoder's output buffer) and call ``commit_rows(n)``."""
         p, pitch = self._rows_at(n)
         return _wrap_device(p, (int(n), self.d), pitch, self.dtype)
 
@@ -167,6 +174,26 @@ class FlatIPIndex:
         if n == 0:
             return torch.empty((0, self.d), dtype=self.dtype, device="cuda")
         return _wrap_device(p - n * pitch * self.dtype.itemsize, (n, self.d), pitch, self.dtype)
+
+    def rows_f32(self, chunk_rows: int = 1 << 16):
+        """The stored rows as float32 CUDA blocks of at most ``chunk_rows`` rows (int8: the dequantised values
+        ``fp32(s * c)``, computed block by block).  Exported embedding files hold these values, so a float32 index
+        rebuilt from them answers bitwise like this one."""
+        n = self.ntotal
+        if self.dtype != torch.int8:
+            rows = self.master_rows()
+            for lo in range(0, n, chunk_rows):
+                yield rows[lo:lo + chunk_rows].float()
+            return
+        p, pitch = self._rows_at(0)
+        if n == 0:
+            return
+        full = _wrap_device(p - n * pitch, (n, pitch), pitch, torch.int8)  # whole rows: codes, padding, scale
+        dpad = (self.d + 15) // 16 * 16
+        for lo in range(0, n, chunk_rows):
+            part = full[lo:lo + chunk_rows]
+            scale = part[:, dpad:dpad + 4].contiguous().view(torch.float32)  # [rows, 1]
+            yield part[:, :self.d].float() * scale
 
     def commit_rows(self, n: int) -> None:
         _lib.check(self._lib.om_index_commit(self._h, int(n), _stream()))
@@ -194,7 +221,8 @@ class _CudaArrayView:
 def _wrap_device(ptr: int, shape, pitch: int, dtype: torch.dtype) -> torch.Tensor:
     size = dtype.itemsize
     strides = None if pitch == shape[1] else (pitch * size, size)
-    return torch.as_tensor(_CudaArrayView(ptr, shape, "<f%d" % size, strides), device="cuda")
+    typestr = "|i1" if dtype == torch.int8 else "<f%d" % size
+    return torch.as_tensor(_CudaArrayView(ptr, shape, typestr, strides), device="cuda")
 
 
 class Comm:

@@ -201,11 +201,15 @@ class DRModel(nn.Module):
     @torch.no_grad()
     def encode_into(self, items, out: Tensor, is_query: bool = False) -> Tensor:
         """Inference only: representations of ``items`` written IN PLACE into ``out`` (fp32 / bf16 / fp16 ``[B, rep_dim]``
-        CUDA tensor with unit column stride — e.g. the rows ``FlatIPIndex.reserve_rows`` handed out), no
+        CUDA tensor with unit column stride — e.g. the rows ``FlatIPIndex.reserve_rows`` handed out, int8 rows of an
+        int8 index included, which the encoder quantises), no
         intermediate ``[B, d]`` tensor and no copy.  Same arithmetic as ``encode`` (:133-155)."""
         model, head = (self.lm_q, self.head_q) if is_query else (self.lm_p, self.head_p)
         input_ids = items["input_ids"]
         if "T5" in type(model).__name__ and not (self.model_args is not None and self.model_args.encoder_only):
+            if out.dtype == torch.int8:
+                raise NotImplementedError("encode_into: int8 index rows need the CUDA encoder; encoder-decoder T5 pooling "
+                                          "is not on it (use --encoder_only, or an fp32 / fp16 index)")
             out.copy_(self.encode(items, model, head, need_hidden=False)[1])  # encoder-decoder pooling: HF module
             return out
         if not input_ids.is_cuda:

@@ -52,9 +52,10 @@ def _results_dict(query_ids: List[str], doc_lookup: np.ndarray, D: np.ndarray, I
 
 def _index_dtype(args) -> torch.dtype:
     name = getattr(args, "index_dtype", "float32")
-    if name not in ("float32", "float16"):
-        raise ValueError("--index_dtype must be 'float32' or 'float16', got %r" % name)
-    return torch.float32 if name == "float32" else torch.float16
+    dtypes = {"float32": torch.float32, "float16": torch.float16, "int8": torch.int8}
+    if name not in dtypes:
+        raise ValueError("--index_dtype must be 'float32', 'float16' or 'int8', got %r" % name)
+    return dtypes[name]
 
 
 class RankArrays:
@@ -98,7 +99,7 @@ class Retriever:
     # ------------------------------------------------------------------ index plumbing
     def _initialize_faiss_index(self, dim: int):
         """Name kept from the reference (:38-41); the index is the HBM-resident flat IP index with the row storage
-        ``--index_dtype`` names (float32 or float16)."""
+        ``--index_dtype`` names (float32, float16 or int8)."""
         self.index = FlatIPIndex(dim, dtype=_index_dtype(self.args))
 
     def _move_index_to_gpu(self):
@@ -133,9 +134,12 @@ class Retriever:
             if into_index:  # foreign model object without encode_into: one device-to-device copy
                 if self.index is None:
                     self._initialize_faiss_index(reps.shape[1])
-                rows = self.index.reserve_rows(reps.shape[0])
-                rows.copy_(reps)
-                self.index.commit_rows(reps.shape[0])
+                if self.index.dtype == torch.int8:  # the index quantises what it adds
+                    self.index.add(reps)
+                else:
+                    rows = self.index.reserve_rows(reps.shape[0])
+                    rows.copy_(reps)
+                    self.index.commit_rows(reps.shape[0])
             else:
                 chunks.append(reps.float())
         return ids, chunks
@@ -234,13 +238,16 @@ class Retriever:
         else:
             # same bytes-on-disk contract as the reference's pickle.dump((encoded, lookup), protocol=4) (:84-86), but the
             # shard is streamed out of HBM through one pinned chunk instead of materialising [n, d] twice on the host
-            write_embedding_file(path, self.index.master_rows(), ids)
+            rows = self.index.rows_f32() if self.index.dtype == torch.int8 else self.index.master_rows()
+            write_embedding_file(path, rows, ids, n=self.index.ntotal, d=self.index.d)
         if self.args.world_size > 1:
             torch.distributed.barrier()
 
     def _index_rows_to_host(self) -> np.ndarray:
         if self.index is None or self.index.ntotal == 0:
             return np.zeros((0, 0), dtype=np.float32)
+        if self.index.dtype == torch.int8:
+            return torch.cat(list(self.index.rows_f32())).cpu().numpy()
         return self.index.master_rows().float().cpu().numpy()  # one D2H copy per corpus shard
 
     def init_index_and_add(self, partition: str = None):
