@@ -42,6 +42,7 @@
 
 #include <algorithm>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 #include "common.h"
@@ -195,67 +196,59 @@ __global__ void __launch_bounds__(256) select_kernel(unsigned long long* cand, i
   }
 }
 
-// Row elements as fp32 for the re-score and the exact scan: group i of 4 consecutive elements (a float4, or one 8-byte
-// load of 4 halves; the row pitch keeps the groups aligned), and element i.  fp16 -> fp32 is exact, so a row stored in
-// fp16 scores bit for bit like the same values held as fp32.
+// Stored row formats, one per row type: the row pitch in elements (host and device), and a view of row r that reads
+// element i, or group i of 4 consecutive elements (d % 4 == 0; the pitch keeps the groups aligned), as fp32.  fp16 -> fp32
+// is exact and an int8 element reads as fp32(s * c), so a stored row scores bit for bit like the same values held as fp32.
+// finite(v): whether a stored value v leaves the row finite, the storage's rule for the rows om_index_commit counts.
 template <typename RowT>
-struct RowQuad;  // the type of one load of 4 row elements
+struct StoredRow;
+// fp32 master rows [n, d]
 template <>
-struct RowQuad<float> {
-  using T = float4;
+struct StoredRow<float> {
+  __host__ __device__ static int pitch(int d) { return d; }
+  const float4* q;  // the row in groups (d % 4 == 0)
+  const float* p;   // the row in elements
+  __device__ StoredRow(const float* xs, size_t r, int d)
+      : q(reinterpret_cast<const float4*>(xs) + r * (pitch(d) >> 2)), p(xs + r * pitch(d)) {}
+  __device__ float4 quad(int i) const { return __ldg(q + i); }
+  __device__ float elem(int i) const { return __ldg(p + i); }
 };
+// fp16 rows [n, dpad], dpad = d rounded up to 8 (om_index_create_typed); a row with a non-finite element is non-finite
 template <>
-struct RowQuad<__half> {
-  using T = uint2;
+struct StoredRow<__half> {
+  __host__ __device__ static int pitch(int d) { return (d + 7) & ~7; }
+  const uint2* q;  // the row in groups of 4 halves
+  const __half* p;
+  __device__ StoredRow(const __half* xs, size_t r, int d)
+      : q(reinterpret_cast<const uint2*>(xs) + r * (pitch(d) >> 2)), p(xs + r * pitch(d)) {}
+  __device__ float4 quad(int i) const {
+    const uint2 u = __ldg(q + i);
+    const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
+    const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
+    return make_float4(lo.x, lo.y, hi.x, hi.y);
+  }
+  __device__ float elem(int i) const { return __half2float(__ldg(p + i)); }
+  __device__ bool finite(float v) const { return isfinite(v); }
 };
-__device__ __forceinline__ float4 quad_f32(float4 v) { return v; }
-__device__ __forceinline__ float4 quad_f32(uint2 u) {
-  const float2 lo = __half22float2(*reinterpret_cast<const __half2*>(&u.x));
-  const float2 hi = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-  return make_float4(lo.x, lo.y, hi.x, hi.y);
-}
-__device__ __forceinline__ float elem_f32(float v) { return v; }
-__device__ __forceinline__ float elem_f32(__half v) { return __half2float(v); }
-// row pitch in elements: fp32 master rows [n, d], fp16 rows [n, dpad] with dpad = d rounded up to 8 (om_index_create),
-// int8 rows of i8_dpad(d) + 16 bytes (quant_i8.cuh)
-template <typename RowT>
-__device__ __forceinline__ int row_pitch(int d) { return sizeof(RowT) == 4 ? d : (d + 7) & ~7; }
+// int8 rows of i8_dpad(d) + 16 bytes (quant_i8.cuh): 4 codes per group, and the row's scale, loaded once per view.  A row
+// is non-finite when its scale is; a finite scale whose products s * c overflow leaves the row accepted.
 template <>
-__device__ __forceinline__ int row_pitch<int8_t>(int d) { return i8_dpad(d) + 16; }
-// the 4-element groups of row r (d % 4 == 0), read with load_quad(group pointer, i)
-template <typename RowT>
-__device__ __forceinline__ const typename RowQuad<RowT>::T* row_quads(const RowT* xs, size_t r, int d) {
-  return reinterpret_cast<const typename RowQuad<RowT>::T*>(xs) + r * (row_pitch<RowT>(d) >> 2);
-}
-// the elements of row r, read with load_elem(element pointer, i)
-template <typename RowT>
-__device__ __forceinline__ const RowT* row_elems(const RowT* xs, size_t r, int d) {
-  return xs + r * row_pitch<RowT>(d);
-}
-template <typename QuadT>
-__device__ __forceinline__ float4 load_quad(const QuadT* x4, int i) { return quad_f32(__ldg(x4 + i)); }
-template <typename RowT>
-__device__ __forceinline__ float load_elem(const RowT* x, int i) { return elem_f32(__ldg(x + i)); }
-// int8 rows: 4 codes per group, and the row's scale; element j reads as fp32(s * c_j), so a row stored in int8 scores bit
-// for bit like the same values held as fp32
-struct I8Row {
+struct StoredRow<int8_t> {
+  __host__ __device__ static int pitch(int d) { return i8_dpad(d) + 16; }
   const int8_t* p;
   float s;
+  __device__ StoredRow(const int8_t* xs, size_t r, int d)
+      : p(xs + r * pitch(d)), s(__ldg(reinterpret_cast<const float*>(p + i8_dpad(d)))) {}
+  __device__ float4 quad(int i) const {
+    const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(p) + i);
+    return make_float4(__fmul_rn(s, static_cast<float>(static_cast<int8_t>(u))),
+                       __fmul_rn(s, static_cast<float>(static_cast<int8_t>(u >> 8))),
+                       __fmul_rn(s, static_cast<float>(static_cast<int8_t>(u >> 16))),
+                       __fmul_rn(s, static_cast<float>(static_cast<int8_t>(u >> 24))));
+  }
+  __device__ float elem(int i) const { return __fmul_rn(s, static_cast<float>(__ldg(p + i))); }
+  __device__ bool finite(float) const { return isfinite(s); }
 };
-__device__ __forceinline__ I8Row i8_row(const int8_t* xs, size_t r, int d) {
-  const int8_t* p = xs + r * row_pitch<int8_t>(d);
-  return {p, __ldg(reinterpret_cast<const float*>(p + i8_dpad(d)))};
-}
-__device__ __forceinline__ I8Row row_quads(const int8_t* xs, size_t r, int d) { return i8_row(xs, r, d); }
-__device__ __forceinline__ I8Row row_elems(const int8_t* xs, size_t r, int d) { return i8_row(xs, r, d); }
-__device__ __forceinline__ float4 load_quad(I8Row x, int i) {
-  const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(x.p) + i);
-  return make_float4(__fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u))),
-                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 8))),
-                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 16))),
-                     __fmul_rn(x.s, static_cast<float>(static_cast<int8_t>(u >> 24))));
-}
-__device__ __forceinline__ float load_elem(I8Row x, int i) { return __fmul_rn(x.s, static_cast<float>(__ldg(x.p + i))); }
 
 // FINAL: one CTA per query: exact fp32 re-score of the candidates against the stored rows (fp32 master rows or fp16
 // rows), sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row
@@ -281,18 +274,18 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
     const uint32_t row = key_row(mine[j]);
     float acc = 0.f;
     if ((d & 3) == 0) {
-      const auto x4 = row_quads(xs, row, d);
+      const StoredRow<RowT> x(xs, row, d);
       const float4* q4 = reinterpret_cast<const float4*>(sq);
       for (int i = lane; i < (d >> 2); i += 32) {
-        const float4 a = load_quad(x4, i), b = q4[i];
+        const float4 a = x.quad(i), b = q4[i];
         acc = fmaf(a.x, b.x, acc);
         acc = fmaf(a.y, b.y, acc);
         acc = fmaf(a.z, b.z, acc);
         acc = fmaf(a.w, b.w, acc);
       }
     } else {
-      const auto x = row_elems(xs, row, d);
-      for (int i = lane; i < d; i += 32) acc = fmaf(load_elem(x, i), sq[i], acc);
+      const StoredRow<RowT> x(xs, row, d);
+      for (int i = lane; i < d; i += 32) acc = fmaf(x.elem(i), sq[i], acc);
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
@@ -376,37 +369,6 @@ __global__ void to_f16_rows_kernel(const T* __restrict__ src, int64_t n, int d, 
   if (nb) atomicAdd(bad, nb);
 }
 
-// fp16 storage, commit: the stored rows x [n, dpad] are read in place.  Running maxima of ||x|| (gstats[0], summed in the
-// order of rows_to_f16_kernel, so an fp32 index of the same values gets the same bits); ||x - x_h|| is 0 and gstats[1]
-// stays as it is.  Rows holding a non-finite element are counted in *nonfinite: searches refuse the index until a reset.
-__global__ void __launch_bounds__(256) commit_f16_rows_kernel(const __half* __restrict__ x, int64_t n, int d, int dpad,
-                                                              float* gstats, int* nonfinite) {
-  const int lane = threadIdx.x & 31;
-  const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
-  float mx = 0.f;
-  int nbad = 0;
-  for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
-    const __half* y = x + r * dpad;
-    float sx = 0.f;
-    bool finite = true;
-    for (int c = 2 * lane; c < d; c += 64) {  // c + 1 < dpad (dpad is a multiple of 8): the pair load stays in the row
-      const float2 v = __half22float2(*reinterpret_cast<const __half2*>(y + c));
-      const float a = v.x, b = c + 1 < d ? v.y : 0.f;
-      finite = finite && isfinite(a) && isfinite(b);
-      sx = fmaf(a, a, fmaf(b, b, sx));
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, o);
-    const float nx = sqrtf(sx);
-    mx = (nx > mx || nx != nx) ? nx : mx;
-    if (!__all_sync(0xffffffffu, finite) && lane == 0) ++nbad;
-  }
-  if (lane == 0) {
-    atomicMax(reinterpret_cast<int*>(gstats), __float_as_int(mx != mx ? __int_as_float(0x7fc00000) : mx));
-    if (nbad) atomicAdd(nonfinite, nbad);
-  }
-}
-
 // int8 storage, add: src [n, d] (fp32 / bf16 / fp16, converted exactly to fp32) -> rows of quant_i8.cuh, one warp per row.
 // Rows holding inf or NaN are counted in *bad: the caller then refuses the whole add.
 template <typename T>
@@ -423,29 +385,31 @@ __global__ void __launch_bounds__(256) quantize_rows_i8_kernel(const T* __restri
   if (lane == 0 && nb) atomicAdd(bad, nb);
 }
 
-// int8 storage, commit: the stored rows are read in place.  Running maximum of ||x^|| over the rows, x^_j = fp32(s c_j)
-// (gstats[0], summed in the order of rows_to_f16_kernel, so an fp32 index of the same values gets the same bits);
-// gstats[1] stays 0 (the stored values are the rows).  Rows with a non-finite scale are counted in *nonfinite: searches
-// refuse the index until a reset.
-__global__ void __launch_bounds__(256) commit_i8_rows_kernel(const int8_t* __restrict__ x, int64_t n, int d, float* gstats,
-                                                             int* nonfinite) {
+// fp16 / int8 storage, commit: the stored rows are read in place.  Running maximum of ||x^|| over the rows, x^_j the stored
+// value of element j (gstats[0], summed in the order of rows_to_f16_kernel, so an fp32 index of the same values gets the
+// same bits); gstats[1] stays as it is (the stored values are the rows).  Rows that StoredRow<RowT>::finite rejects are
+// counted in *nonfinite: searches refuse the index until a reset.
+template <typename RowT>
+__global__ void __launch_bounds__(256) commit_rows_kernel(const RowT* __restrict__ x, int64_t n, int d, float* gstats,
+                                                          int* nonfinite) {
   const int lane = threadIdx.x & 31;
   const int64_t nwarps = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
   float mx = 0.f;
   int nbad = 0;
   for (int64_t r = static_cast<int64_t>(blockIdx.x) * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += nwarps) {
-    const I8Row row = i8_row(x, r, d);
+    const StoredRow<RowT> row(x, r, d);
     float sx = 0.f;
+    bool finite = true;
     for (int c = 2 * lane; c < d; c += 64) {
-      const float a = __fmul_rn(row.s, static_cast<float>(row.p[c]));
-      const float b = c + 1 < d ? __fmul_rn(row.s, static_cast<float>(row.p[c + 1])) : 0.f;
+      const float a = row.elem(c), b = c + 1 < d ? row.elem(c + 1) : 0.f;
+      finite = finite && row.finite(a) && row.finite(b);
       sx = fmaf(a, a, fmaf(b, b, sx));
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) sx += __shfl_xor_sync(0xffffffffu, sx, o);
     const float nx = sqrtf(sx);
     mx = (nx > mx || nx != nx) ? nx : mx;
-    if (lane == 0 && !isfinite(row.s)) ++nbad;
+    if (!__all_sync(0xffffffffu, finite) && lane == 0) ++nbad;
   }
   if (lane == 0) {
     atomicMax(reinterpret_cast<int*>(gstats), __float_as_int(mx != mx ? __int_as_float(0x7fc00000) : mx));
@@ -654,7 +618,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
         float4 a[ROWS];
 #pragma unroll
         for (int rr = 0; rr < ROWS; ++rr)
-          a[rr] = r0 + rr < n_rows ? load_quad(row_quads(xs, r0 + rr, d), i) : make_float4(0.f, 0.f, 0.f, 0.f);
+          a[rr] = r0 + rr < n_rows ? StoredRow<RowT>(xs, r0 + rr, d).quad(i) : make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int j = 0; j < NQT; ++j) {
           if (j < nact) {
@@ -675,7 +639,7 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
       for (int i = lane; i < d; i += 32) {
         float a[ROWS];
 #pragma unroll
-        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? load_elem(row_elems(xs, r0 + rr, d), i) : 0.f;
+        for (int rr = 0; rr < ROWS; ++rr) a[rr] = r0 + rr < n_rows ? StoredRow<RowT>(xs, r0 + rr, d).elem(i) : 0.f;
 #pragma unroll
         for (int j = 0; j < NQT; ++j)
           if (j < nact) {
@@ -783,7 +747,8 @@ struct DevBuf {  // grow-only device scratch
 struct Level {
   int nq = 0, k = 0, kp = 0, kp_target = 0, C = 0, growth = 2, mode = 0, world = 1, kc = 0, nqc_max = 0;
   const float* qf = nullptr;  // [nq, d] fp32 (not owned by the workspace)
-  __half* qh = nullptr;       // [nq, dpad] scan operand (int8 index: q_hi [nq, dpad] then q_lo [nq, dpad], int8)
+  __half* qh = nullptr;       // [nq, dpad] scan operand
+  int8_t* q8 = nullptr;       // int8 index, in qh's region: q_hi [nq, dpad] then q_lo [nq, dpad]
   float2* qsig = nullptr;     // int8 index: per query (sig_hi, sig_lo)
   float *hn = nullptr, *en = nullptr;  // per query ||q_h|| (int8 index: ||sig_hi q_hi|| + ||sig_lo q_lo||), ||q - q_h||
   unsigned long long* cand = nullptr;
@@ -831,50 +796,60 @@ struct om_index {
   int* h_status = nullptr;  // pinned host mirror of Level::status
 };
 
-static inline int64_t i8_pitch(const om_index* ix) { return static_cast<int64_t>(ix->dpad) + 16; }
-
-static int index_grow_i8(om_index* ix, int64_t ncap) {
-  int8_t* nxq = nullptr;
-  OM_CUDA(cudaDeviceSynchronize());  // rows may still be in flight on the caller's stream(s)
-  if (dev_malloc(&nxq, static_cast<size_t>(ncap) * i8_pitch(ix)) != cudaSuccess) {
-    cudaGetLastError();
-    return fail(OM_ENOMEM, "index: cannot allocate the int8 rows for %lld rows", (long long)ncap);
+// Calls f with the index's stored rows as a typed pointer: the fp32 master rows, the fp16 rows or the int8 rows.  Kernels
+// over stored rows deduce their row type from it.
+template <typename F>
+static decltype(auto) with_rows(const om_index* ix, F&& f) {
+  switch (ix->storage) {
+    case OM_I8: return f(ix->xq);
+    case OM_F16: return f(ix->xh);
+    default: return f(ix->xf);
   }
-  if (ix->n > 0) OM_CUDA(cudaMemcpy(nxq, ix->xq, static_cast<size_t>(ix->n) * i8_pitch(ix), cudaMemcpyDeviceToDevice));
-  OM_CUDA(cudaDeviceSynchronize());
-  cudaFree(ix->xq);
-  ix->xq = nxq;
-  ix->cap = ncap;
-  return 0;
 }
 
+// row pitch in elements of the rows behind a typed pointer
+template <typename RowT>
+static int64_t pitch_of(const RowT*, int d) { return StoredRow<RowT>::pitch(d); }
+
+// one row buffer of an index (the index member that holds it) and its bytes per row, named for the out-of-memory message
+struct RowBuf {
+  void** p;
+  size_t row_bytes;
+  const char* name;
+};
+template <typename RowT>
+static RowBuf row_buf(RowT** p, int d, const char* name) {
+  return {reinterpret_cast<void**>(p), StoredRow<RowT>::pitch(d) * sizeof(RowT), name};
+}
+
+// Grows every row buffer of the index's storage to hold at least `need` rows.
 static int index_grow(om_index* ix, int64_t need) {
   if (need <= ix->cap) return 0;
   int64_t ncap = std::max<int64_t>(need, ix->cap + ix->cap / 2);
   ncap = round_up(std::max<int64_t>(ncap, 1024), 256);
-  if (ix->storage == OM_I8) return index_grow_i8(ix, ncap);
-  float* nxf = nullptr;
-  __half* nxh = nullptr;
-  const bool master = ix->storage == OM_F32;
+  std::vector<RowBuf> bufs;
+  switch (ix->storage) {
+    case OM_I8: bufs = {row_buf(&ix->xq, ix->d, "int8")}; break;
+    case OM_F16: bufs = {row_buf(&ix->xh, ix->d, "fp16")}; break;
+    default: bufs = {row_buf(&ix->xf, ix->d, "fp32"), row_buf(&ix->xh, ix->d, "fp16")};  // master rows, scan copy
+  }
+  void* fresh[2] = {};
   // rows may still be in flight on the caller's stream(s) (encoder writing reserved rows, a pending commit)
   OM_CUDA(cudaDeviceSynchronize());
-  if (master) OM_CUDA(dev_malloc(&nxf, static_cast<size_t>(ncap) * ix->d * sizeof(float)));
-  cudaError_t e = dev_malloc(&nxh, static_cast<size_t>(ncap) * ix->dpad * sizeof(__half));
-  if (e != cudaSuccess) {
-    cudaFree(nxf);
-    cudaGetLastError();
-    return fail(OM_ENOMEM, "index: cannot allocate the fp16 rows for %lld rows", (long long)ncap);
-  }
-  if (ix->n > 0) {
-    if (master)
-      OM_CUDA(cudaMemcpy(nxf, ix->xf, static_cast<size_t>(ix->n) * ix->d * sizeof(float), cudaMemcpyDeviceToDevice));
-    OM_CUDA(cudaMemcpy(nxh, ix->xh, static_cast<size_t>(ix->n) * ix->dpad * sizeof(__half), cudaMemcpyDeviceToDevice));
+  for (size_t b = 0; b < bufs.size(); ++b) {
+    if (dev_malloc(&fresh[b], static_cast<size_t>(ncap) * bufs[b].row_bytes) != cudaSuccess) {
+      for (void* p : fresh) cudaFree(p);
+      cudaGetLastError();
+      return fail(OM_ENOMEM, "index: cannot allocate the %s rows for %lld rows", bufs[b].name, (long long)ncap);
+    }
+    if (ix->n > 0)
+      OM_CUDA(cudaMemcpy(fresh[b], *bufs[b].p, static_cast<size_t>(ix->n) * bufs[b].row_bytes, cudaMemcpyDeviceToDevice));
   }
   OM_CUDA(cudaDeviceSynchronize());
-  cudaFree(ix->xf);
-  cudaFree(ix->xh);
-  ix->xf = nxf;
-  ix->xh = nxh;
+  for (size_t b = 0; b < bufs.size(); ++b) {
+    cudaFree(*bufs[b].p);
+    *bufs[b].p = fresh[b];
+  }
   ix->cap = ncap;
   return 0;
 }
@@ -894,6 +869,25 @@ static int settle_reset(om_index* ix, cudaStream_t st) {
   return 0;
 }
 
+// The device rows an add reads: x itself, or for host input a temporary device buffer *tmp filled on st, which the caller
+// frees once st is synchronised.
+static int stage_input(const void* x, om_memkind kind, size_t bytes, cudaStream_t st, const void** src, void** tmp) {
+  *src = x;
+  if (kind != OM_HOST) return 0;
+  OM_CUDA(cudaMalloc(tmp, bytes));
+  OM_CUDA(cudaMemcpyAsync(*tmp, x, bytes, cudaMemcpyHostToDevice, st));
+  *src = *tmp;
+  return 0;
+}
+
+// Calls f with an add's input rows as a typed pointer: fp32, bf16 or fp16.
+template <typename F>
+static decltype(auto) with_input(const void* src, om_dtype dtype, F&& f) {
+  if (dtype == OM_F32) return f(static_cast<const float*>(src));
+  if (dtype == OM_BF16) return f(static_cast<const __nv_bfloat16*>(src));
+  return f(static_cast<const __half*>(src));
+}
+
 extern "C" {
 
 int om_index_create(int d, om_index** out) { return om_index_create_typed(d, OM_F32, out); }
@@ -906,7 +900,7 @@ int om_index_create_typed(int d, om_dtype storage, om_index** out) {
   om_index* ix = new (std::nothrow) om_index();
   if (!ix) return fail(OM_ENOMEM, "om_index_create: out of host memory");
   ix->d = d;
-  ix->dpad = storage == OM_I8 ? i8_dpad(d) : static_cast<int>(round_up(d, 8));  // 16-byte row pitch for TMA
+  ix->dpad = storage == OM_I8 ? i8_dpad(d) : StoredRow<__half>::pitch(d);  // scan operand pitch: 16-byte rows for TMA
   ix->storage = storage;
   if (cudaMalloc(&ix->gstats, 4 * sizeof(float)) != cudaSuccess || cudaMemset(ix->gstats, 0, 4 * sizeof(float)) != cudaSuccess ||
       cudaHostAlloc(&ix->h_status, 8 * sizeof(int), cudaHostAllocDefault) != cudaSuccess) {
@@ -949,16 +943,10 @@ int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row
   if (!ix || n < 0 || !dev_rows || !row_pitch_elems) return fail(OM_EINVAL, "om_index_reserve_rows: bad arguments");
   if (ix->n + n > 0xfffffff0ll) return fail(OM_EINVAL, "index shard limited to 2^32-16 rows; shard the corpus");
   OM_TRY(index_grow(ix, ix->n + n));
-  if (ix->storage == OM_F16) {
-    *dev_rows = ix->xh + static_cast<size_t>(ix->n) * ix->dpad;
-    *row_pitch_elems = ix->dpad;
-  } else if (ix->storage == OM_I8) {
-    *dev_rows = ix->xq + static_cast<size_t>(ix->n) * i8_pitch(ix);
-    *row_pitch_elems = i8_pitch(ix);
-  } else {
-    *dev_rows = ix->xf + static_cast<size_t>(ix->n) * ix->d;
-    *row_pitch_elems = ix->d;
-  }
+  with_rows(ix, [&](auto* xs) {
+    *row_pitch_elems = pitch_of(xs, ix->d);
+    *dev_rows = xs + ix->n * *row_pitch_elems;
+  });
   return 0;
 }
 
@@ -979,16 +967,14 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   OM_TRY(settle_reset(ix, st));
-  if (ix->storage == OM_I8)
-    commit_i8_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xq + static_cast<size_t>(ix->n) * i8_pitch(ix), n, ix->d,
-                                                          ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
-  else if (ix->storage == OM_F16)
-    commit_f16_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d,
-                                                           ix->dpad, ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
-  else
-    rows_to_f16_kernel<<<grid_for(n, 8), 256, 0, st>>>(ix->xf + static_cast<size_t>(ix->n) * ix->d,
-                                                       ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d, ix->dpad,
-                                                       nullptr, nullptr, ix->gstats);
+  with_rows(ix, [&](auto* xs) {
+    auto* rows = xs + ix->n * pitch_of(xs, ix->d);
+    if constexpr (std::is_same<decltype(rows), float*>::value)  // the fp32 commit also writes the fp16 scan copy
+      rows_to_f16_kernel<<<grid_for(n, 8), 256, 0, st>>>(rows, ix->xh + static_cast<size_t>(ix->n) * ix->dpad, n, ix->d,
+                                                         ix->dpad, nullptr, nullptr, ix->gstats);
+    else
+      commit_rows_kernel<<<grid_for(n, 8), 256, 0, st>>>(rows, n, ix->d, ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
+  });
   OM_CUDA(cudaGetLastError());
   ix->n += n;
   return 0;
@@ -1000,42 +986,27 @@ static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype 
   void* rows = nullptr;
   int64_t pitch = 0;
   OM_TRY(om_index_reserve_rows(ix, n, &rows, &pitch));
-  __half* dst = static_cast<__half*>(rows);
-  int8_t* dq = static_cast<int8_t*>(rows);
   const size_t elems = static_cast<size_t>(n) * ix->d;
-  const size_t esize = dtype == OM_F32 ? 4 : 2;
-  const void* src = x;
+  const void* src = nullptr;
   void* tmp = nullptr;
-  if (kind == OM_HOST) {
-    OM_CUDA(cudaMalloc(&tmp, elems * esize));
-    OM_CUDA(cudaMemcpyAsync(tmp, x, elems * esize, cudaMemcpyHostToDevice, st));
-    src = tmp;
-  }
+  OM_TRY(stage_input(x, kind, elems * (dtype == OM_F32 ? 4 : 2), st, &src, &tmp));
+  const bool i8 = ix->storage == OM_I8;  // quantise, else convert to fp16
   int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
   cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(int), st);
-  const int grid = grid_for(static_cast<int64_t>(elems), 256), grid_rows = grid_for(n, 8);
-  if (e == cudaSuccess && ix->storage == OM_I8) {
-    if (dtype == OM_F32)
-      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const float*>(src), n, ix->d, dq, pitch, bad);
-    else if (dtype == OM_BF16)
-      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(src), n, ix->d, dq, pitch, bad);
-    else
-      quantize_rows_i8_kernel<<<grid_rows, 256, 0, st>>>(static_cast<const __half*>(src), n, ix->d, dq, pitch, bad);
-    e = cudaGetLastError();
-  } else if (e == cudaSuccess) {
-    if (dtype == OM_F32)
-      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const float*>(src), n, ix->d, dst, ix->dpad, bad);
-    else if (dtype == OM_BF16)
-      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(src), n, ix->d, dst, ix->dpad, bad);
-    else
-      to_f16_rows_kernel<<<grid, 256, 0, st>>>(static_cast<const __half*>(src), n, ix->d, dst, ix->dpad, bad);
-    e = cudaGetLastError();
-  }
+  if (e == cudaSuccess)
+    e = with_input(src, dtype, [&](const auto* in) {
+      if (i8)
+        quantize_rows_i8_kernel<<<grid_for(n, 8), 256, 0, st>>>(in, n, ix->d, static_cast<int8_t*>(rows), pitch, bad);
+      else
+        to_f16_rows_kernel<<<grid_for(static_cast<int64_t>(elems), 256), 256, 0, st>>>(in, n, ix->d, static_cast<__half*>(rows),
+                                                                                        ix->dpad, bad);
+      return cudaGetLastError();
+    });
   if (e == cudaSuccess) e = cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (tmp) cudaFree(tmp);
   OM_CUDA(e);
-  if (ix->h_status[4] > 0 && ix->storage == OM_I8)
+  if (ix->h_status[4] > 0 && i8)
     return fail(OM_EINVAL, "om_index_add: %d rows hold inf or NaN; int8 storage cannot hold them and no row was added",
                 ix->h_status[4]);
   if (ix->h_status[4] > 0)
@@ -1047,37 +1018,27 @@ static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype 
 int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, void* stream) {
   if (!ix || (!x && n > 0) || n < 0) return fail(OM_EINVAL, "om_index_add: bad arguments");
   if (n == 0) return 0;
+  if (dtype != OM_F32 && dtype != OM_BF16 && dtype != OM_F16) return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (ix->storage != OM_F32) {
-    if (dtype != OM_F32 && dtype != OM_BF16 && dtype != OM_F16)
-      return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
-    return add_converted(ix, x, kind, dtype, n, st);
-  }
+  if (ix->storage != OM_F32) return add_converted(ix, x, kind, dtype, n, st);
   float* dst = nullptr;
   OM_TRY(om_index_reserve(ix, n, &dst));
   const size_t elems = static_cast<size_t>(n) * ix->d;
-  if (dtype == OM_F32) {
-    OM_CUDA(cudaMemcpyAsync(dst, x, elems * 4, kind == OM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice,
-                            st));
-  } else if (dtype == OM_BF16 || dtype == OM_F16) {
-    const void* src = x;
-    void* tmp = nullptr;
-    if (kind == OM_HOST) {
-      OM_CUDA(cudaMalloc(&tmp, elems * 2));
-      OM_CUDA(cudaMemcpyAsync(tmp, x, elems * 2, cudaMemcpyHostToDevice, st));
-      src = tmp;
+  const void* src = x;
+  void* tmp = nullptr;
+  if (dtype != OM_F32) OM_TRY(stage_input(x, kind, elems * 2, st, &src, &tmp));  // fp32 rows are copied straight in
+  OM_TRY(with_input(src, dtype, [&](const auto* in) -> int {
+    if constexpr (std::is_same<decltype(in), const float*>::value) {
+      OM_CUDA(cudaMemcpyAsync(dst, in, elems * 4, kind == OM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
+    } else {
+      to_f32<<<grid_for(elems, 256), 256, 0, st>>>(in, dst, (int64_t)elems);
+      OM_CUDA(cudaGetLastError());
     }
-    if (dtype == OM_BF16)
-      to_f32<<<grid_for(elems, 256), 256, 0, st>>>(static_cast<const __nv_bfloat16*>(src), dst, (int64_t)elems);
-    else
-      to_f32<<<grid_for(elems, 256), 256, 0, st>>>(static_cast<const __half*>(src), dst, (int64_t)elems);
-    OM_CUDA(cudaGetLastError());
-    if (tmp) {
-      OM_CUDA(cudaStreamSynchronize(st));
-      cudaFree(tmp);
-    }
-  } else {
-    return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
+    return 0;
+  }));
+  if (tmp) {
+    OM_CUDA(cudaStreamSynchronize(st));
+    cudaFree(tmp);
   }
   OM_TRY(om_index_commit(ix, n, stream));
   if (kind == OM_HOST) OM_CUDA(cudaStreamSynchronize(st));  // caller may free / reuse its host buffer
@@ -1180,19 +1141,24 @@ void collect_profile(om_index* ix) {
   ix->ev_used = 0;
 }
 
-int once_attrs() {
-  static bool done = false;  // one device per process (enforced by device_sm_count)
-  if (done) return 0;
-  OM_CUDA(cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
-  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
-  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
-  OM_CUDA(cudaFuncSetAttribute(finalize_kernel<int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
-  OM_CUDA(cudaFuncSetAttribute(merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16));
-  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, int8_t>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
-  done = true;
-  return 0;
+// Shared-memory opt-ins, once per process (one device per process, enforced by device_sm_count): the select and merge
+// kernels, and with an index those over its stored rows, once per row type.
+int once_attrs(const om_index* ix) {
+  static bool done = false;
+  if (!done) {
+    OM_CUDA(cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
+    OM_CUDA(cudaFuncSetAttribute(merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16));
+    done = true;
+  }
+  return !ix ? 0 : with_rows(ix, [](const auto* xs) -> int {
+    using RowT = std::decay_t<decltype(*xs)>;
+    static bool rows_done = false;  // one flag per row type: each instantiation of this operator has its own
+    if (rows_done) return 0;
+    OM_CUDA(cudaFuncSetAttribute(finalize_kernel<RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
+    OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    rows_done = true;
+    return 0;
+  });
 }
 
 // Packed per-shard block of the sharded exchange for nqc queries shipping kc entries each:
@@ -1216,7 +1182,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   const int d = ix->d, dpad = ix->dpad;
   if (d > 16384) return fail(OM_EINVAL, "om_index_search: d > 16384 unsupported");
   if (k > kMaxCandidates) return fail(OM_EINVAL, "om_index_search: k = %d exceeds %d", k, kMaxCandidates);
-  OM_TRY(once_attrs());
+  OM_TRY(once_attrs(ix));
   L.qf = qf;
   L.nq = nq;
   L.k = k;
@@ -1262,6 +1228,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   OM_TRY(ix->ws.reserve(off));
   uint8_t* base = static_cast<uint8_t*>(ix->ws.p);
   L.qh = reinterpret_cast<__half*>(base + o_qh);
+  L.q8 = reinterpret_cast<int8_t*>(base + o_qh);
   L.qsig = reinterpret_cast<float2*>(base + o_sig);
   L.hn = reinterpret_cast<float*>(base + o_hn);
   L.en = reinterpret_cast<float*>(base + o_en);
@@ -1272,8 +1239,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   L.send = world > 1 ? base + o_send : nullptr;
   L.recv = world > 1 ? base + o_recv : nullptr;
   if (mode == 0 && ix->storage == OM_I8) {
-    int8_t* q8 = reinterpret_cast<int8_t*>(L.qh);
-    queries_to_i8_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, nq, d, dpad, q8, q8 + static_cast<size_t>(nq) * dpad, L.qsig,
+    queries_to_i8_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, nq, d, dpad, L.q8, L.q8 + static_cast<size_t>(nq) * dpad, L.qsig,
                                                           L.hn, L.en);
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 1;
@@ -1316,17 +1282,17 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
       Timed t(ix, st, 0);
       if (L.mode == 0 && ix->storage == OM_I8) {
         // every round on the int8 scan (pair_scan and the cluster shape do not apply)
-        const int8_t* q8 = reinterpret_cast<const int8_t*>(L.qh);
-        const int8_t* qhi = q8 + static_cast<size_t>(q0) * ix->dpad;
-        const int8_t* qlo = q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
-        const int8_t* xrows = ix->xq + static_cast<size_t>(pos) * i8_pitch(ix);
+        const int8_t* qhi = L.q8 + static_cast<size_t>(q0) * ix->dpad;
+        const int8_t* qlo = L.q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
+        const int64_t pitch = pitch_of(ix->xq, ix->d);
+        const int8_t* xrows = ix->xq + pos * pitch;
         const int ncols = static_cast<int>(step);
         cudaError_t e;
         if (first)
-          e = launch_scan_i8<true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, i8_pitch(ix), ix->dpad, nqc, ncols, ix->d, L.thr,
+          e = launch_scan_i8<true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
                                    L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
         else
-          e = launch_scan_i8<false>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, i8_pitch(ix), ix->dpad, nqc, ncols, ix->d, L.thr,
+          e = launch_scan_i8<false>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
                                     L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
         if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
       } else if (L.mode == 0) {
@@ -1361,18 +1327,10 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
                   static_cast<unsigned>((nqc + nqt - 1) / nqt));
         const size_t smem = static_cast<size_t>(nqt) * ix->d * 4;
-        if (ix->storage == OM_I8)
-          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xq + static_cast<size_t>(pos) * i8_pitch(ix), step,
-                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
-                                                           L.count, overflow, C, first ? 1 : 0);
-        else if (ix->storage == OM_F16)
-          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xh + static_cast<size_t>(pos) * ix->dpad, step,
-                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
-                                                           L.count, overflow, C, first ? 1 : 0);
-        else
-          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(ix->xf + static_cast<size_t>(pos) * ix->d, step,
-                                                           static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand,
-                                                           L.count, overflow, C, first ? 1 : 0);
+        with_rows(ix, [&](const auto* xs) {
+          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf,
+                                                           nqc, ix->d, nqt, L.thr, L.cand, L.count, overflow, C, first ? 1 : 0);
+        });
         OM_CUDA(cudaGetLastError());
       }
     }
@@ -1397,15 +1355,10 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
   {
     Timed t(ix, st, 2);
     const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
-    if (ix->storage == OM_I8)
-      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xq, ix->d, D, I, id_offset, k_out,
+    with_rows(ix, [&](const auto* xs) {
+      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out,
                                                   ix->stage_scores);
-    else if (ix->storage == OM_F16)
-      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xh, ix->d, D, I, id_offset, k_out,
-                                                  ix->stage_scores);
-    else
-      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, ix->xf, ix->d, D, I, id_offset, k_out,
-                                                  ix->stage_scores);
+    });
   }
   OM_CUDA(cudaGetLastError());
   ix->st_launches += 1;
@@ -1421,7 +1374,7 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
 // Merge of nparts [nq, k_in] lists -> [nq, k_out]; more than 8192 entries per query are merged hierarchically.
 int merge_parts(const float* Dp, const int64_t* Ip, int64_t stride_d, int64_t stride_i, int nparts, int nq, int k_in,
                 int k_out, float* D, int64_t* I, cudaStream_t st) {
-  OM_TRY(once_attrs());
+  OM_TRY(once_attrs(nullptr));
   if (k_in > 8192) return fail(OM_EINVAL, "om_topk_merge_n: k_in = %d exceeds 8192", k_in);
   if (static_cast<int64_t>(nparts) * k_in <= 8192) {
     int P = 2;
