@@ -181,7 +181,6 @@ struct EpiBiasActBf16 {
   const float* bias;  // nullable (folded bias W beta + b when the input is normalised)
   int M, N;
   RowNorm norm;
-  static constexpr int kPasses = 1;
   static constexpr bool kPrefetch = false;
   __host__ __device__ static constexpr int smem_bytes(int epi_warps) { return epi_warps * StagedBf16::kBytesPerWarp; }
   struct State {
@@ -233,7 +232,6 @@ struct EpiQKV {
   int M, I2;          // I2 = 2*I
   int valid_rows;     // tokens per attention tile (spt * L)
   RowNorm norm;       // normalisation of the input rows, applied here (see the file header)
-  static constexpr int kPasses = 1;
   static constexpr bool kPrefetch = false;
   __host__ __device__ static constexpr int smem_bytes(int epi_warps) { return epi_warps * StagedBf16::kBytesPerWarp; }
   struct State {
@@ -297,7 +295,6 @@ struct EpiResidNorm {
   int parts;         // column groups per tile (epilogue warps / 4); (N / BN) * parts <= kStatParts
   int M, N;
   int bn;            // tile width (BN of the GEMM): geometry of the static tile schedule, for the L2 prefetch below
-  static constexpr int kPasses = 1;
   static constexpr bool kPrefetch = true;
   static constexpr int kF32Tile = 4096, kBf16Tile = 2048, kPerWarp = kF32Tile + kBf16Tile;
   static constexpr int kMaxN = 1024;     // per-column constants staged in shared memory: 2 * kMaxN floats

@@ -56,10 +56,6 @@ struct GemmCfg {
 //        State object persists across the thread's tiles and finish(State&) is called after the last one
 //   end() runs right after the thread's last chunk: long-latency tails (atomics, global stores) placed there overlap the
 //        next tile's mainloop
-//   static constexpr int kPasses = 1;                          2: the accumulator tile may be read twice:
-//        chunk(..., int pass) runs for pass 0; if need_pass(State&, 1) (warp-uniform) is true, between(State&,
-//        row) and a second sweep with pass 1 follow (the staged tile stays in shared memory until every epilogue thread
-//        is done; the search filter uses this as its overflow path when a thread finds more survivors than its stash holds)
 // Rows >= M and columns >= N contain zeros (TMA out-of-bounds fill) and must be masked by the functor.
 // Named barrier 1 is the functors'; the core uses barrier 2.
 
@@ -202,31 +198,20 @@ gemm_bf16_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_consta
       named_bar_sync(2, 32 * kGemmEpiWarps);
 
       const float* my_row = acc_tile + (ew * 32 + lane) * Cfg::kAccPitch;
+      const int c0 = half * kChunks;
 #pragma unroll 1
-      for (int pass = 0; pass < Epi::kPasses; ++pass) {
-        if constexpr (Epi::kPasses > 1) {
-          if (pass > 0) {
-            if (!epi.need_pass(st, pass)) break;  // warp-uniform decision
-            epi.between(st, row);
-          }
-        }
-        const int c0 = half * kChunks;
-#pragma unroll 1
-        for (int c = c0; c < c0 + kChunks; ++c) {
-          float v[32];
+      for (int c = c0; c < c0 + kChunks; ++c) {
+        float v[32];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 t = *reinterpret_cast<const float4*>(my_row + c * 32 + 4 * i);
-            v[4 * i] = t.x, v[4 * i + 1] = t.y, v[4 * i + 2] = t.z, v[4 * i + 3] = t.w;
-          }
-          const bool has_next = c + 1 < c0 + kChunks;
-          if constexpr (Epi::kPasses > 1)
-            epi.chunk(st, row, n_blk * BN + c * 32, v, pass);
-          else if constexpr (Epi::kPrefetch)
-            epi.chunk(st, row, n_blk * BN + c * 32, v, has_next ? n_blk * BN + (c + 1) * 32 : -1);
-          else
-            epi.chunk(st, row, n_blk * BN + c * 32, v);
+        for (int i = 0; i < 8; ++i) {
+          const float4 t = *reinterpret_cast<const float4*>(my_row + c * 32 + 4 * i);
+          v[4 * i] = t.x, v[4 * i + 1] = t.y, v[4 * i + 2] = t.z, v[4 * i + 3] = t.w;
         }
+        const bool has_next = c + 1 < c0 + kChunks;
+        if constexpr (Epi::kPrefetch)
+          epi.chunk(st, row, n_blk * BN + c * 32, v, has_next ? n_blk * BN + (c + 1) * 32 : -1);
+        else
+          epi.chunk(st, row, n_blk * BN + c * 32, v);
       }
       epi.end(st, row);
     }

@@ -18,14 +18,10 @@
 //               clusters work on neighbouring corpus tiles and the corpus streams from HBM about once.  Every CTA runs
 //               every k block of every tile of its cluster, also when its corpus tile lies past n_cols or its query box
 //               is all padding (TMA zero fill, every column masked): its peers wait on its slices and releases
-//   epilogue    no staging through shared memory: a thread owns two query rows (fragment rows l/4 and l/4 + 8 of its
-//               warp's 16) x 64 corpus columns (8 j + 2 (l % 4) + {0, 1}, j < 32).  One 64-value max per row against the
-//               query's strict threshold rejects the row in the common case; survivors go through a compact bit-mask
-//               loop into a per-thread, double-buffered shared-memory stash.  At the end of a tile the 4 lanes that share
-//               a row reserve their survivors' list slots with ONE atomicAdd (shuffle prefix for the lane offsets); the
-//               atomic's result is consumed one tile later, when the stash is copied to the candidate list, so its L2
-//               round trip hides behind a whole tile of MMA work.  Survivors beyond the stash (dense early rounds) take a
-//               synchronous atomicAdd and are stored at once.  Keys and the overflow flag are those of EpiScan.
+//   epilogue    no staging through shared memory: FragFilter<64> (scan_epilogue.cuh) on the accumulator registers, a
+//               thread owns two query rows x 64 corpus columns.  One 64-value max per row against the query's strict
+//               threshold rejects the row in the common case; survivors go to a double-buffered shared-memory stash and
+//               each quad reserves its list slots with one atomicAdd per row, consumed one tile later
 #pragma once
 #include <cuda_fp16.h>
 
@@ -40,78 +36,11 @@ constexpr int kScanStages = 3;
 constexpr int kScanABytes = kBlockM * kBlockK * 2;           // 16 KB: the CTA's 128 queries
 constexpr int kScanBBytes = kScanBlockN * kBlockK * 2;       // 32 KB: the CTA's corpus tile
 constexpr int kScanStageBytes = kScanABytes + kScanBBytes;
-constexpr int kScanConsumers = 256;                          // two consumer warpgroups
-constexpr int kScanStash = 4;                                // survivors a thread parks per row and tile
+constexpr int kScanConsumers = kStashThreads;                // two consumer warpgroups
 constexpr int kScanStashOffset = kScanStages * kScanStageBytes;
-constexpr int kScanStashBytes = 2 * 2 * kScanStash * kScanConsumers * 8;  // [buffer][row half][slot][thread] keys
-constexpr int kScanBarOffset = kScanStashOffset + kScanStashBytes;
+constexpr int kScanBarOffset = kScanStashOffset + kFragStashBytes;
 constexpr int kScanSmemBytes = kScanBarOffset + 2 * kScanStages * 8 + 1024;  // + slack for 1024-B alignment of the base
 static_assert(kScanSmemBytes <= 232448, "scan ring + stash exceed the 227 KB of shared memory an H100 block may use");
-
-// Value of fragment row H (0: l/4, 1: l/4 + 8) at bit i of the row's 64-bit survivor mask, i = 2 j + b <-> acc[4 j + 2 H + b],
-// for a run-time i without local memory: 6-level select tree (63 SEL).
-template <int H>
-__device__ __forceinline__ float scan_pick(const float (&acc)[128], int i) {
-  float a[32], b[16], c[8], d[4], e[2];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) a[j] = (i & 1) ? acc[4 * j + 2 * H + 1] : acc[4 * j + 2 * H];
-#pragma unroll
-  for (int j = 0; j < 16; ++j) b[j] = (i & 2) ? a[2 * j + 1] : a[2 * j];
-#pragma unroll
-  for (int j = 0; j < 8; ++j) c[j] = (i & 4) ? b[2 * j + 1] : b[2 * j];
-#pragma unroll
-  for (int j = 0; j < 4; ++j) d[j] = (i & 8) ? c[2 * j + 1] : c[2 * j];
-#pragma unroll
-  for (int j = 0; j < 2; ++j) e[j] = (i & 16) ? d[2 * j + 1] : d[2 * j];
-  return (i & 32) ? e[1] : e[0];
-}
-
-// Filter of fragment row H of one tile: returns the number of survivors parked in the stash (<= kScanStash).
-// stash: this thread's slot 0 of (buffer, row H); slot j is at stash[j * kScanConsumers].
-template <int H>
-__device__ __forceinline__ int scan_filter_row(const float (&acc)[128], float t, int row, int lim, int q4, int col0,
-                                               unsigned long long* stash, unsigned long long* cand, int* count,
-                                               int* overflow, int C, uint32_t row_base) {
-  float mx = acc[2 * H];
-#pragma unroll
-  for (int j = 0; j < 32; ++j) mx = fmaxf(mx, fmaxf(acc[4 * j + 2 * H], acc[4 * j + 2 * H + 1]));
-  if (!(mx > t)) return 0;  // common case: nothing in this row's 64 columns beats the threshold
-  // Survivor path.  Kept deliberately COMPACT (a bit mask + a short loop with a select tree): it runs rarely per warp,
-  // so its instructions are cold in the instruction cache and every extra cache line costs hundreds of cycles.
-  uint32_t lo = 0, hi = 0;
-#pragma unroll
-  for (int i = 0; i < 32; ++i) {
-    lo |= (acc[4 * (i >> 1) + 2 * H + (i & 1)] > t ? 1u : 0u) << i;
-    hi |= (acc[4 * (16 + (i >> 1)) + 2 * H + (i & 1)] > t ? 1u : 0u) << i;
-  }
-  unsigned long long mask = (static_cast<unsigned long long>(hi) << 32) | lo;
-  if (lim < kScanBlockN) {  // last corpus tile: columns >= lim hold TMA zero fill, and a zero can beat a negative threshold
-#pragma unroll 1
-    for (int i = 0; i < 64; ++i)
-      if (8 * (i >> 1) + 2 * q4 + (i & 1) >= lim) mask &= ~(1ull << i);
-  }
-  const int n = __popcll(mask);
-  int pos = 0;
-  if (n > kScanStash) {  // more than the stash holds: reserve the excess synchronously
-    pos = atomicAdd(count + row, n - kScanStash);
-    if (pos + (n - kScanStash) > C) *overflow = 1;
-  }
-  unsigned long long* mine = cand + static_cast<size_t>(row) * C;
-  int idx = 0;
-#pragma unroll 1
-  while (mask) {
-    const int i = __ffsll(static_cast<long long>(mask)) - 1;
-    mask &= mask - 1;
-    const unsigned long long key =
-        make_key(scan_pick<H>(acc, i), row_base + static_cast<uint32_t>(col0 + 8 * (i >> 1) + 2 * q4 + (i & 1)));
-    if (idx < kScanStash)
-      stash[idx * kScanConsumers] = key;
-    else if (pos + idx - kScanStash < C)
-      mine[pos + idx - kScanStash] = key;
-    ++idx;
-  }
-  return n < kScanStash ? n : kScanStash;
-}
 
 // Cluster shape CQ x CX and the operand sharing it implies: the one place that knows which CTAs write into which ring
 // and who releases it.  CTA c = (a, b) multicasts its query slice to S_q(c) = {(a, b') : b' < CX} and its corpus slice
@@ -206,26 +135,9 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     // ------------------------------ consumers: wgmma + filter ------------------------------
     const int et = static_cast<int>(threadIdx.x) - kGemmProducerThreads;  // 0 .. 255
     const int wg = et >> 7;                                               // queries [64 wg, +64) of the CTA's 128
-    const int q4 = lane & 3;
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
     Ring<kScanStages> ring;
-    int buf = 0;
-    // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
-    int p_n0 = 0, p_n1 = 0, p_excl0 = 0, p_excl1 = 0, p_pos0 = 0, p_pos1 = 0, p_row = 0, p_buf = 0;
-    auto drain = [&]() {
-      if (!__any_sync(0xffffffffu, (p_n0 | p_n1) != 0)) return;
-      const int b0 = __shfl_sync(0xffffffffu, p_pos0, lane & ~3) + p_excl0;
-      const int b1 = __shfl_sync(0xffffffffu, p_pos1, lane & ~3) + p_excl1;
-      const unsigned long long* s = stash + p_buf * (2 * kScanStash * kScanConsumers) + et;
-      unsigned long long* m0 = cand + static_cast<size_t>(p_row) * C;
-      unsigned long long* m1 = cand + static_cast<size_t>(p_row + 8) * C;
-      for (int j = 0; j < p_n0; ++j)
-        if (b0 + j < C) m0[b0 + j] = s[j * kScanConsumers];
-      for (int j = 0; j < p_n1; ++j)
-        if (b1 + j < C) m1[b1 + j] = s[(kScanStash + j) * kScanConsumers];
-      if ((p_n0 > 0 && b0 + p_n0 > C) || (p_n1 > 0 && b1 + p_n1 > C)) *overflow = 1;
-      p_n0 = p_n1 = 0;
-    };
+    FragFilter<64> filter{stash + et, cand, count, overflow, C, row_base, lane};
 
     // lane 0 of every consumer warp releases a slot on the empty barrier of each CTA of S(c)
     uint32_t peers[Cl::kShare - 1];
@@ -243,6 +155,7 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
       const int m_blk = (tile % qgroups) * CQ + qa;
       const int n_blk = (tile / qgroups) * CX + xb;
       const int row0 = m_blk * kBlockM + frow, row1 = row0 + 8;
+      const int col0 = n_blk * kScanBlockN;
       const float inf = __int_as_float(0x7f800000);
       const float t0 = row0 < nq ? thr[row0] : inf, t1 = row1 < nq ? thr[row1] : inf;
 
@@ -262,36 +175,9 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           release);
       wgmma_fence_regs(acc);
 
-      // ------------------------------ filter on the fragments ------------------------------
-      drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
-      const int col0 = n_blk * kScanBlockN;
-      const int lim = n_cols - col0;  // <= 0: the whole corpus tile lies past n_cols and every column is masked
-      unsigned long long* sb = stash + buf * (2 * kScanStash * kScanConsumers) + et;
-      const int k0 = scan_filter_row<0>(acc, t0, row0, lim, q4, col0, sb, cand, count, overflow, C, row_base);
-      const int k1 = scan_filter_row<1>(acc, t1, row1, lim, q4, col0, sb + kScanStash * kScanConsumers, cand, count,
-                                        overflow, C, row_base);
-      if (__any_sync(0xffffffffu, (k0 | k1) != 0)) {
-        // quad aggregation: lanes 4 i .. 4 i + 3 share both rows; exclusive prefix per lane, one atomic per quad and row
-        int x0 = k0, x1 = k1;
-        int y0 = __shfl_up_sync(0xffffffffu, x0, 1, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 1, 4);
-        if (q4 >= 1) x0 += y0, x1 += y1;
-        y0 = __shfl_up_sync(0xffffffffu, x0, 2, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 2, 4);
-        if (q4 >= 2) x0 += y0, x1 += y1;
-        const int n0 = __shfl_sync(0xffffffffu, x0, lane | 3), n1 = __shfl_sync(0xffffffffu, x1, lane | 3);
-        if (q4 == 0) {
-          if (n0 > 0) p_pos0 = atomicAdd(count + row0, n0);  // result first used by the next drain()
-          if (n1 > 0) p_pos1 = atomicAdd(count + row1, n1);
-        }
-        p_n0 = k0;
-        p_n1 = k1;
-        p_excl0 = x0 - k0;
-        p_excl1 = x1 - k1;
-        p_row = row0;
-        p_buf = buf;
-        buf ^= 1;
-      }
+      filter.tile(acc, t0, t1, row0, col0, n_cols);
     }
-    drain();
+    filter.drain();
   }
 
   __syncthreads();

@@ -13,10 +13,8 @@
 //   score      fp32(s_r * fp32(sig_hi * A_hi + fp32(sig_lo * A_lo))), s_r the row's scale: a few roundings of 2^-24 that
 //              certify_kernel's bound covers (csrc/search.cu)
 //   schedule   persistent, static, queries fastest: every CTA works on neighbouring corpus tiles
-//   filter     as in scan_wide_kernel: a thread owns two query rows (fragment rows l/4, l/4 + 8) x 32 columns; one
-//              32-value max per row against the query's strict threshold, survivors through a bit mask into a
-//              double-buffered stash, one atomicAdd per quad and row whose result is consumed one tile later.  DENSE: every
-//              score stored at position = column
+//   filter     FragFilter<32> (scan_epilogue.cuh) on the combined scores in accumulator fragment order: a thread owns two
+//              query rows x 32 columns, as in scan_wide_kernel.  DENSE: every score stored at position = column
 #pragma once
 #include <stdint.h>
 
@@ -29,53 +27,11 @@ constexpr int kI8BlockN = 128;                        // corpus rows per tile
 constexpr int kI8Stages = 4;
 constexpr int kI8BoxBytes = kBlockM * kI8BlockK;      // 16 KB: 128 rows of one operand
 constexpr int kI8StageBytes = 3 * kI8BoxBytes;        // q_hi, q_lo, corpus
-constexpr int kI8Consumers = 256;                     // two consumer warpgroups
-constexpr int kI8Stash = 4;                           // survivors a thread parks per row and tile
+constexpr int kI8Consumers = kStashThreads;           // two consumer warpgroups
 constexpr int kI8StashOffset = kI8Stages * kI8StageBytes;
-constexpr int kI8StashBytes = 2 * 2 * kI8Stash * kI8Consumers * 8;  // [buffer][row half][slot][thread] keys
-constexpr int kI8BarOffset = kI8StashOffset + kI8StashBytes;
+constexpr int kI8BarOffset = kI8StashOffset + kFragStashBytes;
 constexpr int kI8SmemBytes = kI8BarOffset + 2 * kI8Stages * 8 + 1024;  // + slack for 1024-B alignment of the base
 static_assert(kI8SmemBytes <= 232448, "int8 scan ring + stash exceed the 227 KB of shared memory an H100 block may use");
-
-// Filter of one fragment row (v[i] = column 8 (i >> 1) + 2 q4 + (i & 1) of the tile): returns the number of survivors
-// parked in the stash (<= kI8Stash).  stash: this thread's slot 0 of (buffer, row); slot j is at stash[j * kI8Consumers].
-__device__ __forceinline__ int scan_i8_filter_row(const float (&v)[32], float t, int row, int lim, int q4, int col0,
-                                                  unsigned long long* stash, unsigned long long* cand, int* count,
-                                                  int* overflow, int C, uint32_t row_base) {
-  float mx = v[0];
-#pragma unroll
-  for (int i = 1; i < 32; ++i) mx = fmaxf(mx, v[i]);
-  if (!(mx > t)) return 0;  // common case
-  uint32_t mask = 0;
-#pragma unroll
-  for (int i = 0; i < 32; ++i) mask |= (v[i] > t ? 1u : 0u) << i;
-  if (lim < kI8BlockN) {  // last corpus tile: columns >= lim score 0 (zero scale), which can beat a negative threshold
-#pragma unroll 1
-    for (int i = 0; i < 32; ++i)
-      if (8 * (i >> 1) + 2 * q4 + (i & 1) >= lim) mask &= ~(1u << i);
-  }
-  const int n = __popc(mask);
-  int pos = 0;
-  if (n > kI8Stash) {  // more than the stash holds: reserve the excess synchronously
-    pos = atomicAdd(count + row, n - kI8Stash);
-    if (pos + (n - kI8Stash) > C) *overflow = 1;
-  }
-  unsigned long long* mine = cand + static_cast<size_t>(row) * C;
-  int idx = 0;
-#pragma unroll 1
-  while (mask) {
-    const int i = __ffs(mask) - 1;
-    mask &= mask - 1;
-    const unsigned long long key =
-        make_key(EpiScan<false>::pick32(v, i), row_base + static_cast<uint32_t>(col0 + 8 * (i >> 1) + 2 * q4 + (i & 1)));
-    if (idx < kI8Stash)
-      stash[idx * kI8Consumers] = key;
-    else if (pos + idx - kI8Stash < C)
-      mine[pos + idx - kI8Stash] = key;
-    ++idx;
-  }
-  return n < kI8Stash ? n : kI8Stash;
-}
 
 template <bool DENSE>
 __global__ void __launch_bounds__(kGemmProducerThreads + kI8Consumers, 1)
@@ -131,23 +87,7 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
     const int q4 = lane & 3;
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
     Ring<kI8Stages> ring;
-    int buf = 0;
-    // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
-    int p_n0 = 0, p_n1 = 0, p_excl0 = 0, p_excl1 = 0, p_pos0 = 0, p_pos1 = 0, p_row = 0, p_buf = 0;
-    auto drain = [&]() {
-      if (!__any_sync(0xffffffffu, (p_n0 | p_n1) != 0)) return;
-      const int b0 = __shfl_sync(0xffffffffu, p_pos0, lane & ~3) + p_excl0;
-      const int b1 = __shfl_sync(0xffffffffu, p_pos1, lane & ~3) + p_excl1;
-      const unsigned long long* s = stash + p_buf * (2 * kI8Stash * kI8Consumers) + et;
-      unsigned long long* m0 = cand + static_cast<size_t>(p_row) * C;
-      unsigned long long* m1 = cand + static_cast<size_t>(p_row + 8) * C;
-      for (int j = 0; j < p_n0; ++j)
-        if (b0 + j < C) m0[b0 + j] = s[j * kI8Consumers];
-      for (int j = 0; j < p_n1; ++j)
-        if (b1 + j < C) m1[b1 + j] = s[(kI8Stash + j) * kI8Consumers];
-      if ((p_n0 > 0 && b0 + p_n0 > C) || (p_n1 > 0 && b1 + p_n1 > C)) *overflow = 1;
-      p_n0 = p_n1 = 0;
-    };
+    FragFilter<32> filter{stash + et, cand, count, overflow, C, row_base, lane};
     auto release = [&](uint32_t s) {
       if (lane == 0) mbar_arrive(&empty_bar[s]);
     };
@@ -192,15 +132,15 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
       wgmma_fence_regs(ah);
       wgmma_fence_regs(al);
 
-      // combined scores of fragment rows frow (v0) and frow + 8 (v1): v_H[2 j + b] = accumulator [4 j + 2 H + b]
-      float v0[32], v1[32];
+      // combined scores in accumulator fragment order: v[4 j + 2 H + b] is fragment row frow + 8 H, column 8 j + 2 q4 + b
+      float v[64];
 #pragma unroll
       for (int j = 0; j < 16; ++j)
 #pragma unroll
         for (int b = 0; b < 2; ++b) {
           const int i = 2 * j + b;
-          v0[i] = __fmul_rn(sc[i], __fmaf_rn(g0.x, static_cast<float>(ah[4 * j + b]), __fmul_rn(g0.y, static_cast<float>(al[4 * j + b]))));
-          v1[i] = __fmul_rn(sc[i], __fmaf_rn(g1.x, static_cast<float>(ah[4 * j + 2 + b]), __fmul_rn(g1.y, static_cast<float>(al[4 * j + 2 + b]))));
+          v[4 * j + b] = __fmul_rn(sc[i], __fmaf_rn(g0.x, static_cast<float>(ah[4 * j + b]), __fmul_rn(g0.y, static_cast<float>(al[4 * j + b]))));
+          v[4 * j + 2 + b] = __fmul_rn(sc[i], __fmaf_rn(g1.x, static_cast<float>(ah[4 * j + 2 + b]), __fmul_rn(g1.y, static_cast<float>(al[4 * j + 2 + b]))));
         }
 
       if constexpr (DENSE) {  // first round: every score at position = column
@@ -212,41 +152,15 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
 #pragma unroll
           for (int i = 0; i < 32; ++i) {
             const int c = col0 + 8 * (i >> 1) + 2 * q4 + (i & 1);
-            if (c < n_cols) mine[c] = make_key(h ? v1[i] : v0[i], row_base + static_cast<uint32_t>(c));
+            const int r = 4 * (i >> 1) + (i & 1);
+            if (c < n_cols) mine[c] = make_key(h ? v[r + 2] : v[r], row_base + static_cast<uint32_t>(c));
           }
         }
         continue;
       }
-
-      // ------------------------------ filter on the fragments ------------------------------
-      drain();  // the previous tile's survivors: their atomic was issued a whole tile ago
-      const int lim = n_cols - col0;
-      unsigned long long* sb = stash + buf * (2 * kI8Stash * kI8Consumers) + et;
-      const int k0 = scan_i8_filter_row(v0, t0, row0, lim, q4, col0, sb, cand, count, overflow, C, row_base);
-      const int k1 = scan_i8_filter_row(v1, t1, row1, lim, q4, col0, sb + kI8Stash * kI8Consumers, cand, count, overflow,
-                                        C, row_base);
-      if (__any_sync(0xffffffffu, (k0 | k1) != 0)) {
-        // quad aggregation: lanes 4 i .. 4 i + 3 share both rows; exclusive prefix per lane, one atomic per quad and row
-        int x0 = k0, x1 = k1;
-        int y0 = __shfl_up_sync(0xffffffffu, x0, 1, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 1, 4);
-        if (q4 >= 1) x0 += y0, x1 += y1;
-        y0 = __shfl_up_sync(0xffffffffu, x0, 2, 4), y1 = __shfl_up_sync(0xffffffffu, x1, 2, 4);
-        if (q4 >= 2) x0 += y0, x1 += y1;
-        const int n0 = __shfl_sync(0xffffffffu, x0, lane | 3), n1 = __shfl_sync(0xffffffffu, x1, lane | 3);
-        if (q4 == 0) {
-          if (n0 > 0) p_pos0 = atomicAdd(count + row0, n0);  // result first used by the next drain()
-          if (n1 > 0) p_pos1 = atomicAdd(count + row1, n1);
-        }
-        p_n0 = k0;
-        p_n1 = k1;
-        p_excl0 = x0 - k0;
-        p_excl1 = x1 - k1;
-        p_row = row0;
-        p_buf = buf;
-        buf ^= 1;
-      }
+      filter.tile(v, t0, t1, row0, col0, n_cols);
     }
-    drain();
+    filter.drain();
   }
 
   __syncthreads();

@@ -122,6 +122,53 @@ def test_int8_index_with_k_beyond_its_rows(om):
         assert (Iq[:, 3000:] == -1).all() and (Iq[:, :3000] >= 0).all()
 
 
+def _dequantised_pair(om, x):
+    q8 = om.FlatIPIndex(x.shape[1], dtype=torch.int8)
+    q8.add(x)
+    f = om.FlatIPIndex(x.shape[1])
+    f.add(torch.cat(list(q8.rows_f32())))
+    return q8, f
+
+
+@pytest.mark.parametrize("nq", [9, 300])
+def test_int8_massive_ties(om, nq):
+    # 0/1 data: scores take a handful of values, so tie order decides almost every rank and a thread's row of a tile
+    # holds more survivors than its stash parks
+    rng = np.random.default_rng(7 + nq)
+    x = rng.integers(0, 2, (30000, 64)).astype(np.float32)
+    q = rng.integers(0, 2, (nq, 64)).astype(np.float32)
+    q8, f = _dequantised_pair(om, x)
+    for k in (1, 64, 1000):
+        Dq, Iq, _ = _search(q8, q, k)
+        Df, If, _ = _search(f, q, k)
+        _same(Iq, If, "I k=%d" % k)
+        _same(Dq, Df, "D k=%d" % k)
+
+
+@pytest.mark.parametrize("nq", [3, 300])
+def test_int8_sorted_corpus_forces_overflow_retry(om, nq):
+    # every later row beats every earlier row for every query: each tile's survivors exceed the stash, the doubling
+    # schedule overflows its candidate lists and the overflow-proof schedule must take over.  Column 0 at 127 gives
+    # every row scale 1, so the codes are the rows and every score m * v is exact
+    n, d = 60000, 64
+    v = np.arange(n) // 4  # ascending scores with 4-way ties
+    x = np.zeros((n, d), np.float32)
+    x[:, 0], x[:, 1], x[:, 2] = 127, v // 127, v % 127
+    m = np.arange(nq) % 3 + 1
+    q = np.zeros((nq, d), np.float32)
+    q[:, 1], q[:, 2] = 127 * m, m
+    q8, f = _dequantised_pair(om, x)
+    _check_stored(q8, x, "sorted corpus")
+    Dq, Iq, _ = _search(q8, q, 100)
+    assert q8.stat("overflow_retries") >= 1
+    Df, If, _ = _search(f, q, 100)
+    _same(Iq, If, "I")
+    _same(Dq, Df, "D")
+    Dq, Iq, _ = _search(q8, q, 100, force_safe_rounds=1)
+    _same(Iq, If, "I safe rounds")
+    _same(Dq, Df, "D safe rounds")
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # stored codes and scales == the CPU oracle, every ingest route
 # ---------------------------------------------------------------------------------------------------------------------
