@@ -235,6 +235,32 @@ void om_comm_destroy(om_comm* comm);
 int om_index_search_sharded(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D,
                             int64_t* I, om_memkind out_kind, int64_t id_offset, void* stream);
 
+/* Filtered search: the exact top-k, by fp32 inner product over the stored rows, among the rows the bitmap allows and the
+ * query does not exclude; ties by ascending id.  D and I are bitwise what om_index_search returns on an index built from
+ * the eligible rows only, with ids mapped back; fewer than k eligible rows leave id -1 and score -FLT_MAX slots.
+ *   allow_bits       nullable, device: bit (r & 31) of word r >> 5 set = local row r may be returned
+ *   allow_words      >= ceil(ntotal / 32) when allow_bits is given; bits past ntotal are ignored
+ *   exclude_offsets  nullable, device [nq + 1]: CSR over the queries, non-decreasing; at most 128 ids per query
+ *   exclude_ids      device: ids in the result id space (id_offset + local row), >= 0, any order, duplicates allowed; an
+ *                    id outside [id_offset, id_offset + ntotal) is ignored, so every rank of a sharded search takes the
+ *                    same CSR
+ * A rule broken returns OM_EINVAL before any output is written.  A null filter, or one with both parts null, is
+ * om_index_search / om_index_search_sharded.  The filter buffers are read on `stream`; everything else (tunables, the
+ * synchronous return, the refusal of non-finite rows) is as for the unfiltered calls.  Sharded: allow_bits covers this
+ * rank's rows; every rank calls om_index_search_sharded_filtered, and a rank may pass a null or empty filter while others
+ * pass one (with more than one rank the filters are always checked together, one all-reduce). */
+typedef struct om_search_filter {
+  const uint32_t* allow_bits;
+  int64_t allow_words;
+  const int64_t* exclude_offsets;
+  const int64_t* exclude_ids;
+} om_search_filter;
+int om_index_search_filtered(om_index* idx, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
+                             om_memkind out_kind, int64_t id_offset, const om_search_filter* filter, void* stream);
+int om_index_search_sharded_filtered(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
+                                     float* D, int64_t* I, om_memkind out_kind, int64_t id_offset,
+                                     const om_search_filter* filter, void* stream);
+
 /* Tunables: "rescore_slack" (extra candidate-stage rows kept per query; default max(128, k/5)),
  * "force_safe_rounds" (1 = always use the overflow-proof fixed-size round schedule; testing),
  * "round_growth" (2..8: each scan round covers (g-1) x the rows already seen; default 0 = auto: 2, or 8 for <= 256 queries),

@@ -26,6 +26,12 @@ class EncoderDesc(ctypes.Structure):
                 ("rel_buckets", c_int32), ("rel_max_distance", c_int32), ("max_batch_tokens", c_int32)]
 
 
+class SearchFilter(ctypes.Structure):
+    """om_search_filter: device pointers (0 = absent) of the allowed-row bitmap and of the exclusion CSR."""
+    _fields_ = [("allow_bits", c_void_p), ("allow_words", c_int64), ("exclude_offsets", c_void_p),
+                ("exclude_ids", c_void_p)]
+
+
 # name -> (restype, argtypes); must list every symbol of include/openmatch_b200.h
 SIGNATURES = {
     "om_abi_version": (c_int, []),
@@ -59,6 +65,10 @@ SIGNATURES = {
     "om_comm_destroy": (None, [c_void_p]),
     "om_index_search_sharded": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int,
                                         c_int64, c_void_p]),
+    "om_index_search_filtered": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int64,
+                                         POINTER(SearchFilter), c_void_p]),
+    "om_index_search_sharded_filtered": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p,
+                                                 c_int, c_int64, POINTER(SearchFilter), c_void_p]),
     "om_index_set_param": (c_int, [c_void_p, c_char_p, c_int64]),
     "om_index_get_stat": (c_int64, [c_void_p, c_char_p]),
     "om_index_destroy": (None, [c_void_p]),

@@ -126,6 +126,23 @@ __device__ __forceinline__ int park(const float (&v)[N], SurvivorMask<N> mask, C
   return idx < S ? idx : S;
 }
 
+// Filtered search: the bits of mask whose corpus row row_base + col(i) the allowed-row bitmap keeps (bit r & 31 of word
+// r >> 5 set = row r may be returned).  Called on the survivor path only, after the max test, so a round reads the bitmap
+// for the few rows that beat their query's threshold; the rows of masked-out columns are never read.
+template <int N, class Col>
+__device__ __forceinline__ SurvivorMask<N> allowed(SurvivorMask<N> mask, const uint32_t* allow, uint32_t row_base, Col col) {
+  SurvivorMask<N> keep = 0;
+#pragma unroll 1
+  while (mask) {
+    const int i = mask_ffs(mask) - 1;
+    const SurvivorMask<N> bit = static_cast<SurvivorMask<N>>(1) << i;
+    mask &= ~bit;
+    const uint32_t r = row_base + static_cast<uint32_t>(col(i));
+    if ((__ldg(allow + (r >> 5)) >> (r & 31)) & 1u) keep |= bit;
+  }
+  return keep;
+}
+
 // Copies n parked keys (slot j at stash[j * kStashThreads]) to list[pos ...], whose slots an atomicAdd reserved.
 __device__ __forceinline__ void drain_stash(const unsigned long long* stash, int n, unsigned long long* list, int pos,
                                             int C, int* overflow) {
@@ -145,7 +162,8 @@ __device__ __forceinline__ void drain_stash(const unsigned long long* stash, int
 constexpr int kFragStash = 4;  // survivors a thread parks per row and tile
 constexpr int kFragStashBytes = 2 * 2 * kFragStash * kStashThreads * 8;
 
-template <int COLS>
+// ALLOW: filtered search, survivors are also masked by the allowed-row bitmap `allow` (see allowed()).
+template <int COLS, bool ALLOW = false>
 struct FragFilter {
   unsigned long long* stash;  // this thread's slot 0 of buffer 0, row half 0
   unsigned long long* cand;
@@ -154,6 +172,7 @@ struct FragFilter {
   int C;
   uint32_t row_base;
   int lane;
+  const uint32_t* allow = nullptr;
   int buf = 0;
   // reservation in flight: p_n[h] keys of stash buffer p_buf go to query p_row + 8 h at (quad leader's p_pos[h]) + p_excl[h]
   int p_n[2] = {0, 0}, p_excl[2] = {0, 0}, p_pos[2] = {0, 0}, p_row = 0, p_buf = 0;
@@ -174,6 +193,7 @@ struct FragFilter {
       for (int i = 0; i < COLS; ++i)
         if (col(i) >= lim) mask &= ~(static_cast<SurvivorMask<COLS>>(1) << i);
     }
+    if constexpr (ALLOW) mask = allowed<COLS>(mask, allow, row_base, [&](int i) { return col0 + col(i); });
     return park<kFragStash>(v, mask, [&](int i) { return col0 + col(i); }, 0, sb, row, cand, count, overflow, C,
                             row_base);
   }
@@ -222,8 +242,17 @@ struct FragFilter {
 // DENSE: first round, every score is stored at position = column (no threshold yet).  Otherwise the survivor protocol
 // above with a stash of kStash keys per thread and tile; the thread owns a whole row, so it reserves its own slots.
 // Everything is force-inlined and State never has its address taken, so it lives in registers.
-template <bool DENSE>
-struct EpiScan {
+// ALLOW (threshold rounds only): filtered search, survivors are also masked by the allowed-row bitmap of the base.  The
+// base is empty otherwise, so the functor's layout, and the kernel parameters behind it, stay those of the plain scan.
+template <bool ALLOW>
+struct ScanAllow {};
+template <>
+struct ScanAllow<true> {
+  const uint32_t* allow;  // allowed-row bitmap over the rows of the index shard
+};
+template <bool DENSE, bool ALLOW = false>
+struct EpiScan : ScanAllow<ALLOW> {
+  static_assert(!(DENSE && ALLOW), "a filtered first round runs as a threshold round at -inf");
   const float* thr;          // [nq] strict lower bound per query
   unsigned long long* cand;  // [nq, C]
   int* count;                // [nq]
@@ -297,6 +326,7 @@ struct EpiScan {
     if (!mask) return;  // common case: nothing in this chunk beats the threshold
     const int lim = n_cols - col0;  // columns >= lim are out of range (only in the last tile)
     if (lim < 32) mask &= (1u << lim) - 1u;
+    if constexpr (ALLOW) mask = allowed<32>(mask, this->allow, row_base + col0, [](int i) { return i; });
     s.k = park<kStash>(v, mask, [&](int i) { return col0 + i; }, s.k, slot0(s, s.buf), row, cand, count, overflow, C,
                        row_base);
   }

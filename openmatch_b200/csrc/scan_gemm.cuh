@@ -25,6 +25,8 @@
 #pragma once
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "scan_epilogue.cuh"
 
 namespace om {
@@ -76,11 +78,12 @@ struct ScanCluster {
   }
 };
 
-template <int CQ, int CX>
+// ALLOW: filtered search, survivors are also masked by the allowed-row bitmap `allow` (unread otherwise).
+template <int CQ, int CX, bool ALLOW>
 __global__ void __launch_bounds__(kGemmProducerThreads + kScanConsumers, 1)
 scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmX, int K,
                  const float* __restrict__ thr, unsigned long long* cand, int* count, int* overflow, int nq, int n_cols,
-                 int C, uint32_t row_base) {
+                 int C, uint32_t row_base, const uint32_t* __restrict__ allow) {
   using Cl = ScanCluster<CQ, CX>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -137,7 +140,7 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const int wg = et >> 7;                                               // queries [64 wg, +64) of the CTA's 128
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
     Ring<kScanStages> ring;
-    FragFilter<64> filter{stash + et, cand, count, overflow, C, row_base, lane};
+    FragFilter<64, ALLOW> filter{stash + et, cand, count, overflow, C, row_base, lane, allow};
 
     // lane 0 of every consumer warp releases a slot on the empty barrier of each CTA of S(c)
     uint32_t peers[Cl::kShare - 1];
@@ -186,13 +189,13 @@ scan_wide_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
 // Clusters of the CQ x CX scan that are co-resident on the device (cached per shape, one device per process); 0 when
 // none fits.  The persistent schedule wants every cluster co-resident (a second wave would double the run time).
-template <int CQ, int CX>
+template <int CQ, int CX, bool ALLOW>
 static inline cudaError_t scan_wide_max_clusters(int num_sms, int* out) {
   static int max_clusters = -1;
   if (max_clusters < 0) {
     constexpr int kSize = ScanCluster<CQ, CX>::kSize;
     cudaError_t e =
-        cudaFuncSetAttribute(scan_wide_kernel<CQ, CX>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmemBytes);
+        cudaFuncSetAttribute(scan_wide_kernel<CQ, CX, ALLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kScanSmemBytes);
     if (e != cudaSuccess) return e;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(kSize * (num_sms / kSize));
@@ -204,7 +207,7 @@ static inline cudaError_t scan_wide_max_clusters(int num_sms, int* out) {
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     int n = 0;
-    e = cudaOccupancyMaxActiveClusters(&n, scan_wide_kernel<CQ, CX>, &cfg);
+    e = cudaOccupancyMaxActiveClusters(&n, scan_wide_kernel<CQ, CX, ALLOW>, &cfg);
     if (e != cudaSuccess) return e;
     max_clusters = n < num_sms / kSize ? n : num_sms / kSize;
   }
@@ -212,10 +215,11 @@ static inline cudaError_t scan_wide_max_clusters(int num_sms, int* out) {
   return cudaSuccess;
 }
 
-template <int CQ, int CX>
+template <int CQ, int CX, bool ALLOW>
 static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const __half* X, int64_t ldx, int nq, int n_cols,
                                            int K, const float* thr, unsigned long long* cand, int* count, int* overflow,
-                                           int C, uint32_t row_base, int num_sms, cudaStream_t stream) {
+                                           int C, uint32_t row_base, const uint32_t* allow, int num_sms,
+                                           cudaStream_t stream) {
   using Cl = ScanCluster<CQ, CX>;
   CUtensorMap tmQ, tmX;
   if (make_tmap_bf16_2d(&tmQ, Q, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq * 2, kBlockK, Cl::kQRows) != 0)
@@ -223,7 +227,7 @@ static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const _
   if (make_tmap_bf16_2d(&tmX, X, (uint64_t)K, (uint64_t)n_cols, (uint64_t)ldx * 2, kBlockK, Cl::kXRows) != 0)
     return cudaErrorInvalidValue;
   int max_clusters = 0;
-  cudaError_t e = scan_wide_max_clusters<CQ, CX>(num_sms, &max_clusters);
+  cudaError_t e = scan_wide_max_clusters<CQ, CX, ALLOW>(num_sms, &max_clusters);
   if (e != cudaSuccess) return e;
   if (max_clusters < 1) return cudaErrorNotSupported;
   cudaLaunchConfig_t cfg = {};
@@ -239,39 +243,47 @@ static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const _
   const int64_t num_tiles = static_cast<int64_t>(qgroups) * ((n_cols + CX * kScanBlockN - 1) / (CX * kScanBlockN));
   const int clusters = num_tiles < max_clusters ? static_cast<int>(num_tiles) : max_clusters;
   cfg.gridDim = dim3(Cl::kSize * clusters);
-  return cudaLaunchKernelEx(&cfg, scan_wide_kernel<CQ, CX>, tmQ, tmX, K, thr, cand, count, overflow, nq, n_cols, C,
-                            row_base);
+  return cudaLaunchKernelEx(&cfg, scan_wide_kernel<CQ, CX, ALLOW>, tmQ, tmX, K, thr, cand, count, overflow, nq, n_cols, C,
+                            row_base, allow);
 }
 
 // Host launcher of the wide scan on cq x cx clusters (cq in {2, 4}, cx in {1, 2}).  Q: [nq, K] fp16 queries, row pitch
 // ldq elements; X: [n_cols, K] fp16 corpus rows, row pitch ldx.  Survivors (score > thr[q]) are appended to
-// cand[q * C ...] as make_key(score, row_base + column); a list that would grow beyond C sets *overflow.  Every shape
+// cand[q * C ...] as make_key(score, row_base + column); a list that would grow beyond C sets *overflow.  allow: nullptr, or
+// the allowed-row bitmap of a filtered search (indexed by row_base + column), which survivors must also pass.  Every shape
 // computes each score with the same wgmma sequence, so the candidate lists hold the same keys whatever the shape.
 // Returns cudaSuccess / a CUDA error; tensor-map failures and other shapes map to cudaErrorInvalidValue, and
 // cudaErrorNotSupported means that no cluster of the shape fits on the device.
 static inline cudaError_t launch_scan_cluster(int cq, int cx, const __half* Q, int64_t ldq, const __half* X, int64_t ldx,
                                               int nq, int n_cols, int K, const float* thr, unsigned long long* cand,
-                                              int* count, int* overflow, int C, uint32_t row_base, int num_sms,
-                                              cudaStream_t stream) {
+                                              int* count, int* overflow, int C, uint32_t row_base, const uint32_t* allow,
+                                              int num_sms, cudaStream_t stream) {
   if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
-  if (cq == 2 && cx == 1)
-    return launch_scan_wide<2, 1>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
-  if (cq == 4 && cx == 1)
-    return launch_scan_wide<4, 1>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
-  if (cq == 2 && cx == 2)
-    return launch_scan_wide<2, 2>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
-  if (cq == 4 && cx == 2)
-    return launch_scan_wide<4, 2>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base, num_sms, stream);
+  auto launch = [&](auto cq_c, auto cx_c) {
+    constexpr int CQ = decltype(cq_c)::value, CX = decltype(cx_c)::value;
+    return allow ? launch_scan_wide<CQ, CX, true>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base,
+                                                  allow, num_sms, stream)
+                 : launch_scan_wide<CQ, CX, false>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base,
+                                                   nullptr, num_sms, stream);
+  };
+  using I1 = std::integral_constant<int, 1>;
+  using I2 = std::integral_constant<int, 2>;
+  using I4 = std::integral_constant<int, 4>;
+  if (cq == 2 && cx == 1) return launch(I2{}, I1{});
+  if (cq == 4 && cx == 1) return launch(I4{}, I1{});
+  if (cq == 2 && cx == 2) return launch(I2{}, I2{});
+  if (cq == 4 && cx == 2) return launch(I4{}, I2{});
   return cudaErrorInvalidValue;
 }
 
-// Co-resident clusters of the cq x cx scan on this device (0 when none fits, -1 for another shape).
-static inline cudaError_t scan_cluster_capacity(int cq, int cx, int num_sms, int* out) {
+// Co-resident clusters of the cq x cx scan on this device (0 when none fits, -1 for another shape); filtered: of its
+// bitmap variant.
+static inline cudaError_t scan_cluster_capacity(int cq, int cx, bool filtered, int num_sms, int* out) {
   *out = -1;
-  if (cq == 2 && cx == 1) return scan_wide_max_clusters<2, 1>(num_sms, out);
-  if (cq == 4 && cx == 1) return scan_wide_max_clusters<4, 1>(num_sms, out);
-  if (cq == 2 && cx == 2) return scan_wide_max_clusters<2, 2>(num_sms, out);
-  if (cq == 4 && cx == 2) return scan_wide_max_clusters<4, 2>(num_sms, out);
+  if (cq == 2 && cx == 1) return filtered ? scan_wide_max_clusters<2, 1, true>(num_sms, out) : scan_wide_max_clusters<2, 1, false>(num_sms, out);
+  if (cq == 4 && cx == 1) return filtered ? scan_wide_max_clusters<4, 1, true>(num_sms, out) : scan_wide_max_clusters<4, 1, false>(num_sms, out);
+  if (cq == 2 && cx == 2) return filtered ? scan_wide_max_clusters<2, 2, true>(num_sms, out) : scan_wide_max_clusters<2, 2, false>(num_sms, out);
+  if (cq == 4 && cx == 2) return filtered ? scan_wide_max_clusters<4, 2, true>(num_sms, out) : scan_wide_max_clusters<4, 2, false>(num_sms, out);
   return cudaSuccess;
 }
 

@@ -33,12 +33,14 @@ constexpr int kI8BarOffset = kI8StashOffset + kFragStashBytes;
 constexpr int kI8SmemBytes = kI8BarOffset + 2 * kI8Stages * 8 + 1024;  // + slack for 1024-B alignment of the base
 static_assert(kI8SmemBytes <= 232448, "int8 scan ring + stash exceed the 227 KB of shared memory an H100 block may use");
 
-template <bool DENSE>
+// ALLOW (threshold rounds only): filtered search, survivors are also masked by the allowed-row bitmap `allow`.
+template <bool DENSE, bool ALLOW>
 __global__ void __launch_bounds__(kGemmProducerThreads + kI8Consumers, 1)
 scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__ CUtensorMap tmQl,
                const __grid_constant__ CUtensorMap tmX, int K, const int8_t* __restrict__ xrows, int64_t pitch, int dpad,
                const float2* __restrict__ qsig, const float* __restrict__ thr, unsigned long long* cand, int* count,
-               int* overflow, int nq, int n_cols, int C, uint32_t row_base) {
+               int* overflow, int nq, int n_cols, int C, uint32_t row_base, const uint32_t* __restrict__ allow) {
+  static_assert(!(DENSE && ALLOW), "a filtered first round runs as a threshold round at -inf");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   unsigned long long* stash = reinterpret_cast<unsigned long long*>(smem + kI8StashOffset);
@@ -87,7 +89,7 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
     const int q4 = lane & 3;
     const int frow = 64 * wg + 16 * (warp & 3) + (lane >> 2);             // fragment rows frow, frow + 8
     Ring<kI8Stages> ring;
-    FragFilter<32> filter{stash + et, cand, count, overflow, C, row_base, lane};
+    FragFilter<32, ALLOW> filter{stash + et, cand, count, overflow, C, row_base, lane, allow};
     auto release = [&](uint32_t s) {
       if (lane == 0) mbar_arrive(&empty_bar[s]);
     };
@@ -169,13 +171,15 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
 // Host launcher.  Qh, Ql: [nq, K] int8 query splits, row pitch ldq bytes; qsig [nq] (sig_hi, sig_lo); X: the corpus rows of
 // the round, [n_cols] rows of pitch `pitch` bytes with the scale at byte dpad.  DENSE: every score goes to
 // cand[q * C + column]; otherwise survivors (score > thr[q]) are appended as make_key(score, row_base + column) and a
-// list that would grow beyond C sets *overflow.  Returns cudaSuccess / a CUDA error (tensor-map failures:
+// list that would grow beyond C sets *overflow.  ALLOW: survivors must also pass the allowed-row bitmap `allow` (indexed by
+// row_base + column).  Returns cudaSuccess / a CUDA error (tensor-map failures:
 // cudaErrorInvalidValue).
-template <bool DENSE>
+template <bool DENSE, bool ALLOW = false>
 static inline cudaError_t launch_scan_i8(const int8_t* Qh, const int8_t* Ql, int64_t ldq, const float2* qsig,
                                          const int8_t* X, int64_t pitch, int dpad, int nq, int n_cols, int K,
                                          const float* thr, unsigned long long* cand, int* count, int* overflow, int C,
-                                         uint32_t row_base, int num_sms, cudaStream_t stream) {
+                                         uint32_t row_base, int num_sms, cudaStream_t stream,
+                                         const uint32_t* allow = nullptr) {
   if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
   CUtensorMap tmQh, tmQl, tmX;
   if (make_tmap_2d(&tmQh, Qh, 1, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq, kI8BlockK, kBlockM, 128) != 0 ||
@@ -184,15 +188,15 @@ static inline cudaError_t launch_scan_i8(const int8_t* Qh, const int8_t* Ql, int
     return cudaErrorInvalidValue;
   static bool attr_set = false;  // per instantiation
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(scan_i8_kernel<DENSE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kI8SmemBytes);
+    cudaError_t e = cudaFuncSetAttribute(scan_i8_kernel<DENSE, ALLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kI8SmemBytes);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
   const int64_t num_tiles =
       static_cast<int64_t>((nq + kBlockM - 1) / kBlockM) * ((n_cols + kI8BlockN - 1) / kI8BlockN);
   const int grid = static_cast<int>(num_tiles < num_sms ? num_tiles : num_sms);
-  scan_i8_kernel<DENSE><<<grid, kGemmProducerThreads + kI8Consumers, kI8SmemBytes, stream>>>(
-      tmQh, tmQl, tmX, K, X, pitch, dpad, qsig, thr, cand, count, overflow, nq, n_cols, C, row_base);
+  scan_i8_kernel<DENSE, ALLOW><<<grid, kGemmProducerThreads + kI8Consumers, kI8SmemBytes, stream>>>(
+      tmQh, tmQl, tmX, K, X, pitch, dpad, qsig, thr, cand, count, overflow, nq, n_cols, C, row_base, allow);
   return cudaGetLastError();
 }
 

@@ -250,14 +250,42 @@ struct StoredRow<int8_t> {
   __device__ bool finite(float) const { return isfinite(s); }
 };
 
+// Excluded ids of a filtered search: CSR offsets over the caller's queries and ids in the result id space (id_offset +
+// local row).  Query q of a launch is the caller's query qmap[q_base + q] (an escalation level's sub-batch), or q_base + q
+// without a map.  At most kMaxExcluded ids per query, the smallest re-score slack: a full first-level list then still
+// holds k rows that are not excluded.
+constexpr int kMaxExcluded = 128;
+struct Excluded {
+  const int64_t* off;  // nullptr: no exclusions
+  const int64_t* ids;
+  const int* qmap;
+  int q_base;
+  int64_t id_offset;
+  // Query q's excluded ids as local rows in s[0], s[stride], ... s[(n - 1) stride], loaded by threads tid, tid + nthreads,
+  // ...; returns n.  An id outside [id_offset, id_offset + 2^32 - 1) becomes 0xffffffff, which is no row of a shard.
+  __device__ int load(int q, uint32_t* s, int stride, int tid, int nthreads) const {
+    if (!off) return 0;
+    const int g = qmap ? qmap[q_base + q] : q_base + q;
+    const int64_t a = off[g];
+    const int n = static_cast<int>(off[g + 1] - a);
+    for (int i = tid; i < n; i += nthreads) {
+      const int64_t r = ids[a + i] - id_offset;
+      s[i * stride] = (r >= 0 && r < 0xffffffffll) ? static_cast<uint32_t>(r) : 0xffffffffu;
+    }
+    return n;
+  }
+};
+
 // FINAL: one CTA per query: exact fp32 re-score of the candidates against the stored rows (fp32 master rows or fp16
 // rows), sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row
 // gathers are HBM-bound and want every warp resident.
-template <typename RowT>
+// FILTER: candidates whose rows the query excludes (ex, <= kMaxExcluded ids in shared memory after the query) are dropped
+// before their re-score; their keys (0) sort last and are emitted as missing slots.
+template <typename RowT, bool FILTER = false>
 __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long long* cand, const int* count, int C,
                                                           const float* __restrict__ qf, const RowT* __restrict__ xs,
                                                           int d, float* D, int64_t* I, int64_t id_offset, int k_out,
-                                                          int stage_scores) {
+                                                          int stage_scores, Excluded ex) {
   extern __shared__ unsigned long long fsm[];
   const int q = blockIdx.x;
   const int cnt = count[q];
@@ -267,11 +295,22 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
   float* sq = reinterpret_cast<float*>(fsm + P);
   for (int i = threadIdx.x; i < d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q) * d + i];
   for (int i = cnt + threadIdx.x; i < P; i += blockDim.x) skeys[i] = 0ull;
+  uint32_t* sx = reinterpret_cast<uint32_t*>(sq + d);
+  int nx = 0;
+  if constexpr (FILTER) nx = ex.load(q, sx, 1, threadIdx.x, blockDim.x);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nw = blockDim.x >> 5;
   const unsigned long long* mine = cand + static_cast<size_t>(q) * C;
   for (int j = warp; j < cnt; j += nw) {
     const uint32_t row = key_row(mine[j]);
+    if constexpr (FILTER) {
+      bool hit = false;
+      for (int e = lane; e < nx; e += 32) hit |= sx[e] == row;
+      if (__any_sync(0xffffffffu, hit)) {
+        if (lane == 0) skeys[j] = 0ull;
+        continue;
+      }
+    }
     float acc = 0.f;
     if ((d & 3) == 0) {
       const StoredRow<RowT> x(xs, row, d);
@@ -298,7 +337,7 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
   for (int r = threadIdx.x; r < k_out; r += blockDim.x) {
     float s = -FLT_MAX;
     int64_t id = -1;
-    if (r < cnt) {
+    if (r < cnt && (!FILTER || skeys[r] != 0ull)) {
       s = key_score(skeys[r]);
       id = id_offset + static_cast<int64_t>(key_row(skeys[r]));
     }
@@ -591,18 +630,31 @@ __global__ void __launch_bounds__(1024) compact_flags_kernel(const int* __restri
 // xor-butterfly), so both produce bit-identical scores.
 // Survivors (score > the query's strict threshold) are appended to the same candidate lists the tensor-core scan
 // uses; dense = 1: first round, every score stored at position = column.
-template <int NQT, int ROWS, typename RowT>
+// FILTER (dense = 0 only: a filtered first round runs at threshold -inf): survivors must also be allowed by the bitmap
+// `allow` (nullable) and not excluded by their query (ex: kMaxExcluded x NQT ids in shared memory after the queries,
+// interleaved, id e of query j at e * NQT + j, so the lanes of the active queries read consecutive words).
+template <int NQT, int ROWS, typename RowT, bool FILTER = false>
 __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict__ xs, int64_t n_rows,
                                                          uint32_t row_base,
                                                          const float* __restrict__ qf, int nq, int d, int nqt,
                                                          const float* __restrict__ thr, unsigned long long* cand,
-                                                         int* count, int* overflow, int C, int dense) {
+                                                         int* count, int* overflow, int C, int dense,
+                                                         const uint32_t* __restrict__ allow, Excluded ex) {
   extern __shared__ float sq[];
   const int q0 = blockIdx.y * nqt;
   const int nact = min(nqt, nq - q0);
   for (int i = threadIdx.x; i < nact * d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q0) * d + i];
+  int nx = 0;  // lane j: query j's excluded rows, sx[0, nx)
+  if constexpr (FILTER) {
+    for (int j = 0; j < nact; ++j) {
+      const int n = ex.load(q0 + j, reinterpret_cast<uint32_t*>(sq + static_cast<size_t>(nqt) * d) + j, NQT, threadIdx.x,
+                            blockDim.x);
+      if (static_cast<int>(threadIdx.x & 31) == j) nx = n;
+    }
+  }
   __syncthreads();
   const int lane = threadIdx.x & 31;
+  const uint32_t* sx = reinterpret_cast<const uint32_t*>(sq + static_cast<size_t>(nqt) * d) + lane;
   float t = __int_as_float(0x7f800000);
   if (lane < nact && !dense) t = thr[q0 + lane];
   const int64_t wg = static_cast<int64_t>(blockIdx.x) * 8 + (threadIdx.x >> 5), nw = static_cast<int64_t>(gridDim.x) * 8;
@@ -668,6 +720,12 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
         if (dense) {
           cand[static_cast<size_t>(q) * C + col] = key;
         } else if (mine > t) {
+          if constexpr (FILTER) {
+            const uint32_t r = row_base + static_cast<uint32_t>(col);
+            bool keep = !allow || ((__ldg(allow + (r >> 5)) >> (r & 31)) & 1u);
+            for (int e = 0; keep && e < nx; ++e) keep = sx[e * NQT] != r;
+            if (!keep) continue;
+          }
           const int pos = atomicAdd(count + q, 1);
           if (pos < C)
             cand[static_cast<size_t>(q) * C + pos] = key;
@@ -676,6 +734,37 @@ __global__ void __launch_bounds__(256) exact_scan_kernel(const RowT* __restrict_
         }
       }
     }
+  }
+}
+
+// Argument rules of a filter's exclusions, per query: *bad |= 1 for decreasing offsets (or a negative first one, or ids
+// missing), 2 for more than kMaxExcluded ids, 4 for a negative id.
+__global__ void check_exclusions_kernel(const int64_t* __restrict__ off, const int64_t* __restrict__ ids, int nq, int* bad) {
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x) {
+    const int64_t a = off[q], b = off[q + 1];
+    int f = 0;
+    if (a < 0 || b < a || (b > a && !ids))
+      f = 1;
+    else if (b - a > kMaxExcluded)
+      f = 2;
+    else
+      for (int64_t i = a; i < b; ++i) f |= ids[i] < 0 ? 4 : 0;
+    if (f) atomicOr(bad, f);
+  }
+}
+
+// Allowed rows of a filtered search's bitmap in each 256-row block of the shard's n rows (bits past n are ignored).
+__global__ void allow_block_counts_kernel(const uint32_t* __restrict__ allow, int64_t n, int64_t nblocks, int* __restrict__ out) {
+  for (int64_t b = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; b < nblocks;
+       b += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+    int c = 0;
+    for (int w = 0; w < 8 && b * 256 + 32 * w < n; ++w) {
+      const int64_t r0 = b * 256 + 32 * w;
+      uint32_t m = allow[r0 >> 5];
+      if (n - r0 < 32) m &= (1u << (n - r0)) - 1u;
+      c += __popc(m);
+    }
+    out[b] = c;
   }
 }
 
@@ -756,6 +845,8 @@ struct Level {
   float* thr = nullptr;
   int* status = nullptr;  // [0] list overflow, [2] uncertified queries
   uint8_t *send = nullptr, *recv = nullptr;
+  const uint32_t* allow = nullptr;  // filtered search: the shard's allowed-row bitmap
+  Excluded ex{};  // filtered search: excluded ids (ex.off nullptr: none), ex.qmap the level's queries in the caller's batch
 };
 
 }  // namespace
@@ -793,6 +884,8 @@ struct om_index {
   std::vector<int> ev_kind;     // 0 scan, 1 select, 2 finalize, 3 exchange / merge / certify
   size_t ev_used = 0;
   DevBuf ws, ows, sws;  // level workspace / whole-search staging / escalation sub-batch
+  // filtered search with a bitmap: allowed rows in [0, min(256 b, n)) for b = 0 .. ceil(n / 256), set by check_filter
+  std::vector<int64_t> allow_prefix;
   int* h_status = nullptr;  // pinned host mirror of Level::status
 };
 
@@ -1156,6 +1249,10 @@ int once_attrs(const om_index* ix) {
     if (rows_done) return 0;
     OM_CUDA(cudaFuncSetAttribute(finalize_kernel<RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxCandidates * 8 + 65536));
     OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 96 * 1024));
+    OM_CUDA(cudaFuncSetAttribute(finalize_kernel<RowT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 kMaxCandidates * 8 + 65536 + kMaxExcluded * 4));
+    OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, RowT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 96 * 1024 + 8 * kMaxExcluded * 4));
     rows_done = true;
     return 0;
   });
@@ -1270,14 +1367,45 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
   int64_t pos = 0;
   const size_t sel_smem = static_cast<size_t>(C) * 8;
   bool first = true;
+  // Filtered search: the scan must not store the rows the filter drops, so instead of the dense first round (every score
+  // at position = column, kp counted over all C rows) the first round is a threshold round at -inf: every allowed row
+  // survives, and select counts the list, which holds allowed rows only.  Later rounds filter as usual.  The exact scan
+  // drops excluded ids as well, so its lists (k rows) hold no excluded row either.
+  const bool sparse_first = L.allow || (L.mode == 1 && L.ex.off);
+  const bool exact_filter = L.mode == 1 && sparse_first;
+  Excluded ex = L.ex;
+  ex.q_base = q0;
+  // With a bitmap, rounds are sized in allowed rows (ix->allow_prefix, per 256-row block), as they would be in rows on an
+  // index of the allowed rows alone: the first round takes up to C allowed rows, a doubling round (growth - 1) x the
+  // allowed rows seen, a safe round C - kp.  So a round at threshold -inf (fewer than kp allowed rows seen) cannot
+  // overflow its list however the allowed rows are placed, and stretches of disallowed rows join the next round.
+  // Returns the end of the round from pos: the last block boundary (or N) whose allowed rows since pos stay within
+  // budget, one block at least.
+  const std::vector<int64_t>& A = ix->allow_prefix;
+  auto allowed_end = [&](int64_t from, int64_t budget) -> int64_t {
+    const int64_t b0 = from / 256;
+    int64_t b = std::upper_bound(A.begin() + b0 + 1, A.end(), A[b0] + budget) - A.begin() - 1;
+    b = std::max(b, b0 + 1);
+    return std::min<int64_t>(b * 256, N);
+  };
+  if (sparse_first) {
+    fill_i32<<<(nqc + 255) / 256, 256, 0, st>>>(L.count, 0, nqc);
+    fill_i32<<<(nqc + 255) / 256, 256, 0, st>>>(reinterpret_cast<int*>(L.thr), static_cast<int>(0xff800000), nqc);
+    OM_CUDA(cudaGetLastError());
+  }
   while (pos < N) {
     int64_t step;
-    if (first)
+    if (L.allow)
+      step = allowed_end(pos, first ? C : safe ? C - kp : (growth - 1) * (A[pos / 256])) - pos;
+    else if (first)
       step = std::min<int64_t>(N, C);
     else if (safe)
       step = std::min<int64_t>(N - pos, std::max<int64_t>(256, ((C - kp) / 256) * 256));
     else
       step = std::min<int64_t>(N - pos, (growth - 1) * pos);
+    // a first round of allowed rows only (an allow-all bitmap, a sub-collection at the start of the shard) stores densely
+    // as the unfiltered search does: nothing there for the filter to drop
+    const bool dense = first && (!sparse_first || (L.mode == 0 && L.allow && A[(pos + step + 255) / 256] == step));
     {
       Timed t(ix, st, 0);
       if (L.mode == 0 && ix->storage == OM_I8) {
@@ -1288,9 +1416,12 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         const int8_t* xrows = ix->xq + pos * pitch;
         const int ncols = static_cast<int>(step);
         cudaError_t e;
-        if (first)
+        if (dense)
           e = launch_scan_i8<true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
                                    L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
+        else if (L.allow)
+          e = launch_scan_i8<false, true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
+                                          L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st, L.allow);
         else
           e = launch_scan_i8<false>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
                                     L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
@@ -1303,8 +1434,8 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
         // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
         // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
         const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
-        if (first) {
-          EpiScan<true> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
+        if (dense) {
+          EpiScan<true> epi{{}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         } else if (pair) {
           // cluster shape CQ x CX: the index parameters, else 2 x 1.  The wider shapes cut L2 -> SM traffic by 25 - 50 %, but
@@ -1313,12 +1444,16 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
           const int cq = ix->scan_cq ? ix->scan_cq : 2, cx = ix->scan_cx ? ix->scan_cx : 1;
           int clusters = 0;
           e = launch_scan_cluster(cq, cx, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
-                                  overflow, C, static_cast<uint32_t>(pos), sms, st);
-          if (e == cudaSuccess) e = scan_cluster_capacity(cq, cx, sms, &clusters);
+                                  overflow, C, static_cast<uint32_t>(pos), L.allow, sms, st);
+          if (e == cudaSuccess) e = scan_cluster_capacity(cq, cx, L.allow != nullptr, sms, &clusters);
           ix->st_scan_cluster = 10 * cq + cx;
           ix->st_scan_clusters = clusters;
+        } else if (L.allow) {
+          EpiScan<false, true> epi{{L.allow}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
+          e = launch_gemm<128, 3, true, EpiScan<false, true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st,
+                                                                   /*dynamic_sched=*/true);
         } else {
-          EpiScan<false> epi{L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
+          EpiScan<false> epi{{}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
           e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
         }
         if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
@@ -1328,15 +1463,22 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
                   static_cast<unsigned>((nqc + nqt - 1) / nqt));
         const size_t smem = static_cast<size_t>(nqt) * ix->d * 4;
         with_rows(ix, [&](const auto* xs) {
-          exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf,
-                                                           nqc, ix->d, nqt, L.thr, L.cand, L.count, overflow, C, first ? 1 : 0);
+          using RowT = std::decay_t<decltype(*xs)>;
+          if (exact_filter)
+            exact_scan_kernel<8, 2, RowT, true><<<grid, 256, smem + 8 * kMaxExcluded * 4, st>>>(
+                xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand, L.count,
+                overflow, C, 0, L.allow, ex);
+          else
+            exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf,
+                                                             nqc, ix->d, nqt, L.thr, L.cand, L.count, overflow, C, first ? 1 : 0,
+                                                             nullptr, Excluded{});
         });
         OM_CUDA(cudaGetLastError());
       }
     }
     {
       Timed t(ix, st, 1);
-      select_kernel<<<nqc, 256, sel_smem, st>>>(L.cand, L.count, L.thr, C, kp, first ? static_cast<int>(step) : -1);
+      select_kernel<<<nqc, 256, sel_smem, st>>>(L.cand, L.count, L.thr, C, kp, dense ? static_cast<int>(step) : -1);
     }
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 2;
@@ -1356,8 +1498,15 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
     Timed t(ix, st, 2);
     const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
     with_rows(ix, [&](const auto* xs) {
-      finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out,
-                                                  ix->stage_scores);
+      using RowT = std::decay_t<decltype(*xs)>;
+      Excluded ex = L.ex;
+      ex.q_base = q0;
+      if (ex.off)
+        finalize_kernel<RowT, true><<<nqc, 256, fin_smem + kMaxExcluded * 4, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I,
+                                                                                  id_offset, k_out, ix->stage_scores, ex);
+      else
+        finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out,
+                                                    ix->stage_scores, Excluded{});
     });
   }
   OM_CUDA(cudaGetLastError());
@@ -1508,10 +1657,51 @@ int check_finite_rows(om_index* ix, om_comm* comm, cudaStream_t st) {
   return 0;
 }
 
+// A search filter's argument rules (om_search_filter), checked on `st` before the search writes anything: the bitmap
+// covers the shard, and every query excludes at most kMaxExcluded ids, none negative, through monotone offsets.
+// Sharded: every rank takes part (its filter may be null or empty) and takes the decision of all of them.  A valid bitmap
+// also leaves its allowed rows per 256-row block in ix->allow_prefix, from which sweep_chunk sizes the rounds.  One host
+// synchronisation.
+int check_filter(om_index* ix, om_comm* comm, const om_search_filter* f, int nq, cudaStream_t st) {
+  const om_search_filter none = {nullptr, 0, nullptr, nullptr};
+  if (!f) f = &none;
+  const bool sharded = comm && comm->world > 1;
+  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
+  const bool short_bits = f->allow_bits && f->allow_words < (ix->n + 31) / 32;
+  fill_i32<<<1, 1, 0, st>>>(bad, short_bits ? 8 : 0, 1);
+  if (f->exclude_offsets)
+    check_exclusions_kernel<<<grid_for(nq, 256), 256, 0, st>>>(f->exclude_offsets, f->exclude_ids, nq, bad);
+  OM_CUDA(cudaGetLastError());
+  const int64_t nblocks = (ix->n + 255) / 256;
+  std::vector<int> counts;
+  if (f->allow_bits && !short_bits && nblocks > 0) {
+    OM_TRY(ix->ows.reserve(static_cast<size_t>(nblocks) * 4));
+    allow_block_counts_kernel<<<grid_for(nblocks, 256), 256, 0, st>>>(f->allow_bits, ix->n, nblocks,
+                                                                       static_cast<int*>(ix->ows.p));
+    OM_CUDA(cudaGetLastError());
+    counts.resize(nblocks);
+    OM_CUDA(cudaMemcpyAsync(counts.data(), ix->ows.p, static_cast<size_t>(nblocks) * 4, cudaMemcpyDeviceToHost, st));
+  }
+  if (sharded) OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
+  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  ix->allow_prefix.assign(1, 0);
+  for (int c : counts) ix->allow_prefix.push_back(ix->allow_prefix.back() + c);
+  const int b = ix->h_status[4];
+  if (b & 8)
+    return fail(OM_EINVAL, "search filter: allow_words = %lld is fewer than the %lld words of the %lld rows%s",
+                (long long)f->allow_words, (long long)((ix->n + 31) / 32), (long long)ix->n, sharded ? " (or on another rank)" : "");
+  if (b & 2) return fail(OM_EINVAL, "search filter: a query excludes more than %d ids", kMaxExcluded);
+  if (b & 1) return fail(OM_EINVAL, "search filter: exclude_offsets must be non-negative and non-decreasing, with exclude_ids given");
+  if (b & 4) return fail(OM_EINVAL, "search filter: an excluded id is negative");
+  return 0;
+}
+
 // The whole search: level 0 (all queries, k + slack candidates) -> level 1 (uncertified queries, widest list) ->
-// level 2 (still uncertified: exact fp32 scan).  comm == nullptr / world 1: single shard.
+// level 2 (still uncertified: exact fp32 scan).  comm == nullptr / world 1: single shard.  f: nullptr, or a checked filter
+// with at least one part.
 int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
-                om_memkind out_kind, int64_t id_offset, cudaStream_t st) {
+                om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
   NvtxRange nvtx("om.search");
   const int d = ix->d;
   const int world = comm ? comm->world : 1;
@@ -1549,12 +1739,19 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   int* sub_flags = reinterpret_cast<int*>(ob + o_sub);
   int* flag_list2 = reinterpret_cast<int*>(ob + o_flag2);
 
+  // the filter of every level: the bitmap, and the exclusions of the level's queries (qmap: the escalated ones)
+  auto filter = [&](Level& L, const int* qmap) {
+    if (!f) return;
+    L.allow = f->allow_bits;
+    L.ex = Excluded{f->exclude_offsets, f->exclude_ids, qmap, 0, id_offset};
+  };
   const int64_t slack = ix->rescore_slack >= 0 ? ix->rescore_slack : std::max<int64_t>(128, k / 5);
   const int kp0 = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(k) + slack, kMaxCandidates));
   int nf = 0;
   if (!ix->exact_only) {
     Level L;
     OM_TRY(level_prepare(ix, L, qf, nq, k, kp0, 0, world, st));
+    filter(L, nullptr);
     OM_TRY(run_level(ix, comm, L, dD, dI, id_offset, flags, flag_list, &nf, st));
     ix->st_flagged = nf;
   }
@@ -1564,6 +1761,7 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
     Level Ls;
     if (!list) {
       OM_TRY(level_prepare(ix, Ls, qf, n_sub, k, kp_target, mode, world, st));
+      filter(Ls, nullptr);
       return run_level(ix, comm, Ls, dD, dI, id_offset, flags, sub_flags, nf_out, st);
     }
     size_t so = 0;
@@ -1582,6 +1780,7 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
     gather_rows_kernel<<<grid_for(static_cast<int64_t>(n_sub) * d, 256), 256, 0, st>>>(qf, list, n_sub, d, qsub);
     OM_CUDA(cudaGetLastError());
     OM_TRY(level_prepare(ix, Ls, qsub, n_sub, k, kp_target, mode, world, st));
+    filter(Ls, list);
     OM_TRY(run_level(ix, comm, Ls, Ds, Is, id_offset, flags, sub_flags, nf_out, st));
     scatter_results_kernel<<<grid_for(static_cast<int64_t>(n_sub) * k, 256), 256, 0, st>>>(Ds, Is, list, n_sub, k, dD, dI);
     OM_CUDA(cudaGetLastError());
@@ -1631,7 +1830,22 @@ extern "C" int om_index_search(om_index* ix, const void* q, om_memkind q_kind, i
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
   OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
-  return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, static_cast<cudaStream_t>(stream));
+  return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int om_index_search_filtered(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D,
+                                        int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
+                                        void* stream) {
+  if (!filter || (!filter->allow_bits && !filter->exclude_offsets))
+    return om_index_search(ix, q, q_kind, nq, k, D, I, out_kind, id_offset, stream);
+  if (!ix || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
+    return fail(OM_EINVAL, "om_index_search_filtered: bad arguments (nq=%d k=%d)", nq, k);
+  if (nq == 0) return 0;
+  OM_TRY(device_sm_count());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  OM_TRY(settle_reset(ix, st));
+  OM_TRY(check_filter(ix, nullptr, filter, nq, st));
+  return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, st);
 }
 
 // ---- row-sharded search with the exchange inside the library (NCCL over NVLink) -----------------------------------
@@ -1678,7 +1892,25 @@ extern "C" int om_index_search_sharded(om_index* ix, om_comm* comm, const void* 
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
   OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
-  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, static_cast<cudaStream_t>(stream));
+  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int om_index_search_sharded_filtered(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                                                int k, float* D, int64_t* I, om_memkind out_kind, int64_t id_offset,
+                                                const om_search_filter* filter, void* stream) {
+  // Collective whatever this rank's filter: with more than one rank every rank checks the filters together (one all-reduce),
+  // also a rank whose filter is null or empty, so the ranks' collectives stay in step when only some pass a filter.
+  const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
+  if (!local && !(comm && comm->world > 1))
+    return om_index_search_sharded(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, stream);
+  if (!ix || !comm || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
+    return fail(OM_EINVAL, "om_index_search_sharded_filtered: bad arguments (nq=%d k=%d)", nq, k);
+  if (nq == 0) return 0;
+  OM_TRY(device_sm_count());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  OM_TRY(settle_reset(ix, st));
+  OM_TRY(check_filter(ix, comm, filter, nq, st));
+  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
 }
 
 extern "C" int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k_in, int k_out,

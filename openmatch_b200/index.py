@@ -23,6 +23,89 @@ def _stream() -> int:
 _STORAGE = {torch.float32: _lib.OM_F32, torch.float16: _lib.OM_F16, torch.int8: _lib.OM_I8}
 
 
+# ---- search filters (om_search_filter): the allowed-row bitmap and the per-query excluded ids ----
+def _as_tensor(a) -> torch.Tensor:
+    if isinstance(a, np.ndarray):
+        if a.dtype == np.uint32:
+            a = a.view(np.int32)
+        return torch.from_numpy(np.ascontiguousarray(a))
+    if isinstance(a, torch.Tensor):
+        return a.detach()
+    raise TypeError("expected a torch tensor or a numpy array, got %s" % type(a).__name__)
+
+
+def pack_allow(allow, n: int, device=None) -> torch.Tensor:
+    """The allowed-row bitmap of ``n`` rows as int32 words (bit ``r & 31`` of word ``r >> 5`` = row ``r``), packed on
+    ``device`` with torch ops.  ``allow``: a bool tensor or ndarray ``[n]``, or words already packed (int32 / uint32,
+    at least ``ceil(n / 32)`` of them), which are passed as they are."""
+    a = _as_tensor(allow)
+    if device is not None:
+        a = a.to(device)
+    if a.dim() != 1:
+        raise ValueError("allow must be one-dimensional, got shape %s" % (tuple(a.shape),))
+    if a.dtype == torch.int32:
+        if a.numel() < (n + 31) // 32:
+            raise ValueError("allow holds %d packed words; %d rows need %d" % (a.numel(), n, (n + 31) // 32))
+        return a.contiguous()
+    if a.dtype != torch.bool:
+        raise ValueError("allow must be bool [%d] or packed int32 words, got %s" % (n, a.dtype))
+    if a.numel() != n:
+        raise ValueError("allow has %d entries for %d rows" % (a.numel(), n))
+    words = (n + 31) // 32
+    bits = torch.zeros(words * 32, dtype=torch.int64, device=a.device)
+    bits[:n] = a.to(torch.int64)
+    w = (bits.view(words, 32) << torch.arange(32, device=a.device)).sum(1)
+    return torch.where(w >= 1 << 31, w - (1 << 32), w).to(torch.int32)
+
+
+def unpack_allow(words: torch.Tensor, n: int) -> torch.Tensor:
+    """Inverse of :func:`pack_allow`: bool ``[n]`` on the words' device."""
+    w = words.to(torch.int64) & 0xFFFFFFFF
+    bits = (w.view(-1, 1) >> torch.arange(32, device=w.device)) & 1
+    return bits.view(-1)[:n].bool()
+
+
+def exclusion_csr(exclude, nq: int, device=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(offsets int64 [nq + 1], ids int64) of the per-query excluded ids.  ``exclude``: a list of ``nq`` id lists, or an
+    ``(offsets, ids)`` pair of tensors / ndarrays that is passed as it is."""
+    if isinstance(exclude, tuple):
+        if len(exclude) != 2:
+            raise ValueError("exclude as a tuple must be (offsets, ids)")
+        off, ids = (_as_tensor(t) for t in exclude)
+        if off.dim() != 1 or off.numel() != nq + 1 or ids.dim() != 1:
+            raise ValueError("exclude offsets must be [nq + 1] = [%d] and ids one-dimensional" % (nq + 1))
+        if off.is_floating_point() or ids.is_floating_point() or off.dtype == torch.bool or ids.dtype == torch.bool:
+            raise ValueError("exclude offsets and ids must be integer tensors")
+    else:
+        exclude = list(exclude)
+        if len(exclude) != nq:
+            raise ValueError("exclude has %d id lists for %d queries" % (len(exclude), nq))
+        lens = [len(e) for e in exclude]
+        off = torch.from_numpy(np.concatenate([[0], np.cumsum(lens, dtype=np.int64)]).astype(np.int64))
+        ids = torch.from_numpy(np.fromiter((int(i) for e in exclude for i in e), dtype=np.int64, count=sum(lens)))
+    off, ids = off.to(torch.int64).contiguous(), ids.to(torch.int64).contiguous()
+    if device is not None:
+        off, ids = off.to(device), ids.to(device)
+    return off, ids
+
+
+def _filter(n: int, nq: int, device, allow, exclude):
+    """(om_search_filter or None, the tensors it points into, to be kept alive for the call)"""
+    if allow is None and exclude is None:
+        return None, ()
+    f = _lib.SearchFilter()
+    keep = []
+    if allow is not None:
+        words = pack_allow(allow, n, device)
+        f.allow_bits, f.allow_words = words.data_ptr() or None, words.numel()
+        keep.append(words)
+    if exclude is not None:
+        off, ids = exclusion_csr(exclude, nq, device)
+        f.exclude_offsets, f.exclude_ids = off.data_ptr(), ids.data_ptr() if ids.numel() else None
+        keep += [off, ids]
+    return f, keep
+
+
 class FlatIPIndex:
     """``faiss.IndexFlatIP`` duck type (``d``, ``ntotal``, ``add``, ``search``, ``reset``) living on the
     current CUDA device.
@@ -88,8 +171,19 @@ class FlatIPIndex:
     def reset(self) -> None:
         _lib.check(self._lib.om_index_reset(self._h))
 
-    def search(self, q, k: int, id_offset: int = 0) -> Tuple[np.ndarray, np.ndarray]:
-        """``D, I = index.search(q, k)`` with numpy outputs (float32 [nq, k], int64 [nq, k])."""
+    def search(self, q, k: int, id_offset: int = 0, allow=None, exclude=None) -> Tuple[np.ndarray, np.ndarray]:
+        """``D, I = index.search(q, k)`` with numpy outputs (float32 [nq, k], int64 [nq, k]).
+
+        Filtered search (``om_index_search_filtered``): ``allow`` restricts the result to the rows it allows (bool
+        ``[ntotal]``, tensor or ndarray, or int32 words packed as :func:`pack_allow` does); ``exclude`` drops ids per
+        query (a list of ``nq`` id lists, or an ``(offsets, ids)`` CSR pair; at most 128 ids per query; ids are
+        ``id_offset`` + row).  The result is the exact top-k among the eligible rows, bitwise what an index of those rows
+        alone returns with ids mapped back; missing slots hold id -1.  ``None`` keeps the unfiltered search."""
+        if allow is not None or exclude is not None:
+            if not isinstance(q, torch.Tensor):
+                q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
+            D, I = self.search_device(q.cuda(), k, id_offset, allow=allow, exclude=exclude)
+            return D.cpu().numpy(), I.cpu().numpy()
         if isinstance(q, torch.Tensor) and q.is_cuda:
             D, I = self.search_device(q, k, id_offset)
             return D.cpu().numpy(), I.cpu().numpy()
@@ -116,25 +210,44 @@ class FlatIPIndex:
             raise ValueError("out must be contiguous CUDA tensors (float32 [nq, k], int64 [nq, k])")
         return D, I
 
-    def search_device(self, q: torch.Tensor, k: int, id_offset: int = 0, out=None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``out=(D, I)``: write into caller-owned CUDA tensors (no allocation on the search path)."""
+    def search_device(self, q: torch.Tensor, k: int, id_offset: int = 0, out=None, allow=None,
+                      exclude=None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``out=(D, I)``: write into caller-owned CUDA tensors (no allocation on the search path).  ``allow`` /
+        ``exclude``: the filter of :meth:`search`, packed on the query's device."""
         q = q.contiguous().float()
         self._check_shape(q.shape)
         nq = q.shape[0]
+        f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         D, I = self._outputs(nq, int(k), q.device, out)
-        _lib.check(self._lib.om_index_search(self._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k), D.data_ptr(),
-                                             I.data_ptr(), _lib.OM_DEVICE, int(id_offset), _stream()))
+        if f is None:
+            _lib.check(self._lib.om_index_search(self._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k), D.data_ptr(),
+                                                 I.data_ptr(), _lib.OM_DEVICE, int(id_offset), _stream()))
+        else:
+            _lib.check(self._lib.om_index_search_filtered(self._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k), D.data_ptr(),
+                                                          I.data_ptr(), _lib.OM_DEVICE, int(id_offset), ctypes.byref(f),
+                                                          _stream()))
         return D, I
 
-    def search_sharded_device(self, comm: "Comm", q: torch.Tensor, k: int, id_offset: int = 0, out=None):
+    def search_sharded_device(self, comm: "Comm", q: torch.Tensor, k: int, id_offset: int = 0, out=None, allow=None,
+                              exclude=None):
         """This rank's call of the row-sharded search (``om_index_search_sharded``): collective over ``comm``; every
-        rank passes the same queries and receives the same global (D, I) [nq, k] on its device."""
+        rank passes the same queries and receives the same global (D, I) [nq, k] on its device.  ``allow`` covers THIS
+        rank's rows (``ntotal`` of them); ``exclude`` holds global ids and may be the same on every rank.  Every rank
+        passes a filter or none does; a rank's filter may be empty (a shard without rows packs to no words), which
+        still takes the filtered call, so the ranks' collectives stay in step."""
         q = q.contiguous().float()
         self._check_shape(q.shape)
         nq = q.shape[0]
+        f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         D, I = self._outputs(nq, int(k), q.device, out)
-        _lib.check(self._lib.om_index_search_sharded(self._h, comm._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k),
-                                                     D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, int(id_offset), _stream()))
+        if f is None:
+            _lib.check(self._lib.om_index_search_sharded(self._h, comm._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k),
+                                                         D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, int(id_offset),
+                                                         _stream()))
+        else:
+            _lib.check(self._lib.om_index_search_sharded_filtered(self._h, comm._h, q.data_ptr(), _lib.OM_DEVICE, nq,
+                                                                  int(k), D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE,
+                                                                  int(id_offset), ctypes.byref(f), _stream()))
         return D, I
 
     def search_sharded_pinned(self, comm: "Comm", q_host: torch.Tensor, k: int, D_out: torch.Tensor, I_out: torch.Tensor,
@@ -276,15 +389,36 @@ def merge_topk_device(D_parts: torch.Tensor, I_parts: torch.Tensor, k: int) -> T
     return D, I
 
 
-def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offset: int, group=None):
+def local_allow(allow, id_offset: int, n_local: int, device=None):
+    """A shard's slice ``[id_offset, id_offset + n_local)`` of an allowed-row bitmap over global ids (bool, or int32 words
+    packed as :func:`pack_allow` does), as bool ``[n_local]``; ``None`` stays ``None``."""
+    if allow is None:
+        return None
+    a = _as_tensor(allow)
+    if device is not None:
+        a = a.to(device)
+    if a.dtype == torch.int32:
+        a = unpack_allow(a, a.numel() * 32)
+    if a.dtype != torch.bool or a.dim() != 1:
+        raise ValueError("allow must be bool [ntotal] or packed int32 words, got %s %s" % (a.dtype, tuple(a.shape)))
+    if a.numel() < id_offset + n_local:
+        raise ValueError("allow covers %d ids; this shard holds ids [%d, %d)" % (a.numel(), id_offset, id_offset + n_local))
+    return a[id_offset:id_offset + n_local]
+
+
+def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offset: int, group=None, allow=None,
+                          exclude=None):
     """Row-sharded exact search: every rank passes the same queries and its own shard's ``id_offset`` and receives
     the same global (D, I) [nq, k].  Scan, exchange, merge and the exactness certificate run inside the library
     (``om_index_search_sharded``) over the library's NCCL communicator for ``group``, which is created on first
-    use whatever the group's backend.  Without a process group, or with one rank: the single-shard search."""
+    use whatever the group's backend.  Without a process group, or with one rank: the single-shard search.
+    ``allow`` (over global ids; each rank takes its slice) and ``exclude`` (global ids) filter as in
+    :meth:`FlatIPIndex.search`."""
     import torch.distributed as dist
+    allow = local_allow(allow, int(id_offset), index.ntotal, q.device)
     if not dist.is_initialized() or dist.get_world_size(group) == 1:
-        return index.search_device(q, k, id_offset=id_offset)
-    return index.search_sharded_device(comm_for(group), q, k, id_offset)
+        return index.search_device(q, k, id_offset=id_offset, allow=allow, exclude=exclude)
+    return index.search_sharded_device(comm_for(group), q, k, id_offset, allow=allow, exclude=exclude)
 
 
 def shard_offsets(n_local: int, group=None):
@@ -324,11 +458,12 @@ class ShardedFlatIPIndex:
     def ntotal(self) -> int:
         return self._ntotal
 
-    def search_device(self, q: torch.Tensor, k: int):
-        return sharded_search_device(self.local, q, k, self.offset, self.group)
+    def search_device(self, q: torch.Tensor, k: int, allow=None, exclude=None):
+        """``allow``: bitmap over the global ids (each rank uses its slice); ``exclude``: global ids per query."""
+        return sharded_search_device(self.local, q, k, self.offset, self.group, allow=allow, exclude=exclude)
 
-    def search(self, q, k: int):
+    def search(self, q, k: int, allow=None, exclude=None):
         if not isinstance(q, torch.Tensor):
             q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        D, I = self.search_device(q.cuda(), k)
+        D, I = self.search_device(q.cuda(), k, allow=allow, exclude=exclude)
         return D.cpu().numpy(), I.cpu().numpy()

@@ -30,7 +30,7 @@ from tqdm import tqdm
 from ..arguments import InferenceArguments as EncodingArguments
 from ..dataset import DRInferenceCollator
 from ..embedding_store import EmbeddingFile, write_embedding_file
-from ..index import FlatIPIndex, shard_offsets, sharded_search_device
+from ..index import FlatIPIndex, comm_for, shard_offsets, sharded_search_device
 from ..modeling import DRModelForInference
 from ..utils import merge_retrieval_results_by_score
 
@@ -48,6 +48,24 @@ def _results_dict(query_ids: List[str], doc_lookup: np.ndarray, D: np.ndarray, I
         out[str(qid)] = dict(zip(names, scores[qi][: len(names)])) if valid.all() else \
             dict(zip(names, np.asarray(scores[qi])[valid].tolist()))
     return out
+
+
+def doc_filter(doc_lookup, query_ids, allowed_docs=None, exclude=None, id_offset: int = 0):
+    """Maps a search filter over doc-id strings onto index rows: ``(allow, excluded)`` with ``allow`` a bool array over
+    the rows of ``doc_lookup`` (None: every row) and ``excluded`` one list of ids (``id_offset`` + row) per query of
+    ``query_ids`` (None: no exclusions).  ``allowed_docs``: iterable of doc ids; ``exclude``: ``{qid: [doc ids]}``.  Doc
+    ids the lookup does not hold are ignored, so every rank of a sharded index maps the same arguments on its own rows."""
+    if allowed_docs is None and exclude is None:
+        return None, None
+    row = {d: i for i, d in enumerate(doc_lookup)}
+    allow = None
+    if allowed_docs is not None:
+        allow = np.zeros(len(doc_lookup), dtype=bool)
+        allow[[row[d] for d in allowed_docs if d in row]] = True
+    excluded = None
+    if exclude is not None:
+        excluded = [[id_offset + row[d] for d in exclude.get(q, ()) if d in row] for q in query_ids]
+    return allow, excluded
 
 
 def _index_dtype(args) -> torch.dtype:
@@ -326,21 +344,29 @@ class Retriever:
             self.query_lookup.extend(lookup)
         return np.concatenate(encoded)
 
-    def search(self, topk: int = 100, as_arrays: bool = False):
+    def search(self, topk: int = 100, as_arrays: bool = False, allowed_docs=None, exclude=None):
         """Reference contract (:166-192): ``{qid: {docid: score}}``.  ``as_arrays=True`` returns the same ranking as
-        a :class:`RankArrays` (no per-result Python objects; rank 0 only when sharded)."""
+        a :class:`RankArrays` (no per-result Python objects; rank 0 only when sharded).
+
+        ``allowed_docs`` (doc ids) restricts the ranking to those documents and ``exclude`` (``{qid: [doc ids]}``, at
+        most 128 per query) drops documents per query, e.g. the query's positives or the query itself; the ranking is the
+        exact top-k among the remaining documents (``FlatIPIndex.search``'s filter).  Unknown doc ids are ignored."""
         logger.info("Searching")
         if self.index is None:
             raise ValueError("Index is not initialized")
         encoded = self._load_queries()
         if self.args.world_size > 1:
-            return self._search_sharded(encoded, topk, as_arrays)
-        D, I = self.index.search(encoded, topk)
+            return self._search_sharded(encoded, topk, as_arrays, allowed_docs, exclude)
+        if allowed_docs is None and exclude is None:
+            D, I = self.index.search(encoded, topk)
+        else:
+            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude)
+            D, I = self.index.search(encoded, topk, allow=allow, exclude=excluded)
         result = RankArrays(self.query_lookup, np.array(self.doc_lookup), D, I)
         logger.info("End searching with %d queries", len(result))
         return result if as_arrays else result.to_dict()
 
-    def _search_sharded(self, encoded: np.ndarray, topk: int, as_arrays: bool = False):
+    def _search_sharded(self, encoded: np.ndarray, topk: int, as_arrays: bool = False, allowed_docs=None, exclude=None):
         """Every rank: all queries x local shard -> all-gather [nq, k] lists over NCCL -> merge; doc-id strings
         are gathered to rank 0, which alone builds the result dict (like the reference, :200-203)."""
         dist = torch.distributed
@@ -349,7 +375,12 @@ class Retriever:
             self._initialize_faiss_index(encoded.shape[1])
         offset, _ = shard_offsets(len(self.doc_lookup))
         q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
-        D, I = sharded_search_device(self.index, q, topk, offset)
+        if allowed_docs is None and exclude is None:
+            D, I = sharded_search_device(self.index, q, topk, offset)
+        else:
+            # each rank maps the filter on its own rows (its slice of the bitmap, exclusions among its own documents)
+            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
+            D, I = self.index.search_sharded_device(comm_for(None), q, topk, offset, allow=allow, exclude=excluded)
         lookups = [None] * W if r == 0 else None
         dist.gather_object(self.doc_lookup, lookups, dst=0)
         if r != 0:
@@ -358,16 +389,19 @@ class Retriever:
         result = RankArrays(self.query_lookup, names, D.cpu().numpy(), I.cpu().numpy())
         return result if as_arrays else result.to_dict()
 
-    def retrieve(self, query_dataset: IterableDataset, topk: int = 100, as_arrays: bool = False):
+    def retrieve(self, query_dataset: IterableDataset, topk: int = 100, as_arrays: bool = False, allowed_docs=None,
+                 exclude=None):
+        """Encodes the queries and searches them; ``allowed_docs`` / ``exclude`` filter as in :meth:`search`."""
         self.query_embedding_inference(query_dataset)
         self.model.cpu()
         del self.model
         torch.cuda.empty_cache()
         if self.args.world_size > 1:
-            results = self.search(topk, as_arrays)  # collective: every rank takes part, rank 0 gets the result
+            # collective: every rank takes part, rank 0 gets the result
+            results = self.search(topk, as_arrays, allowed_docs, exclude)
             torch.distributed.barrier()
             return results
-        return self.search(topk, as_arrays)
+        return self.search(topk, as_arrays, allowed_docs, exclude)
 
 
 class SuccessiveRetriever(Retriever):
