@@ -1,6 +1,7 @@
 // Candidate key encoding and the top-k filter of the search scans: the survivor protocol, the fragment filter of the
-// wide and int8 scans and the fused epilogue of the GEMM core.
+// wide and int8 scans and the fused epilogue of the GEMM core and its launcher.
 #pragma once
+#include <cuda_fp16.h>
 #include <string.h>
 
 #include <type_traits>
@@ -331,5 +332,22 @@ struct EpiScan : ScanAllow<ALLOW> {
                        row_base);
   }
 };
+
+// Host launcher of the scan on the GEMM core (128-row corpus tiles from a dynamic tile queue).  Q: [nq, K] fp16 queries,
+// row pitch ldq elements; X: [n_cols, K] fp16 corpus rows, row pitch ldx.  dense: every score goes to cand[q * C + column],
+// and allow is not read; otherwise survivors (score > thr[q]) are appended as make_key(score, row_base + column).  allow:
+// nullptr, or the allowed-row bitmap of a filtered search, which survivors must also pass.
+static inline cudaError_t launch_scan_core(bool dense, const uint32_t* allow, const __half* Q, int64_t ldq, const __half* X,
+                                           int64_t ldx, int nq, int n_cols, int K, const float* thr,
+                                           unsigned long long* cand, int* count, int* overflow, int C, uint32_t row_base,
+                                           int num_sms, cudaStream_t stream) {
+  auto launch = [&](const auto& epi) {
+    return launch_gemm<128, 3, true, std::decay_t<decltype(epi)>, true>(Q, ldq, X, ldx, nq, n_cols, K, epi, num_sms, stream,
+                                                                       /*dynamic_sched=*/true);
+  };
+  if (dense) return launch(EpiScan<true>{{}, thr, cand, count, overflow, nq, n_cols, C, row_base});
+  if (allow) return launch(EpiScan<false, true>{{allow}, thr, cand, count, overflow, nq, n_cols, C, row_base});
+  return launch(EpiScan<false>{{}, thr, cand, count, overflow, nq, n_cols, C, row_base});
+}
 
 }  // namespace om

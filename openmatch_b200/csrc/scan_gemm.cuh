@@ -219,7 +219,7 @@ template <int CQ, int CX, bool ALLOW>
 static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const __half* X, int64_t ldx, int nq, int n_cols,
                                            int K, const float* thr, unsigned long long* cand, int* count, int* overflow,
                                            int C, uint32_t row_base, const uint32_t* allow, int num_sms,
-                                           cudaStream_t stream) {
+                                           cudaStream_t stream, int* max_clusters_out) {
   using Cl = ScanCluster<CQ, CX>;
   CUtensorMap tmQ, tmX;
   if (make_tmap_bf16_2d(&tmQ, Q, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq * 2, kBlockK, Cl::kQRows) != 0)
@@ -229,6 +229,7 @@ static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const _
   int max_clusters = 0;
   cudaError_t e = scan_wide_max_clusters<CQ, CX, ALLOW>(num_sms, &max_clusters);
   if (e != cudaSuccess) return e;
+  *max_clusters_out = max_clusters;
   if (max_clusters < 1) return cudaErrorNotSupported;
   cudaLaunchConfig_t cfg = {};
   cfg.blockDim = dim3(kGemmProducerThreads + kScanConsumers);
@@ -252,19 +253,21 @@ static inline cudaError_t launch_scan_wide(const __half* Q, int64_t ldq, const _
 // cand[q * C ...] as make_key(score, row_base + column); a list that would grow beyond C sets *overflow.  allow: nullptr, or
 // the allowed-row bitmap of a filtered search (indexed by row_base + column), which survivors must also pass.  Every shape
 // computes each score with the same wgmma sequence, so the candidate lists hold the same keys whatever the shape.
-// Returns cudaSuccess / a CUDA error; tensor-map failures and other shapes map to cudaErrorInvalidValue, and
-// cudaErrorNotSupported means that no cluster of the shape fits on the device.
+// *max_clusters: the clusters of the shape (of its bitmap variant with allow) that are co-resident on the device, 0 when
+// none fits or the shape is not one of the four.  Returns cudaSuccess / a CUDA error; tensor-map failures and other
+// shapes map to cudaErrorInvalidValue, and cudaErrorNotSupported means that no cluster of the shape fits on the device.
 static inline cudaError_t launch_scan_cluster(int cq, int cx, const __half* Q, int64_t ldq, const __half* X, int64_t ldx,
                                               int nq, int n_cols, int K, const float* thr, unsigned long long* cand,
                                               int* count, int* overflow, int C, uint32_t row_base, const uint32_t* allow,
-                                              int num_sms, cudaStream_t stream) {
+                                              int num_sms, cudaStream_t stream, int* max_clusters) {
+  *max_clusters = 0;
   if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
   auto launch = [&](auto cq_c, auto cx_c) {
     constexpr int CQ = decltype(cq_c)::value, CX = decltype(cx_c)::value;
     return allow ? launch_scan_wide<CQ, CX, true>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base,
-                                                  allow, num_sms, stream)
+                                                  allow, num_sms, stream, max_clusters)
                  : launch_scan_wide<CQ, CX, false>(Q, ldq, X, ldx, nq, n_cols, K, thr, cand, count, overflow, C, row_base,
-                                                   nullptr, num_sms, stream);
+                                                   nullptr, num_sms, stream, max_clusters);
   };
   using I1 = std::integral_constant<int, 1>;
   using I2 = std::integral_constant<int, 2>;
@@ -274,17 +277,6 @@ static inline cudaError_t launch_scan_cluster(int cq, int cx, const __half* Q, i
   if (cq == 2 && cx == 2) return launch(I2{}, I2{});
   if (cq == 4 && cx == 2) return launch(I4{}, I2{});
   return cudaErrorInvalidValue;
-}
-
-// Co-resident clusters of the cq x cx scan on this device (0 when none fits, -1 for another shape); filtered: of its
-// bitmap variant.
-static inline cudaError_t scan_cluster_capacity(int cq, int cx, bool filtered, int num_sms, int* out) {
-  *out = -1;
-  if (cq == 2 && cx == 1) return filtered ? scan_wide_max_clusters<2, 1, true>(num_sms, out) : scan_wide_max_clusters<2, 1, false>(num_sms, out);
-  if (cq == 4 && cx == 1) return filtered ? scan_wide_max_clusters<4, 1, true>(num_sms, out) : scan_wide_max_clusters<4, 1, false>(num_sms, out);
-  if (cq == 2 && cx == 2) return filtered ? scan_wide_max_clusters<2, 2, true>(num_sms, out) : scan_wide_max_clusters<2, 2, false>(num_sms, out);
-  if (cq == 4 && cx == 2) return filtered ? scan_wide_max_clusters<4, 2, true>(num_sms, out) : scan_wide_max_clusters<4, 2, false>(num_sms, out);
-  return cudaSuccess;
 }
 
 }  // namespace om

@@ -18,6 +18,8 @@
 #pragma once
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "scan_epilogue.cuh"
 
 namespace om {
@@ -169,35 +171,42 @@ scan_i8_kernel(const __grid_constant__ CUtensorMap tmQh, const __grid_constant__
 }
 
 // Host launcher.  Qh, Ql: [nq, K] int8 query splits, row pitch ldq bytes; qsig [nq] (sig_hi, sig_lo); X: the corpus rows of
-// the round, [n_cols] rows of pitch `pitch` bytes with the scale at byte dpad.  DENSE: every score goes to
-// cand[q * C + column]; otherwise survivors (score > thr[q]) are appended as make_key(score, row_base + column) and a
-// list that would grow beyond C sets *overflow.  ALLOW: survivors must also pass the allowed-row bitmap `allow` (indexed by
-// row_base + column).  Returns cudaSuccess / a CUDA error (tensor-map failures:
-// cudaErrorInvalidValue).
-template <bool DENSE, bool ALLOW = false>
-static inline cudaError_t launch_scan_i8(const int8_t* Qh, const int8_t* Ql, int64_t ldq, const float2* qsig,
-                                         const int8_t* X, int64_t pitch, int dpad, int nq, int n_cols, int K,
-                                         const float* thr, unsigned long long* cand, int* count, int* overflow, int C,
-                                         uint32_t row_base, int num_sms, cudaStream_t stream,
-                                         const uint32_t* allow = nullptr) {
+// the round, [n_cols] rows of pitch `pitch` bytes with the scale at byte dpad.  dense: every score goes to
+// cand[q * C + column], and allow is not read; otherwise survivors (score > thr[q]) are appended as
+// make_key(score, row_base + column) and a list that would grow beyond C sets *overflow.  allow: nullptr, or the
+// allowed-row bitmap of a filtered search (indexed by row_base + column), which survivors must also pass.  Returns
+// cudaSuccess / a CUDA error (tensor-map failures: cudaErrorInvalidValue).
+static inline cudaError_t launch_scan_i8(bool dense, const uint32_t* allow, const int8_t* Qh, const int8_t* Ql, int64_t ldq,
+                                         const float2* qsig, const int8_t* X, int64_t pitch, int dpad, int nq, int n_cols,
+                                         int K, const float* thr, unsigned long long* cand, int* count, int* overflow, int C,
+                                         uint32_t row_base, int num_sms, cudaStream_t stream) {
   if (nq <= 0 || n_cols <= 0 || K <= 0) return cudaSuccess;
   CUtensorMap tmQh, tmQl, tmX;
   if (make_tmap_2d(&tmQh, Qh, 1, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq, kI8BlockK, kBlockM, 128) != 0 ||
       make_tmap_2d(&tmQl, Ql, 1, (uint64_t)K, (uint64_t)nq, (uint64_t)ldq, kI8BlockK, kBlockM, 128) != 0 ||
       make_tmap_2d(&tmX, X, 1, (uint64_t)K, (uint64_t)n_cols, (uint64_t)pitch, kI8BlockK, kI8BlockN, 128) != 0)
     return cudaErrorInvalidValue;
-  static bool attr_set = false;  // per instantiation
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(scan_i8_kernel<DENSE, ALLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kI8SmemBytes);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
   const int64_t num_tiles =
       static_cast<int64_t>((nq + kBlockM - 1) / kBlockM) * ((n_cols + kI8BlockN - 1) / kI8BlockN);
   const int grid = static_cast<int>(num_tiles < num_sms ? num_tiles : num_sms);
-  scan_i8_kernel<DENSE, ALLOW><<<grid, kGemmProducerThreads + kI8Consumers, kI8SmemBytes, stream>>>(
-      tmQh, tmQl, tmX, K, X, pitch, dpad, qsig, thr, cand, count, overflow, nq, n_cols, C, row_base, allow);
-  return cudaGetLastError();
+  auto launch = [&](auto dense_c, auto allow_c) {
+    constexpr bool DENSE = decltype(dense_c)::value, ALLOW = decltype(allow_c)::value;
+    static bool attr_set = false;  // per instantiation
+    if (!attr_set) {
+      cudaError_t e =
+          cudaFuncSetAttribute(scan_i8_kernel<DENSE, ALLOW>, cudaFuncAttributeMaxDynamicSharedMemorySize, kI8SmemBytes);
+      if (e != cudaSuccess) return e;
+      attr_set = true;
+    }
+    scan_i8_kernel<DENSE, ALLOW><<<grid, kGemmProducerThreads + kI8Consumers, kI8SmemBytes, stream>>>(
+        tmQh, tmQl, tmX, K, X, pitch, dpad, qsig, thr, cand, count, overflow, nq, n_cols, C, row_base,
+        ALLOW ? allow : nullptr);
+    return cudaGetLastError();
+  };
+  // a dense round stores every score, so the filter variant exists for threshold rounds only
+  if (dense) return launch(std::true_type{}, std::false_type{});
+  if (allow) return launch(std::false_type{}, std::true_type{});
+  return launch(std::false_type{}, std::false_type{});
 }
 
 }  // namespace om

@@ -1408,70 +1408,50 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
     const bool dense = first && (!sparse_first || (L.mode == 0 && L.allow && A[(pos + step + 255) / 256] == step));
     {
       Timed t(ix, st, 0);
+      const int ncols = static_cast<int>(step);
+      const uint32_t row_base = static_cast<uint32_t>(pos);
       if (L.mode == 0 && ix->storage == OM_I8) {
         // every round on the int8 scan (pair_scan and the cluster shape do not apply)
         const int8_t* qhi = L.q8 + static_cast<size_t>(q0) * ix->dpad;
         const int8_t* qlo = L.q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
         const int64_t pitch = pitch_of(ix->xq, ix->d);
-        const int8_t* xrows = ix->xq + pos * pitch;
-        const int ncols = static_cast<int>(step);
-        cudaError_t e;
-        if (dense)
-          e = launch_scan_i8<true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
-                                   L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
-        else if (L.allow)
-          e = launch_scan_i8<false, true>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
-                                          L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st, L.allow);
-        else
-          e = launch_scan_i8<false>(qhi, qlo, ix->dpad, L.qsig + q0, xrows, pitch, ix->dpad, nqc, ncols, ix->d, L.thr,
-                                    L.cand, L.count, overflow, C, static_cast<uint32_t>(pos), sms, st);
+        const cudaError_t e = launch_scan_i8(dense, L.allow, qhi, qlo, ix->dpad, L.qsig + q0, ix->xq + pos * pitch, pitch,
+                                             ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C, row_base, sms,
+                                             st);
         if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
       } else if (L.mode == 0) {
         const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
         cudaError_t e;
-        const int ncols = static_cast<int>(step);
         // a cluster owns at least 2 x 128 query rows per tile: with <= 128 queries the peers' boxes would be padding (and the sweep is
         // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
         // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
         const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
-        if (dense) {
-          EpiScan<true> epi{{}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          e = launch_gemm<128, 3, true, EpiScan<true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
-        } else if (pair) {
+        if (!dense && pair) {
           // cluster shape CQ x CX: the index parameters, else 2 x 1.  The wider shapes cut L2 -> SM traffic by 25 - 50 %, but
           // only 30 clusters of 4 and 15 of 8 CTAs fit an H100 SXM (120 SMs, against 66 pairs on all 132), and the whole
           // search measured no faster on any of them beyond run-to-run noise at C2 and slower at C5 (DESIGN §7)
           const int cq = ix->scan_cq ? ix->scan_cq : 2, cx = ix->scan_cx ? ix->scan_cx : 1;
           int clusters = 0;
           e = launch_scan_cluster(cq, cx, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
-                                  overflow, C, static_cast<uint32_t>(pos), L.allow, sms, st);
-          if (e == cudaSuccess) e = scan_cluster_capacity(cq, cx, L.allow != nullptr, sms, &clusters);
+                                  overflow, C, row_base, L.allow, sms, st, &clusters);
           ix->st_scan_cluster = 10 * cq + cx;
           ix->st_scan_clusters = clusters;
-        } else if (L.allow) {
-          EpiScan<false, true> epi{{L.allow}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          e = launch_gemm<128, 3, true, EpiScan<false, true>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st,
-                                                                   /*dynamic_sched=*/true);
         } else {
-          EpiScan<false> epi{{}, L.thr, L.cand, L.count, overflow, nqc, ncols, C, static_cast<uint32_t>(pos)};
-          e = launch_gemm<128, 3, true, EpiScan<false>, true>(qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, epi, sms, st, /*dynamic_sched=*/true);
+          e = launch_scan_core(dense, L.allow, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
+                               overflow, C, row_base, sms, st);
         }
         if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
       } else {
         const int nqt = std::max(1, std::min(8, (96 * 1024) / (ix->d * 4)));
         dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
                   static_cast<unsigned>((nqc + nqt - 1) / nqt));
-        const size_t smem = static_cast<size_t>(nqt) * ix->d * 4;
+        // the filter variant keeps the queries' excluded ids in shared memory after the queries
+        const size_t smem = static_cast<size_t>(nqt) * ix->d * 4 + (exact_filter ? 8 * kMaxExcluded * 4 : 0);
         with_rows(ix, [&](const auto* xs) {
           using RowT = std::decay_t<decltype(*xs)>;
-          if (exact_filter)
-            exact_scan_kernel<8, 2, RowT, true><<<grid, 256, smem + 8 * kMaxExcluded * 4, st>>>(
-                xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf, nqc, ix->d, nqt, L.thr, L.cand, L.count,
-                overflow, C, 0, L.allow, ex);
-          else
-            exact_scan_kernel<8, 2><<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, static_cast<uint32_t>(pos), qf,
-                                                             nqc, ix->d, nqt, L.thr, L.cand, L.count, overflow, C, first ? 1 : 0,
-                                                             nullptr, Excluded{});
+          const auto kernel = exact_filter ? exact_scan_kernel<8, 2, RowT, true> : exact_scan_kernel<8, 2, RowT>;
+          kernel<<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, row_base, qf, nqc, ix->d, nqt, L.thr, L.cand,
+                                          L.count, overflow, C, dense ? 1 : 0, L.allow, exact_filter ? ex : Excluded{});
         });
         OM_CUDA(cudaGetLastError());
       }
@@ -1493,20 +1473,18 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
                    cudaStream_t st) {
   int P2 = 2;
   while (P2 < L.kp) P2 <<= 1;
-  const size_t fin_smem = static_cast<size_t>(P2) * 8 + static_cast<size_t>(ix->d) * 4;
+  const bool filter = L.ex.off != nullptr;  // the filter variant keeps the query's excluded ids after the query
+  const size_t fin_smem = static_cast<size_t>(P2) * 8 + static_cast<size_t>(ix->d) * 4 + (filter ? kMaxExcluded * 4 : 0);
   {
     Timed t(ix, st, 2);
     const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
+    Excluded ex = L.ex;
+    ex.q_base = q0;
     with_rows(ix, [&](const auto* xs) {
       using RowT = std::decay_t<decltype(*xs)>;
-      Excluded ex = L.ex;
-      ex.q_base = q0;
-      if (ex.off)
-        finalize_kernel<RowT, true><<<nqc, 256, fin_smem + kMaxExcluded * 4, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I,
-                                                                                  id_offset, k_out, ix->stage_scores, ex);
-      else
-        finalize_kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out,
-                                                    ix->stage_scores, Excluded{});
+      const auto kernel = filter ? finalize_kernel<RowT, true> : finalize_kernel<RowT>;
+      kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out, ix->stage_scores,
+                                         filter ? ex : Excluded{});
     });
   }
   OM_CUDA(cudaGetLastError());
@@ -1821,31 +1799,38 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   return 0;
 }
 
+// The four exported searches: sharded, the entries that take a communicator (required); filtered, the _filtered entries.
+// The filter is checked before the search when it has a part and, through the sharded entry with more than one rank,
+// always: every rank checks the filters together (one all-reduce), also a rank whose filter is null or empty, so the
+// ranks' collectives stay in step when only some pass a filter.  Any other call is the plain search, and its messages
+// name the plain entry.
+int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
+                 float* D, int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter, void* stream) {
+  const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
+  const bool check = local || (filtered && comm && comm->world > 1);
+  const char* who = sharded ? (check ? "om_index_search_sharded_filtered" : "om_index_search_sharded")
+                            : (check ? "om_index_search_filtered" : "om_index_search");
+  if (!ix || (sharded && !comm) || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
+    return fail(OM_EINVAL, "%s: bad arguments (nq=%d k=%d)", who, nq, k);
+  if (nq == 0) return 0;
+  OM_TRY(device_sm_count());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  OM_TRY(settle_reset(ix, st));
+  if (check) OM_TRY(check_filter(ix, comm, filter, nq, st));
+  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
+}
+
 }  // namespace
 
 extern "C" int om_index_search(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
                                om_memkind out_kind, int64_t id_offset, void* stream) {
-  if (!ix || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
-    return fail(OM_EINVAL, "om_index_search: bad arguments (nq=%d k=%d)", nq, k);
-  if (nq == 0) return 0;
-  OM_TRY(device_sm_count());
-  OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
-  return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, static_cast<cudaStream_t>(stream));
+  return search_entry(false, false, ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, stream);
 }
 
 extern "C" int om_index_search_filtered(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D,
                                         int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
                                         void* stream) {
-  if (!filter || (!filter->allow_bits && !filter->exclude_offsets))
-    return om_index_search(ix, q, q_kind, nq, k, D, I, out_kind, id_offset, stream);
-  if (!ix || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
-    return fail(OM_EINVAL, "om_index_search_filtered: bad arguments (nq=%d k=%d)", nq, k);
-  if (nq == 0) return 0;
-  OM_TRY(device_sm_count());
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  OM_TRY(settle_reset(ix, st));
-  OM_TRY(check_filter(ix, nullptr, filter, nq, st));
-  return search_impl(ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, st);
+  return search_entry(false, true, ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, stream);
 }
 
 // ---- row-sharded search with the exchange inside the library (NCCL over NVLink) -----------------------------------
@@ -1887,30 +1872,13 @@ extern "C" void om_comm_destroy(om_comm* c) {
 
 extern "C" int om_index_search_sharded(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
                                        float* D, int64_t* I, om_memkind out_kind, int64_t id_offset, void* stream) {
-  if (!ix || !comm || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
-    return fail(OM_EINVAL, "om_index_search_sharded: bad arguments (nq=%d k=%d)", nq, k);
-  if (nq == 0) return 0;
-  OM_TRY(device_sm_count());
-  OM_TRY(settle_reset(ix, static_cast<cudaStream_t>(stream)));
-  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, static_cast<cudaStream_t>(stream));
+  return search_entry(true, false, ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, stream);
 }
 
 extern "C" int om_index_search_sharded_filtered(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                                 int k, float* D, int64_t* I, om_memkind out_kind, int64_t id_offset,
                                                 const om_search_filter* filter, void* stream) {
-  // Collective whatever this rank's filter: with more than one rank every rank checks the filters together (one all-reduce),
-  // also a rank whose filter is null or empty, so the ranks' collectives stay in step when only some pass a filter.
-  const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
-  if (!local && !(comm && comm->world > 1))
-    return om_index_search_sharded(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, stream);
-  if (!ix || !comm || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
-    return fail(OM_EINVAL, "om_index_search_sharded_filtered: bad arguments (nq=%d k=%d)", nq, k);
-  if (nq == 0) return 0;
-  OM_TRY(device_sm_count());
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  OM_TRY(settle_reset(ix, st));
-  OM_TRY(check_filter(ix, comm, filter, nq, st));
-  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
+  return search_entry(true, true, ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, stream);
 }
 
 extern "C" int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k_in, int k_out,

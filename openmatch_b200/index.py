@@ -194,9 +194,22 @@ class FlatIPIndex:
         nq = q.shape[0]
         D = np.empty((nq, k), dtype=np.float32)
         I = np.empty((nq, k), dtype=np.int64)
-        _lib.check(self._lib.om_index_search(self._h, q.ctypes.data, _lib.OM_HOST, nq, int(k), D.ctypes.data,
-                                             I.ctypes.data, _lib.OM_HOST, int(id_offset), _stream()))
+        self._search(None, q.ctypes.data, _lib.OM_HOST, nq, k, D.ctypes.data, I.ctypes.data, _lib.OM_HOST, id_offset)
         return D, I
+
+    def _search(self, comm, q_ptr, q_kind, nq, k, D_ptr, I_ptr, out_kind, id_offset, f=None) -> None:
+        """One search call of the C ABI: ``om_index_search``, ``_sharded`` with ``comm``, ``_filtered`` with the
+        filter ``f``.  An unfiltered call never takes a ``_filtered`` entry: with more than one rank that would add a
+        collective filter check."""
+        lib = self._lib
+        if comm is None:
+            head = (self._h,)
+            fn = lib.om_index_search if f is None else lib.om_index_search_filtered
+        else:
+            head = (self._h, comm._h)
+            fn = lib.om_index_search_sharded if f is None else lib.om_index_search_sharded_filtered
+        tail = (_stream(),) if f is None else (ctypes.byref(f), _stream())
+        _lib.check(fn(*head, q_ptr, q_kind, nq, int(k), D_ptr, I_ptr, out_kind, int(id_offset), *tail))
 
     # ---- device-resident variants ----
     @staticmethod
@@ -219,13 +232,7 @@ class FlatIPIndex:
         nq = q.shape[0]
         f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         D, I = self._outputs(nq, int(k), q.device, out)
-        if f is None:
-            _lib.check(self._lib.om_index_search(self._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k), D.data_ptr(),
-                                                 I.data_ptr(), _lib.OM_DEVICE, int(id_offset), _stream()))
-        else:
-            _lib.check(self._lib.om_index_search_filtered(self._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k), D.data_ptr(),
-                                                          I.data_ptr(), _lib.OM_DEVICE, int(id_offset), ctypes.byref(f),
-                                                          _stream()))
+        self._search(None, q.data_ptr(), _lib.OM_DEVICE, nq, k, D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, id_offset, f)
         return D, I
 
     def search_sharded_device(self, comm: "Comm", q: torch.Tensor, k: int, id_offset: int = 0, out=None, allow=None,
@@ -240,31 +247,22 @@ class FlatIPIndex:
         nq = q.shape[0]
         f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         D, I = self._outputs(nq, int(k), q.device, out)
-        if f is None:
-            _lib.check(self._lib.om_index_search_sharded(self._h, comm._h, q.data_ptr(), _lib.OM_DEVICE, nq, int(k),
-                                                         D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, int(id_offset),
-                                                         _stream()))
-        else:
-            _lib.check(self._lib.om_index_search_sharded_filtered(self._h, comm._h, q.data_ptr(), _lib.OM_DEVICE, nq,
-                                                                  int(k), D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE,
-                                                                  int(id_offset), ctypes.byref(f), _stream()))
+        self._search(comm, q.data_ptr(), _lib.OM_DEVICE, nq, k, D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, id_offset, f)
         return D, I
 
     def search_sharded_pinned(self, comm: "Comm", q_host: torch.Tensor, k: int, D_out: torch.Tensor, I_out: torch.Tensor,
                               id_offset: int = 0) -> None:
         """Host (pinned) queries in; results into ``D_out`` / ``I_out`` (pinned host on the rank that wants them,
         device tensors elsewhere)."""
-        nq = q_host.shape[0]
         kind = _lib.OM_DEVICE if D_out.is_cuda else _lib.OM_HOST
-        _lib.check(self._lib.om_index_search_sharded(self._h, comm._h, q_host.data_ptr(), _lib.OM_HOST, nq, int(k),
-                                                     D_out.data_ptr(), I_out.data_ptr(), kind, int(id_offset), _stream()))
+        self._search(comm, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], k, D_out.data_ptr(), I_out.data_ptr(), kind,
+                     id_offset)
 
     def search_pinned(self, q_host: torch.Tensor, k: int, D_host: torch.Tensor, I_host: torch.Tensor,
                       id_offset: int = 0) -> None:
         """Host (pinned) in, host (pinned) out — the end-to-end call the benchmark times."""
-        nq = q_host.shape[0]
-        _lib.check(self._lib.om_index_search(self._h, q_host.data_ptr(), _lib.OM_HOST, nq, int(k), D_host.data_ptr(),
-                                             I_host.data_ptr(), _lib.OM_HOST, int(id_offset), _stream()))
+        self._search(None, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], k, D_host.data_ptr(), I_host.data_ptr(),
+                     _lib.OM_HOST, id_offset)
 
     def _rows_at(self, n: int):
         """(device address, row pitch in elements) of the shard's rows after reserving room for n more"""

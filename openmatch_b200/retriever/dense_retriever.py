@@ -30,7 +30,7 @@ from tqdm import tqdm
 from ..arguments import InferenceArguments as EncodingArguments
 from ..dataset import DRInferenceCollator
 from ..embedding_store import EmbeddingFile, write_embedding_file
-from ..index import FlatIPIndex, comm_for, shard_offsets, sharded_search_device
+from ..index import FlatIPIndex, comm_for, shard_offsets
 from ..modeling import DRModelForInference
 from ..utils import merge_retrieval_results_by_score
 
@@ -261,13 +261,6 @@ class Retriever:
         if self.args.world_size > 1:
             torch.distributed.barrier()
 
-    def _index_rows_to_host(self) -> np.ndarray:
-        if self.index is None or self.index.ntotal == 0:
-            return np.zeros((0, 0), dtype=np.float32)
-        if self.index.dtype == torch.int8:
-            return torch.cat(list(self.index.rows_f32())).cpu().numpy()
-        return self.index.master_rows().float().cpu().numpy()  # one D2H copy per corpus shard
-
     def init_index_and_add(self, partition: str = None):
         logger.info("Initializing index from pre-computed document embeddings")
         files = [partition] if partition is not None else sorted(
@@ -375,12 +368,9 @@ class Retriever:
             self._initialize_faiss_index(encoded.shape[1])
         offset, _ = shard_offsets(len(self.doc_lookup))
         q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
-        if allowed_docs is None and exclude is None:
-            D, I = sharded_search_device(self.index, q, topk, offset)
-        else:
-            # each rank maps the filter on its own rows (its slice of the bitmap, exclusions among its own documents)
-            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
-            D, I = self.index.search_sharded_device(comm_for(None), q, topk, offset, allow=allow, exclude=excluded)
+        # each rank maps the filter on its own rows (its slice of the bitmap, exclusions among its own documents)
+        allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
+        D, I = self.index.search_sharded_device(comm_for(None), q, topk, offset, allow=allow, exclude=excluded)
         lookups = [None] * W if r == 0 else None
         dist.gather_object(self.doc_lookup, lookups, dst=0)
         if r != 0:
