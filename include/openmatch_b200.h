@@ -261,6 +261,27 @@ int om_index_search_sharded_filtered(om_index* idx, om_comm* comm, const void* q
                                      float* D, int64_t* I, om_memkind out_kind, int64_t id_offset,
                                      const om_search_filter* filter, void* stream);
 
+/* Range search (faiss IndexFlatIP.range_search): for query i every row whose fp32 score, as om_index_search computes it,
+ * is strictly greater than radius[i], ordered by (score desc, id asc).  For every j <= min(count, 4096) the first j results
+ * of a query are bitwise om_index_search(q, j)'s D and I.  Exact on every storage (fp16 / int8: with respect to the stored
+ * values) with no certificate to fail: one sweep at radius - E(q) (the certificate's error bound) collects a superset,
+ * which is re-scored exactly and cut at the radius; queries without a finite bound take the exact fp32 scan.
+ * radius: [nq] fp32, same memkind as q; NaN returns OM_EINVAL before any write.  radius -inf returns every row, +inf none.
+ * lims: [nq + 1] int64 written to out_kind memory; query i's results are [lims[i], lims[i + 1]), lims[nq] = total results.
+ * The results stay in the handle until its next search / range search / reset / destroy: the caller learns the total
+ * before it allocates, and om_index_range_results copies them out.  Synchronous on return.
+ * Sharded: every rank passes the same queries and radii and its own id_offset and receives the same lims and results,
+ * bitwise the range search of one index over the concatenated shards.  Tunables that apply: "pair_scan",
+ * "scan_cluster_q" / "_x", "exact_only" and "range_list" (first candidate list length per query, default 4096; a query
+ * with more candidates is swept again with a list sized from its count); stats "range_candidates" (rows re-scored),
+ * "range_resweeps" (queries swept again) and "exact_queries". */
+int om_index_range_search(om_index* idx, const void* q, om_memkind q_kind, int nq, const float* radius, int64_t* lims,
+                          om_memkind out_kind, int64_t id_offset, void* stream);
+int om_index_range_search_sharded(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                                  const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream);
+/* D fp32 [lims[nq]], I int64 [lims[nq]] of the last range search on idx; OM_ESTATE if there is none. */
+int om_index_range_results(const om_index* idx, float* D, int64_t* I, om_memkind out_kind, void* stream);
+
 /* Tunables: "rescore_slack" (extra candidate-stage rows kept per query; default max(128, k/5)),
  * "force_safe_rounds" (1 = always use the overflow-proof fixed-size round schedule; testing),
  * "round_growth" (2..8: each scan round covers (g-1) x the rows already seen; default 0 = auto: 2, or 8 for <= 256 queries),

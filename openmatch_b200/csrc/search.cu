@@ -36,6 +36,7 @@
 //              always the exact top-k by fp32 inner product, ties by row id — never "top-k up to fp16 noise".
 #include <cuda_fp16.h>
 #include <float.h>
+#include <limits.h>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -276,6 +277,31 @@ struct Excluded {
   }
 };
 
+// The fp32 score of stored row `row` against the query sq (d floats in shared memory), computed by one warp: a lane-strided
+// 4-element FMA chain, then the xor-butterfly; every lane returns the sum.  FINAL and the range re-score share it, so a
+// range result scores bit for bit as search reports the same row.
+template <typename RowT>
+__device__ __forceinline__ float row_dot(const RowT* __restrict__ xs, uint32_t row, int d, const float* sq, int lane) {
+  float acc = 0.f;
+  if ((d & 3) == 0) {
+    const StoredRow<RowT> x(xs, row, d);
+    const float4* q4 = reinterpret_cast<const float4*>(sq);
+    for (int i = lane; i < (d >> 2); i += 32) {
+      const float4 a = x.quad(i), b = q4[i];
+      acc = fmaf(a.x, b.x, acc);
+      acc = fmaf(a.y, b.y, acc);
+      acc = fmaf(a.z, b.z, acc);
+      acc = fmaf(a.w, b.w, acc);
+    }
+  } else {
+    const StoredRow<RowT> x(xs, row, d);
+    for (int i = lane; i < d; i += 32) acc = fmaf(x.elem(i), sq[i], acc);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  return acc;
+}
+
 // FINAL: one CTA per query: exact fp32 re-score of the candidates against the stored rows (fp32 master rows or fp16
 // rows), sort by (score desc, row asc), emit the top k_out.  8 CTAs per SM (32 registers): the row
 // gathers are HBM-bound and want every warp resident.
@@ -311,23 +337,7 @@ __global__ void __launch_bounds__(256, 8) finalize_kernel(const unsigned long lo
         continue;
       }
     }
-    float acc = 0.f;
-    if ((d & 3) == 0) {
-      const StoredRow<RowT> x(xs, row, d);
-      const float4* q4 = reinterpret_cast<const float4*>(sq);
-      for (int i = lane; i < (d >> 2); i += 32) {
-        const float4 a = x.quad(i), b = q4[i];
-        acc = fmaf(a.x, b.x, acc);
-        acc = fmaf(a.y, b.y, acc);
-        acc = fmaf(a.z, b.z, acc);
-        acc = fmaf(a.w, b.w, acc);
-      }
-    } else {
-      const StoredRow<RowT> x(xs, row, d);
-      for (int i = lane; i < d; i += 32) acc = fmaf(x.elem(i), sq[i], acc);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+    float acc = row_dot(xs, row, d, sq, lane);
     if (stage_scores) acc = key_score(mine[j]);  // debug: report the candidate-stage score instead
     if (lane == 0) skeys[j] = make_key(acc, row);
   }
@@ -570,6 +580,11 @@ __global__ void __launch_bounds__(256) merge_kernel(const float* Dp, const int64
 // with the corpus norms replaced by their maxima over the index (kept by rows_to_f16_kernel; sharded search: over all
 // shards).  tau is the kp-th stage score of the candidate list — sharded search: the largest of the shards' floors.
 // A NaN anywhere makes the comparison false: the query is flagged and answered by the exact path.
+// cert_bound: E(q) from the query's hn = ||q_h||, en = ||q - q_h|| and the corpus maxima xmax, exmax (the 1.001 covers the
+// roundings of this fp32 expression itself).
+__device__ __forceinline__ float cert_bound(float hn, float en, float xmax, float exmax, int d) {
+  return 1.001f * (hn * exmax + en * xmax + static_cast<float>(d + 16) * 2.384185791015625e-07f * (hn + en) * (xmax + exmax));
+}
 __global__ void __launch_bounds__(256) certify_kernel(const float* __restrict__ D, const int64_t* __restrict__ I, int k,
                                                       const float* __restrict__ floors, int64_t floor_stride, int nparts,
                                                       const float* __restrict__ gstats, int64_t stats_stride,
@@ -586,8 +601,7 @@ __global__ void __launch_bounds__(256) certify_kernel(const float* __restrict__ 
     xmax = (a > xmax || a != a) ? a : xmax;  // NaN sticks: the comparison below then fails
     exmax = (b > exmax || b != b) ? b : exmax;
   }
-  const float a = hn[q], b = en[q];
-  const float E = 1.001f * (a * exmax + b * xmax + static_cast<float>(d + 16) * 2.384185791015625e-07f * (a + b) * (xmax + exmax));
+  const float E = cert_bound(hn[q], en[q], xmax, exmax, d);
   // tau = -inf: every list holds every row of its shard, nothing was left out.  Otherwise k results are needed to compare.
   const bool full = I[static_cast<size_t>(q) * k + (k - 1)] >= 0;
   const bool ok = !(tau > __int_as_float(0xff800000)) ? true : (full && D[static_cast<size_t>(q) * k + (k - 1)] - tau > E);
@@ -795,6 +809,201 @@ __global__ void compose_list_kernel(const int* __restrict__ outer, const int* __
   if (i < n) out[i] = outer[inner[i]];
 }
 
+// ---------------------------------------------------------------------------------------------------
+// range search: every row whose fp32 score is strictly above the query's radius rho
+// ---------------------------------------------------------------------------------------------------
+// THRESHOLD of the one sweep.  Every row has |b - s| <= E(q) (the certificate's bound, b the stage score, s the fp32
+// score), so a row with s > rho has b >= s - E > rho - E >= t with t = rho - E rounded toward -inf: b > t, the scans'
+// strict test, keeps it.  The sweep's candidate set therefore holds every row of the answer, at any threshold round and
+// on any scan kernel, and the exact re-score decides.  t <= rho is never NaN while E is finite; t = -inf (rho = -inf, or
+// rho - E below -FLT_MAX) keeps every row, still a superset.  A non-finite E (a query holding inf / NaN, overflowed norms)
+// proves nothing: the query gets t = +inf here (no candidates) and is answered by the exact scan, which compares exact
+// scores with rho itself (exact = 1 sweeps: thr = rho).
+__global__ void range_threshold_kernel(const float* __restrict__ rho, const float* __restrict__ hn, const float* __restrict__ en,
+                                       const float* __restrict__ gstats, int d, int nq, int exact, float* __restrict__ thr,
+                                       int* __restrict__ to_exact) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  if (exact) {
+    thr[q] = rho[q];
+    to_exact[q] = 0;
+    return;
+  }
+  const float E = cert_bound(hn[q], en[q], gstats[0], gstats[1], d);
+  const bool ok = isfinite(E);
+  thr[q] = ok ? __fsub_rd(rho[q], E) : __int_as_float(0x7f800000);
+  to_exact[q] = ok ? 0 : 1;
+}
+
+// After each round: the scans count every survivor (atomicAdd on count) but store only below C.  The round's survivors
+// are added to the 64-bit total and count is clamped back to the list's fill, so no round (< 2^30 columns) can wrap it.
+__global__ void range_fold_kernel(int* __restrict__ count, int* __restrict__ filled, long long* __restrict__ total, int C, int nq) {
+  const int q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nq) return;
+  const int c = count[q];
+  total[q] += c - filled[q];
+  const int f = min(c, C);
+  filled[q] = f;
+  count[q] = f;
+}
+
+// RE-SCORE and CUT: one warp per candidate (grid.y = query), the query in shared memory, the score of FINAL (row_dot).  A
+// candidate becomes make_key(s, row) if s > rho, else 0, which is no row's key and sorts last; surv counts the kept ones.
+// Queries whose list overflowed (total > C) are swept again and skipped here.
+template <typename RowT>
+__global__ void __launch_bounds__(256, 4) range_rescore_kernel(unsigned long long* __restrict__ cand, const int* __restrict__ count,
+                                                            const long long* __restrict__ total, int C,
+                                                            const float* __restrict__ qf, const RowT* __restrict__ xs, int d,
+                                                            const float* __restrict__ rho, int* __restrict__ surv) {
+  extern __shared__ float4 rsm[];
+  float* sq = reinterpret_cast<float*>(rsm);
+  const int q = blockIdx.y;
+  const int cnt = count[q];
+  if (total[q] > C || static_cast<int>(blockIdx.x) * 8 >= cnt) return;
+  for (int i = threadIdx.x; i < d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q) * d + i];
+  __syncthreads();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const float r = rho[q];
+  unsigned long long* mine = cand + static_cast<size_t>(q) * C;
+  int kept = 0;
+  for (int j = blockIdx.x * 8 + warp; j < cnt; j += gridDim.x * 8) {
+    const uint32_t row = key_row(mine[j]);
+    const float s = row_dot(xs, row, d, sq, lane);
+    const bool keep = s > r;
+    if (lane == 0) mine[j] = keep ? make_key(s, row) : 0ull;
+    kept += keep ? 1 : 0;
+  }
+  if (lane == 0 && kept) atomicAdd(surv + q, kept);
+}
+
+// SORT, step 1: every block of kRangeSortKeys keys of a query's list (grid.x = block, grid.y = query) is sorted descending in
+// shared memory.  A list of at most kRangeSortKeys keys is then sorted; longer ones are merged by range_merge_kernel.
+constexpr int kRangeSortKeys = 16384;
+__global__ void __launch_bounds__(512) range_sort_kernel(unsigned long long* __restrict__ cand, const int* __restrict__ count,
+                                                         const long long* __restrict__ total, int C) {
+  extern __shared__ unsigned long long ssk[];
+  const int q = blockIdx.y;
+  const int cnt = count[q], base = blockIdx.x * kRangeSortKeys;
+  if (total[q] > C || base >= cnt) return;
+  const int n = min(cnt - base, kRangeSortKeys);
+  int P = 2;
+  while (P < n) P <<= 1;
+  unsigned long long* mine = cand + static_cast<size_t>(q) * C + base;
+  for (int i = threadIdx.x; i < P; i += blockDim.x) ssk[i] = i < n ? mine[i] : 0ull;
+  __syncthreads();
+  bitonic_sort_desc(ssk, P, threadIdx.x, blockDim.x);
+  for (int i = threadIdx.x; i < n; i += blockDim.x) mine[i] = ssk[i];
+}
+
+// SORT, step 2 (lists longer than kRangeSortKeys): merges the sorted runs of w keys pairwise, src -> dst.  Each key goes to
+// its run's start + its place in its run + the keys of the partner run before it: those greater than it for a key of the
+// left run, those not smaller for one of the right run, so the cut keys (0, repeated) also land on distinct places.
+__global__ void __launch_bounds__(256) range_merge_kernel(const unsigned long long* __restrict__ src, unsigned long long* __restrict__ dst,
+                                                          const int* __restrict__ count, const long long* __restrict__ total,
+                                                          int C, int w) {
+  const int q = blockIdx.y;
+  const int cnt = count[q];
+  if (total[q] > C || cnt <= kRangeSortKeys) return;
+  const unsigned long long* s = src + static_cast<size_t>(q) * C;
+  unsigned long long* o = dst + static_cast<size_t>(q) * C;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += gridDim.x * blockDim.x) {
+    const int run = i / w, j = i - run * w, p0 = (run ^ 1) * w;
+    const int plen = max(0, min(cnt - p0, w));
+    const unsigned long long key = s[i];
+    const bool left = (run & 1) == 0;
+    int lo = 0, hi = plen;  // first partner place whose key does not precede this one
+    while (lo < hi) {
+      const int mid = (lo + hi) >> 1;
+      const unsigned long long pk = s[p0 + mid];
+      if (left ? pk > key : pk >= key)
+        lo = mid + 1;
+      else
+        hi = mid;
+    }
+    o[min(run, run ^ 1) * w + j + lo] = key;
+  }
+}
+
+// EMIT: the sorted survivors of the queries a sweep answered (off[q] >= 0) to the results' key store at off[q].  Lists
+// longer than kRangeSortKeys ended in `alt` when their merge took an odd number of steps.
+__global__ void __launch_bounds__(256) range_emit_kernel(const unsigned long long* __restrict__ cand,
+                                                         const unsigned long long* __restrict__ alt, int alt_above,
+                                                         const int* __restrict__ count, const int* __restrict__ surv,
+                                                         const long long* __restrict__ off, int C,
+                                                         unsigned long long* __restrict__ store) {
+  const int q = blockIdx.y;
+  const long long o = off[q];
+  if (o < 0) return;
+  const unsigned long long* s = (count[q] > alt_above ? alt : cand) + static_cast<size_t>(q) * C;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < surv[q]; i += gridDim.x * blockDim.x) store[o + i] = s[i];
+}
+
+// Results of a shard in query order: query q's keys store[src[q] ...] -> (score, id_offset + row) at lims[q] (grid.x =
+// query, grid.y = CTAs per query).
+__global__ void __launch_bounds__(256) range_gather_kernel(const unsigned long long* __restrict__ store,
+                                                           const long long* __restrict__ src, const long long* __restrict__ lims,
+                                                           int64_t id_offset, float* __restrict__ D, int64_t* __restrict__ I) {
+  const int q = blockIdx.x;
+  const long long a = lims[q], n = lims[q + 1] - a, s = src[q];
+  for (long long i = blockIdx.y * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+       i += static_cast<long long>(gridDim.y) * blockDim.x) {
+    const unsigned long long k = store[s + i];
+    D[a + i] = key_score(k);
+    I[a + i] = id_offset + static_cast<int64_t>(key_row(k));
+  }
+}
+
+// MERGE of a sharded range search: part p's results (Dp + p stride_d, Ip + p stride_i; its lims at plims + p (nq + 1))
+// are sorted runs per query by (score desc, id asc).  Each entry goes to glims[q] + its place in its run + the entries of
+// the other parts' runs that precede it: higher score, or equal score and lower id (equal ids: lower part).  Ids are
+// compared themselves, so any id_offset per rank gives the single-index order.  grid.y = part.
+__global__ void __launch_bounds__(256, 4) range_merge_parts_kernel(const float* __restrict__ Dp, const int64_t* __restrict__ Ip,
+                                                                int64_t stride_d, int64_t stride_i,
+                                                                const long long* __restrict__ plims, int W, int nq,
+                                                                const long long* __restrict__ glims, float* __restrict__ D,
+                                                                int64_t* __restrict__ I) {
+  const int p = blockIdx.y;
+  const long long* lp = plims + static_cast<size_t>(p) * (nq + 1);
+  const long long T = lp[nq];
+  for (long long e = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; e < T;
+       e += static_cast<long long>(gridDim.x) * blockDim.x) {
+    int lo = 0, hi = nq;  // the query: the last q with lp[q] <= e
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (lp[mid] <= e) lo = mid; else hi = mid;
+    }
+    const int q = lo;
+    const float s = Dp[p * stride_d + e];
+    const int64_t id = Ip[p * stride_i + e];
+    long long pos = glims[q] + (e - lp[q]);
+    for (int p2 = 0; p2 < W; ++p2) {
+      if (p2 == p) continue;
+      const long long* l2 = plims + static_cast<size_t>(p2) * (nq + 1);
+      const float* D2 = Dp + p2 * stride_d;
+      const int64_t* I2 = Ip + p2 * stride_i;
+      long long a = l2[q], b = l2[q + 1];
+      while (a < b) {  // first entry of the run that does not precede (s, id, p)
+        const long long mid = (a + b) >> 1;
+        const float s2 = D2[mid];
+        const int64_t id2 = I2[mid];
+        if (s2 > s || (s2 == s && (id2 < id || (id2 == id && p2 < p))))
+          a = mid + 1;
+        else
+          b = mid;
+      }
+      pos += a - l2[q];
+    }
+    D[pos] = s;
+    I[pos] = id;
+  }
+}
+
+// 1 in *bad if any radius is NaN
+__global__ void check_radius_kernel(const float* __restrict__ rho, int nq, int* bad) {
+  for (int q = blockIdx.x * blockDim.x + threadIdx.x; q < nq; q += gridDim.x * blockDim.x)
+    if (rho[q] != rho[q]) atomicOr(bad, 1);
+}
+
 }  // namespace om
 
 using namespace om;
@@ -887,6 +1096,13 @@ struct om_index {
   // filtered search with a bitmap: allowed rows in [0, min(256 b, n)) for b = 0 .. ceil(n / 256), set by check_filter
   std::vector<int64_t> allow_prefix;
   int* h_status = nullptr;  // pinned host mirror of Level::status
+  // range search: first list capacity per query; the last range search's results (D fp32 then I int64, r_total of each) in
+  // rout, r_total = -1 when there are none (before any range search, after a search or a reset); rkeys: its key store
+  int range_list = 4096;
+  int64_t r_total = -1;
+  DevBuf rkeys, rout;
+  size_t r_keep_ws = 0;  // the workspace of the last range search's first sweeps (kept after the call)
+  int64_t st_range_candidates = 0, st_range_resweeps = 0;
 };
 
 // Calls f with the index's stored rows as a typed pointer: the fp32 master rows, the fp16 rows or the int8 rows.  Kernels
@@ -1016,6 +1232,8 @@ void om_index_destroy(om_index* ix) {
   ix->ws.release();
   ix->ows.release();
   ix->sws.release();
+  ix->rkeys.release();
+  ix->rout.release();
   for (cudaEvent_t e : ix->ev) cudaEventDestroy(e);
   delete ix;
 }
@@ -1029,6 +1247,8 @@ int om_index_reset(om_index* ix) {
   ix->n = 0;
   ix->gstats_stale = true;  // host only: see settle_reset
   ix->st_nonfinite = 0;
+  ix->r_total = -1;
+  ix->rout.release();
   return 0;
 }
 
@@ -1163,6 +1383,9 @@ int om_index_set_param(om_index* ix, const char* name, int64_t value) {
     ix->exact_only = value != 0;
   } else if (!strcmp(name, "debug_stage_scores")) {
     ix->stage_scores = value != 0;
+  } else if (!strcmp(name, "range_list")) {
+    if (value < 256 || value > (1 << 24)) return fail(OM_EINVAL, "range_list must be in [256, 2^24]");
+    ix->range_list = static_cast<int>(value);
   } else {
     return fail(OM_EINVAL, "om_index_set_param: unknown parameter '%s'", name);
   }
@@ -1185,6 +1408,8 @@ int64_t om_index_get_stat(const om_index* ix, const char* name) {
   if (!strcmp(name, "select_ns")) return static_cast<int64_t>(ix->st_select_us * 1e3);
   if (!strcmp(name, "finalize_ns")) return static_cast<int64_t>(ix->st_final_us * 1e3);
   if (!strcmp(name, "other_ns")) return static_cast<int64_t>(ix->st_other_us * 1e3);
+  if (!strcmp(name, "range_candidates")) return ix->st_range_candidates;
+  if (!strcmp(name, "range_resweeps")) return ix->st_range_resweeps;
   return -1;
 }
 
@@ -1241,6 +1466,7 @@ int once_attrs(const om_index* ix) {
   if (!done) {
     OM_CUDA(cudaFuncSetAttribute(select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8));
     OM_CUDA(cudaFuncSetAttribute(merge_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 8192 * 16));
+    OM_CUDA(cudaFuncSetAttribute(range_sort_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kRangeSortKeys * 8));
     done = true;
   }
   return !ix ? 0 : with_rows(ix, [](const auto* xs) -> int {
@@ -1253,6 +1479,7 @@ int once_attrs(const om_index* ix) {
                                  kMaxCandidates * 8 + 65536 + kMaxExcluded * 4));
     OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, RowT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  96 * 1024 + 8 * kMaxExcluded * 4));
+    OM_CUDA(cudaFuncSetAttribute(range_rescore_kernel<RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
     rows_done = true;
     return 0;
   });
@@ -1272,6 +1499,20 @@ inline ExchangeBlock exchange_block(size_t nqc, size_t kc) {
   return b;
 }
 inline size_t exchange_block_bytes(size_t nqc, size_t kc) { return exchange_block(nqc, kc).bytes; }
+
+// The tensor-core scan operand of the level's queries L.qf (fp16, or the int8 split of an int8 index) and their
+// certificate norms L.hn, L.en.
+int convert_queries(om_index* ix, Level& L, cudaStream_t st) {
+  const int nq = L.nq, d = ix->d, dpad = ix->dpad;
+  if (ix->storage == OM_I8)
+    queries_to_i8_kernel<<<grid_for(nq, 8), 256, 0, st>>>(L.qf, nq, d, dpad, L.q8, L.q8 + static_cast<size_t>(nq) * dpad, L.qsig,
+                                                          L.hn, L.en);
+  else
+    rows_to_f16_kernel<<<grid_for(nq, 8), 256, 0, st>>>(L.qf, L.qh, nq, d, dpad, L.hn, L.en, nullptr);
+  OM_CUDA(cudaGetLastError());
+  ix->st_launches += 1;
+  return 0;
+}
 
 // sizes the candidate lists of a level, carves the level workspace and converts the queries
 int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp_target, int mode, int world,
@@ -1335,15 +1576,67 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   L.status = reinterpret_cast<int*>(base + o_status);
   L.send = world > 1 ? base + o_send : nullptr;
   L.recv = world > 1 ? base + o_recv : nullptr;
-  if (mode == 0 && ix->storage == OM_I8) {
-    queries_to_i8_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, nq, d, dpad, L.q8, L.q8 + static_cast<size_t>(nq) * dpad, L.qsig,
-                                                          L.hn, L.en);
+  return mode == 0 ? convert_queries(ix, L, st) : 0;
+}
+
+// One scan round over rows [pos, pos + step) of the shard for queries [q0, q0 + nqc) of the level, on the kernel the level
+// and the storage choose: mode 1 the exact fp32 scan; mode 0 the int8 scan on an int8 index, else the wide cluster scan
+// for threshold rounds of more than 128 queries with pair_scan on, else the GEMM core.  Survivors of thr go to the level's
+// lists; dense: every score at position = column.
+int scan_round(om_index* ix, const Level& L, int q0, int nqc, int64_t pos, int64_t step, bool dense, int sms, cudaStream_t st) {
+  Timed t(ix, st, 0);
+  const int C = L.C;
+  int* overflow = L.status;
+  const int ncols = static_cast<int>(step);
+  const uint32_t row_base = static_cast<uint32_t>(pos);
+  if (L.mode == 0 && ix->storage == OM_I8) {
+    // every round on the int8 scan (pair_scan and the cluster shape do not apply)
+    const int8_t* qhi = L.q8 + static_cast<size_t>(q0) * ix->dpad;
+    const int8_t* qlo = L.q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
+    const int64_t pitch = pitch_of(ix->xq, ix->d);
+    const cudaError_t e = launch_scan_i8(dense, L.allow, qhi, qlo, ix->dpad, L.qsig + q0, ix->xq + pos * pitch, pitch,
+                                         ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C, row_base, sms, st);
+    if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
+  } else if (L.mode == 0) {
+    const __half* qh = L.qh + static_cast<size_t>(q0) * ix->dpad;
+    const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
+    cudaError_t e;
+    // a cluster owns at least 2 x 128 query rows per tile: with <= 128 queries the peers' boxes would be padding (and the sweep is
+    // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
+    // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
+    const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
+    if (!dense && pair) {
+      // cluster shape CQ x CX: the index parameters, else 2 x 1.  The wider shapes cut L2 -> SM traffic by 25 - 50 %, but
+      // only 30 clusters of 4 and 15 of 8 CTAs fit an H100 SXM (120 SMs, against 66 pairs on all 132), and the whole
+      // search measured no faster on any of them beyond run-to-run noise at C2 and slower at C5 (DESIGN §7)
+      const int cq = ix->scan_cq ? ix->scan_cq : 2, cx = ix->scan_cx ? ix->scan_cx : 1;
+      int clusters = 0;
+      e = launch_scan_cluster(cq, cx, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C,
+                              row_base, L.allow, sms, st, &clusters);
+      ix->st_scan_cluster = 10 * cq + cx;
+      ix->st_scan_clusters = clusters;
+    } else {
+      e = launch_scan_core(dense, L.allow, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow,
+                           C, row_base, sms, st);
+    }
+    if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
+  } else {
+    // the filter variant (a filtered exact round) keeps the queries' excluded ids in shared memory after the queries
+    const bool exact_filter = L.allow || L.ex.off;
+    Excluded ex = L.ex;
+    ex.q_base = q0;
+    const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
+    const int nqt = std::max(1, std::min(8, (96 * 1024) / (ix->d * 4)));
+    dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
+              static_cast<unsigned>((nqc + nqt - 1) / nqt));
+    const size_t smem = static_cast<size_t>(nqt) * ix->d * 4 + (exact_filter ? 8 * kMaxExcluded * 4 : 0);
+    with_rows(ix, [&](const auto* xs) {
+      using RowT = std::decay_t<decltype(*xs)>;
+      const auto kernel = exact_filter ? exact_scan_kernel<8, 2, RowT, true> : exact_scan_kernel<8, 2, RowT>;
+      kernel<<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, row_base, qf, nqc, ix->d, nqt, L.thr, L.cand,
+                                      L.count, overflow, C, dense ? 1 : 0, L.allow, exact_filter ? ex : Excluded{});
+    });
     OM_CUDA(cudaGetLastError());
-    ix->st_launches += 1;
-  } else if (mode == 0) {
-    rows_to_f16_kernel<<<grid_for(nq, 8), 256, 0, st>>>(qf, L.qh, nq, d, dpad, L.hn, L.en, nullptr);
-    OM_CUDA(cudaGetLastError());
-    ix->st_launches += 1;
   }
   return 0;
 }
@@ -1361,9 +1654,6 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
     OM_CUDA(cudaGetLastError());
     return 0;
   }
-  const __half* qh = L.qh + static_cast<size_t>(q0) * ix->dpad;
-  const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
-  int* overflow = L.status;
   int64_t pos = 0;
   const size_t sel_smem = static_cast<size_t>(C) * 8;
   bool first = true;
@@ -1372,9 +1662,6 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
   // survives, and select counts the list, which holds allowed rows only.  Later rounds filter as usual.  The exact scan
   // drops excluded ids as well, so its lists (k rows) hold no excluded row either.
   const bool sparse_first = L.allow || (L.mode == 1 && L.ex.off);
-  const bool exact_filter = L.mode == 1 && sparse_first;
-  Excluded ex = L.ex;
-  ex.q_base = q0;
   // With a bitmap, rounds are sized in allowed rows (ix->allow_prefix, per 256-row block), as they would be in rows on an
   // index of the allowed rows alone: the first round takes up to C allowed rows, a doubling round (growth - 1) x the
   // allowed rows seen, a safe round C - kp.  So a round at threshold -inf (fewer than kp allowed rows seen) cannot
@@ -1406,56 +1693,7 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
     // a first round of allowed rows only (an allow-all bitmap, a sub-collection at the start of the shard) stores densely
     // as the unfiltered search does: nothing there for the filter to drop
     const bool dense = first && (!sparse_first || (L.mode == 0 && L.allow && A[(pos + step + 255) / 256] == step));
-    {
-      Timed t(ix, st, 0);
-      const int ncols = static_cast<int>(step);
-      const uint32_t row_base = static_cast<uint32_t>(pos);
-      if (L.mode == 0 && ix->storage == OM_I8) {
-        // every round on the int8 scan (pair_scan and the cluster shape do not apply)
-        const int8_t* qhi = L.q8 + static_cast<size_t>(q0) * ix->dpad;
-        const int8_t* qlo = L.q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
-        const int64_t pitch = pitch_of(ix->xq, ix->d);
-        const cudaError_t e = launch_scan_i8(dense, L.allow, qhi, qlo, ix->dpad, L.qsig + q0, ix->xq + pos * pitch, pitch,
-                                             ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C, row_base, sms,
-                                             st);
-        if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
-      } else if (L.mode == 0) {
-        const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
-        cudaError_t e;
-        // a cluster owns at least 2 x 128 query rows per tile: with <= 128 queries the peers' boxes would be padding (and the sweep is
-        // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
-        // first, dense round (C rows, every score stored) stays on the single-CTA kernel as well.
-        const bool pair = ix->pair_scan != 0 && nqc > kBlockM;
-        if (!dense && pair) {
-          // cluster shape CQ x CX: the index parameters, else 2 x 1.  The wider shapes cut L2 -> SM traffic by 25 - 50 %, but
-          // only 30 clusters of 4 and 15 of 8 CTAs fit an H100 SXM (120 SMs, against 66 pairs on all 132), and the whole
-          // search measured no faster on any of them beyond run-to-run noise at C2 and slower at C5 (DESIGN §7)
-          const int cq = ix->scan_cq ? ix->scan_cq : 2, cx = ix->scan_cx ? ix->scan_cx : 1;
-          int clusters = 0;
-          e = launch_scan_cluster(cq, cx, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
-                                  overflow, C, row_base, L.allow, sms, st, &clusters);
-          ix->st_scan_cluster = 10 * cq + cx;
-          ix->st_scan_clusters = clusters;
-        } else {
-          e = launch_scan_core(dense, L.allow, qh, ix->dpad, xrows, ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count,
-                               overflow, C, row_base, sms, st);
-        }
-        if (e != cudaSuccess) return fail(OM_ECUDA, "scan kernel launch failed: %s", cudaGetErrorString(e));
-      } else {
-        const int nqt = std::max(1, std::min(8, (96 * 1024) / (ix->d * 4)));
-        dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
-                  static_cast<unsigned>((nqc + nqt - 1) / nqt));
-        // the filter variant keeps the queries' excluded ids in shared memory after the queries
-        const size_t smem = static_cast<size_t>(nqt) * ix->d * 4 + (exact_filter ? 8 * kMaxExcluded * 4 : 0);
-        with_rows(ix, [&](const auto* xs) {
-          using RowT = std::decay_t<decltype(*xs)>;
-          const auto kernel = exact_filter ? exact_scan_kernel<8, 2, RowT, true> : exact_scan_kernel<8, 2, RowT>;
-          kernel<<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, row_base, qf, nqc, ix->d, nqt, L.thr, L.cand,
-                                          L.count, overflow, C, dense ? 1 : 0, L.allow, exact_filter ? ex : Excluded{});
-        });
-        OM_CUDA(cudaGetLastError());
-      }
-    }
+    OM_TRY(scan_round(ix, L, q0, nqc, pos, step, dense, sms, st));
     {
       Timed t(ix, st, 1);
       select_kernel<<<nqc, 256, sel_smem, st>>>(L.cand, L.count, L.thr, C, kp, dense ? static_cast<int>(step) : -1);
@@ -1812,6 +2050,8 @@ int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const
                             : (check ? "om_index_search_filtered" : "om_index_search");
   if (!ix || (sharded && !comm) || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
     return fail(OM_EINVAL, "%s: bad arguments (nq=%d k=%d)", who, nq, k);
+  ix->r_total = -1;  // a search ends the last range search's results
+  ix->rout.release();
   if (nq == 0) return 0;
   OM_TRY(device_sm_count());
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1820,7 +2060,453 @@ int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const
   return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
 }
 
+// ---- range search ---------------------------------------------------------------------------------------------------
+// A list count starts a round at most kRangeMaxList (its fill) and a round adds at most kRangeRound: 2^30 + 2^29 < 2^31, so
+// the scans' int counters cannot wrap.
+constexpr int64_t kRangeRound = int64_t(1) << 29;  // rows per scan round
+constexpr int kRangeMaxList = 1 << 30;             // longest candidate list of one query
+
+// Grows b to `need` bytes, keeping its first `keep` bytes.
+int grow_keep(DevBuf& b, size_t keep, size_t need, cudaStream_t st) {
+  if (need <= b.bytes) return 0;
+  need = std::max(need, b.bytes + b.bytes / 2);
+  void* p = nullptr;
+  if (dev_malloc(&p, need) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(OM_ENOMEM, "range search: cannot allocate %zu bytes of results", need);
+  }
+  if (keep) OM_CUDA(cudaMemcpyAsync(p, b.p, keep, cudaMemcpyDeviceToDevice, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  b.release();
+  b.p = p;
+  b.bytes = need;
+  return 0;
+}
+
+// Per query of one range sweep: the candidates the scans counted, the rows above rho among them (when they fit) and
+// whether the query needs the exact scan.
+struct RangeSweep {
+  std::vector<long long> total;
+  std::vector<int> surv, to_exact;
+};
+
+// One sweep of a range search over queries list[0, m) (rows of qf / rho) with lists of C keys: mode 0 the tensor-core
+// scan at t(q), mode 1 the exact scan at rho; then re-score, cut and sort of every list that holds all its query's
+// candidates.  One host synchronisation; the answered queries' sorted keys are appended to ix->rkeys at *stored, and
+// src[g] / cnt[g] record where and how many for query g.
+int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vector<int>& list, int mode, int C, int sms,
+                int64_t* stored, std::vector<int64_t>& src, std::vector<int64_t>& cnt, RangeSweep& r, cudaStream_t st) {
+  const int m = static_cast<int>(list.size()), d = ix->d;
+  const size_t M = m;
+  const bool long_lists = C > kRangeSortKeys;
+  size_t off = 0;
+  auto carve = [&](size_t bytes) {
+    size_t o = off;
+    off += round_up(bytes, 256);
+    return o;
+  };
+  const size_t o_list = carve(M * 4), o_q = carve(M * d * 4), o_rho = carve(M * 4), o_qh = carve(M * ix->dpad * 2),
+               o_hn = carve(M * 4), o_en = carve(M * 4), o_sig = carve(M * 8), o_cand = carve(M * C * 8),
+               o_alt = carve(long_lists ? M * C * 8 : 0), o_count = carve(M * 4), o_filled = carve(M * 4),
+               o_total = carve(M * 8), o_thr = carve(M * 4), o_surv = carve(M * 4), o_exact = carve(M * 4),
+               o_off = carve(M * 8), o_status = carve(256);
+  if (C == ix->range_list) ix->r_keep_ws = std::max(ix->r_keep_ws, off);  // a first sweep's workspace
+  if (ix->ws.reserve(off) != 0) {
+    cudaGetLastError();
+    return fail(OM_ENOMEM, "range search: cannot allocate candidate lists of %d queries x %d rows", m, C);
+  }
+  uint8_t* b = static_cast<uint8_t*>(ix->ws.p);
+  int* dlist = reinterpret_cast<int*>(b + o_list);
+  float* q = reinterpret_cast<float*>(b + o_q);
+  float* rq = reinterpret_cast<float*>(b + o_rho);
+  int* filled = reinterpret_cast<int*>(b + o_filled);
+  long long* total = reinterpret_cast<long long*>(b + o_total);
+  int* surv = reinterpret_cast<int*>(b + o_surv);
+  int* to_exact = reinterpret_cast<int*>(b + o_exact);
+  long long* doff = reinterpret_cast<long long*>(b + o_off);
+  unsigned long long* alt = reinterpret_cast<unsigned long long*>(b + o_alt);
+  Level L;
+  L.nq = m;
+  L.C = C;
+  L.mode = mode;
+  L.qf = q;
+  L.qh = reinterpret_cast<__half*>(b + o_qh);
+  L.q8 = reinterpret_cast<int8_t*>(b + o_qh);
+  L.qsig = reinterpret_cast<float2*>(b + o_sig);
+  L.hn = reinterpret_cast<float*>(b + o_hn);
+  L.en = reinterpret_cast<float*>(b + o_en);
+  L.cand = reinterpret_cast<unsigned long long*>(b + o_cand);
+  L.count = reinterpret_cast<int*>(b + o_count);
+  L.thr = reinterpret_cast<float*>(b + o_thr);
+  L.status = reinterpret_cast<int*>(b + o_status);
+  OM_CUDA(cudaMemcpyAsync(dlist, list.data(), M * 4, cudaMemcpyHostToDevice, st));
+  gather_rows_kernel<<<grid_for(static_cast<int64_t>(m) * d, 256), 256, 0, st>>>(qf, dlist, m, d, q);
+  gather_rows_kernel<<<grid_for(m, 256), 256, 0, st>>>(rho, dlist, m, 1, rq);
+  OM_CUDA(cudaGetLastError());
+  if (mode == 0) OM_TRY(convert_queries(ix, L, st));
+  range_threshold_kernel<<<(m + 255) / 256, 256, 0, st>>>(rq, L.hn, L.en, ix->gstats, d, m, mode, L.thr, to_exact);
+  OM_CUDA(cudaMemsetAsync(L.count, 0, M * 4, st));
+  OM_CUDA(cudaMemsetAsync(filled, 0, M * 4, st));
+  OM_CUDA(cudaMemsetAsync(total, 0, M * 8, st));
+  OM_CUDA(cudaMemsetAsync(surv, 0, M * 4, st));
+  OM_CUDA(cudaMemsetAsync(L.status, 0, 32, st));
+  ix->st_launches += 4;
+  // the sweep: one pass over the shard at the fixed thresholds, in rounds only to keep the column counts in an int
+  for (int64_t pos = 0; pos < ix->n; pos += kRangeRound) {
+    OM_TRY(scan_round(ix, L, 0, m, pos, std::min(ix->n - pos, kRangeRound), false, sms, st));
+    range_fold_kernel<<<(m + 255) / 256, 256, 0, st>>>(L.count, filled, total, C, m);
+    OM_CUDA(cudaGetLastError());
+    ix->st_rounds++;
+    ix->st_launches += 2;
+  }
+  {
+    Timed t(ix, st, 2);
+    with_rows(ix, [&](const auto* xs) {
+      using RowT = std::decay_t<decltype(*xs)>;
+      // at least 32 CTAs per query, more when few queries would leave SMs idle (a handful of long lists)
+      const int gx = std::min((C + 63) / 64, std::max(32, (8 * sms + m - 1) / m));
+      range_rescore_kernel<RowT><<<dim3(gx, m), 256, static_cast<size_t>(d) * 4, st>>>(
+          L.cand, L.count, total, C, q, xs, d, rq, surv);
+    });
+    int P = 2;
+    while (P < std::min(C, kRangeSortKeys)) P <<= 1;
+    range_sort_kernel<<<dim3((C + kRangeSortKeys - 1) / kRangeSortKeys, m), 512, static_cast<size_t>(P) * 8, st>>>(L.cand, L.count,
+                                                                                                                  total, C);
+    ix->st_launches += 2;
+  }
+  OM_CUDA(cudaGetLastError());
+  unsigned long long *from = L.cand, *to = alt;
+  int merges = 0;
+  for (int w = kRangeSortKeys; w < C; w <<= 1, ++merges) {
+    range_merge_kernel<<<dim3(std::min((C + 255) / 256, 4096), m), 256, 0, st>>>(from, to, L.count, total, C, w);
+    std::swap(from, to);
+    ix->st_launches += 1;
+  }
+  OM_CUDA(cudaGetLastError());
+  r.total.resize(m);
+  r.surv.resize(m);
+  r.to_exact.resize(m);
+  OM_CUDA(cudaMemcpyAsync(r.total.data(), total, M * 8, cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaMemcpyAsync(r.surv.data(), surv, M * 4, cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaMemcpyAsync(r.to_exact.data(), to_exact, M * 4, cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  const unsigned int fault = read_clear_dev_fault();
+  if (fault) return fail(OM_EFAULT, "scan kernel pipeline fault 0x%08x", fault);
+  // the queries this sweep answered: their keys go to the store, in list order
+  std::vector<long long> hoff(m, -1);
+  int64_t add = 0;
+  for (int i = 0; i < m; ++i) {
+    if ((mode == 0 && r.to_exact[i]) || r.total[i] > C) continue;
+    hoff[i] = *stored + add;
+    src[list[i]] = hoff[i];
+    cnt[list[i]] = r.surv[i];
+    add += r.surv[i];
+    ix->st_range_candidates += r.total[i];
+  }
+  if (add == 0) return 0;
+  OM_TRY(grow_keep(ix->rkeys, static_cast<size_t>(*stored) * 8, static_cast<size_t>(*stored + add) * 8, st));
+  OM_CUDA(cudaMemcpyAsync(doff, hoff.data(), M * 8, cudaMemcpyHostToDevice, st));
+  range_emit_kernel<<<dim3(std::min((C + 255) / 256, 1024), m), 256, 0, st>>>(
+      L.cand, alt, (merges & 1) ? kRangeSortKeys : INT_MAX, L.count, surv, doff, C, static_cast<unsigned long long*>(ix->rkeys.p));
+  OM_CUDA(cudaGetLastError());
+  ix->st_launches += 1;
+  *stored += add;
+  return 0;
+}
+
+// The range search on this shard: every query swept once with lists of range_list keys; the queries whose candidates
+// overflowed their list are swept again in groups that fit the device, with lists sized from their counts (a re-sweep may
+// run another scan kernel, whose stage scores can differ in the last bit: hence the head-room and a bounded number of
+// attempts); queries without a finite certificate bound are swept by the exact scan.  cnt[g] rows above rho for query g
+// end sorted at ix->rkeys + src[g]; *stored keys in all.
+int range_local(om_index* ix, const float* qf, const float* rho, int nq, std::vector<int64_t>& src, std::vector<int64_t>& cnt,
+                int64_t* stored, cudaStream_t st) {
+  const int sms = device_sm_count();
+  if (sms < 0) return sms;
+  struct Job {
+    std::vector<int> qs;
+    int mode, C;
+  };
+  std::vector<Job> jobs;
+  auto add_chunks = [&](const std::vector<int>& qs, int mode) {
+    for (size_t i = 0; i < qs.size(); i += kQueryChunk)
+      jobs.push_back({std::vector<int>(qs.begin() + i, qs.begin() + std::min(qs.size(), i + kQueryChunk)), mode, ix->range_list});
+  };
+  src.assign(nq, -1);
+  cnt.assign(nq, 0);
+  *stored = 0;
+  std::vector<int> all(nq), tries(nq, 0);
+  for (int i = 0; i < nq; ++i) all[i] = i;
+  add_chunks(all, ix->exact_only ? 1 : 0);
+  ix->st_exact = ix->exact_only ? nq : 0;
+  for (size_t j = 0; j < jobs.size(); ++j) {
+    const Job job = jobs[j];  // a copy: jobs grows below
+    RangeSweep r;
+    OM_TRY(range_sweep(ix, qf, rho, job.qs, job.mode, job.C, sms, stored, src, cnt, r, st));
+    std::vector<int> exact;
+    std::vector<std::pair<long long, int>> over;  // (candidates, query)
+    for (size_t i = 0; i < job.qs.size(); ++i) {
+      if (job.mode == 0 && r.to_exact[i])
+        exact.push_back(job.qs[i]);
+      else if (r.total[i] > job.C)
+        over.push_back({r.total[i], job.qs[i]});
+    }
+    ix->st_exact += static_cast<int64_t>(exact.size());
+    add_chunks(exact, 1);
+    if (over.empty()) continue;
+    ix->st_range_resweeps += static_cast<int64_t>(over.size());
+    std::sort(over.begin(), over.end(), std::greater<std::pair<long long, int>>());
+    size_t free_b = 0, total_b = 0;
+    OM_CUDA(cudaMemGetInfo(&free_b, &total_b));
+    const size_t budget = (free_b + ix->ws.bytes) / 2;
+    for (size_t i = 0; i < over.size();) {
+      // the group's lists: the longest count of the group (the first) + 1/8 + 1024 of head-room
+      const long long cap = round_up(over[i].first + over[i].first / 8 + 1024, 256);
+      if (cap > kRangeMaxList)
+        return fail(OM_ENOMEM, "range search: query %d has %lld candidates; a list holds at most %d", over[i].second,
+                    over[i].first, kRangeMaxList);
+      const size_t per = static_cast<size_t>(cap) * 8 * (cap > kRangeSortKeys ? 2 : 1) + static_cast<size_t>(ix->d) * 8 + 256;
+      Job g{{}, job.mode, static_cast<int>(cap)};
+      do {
+        if (++tries[over[i].second] > 3) return fail(OM_EFAULT, "range search: a candidate list did not converge (bug)");
+        g.qs.push_back(over[i++].second);
+      } while (i < over.size() && g.qs.size() < static_cast<size_t>(kQueryChunk) && (g.qs.size() + 1) * per <= budget);
+      jobs.push_back(std::move(g));
+    }
+  }
+  return 0;
+}
+
+// The whole range search, unsharded or this rank's part of a sharded one: argument rules (a NaN radius, fp16 / int8 rows
+// holding inf or NaN) checked before anything is written, the shard's results, then with several ranks one all-gather of
+// the per-query counts, one all-gather of every shard's sorted results (padded to the largest) and the merge.  The lims
+// go to the caller, the results stay in the index (rout).
+int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, const float* radius, int64_t* lims,
+               om_memkind out_kind, int64_t id_offset, cudaStream_t st) {
+  NvtxRange nvtx("om.range_search");
+  const int d = ix->d;
+  // the sharded entry runs the exchange at every world size, one rank included
+  const bool sharded = comm != nullptr;
+  const int W = sharded ? comm->world : 1;
+  const int sms = device_sm_count();
+  if (sms < 0) return sms;
+  // What only long lists grow is returned when the call ends, however it ends: the level workspace beyond what it held
+  // before and what a first sweep needs (re-sweeps, the exchange), and a key store beyond 64 MB.  Smaller scratch stays
+  // for the next call; the results (rout) stay until the next search, range search, reset or destroy.
+  struct Scratch {
+    om_index* ix;
+    size_t ws0;
+    ~Scratch() {
+      if (ix->rkeys.bytes > (size_t(64) << 20)) ix->rkeys.release();
+      if (ix->ws.bytes > std::max(ws0, ix->r_keep_ws)) ix->ws.release();
+    }
+  } scratch{ix, ix->ws.bytes};
+  ix->r_keep_ws = 0;
+  ix->st_rounds = ix->st_retries = ix->st_launches = 0;
+  ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
+  ix->st_scan_cluster = ix->st_scan_clusters = 0;
+  ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
+  ix->st_range_candidates = ix->st_range_resweeps = 0;
+  ix->ev_used = 0;
+  OM_TRY(once_attrs(ix));
+  if (d > 16384) return fail(OM_EINVAL, "om_index_range_search: d > 16384 unsupported");
+  // whole-call staging: queries and radii that arrive from the host
+  const size_t o_q = 0, o_rho = round_up(q_kind == OM_HOST ? static_cast<size_t>(nq) * d * 4 : 0, 256);
+  OM_TRY(ix->ows.reserve(o_rho + round_up(static_cast<size_t>(nq) * 4, 256)));
+  uint8_t* ob = static_cast<uint8_t*>(ix->ows.p);
+  const float* qf = static_cast<const float*>(q);
+  const float* rho = radius;
+  if (q_kind == OM_HOST) {
+    OM_CUDA(cudaMemcpyAsync(ob + o_q, q, static_cast<size_t>(nq) * d * 4, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(ob + o_rho, radius, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, st));
+    qf = reinterpret_cast<const float*>(ob + o_q);
+    rho = reinterpret_cast<const float*>(ob + o_rho);
+  }
+  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
+  OM_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
+  check_radius_kernel<<<grid_for(nq, 256), 256, 0, st>>>(rho, nq, bad);
+  OM_CUDA(cudaGetLastError());
+  if (sharded) OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
+  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  if (ix->h_status[4]) return fail(OM_EINVAL, "om_index_range_search: a radius is NaN%s", sharded ? " (on some rank)" : "");
+  OM_TRY(check_finite_rows(ix, comm, st));
+
+  std::vector<int64_t> src, cnt;
+  int64_t stored = 0;
+  int rc = range_local(ix, qf, rho, nq, src, cnt, &stored, st);
+  // Every rank takes the same decision after a step that can fail on one rank alone (a re-sweep, an allocation): the
+  // largest error code of all ranks, through one all-reduce, before the next collective.
+  auto agree = [&](int rc_local) -> int {
+    if (!sharded) return rc_local;
+    cudaGetLastError();
+    fill_i32<<<1, 1, 0, st>>>(bad, rc_local < 0 ? -rc_local : 0, 1);
+    OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
+    OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
+    OM_CUDA(cudaStreamSynchronize(st));
+    if (rc_local == 0 && ix->h_status[4]) return fail(-ix->h_status[4], "om_index_range_search_sharded: another rank failed");
+    return rc_local;
+  };
+
+  std::vector<long long> ll(nq + 1, 0);  // this shard's lims
+  for (int i = 0; i < nq && rc == 0; ++i) ll[i + 1] = ll[i] + cnt[i];
+  const size_t NQ1 = static_cast<size_t>(nq) + 1;
+  std::vector<long long> plims, glims;  // every part's lims [W][nq + 1], the merged lims
+  size_t off = 0;
+  auto carve = [&](size_t bytes) {
+    size_t o = off;
+    off += round_up(bytes, 256);
+    return o;
+  };
+  const size_t o_src = carve(nq * 8), o_ll = carve(NQ1 * 8), o_plims = carve(W * NQ1 * 8), o_glims = carve(NQ1 * 8),
+               o_cnt = carve(nq * 8), o_all = carve(static_cast<size_t>(W) * nq * 8);
+  if (rc == 0 && ix->ws.reserve(off) != 0) {
+    cudaGetLastError();
+    rc = fail(OM_ENOMEM, "range search: cannot allocate the lims of %d queries", nq);
+  }
+  OM_TRY(agree(rc));
+  uint8_t* b = static_cast<uint8_t*>(ix->ws.p);
+  const unsigned long long* keys = static_cast<const unsigned long long*>(ix->rkeys.p);
+  auto outputs = [&](int64_t T, float** D, int64_t** I) -> int {
+    if (ix->rout.reserve(round_up(T * 4, 256) + T * 8 + 256) != 0) {
+      cudaGetLastError();
+      return fail(OM_ENOMEM, "range search: cannot allocate %lld results", (long long)T);
+    }
+    *D = static_cast<float*>(ix->rout.p);
+    *I = reinterpret_cast<int64_t*>(static_cast<uint8_t*>(ix->rout.p) + round_up(T * 4, 256));
+    return 0;
+  };
+  // this shard's results in query order: one CTA row per query, enough CTAs per query to fill the device when few
+  // queries hold long lists
+  const long long cmax = nq > 0 ? *std::max_element(cnt.begin(), cnt.end()) : 0;
+  const dim3 gather_grid(static_cast<unsigned>(nq),
+                         static_cast<unsigned>(std::max<long long>(1, std::min<long long>({(cmax + 255) / 256,
+                                                                                          (8LL * sms + nq - 1) / nq, 65535}))));
+  auto gather = [&](float* D, int64_t* I) -> int {
+    OM_CUDA(cudaMemcpyAsync(b + o_src, src.data(), nq * 8, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(b + o_ll, ll.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
+    if (cmax > 0)
+      range_gather_kernel<<<gather_grid, 256, 0, st>>>(keys, reinterpret_cast<long long*>(b + o_src),
+                                                       reinterpret_cast<long long*>(b + o_ll), id_offset, D, I);
+    OM_CUDA(cudaGetLastError());
+    ix->st_launches += 1;
+    return 0;
+  };
+  int64_t T = ll[nq];
+  if (!sharded) {
+    float* D;
+    int64_t* I;
+    OM_TRY(outputs(T, &D, &I));
+    OM_TRY(gather(D, I));
+    glims = ll;
+  } else {
+    NcclApi& nc = nccl_api();
+    Timed t(ix, st, 3);
+    // counts of every shard
+    OM_CUDA(cudaMemcpyAsync(b + o_cnt, cnt.data(), nq * 8, cudaMemcpyHostToDevice, st));
+    OM_NCCL(nc.AllGather(b + o_cnt, b + o_all, static_cast<size_t>(nq) * 8, kNcclInt8, comm->nccl, st));
+    std::vector<long long> all(static_cast<size_t>(W) * nq);
+    OM_CUDA(cudaMemcpyAsync(all.data(), b + o_all, all.size() * 8, cudaMemcpyDeviceToHost, st));
+    OM_CUDA(cudaStreamSynchronize(st));
+    plims.assign(W * NQ1, 0);
+    glims.assign(NQ1, 0);
+    long long tmax = 0;
+    for (int p = 0; p < W; ++p) {
+      for (int i = 0; i < nq; ++i) plims[p * NQ1 + i + 1] = plims[p * NQ1 + i] + all[static_cast<size_t>(p) * nq + i];
+      tmax = std::max(tmax, plims[p * NQ1 + nq]);
+    }
+    for (int i = 0; i < nq; ++i) {
+      long long c = 0;
+      for (int p = 0; p < W; ++p) c += all[static_cast<size_t>(p) * nq + i];
+      glims[i + 1] = glims[i] + c;
+    }
+    T = glims[nq];
+    // every shard's sorted results, padded to the longest: [D f32 tmax | I i64 tmax], and the merged results; both
+    // allocated, and the outcome agreed, before the results' all-gather
+    const size_t o_i = round_up(tmax * 4, 256), blk = o_i + round_up(tmax * 8, 256) + 256;
+    const size_t o_send = carve(blk), o_recv = carve(blk * W);
+    float* D = nullptr;
+    int64_t* I = nullptr;
+    int rc2 = 0;
+    if (ix->ws.reserve(off) != 0) {
+      cudaGetLastError();
+      rc2 = fail(OM_ENOMEM, "range search: cannot allocate the exchange of %lld results per shard", tmax);
+    }
+    if (rc2 == 0) rc2 = outputs(T, &D, &I);
+    OM_TRY(agree(rc2));
+    b = static_cast<uint8_t*>(ix->ws.p);  // possibly a new buffer: the uploads above were read by the all-gather already
+    OM_CUDA(cudaMemcpyAsync(b + o_plims, plims.data(), W * NQ1 * 8, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(b + o_glims, glims.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
+    OM_TRY(gather(reinterpret_cast<float*>(b + o_send), reinterpret_cast<int64_t*>(b + o_send + o_i)));
+    OM_NCCL(nc.AllGather(b + o_send, b + o_recv, blk, kNcclInt8, comm->nccl, st));
+    if (tmax > 0)
+      range_merge_parts_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((tmax + 255) / 256, 4096)), W), 256, 0, st>>>(
+          reinterpret_cast<const float*>(b + o_recv), reinterpret_cast<const int64_t*>(b + o_recv + o_i),
+          static_cast<int64_t>(blk / 4), static_cast<int64_t>(blk / 8), reinterpret_cast<const long long*>(b + o_plims), W, nq,
+          reinterpret_cast<const long long*>(b + o_glims), D, I);
+    OM_CUDA(cudaGetLastError());
+    ix->st_launches += 3;
+  }
+  if (out_kind == OM_HOST)
+    memcpy(lims, glims.data(), NQ1 * 8);
+  else
+    OM_CUDA(cudaMemcpyAsync(lims, glims.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  if (ix->profile) collect_profile(ix);
+  ix->r_total = T;
+  return 0;
+}
+
+int range_entry(bool sharded, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, const float* radius,
+                int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream) {
+  const char* who = sharded ? "om_index_range_search_sharded" : "om_index_range_search";
+  if (!ix || (sharded && !comm) || nq < 0 || !lims || (nq > 0 && (!q || !radius)))
+    return fail(OM_EINVAL, "%s: bad arguments (nq=%d)", who, nq);
+  ix->r_total = -1;
+  OM_TRY(device_sm_count());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (nq == 0) {  // lims = {0}, no results
+    if (out_kind == OM_HOST) {
+      lims[0] = 0;
+    } else {
+      OM_CUDA(cudaMemsetAsync(lims, 0, 8, st));
+      OM_CUDA(cudaStreamSynchronize(st));
+    }
+    ix->r_total = 0;
+    return 0;
+  }
+  OM_TRY(settle_reset(ix, st));
+  return range_impl(ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, st);
+}
+
 }  // namespace
+
+extern "C" int om_index_range_search(om_index* ix, const void* q, om_memkind q_kind, int nq, const float* radius,
+                                     int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream) {
+  return range_entry(false, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, stream);
+}
+
+extern "C" int om_index_range_search_sharded(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                                             const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset,
+                                             void* stream) {
+  return range_entry(true, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, stream);
+}
+
+extern "C" int om_index_range_results(const om_index* ix, float* D, int64_t* I, om_memkind out_kind, void* stream) {
+  if (!ix) return fail(OM_EINVAL, "om_index_range_results: null index");
+  if (ix->r_total < 0) return fail(OM_ESTATE, "om_index_range_results: no range search result on this index");
+  const int64_t T = ix->r_total;
+  if (T == 0) return 0;
+  if (!D || !I) return fail(OM_EINVAL, "om_index_range_results: null output");
+  OM_TRY(device_sm_count());
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const cudaMemcpyKind kind = out_kind == OM_HOST ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+  const uint8_t* p = static_cast<const uint8_t*>(ix->rout.p);
+  OM_CUDA(cudaMemcpyAsync(D, p, T * 4, kind, st));
+  OM_CUDA(cudaMemcpyAsync(I, p + round_up(T * 4, 256), T * 8, kind, st));
+  OM_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
 
 extern "C" int om_index_search(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
                                om_memkind out_kind, int64_t id_offset, void* stream) {

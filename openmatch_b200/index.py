@@ -106,6 +106,22 @@ def _filter(n: int, nq: int, device, allow, exclude):
     return f, keep
 
 
+def range_radius(radius, nq: int, device=None) -> torch.Tensor:
+    """The per-query radii of a range search as float32 ``[nq]``: a number is broadcast, an array must hold ``nq``."""
+    if isinstance(radius, (int, float, np.floating, np.integer)):
+        r = torch.full((nq,), float(radius), dtype=torch.float32)
+    else:
+        r = _as_tensor(np.asarray(radius, dtype=np.float32) if isinstance(radius, (list, tuple)) else radius)
+        if r.dim() == 0:
+            r = r.reshape(1).expand(nq)
+        if r.dim() != 1 or r.numel() != nq:
+            raise ValueError("radius must be a number or hold one value per query ([%d]), got shape %s"
+                             % (nq, tuple(r.shape)))
+        r = r.float()
+    r = r.contiguous()
+    return r.to(device) if device is not None else r
+
+
 class FlatIPIndex:
     """``faiss.IndexFlatIP`` duck type (``d``, ``ntotal``, ``add``, ``search``, ``reset``) living on the
     current CUDA device.
@@ -264,6 +280,43 @@ class FlatIPIndex:
         self._search(None, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], k, D_host.data_ptr(), I_host.data_ptr(),
                      _lib.OM_HOST, id_offset)
 
+    # ---- range search ----
+    def range_search(self, q, radius, id_offset: int = 0) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """``lims, D, I = index.range_search(q, radius)`` (faiss's signature): for query i every row whose score is
+        strictly greater than ``radius`` (a float, or one per query), at ``D[lims[i]:lims[i + 1]]`` /
+        ``I[lims[i]:lims[i + 1]]`` ordered by (score desc, id asc).  The first j results of a query are bitwise
+        ``search(q, j)``'s for j <= 4096.  numpy outputs (int64 [nq + 1], float32, int64)."""
+        if not isinstance(q, torch.Tensor):
+            q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
+        lims, D, I = self.range_search_device(q.cuda(), radius, id_offset)
+        return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()
+
+    def range_search_device(self, q: torch.Tensor, radius, id_offset: int = 0):
+        """:meth:`range_search` with CUDA tensors in and out: (lims int64 [nq + 1], D float32, I int64)."""
+        return self._range(None, q, radius, id_offset)
+
+    def range_search_sharded_device(self, comm: "Comm", q: torch.Tensor, radius, id_offset: int = 0):
+        """This rank's call of the row-sharded range search (``om_index_range_search_sharded``): collective over
+        ``comm``; every rank passes the same queries and radii and receives the same global (lims, D, I)."""
+        return self._range(comm, q, radius, id_offset)
+
+    def _range(self, comm, q: torch.Tensor, radius, id_offset: int):
+        q = q.detach().contiguous().float()
+        self._check_shape(q.shape)
+        nq = q.shape[0]
+        rho = range_radius(radius, nq, q.device)
+        lims = torch.empty(nq + 1, dtype=torch.int64)
+        head = (self._h,) if comm is None else (self._h, comm._h)
+        fn = self._lib.om_index_range_search if comm is None else self._lib.om_index_range_search_sharded
+        _lib.check(fn(*head, q.data_ptr(), _lib.OM_DEVICE, nq, rho.data_ptr(), lims.data_ptr(), _lib.OM_HOST,
+                      int(id_offset), _stream()))
+        total = int(lims[-1])
+        D = torch.empty(total, dtype=torch.float32, device=q.device)
+        I = torch.empty(total, dtype=torch.int64, device=q.device)
+        _lib.check(self._lib.om_index_range_results(self._h, D.data_ptr() or None, I.data_ptr() or None, _lib.OM_DEVICE,
+                                                    _stream()))
+        return lims.to(q.device), D, I
+
     def _rows_at(self, n: int):
         """(device address, row pitch in elements) of the shard's rows after reserving room for n more"""
         p, pitch = ctypes.c_void_p(), ctypes.c_int64()
@@ -419,6 +472,16 @@ def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offs
     return index.search_sharded_device(comm_for(group), q, k, id_offset, allow=allow, exclude=exclude)
 
 
+def sharded_range_search_device(index: "FlatIPIndex", q: torch.Tensor, radius, id_offset: int, group=None):
+    """Row-sharded exact range search: every rank passes the same queries and radii and its own shard's ``id_offset``
+    and receives the same global (lims, D, I), bitwise one index's range search over the concatenated shards.  Without
+    a process group, or with one rank: the single-shard range search."""
+    import torch.distributed as dist
+    if not dist.is_initialized() or dist.get_world_size(group) == 1:
+        return index.range_search_device(q, radius, id_offset)
+    return index.range_search_sharded_device(comm_for(group), q, radius, id_offset)
+
+
 def shard_offsets(n_local: int, group=None):
     """(global id of this rank's first row, total rows) for rank-major contiguous shards."""
     import torch.distributed as dist
@@ -465,3 +528,13 @@ class ShardedFlatIPIndex:
             q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
         D, I = self.search_device(q.cuda(), k, allow=allow, exclude=exclude)
         return D.cpu().numpy(), I.cpu().numpy()
+
+    def range_search_device(self, q: torch.Tensor, radius):
+        return sharded_range_search_device(self.local, q, radius, self.offset, self.group)
+
+    def range_search(self, q, radius):
+        """(lims, D, I) numpy over the global ids, the same on every rank."""
+        if not isinstance(q, torch.Tensor):
+            q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
+        lims, D, I = self.range_search_device(q.cuda(), radius)
+        return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()

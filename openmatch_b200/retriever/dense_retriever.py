@@ -30,7 +30,7 @@ from tqdm import tqdm
 from ..arguments import InferenceArguments as EncodingArguments
 from ..dataset import DRInferenceCollator
 from ..embedding_store import EmbeddingFile, write_embedding_file
-from ..index import FlatIPIndex, comm_for, shard_offsets
+from ..index import FlatIPIndex, comm_for, range_radius, shard_offsets
 from ..modeling import DRModelForInference
 from ..utils import merge_retrieval_results_by_score
 
@@ -48,6 +48,14 @@ def _results_dict(query_ids: List[str], doc_lookup: np.ndarray, D: np.ndarray, I
         out[str(qid)] = dict(zip(names, scores[qi][: len(names)])) if valid.all() else \
             dict(zip(names, np.asarray(scores[qi])[valid].tolist()))
     return out
+
+
+def _range_dict(query_ids: List[str], doc_lookup: np.ndarray, lims: np.ndarray, D: np.ndarray, I: np.ndarray):
+    """{qid: {docid: score}} of a range search, each query's documents in rank order."""
+    scores = D.tolist()
+    names = doc_lookup[I].tolist() if len(I) else []
+    return {str(qid): dict(zip(names[lims[qi]:lims[qi + 1]], scores[lims[qi]:lims[qi + 1]]))
+            for qi, qid in enumerate(query_ids)}
 
 
 def doc_filter(doc_lookup, query_ids, allowed_docs=None, exclude=None, id_offset: int = 0):
@@ -378,6 +386,34 @@ class Retriever:
         names = np.array([d for part in lookups for d in part])
         result = RankArrays(self.query_lookup, names, D.cpu().numpy(), I.cpu().numpy())
         return result if as_arrays else result.to_dict()
+
+    def range_search(self, radius):
+        """Every document whose score is strictly above ``radius`` (a float, or one per query in query order) as
+        ``{qid: {docid: score}}``, each query's documents in rank order (``FlatIPIndex.range_search``).  Sharded: every
+        rank takes part and rank 0 builds the result; the other ranks return ``{}``."""
+        if self.index is None:
+            raise ValueError("Index is not initialized")
+        encoded = self._load_queries()
+        radius = range_radius(radius, encoded.shape[0]).numpy()
+        if self.args.world_size > 1:
+            return self._range_search_sharded(encoded, radius)
+        lims, D, I = self.index.range_search(encoded, radius)
+        return _range_dict(self.query_lookup, np.array(self.doc_lookup), lims, D, I)
+
+    def _range_search_sharded(self, encoded: np.ndarray, radius: np.ndarray):
+        dist = torch.distributed
+        W, r = self.args.world_size, self.args.process_index
+        if self.index is None:  # this rank holds no rows (fewer embedding files than ranks)
+            self._initialize_faiss_index(encoded.shape[1])
+        offset, _ = shard_offsets(len(self.doc_lookup))
+        q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
+        lims, D, I = self.index.range_search_sharded_device(comm_for(None), q, torch.from_numpy(radius), offset)
+        lookups = [None] * W if r == 0 else None
+        dist.gather_object(self.doc_lookup, lookups, dst=0)
+        if r != 0:
+            return {}
+        names = np.array([d for part in lookups for d in part])
+        return _range_dict(self.query_lookup, names, lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy())
 
     def retrieve(self, query_dataset: IterableDataset, topk: int = 100, as_arrays: bool = False, allowed_docs=None,
                  exclude=None):
