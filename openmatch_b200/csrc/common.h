@@ -43,6 +43,22 @@ int device_sm_count();
 
 static inline int64_t round_up(int64_t x, int64_t m) { return (x + m - 1) / m * m; }
 
+// Layout of one device workspace: add() places a region of `region_bytes` at the next 256-byte boundary and returns its
+// byte offset; `bytes` is the size the regions need.
+struct Layout {
+  size_t bytes = 0;
+  size_t add(size_t region_bytes) {
+    const size_t o = bytes;
+    bytes += round_up(region_bytes, 256);
+    return o;
+  }
+};
+// The region at byte offset `off` of the workspace at `base`.
+template <class T>
+static inline T* region(void* base, size_t off) {
+  return reinterpret_cast<T*>(static_cast<uint8_t*>(base) + off);
+}
+
 // cudaMalloc for the handles' storage and workspaces.  With OPENMATCH_B200_POISON_ALLOC=1 in the environment every fresh
 // buffer is first filled with 0xFF bytes (NaN in fp32, bf16 and fp16), so that tests can tell a read of never-written
 // memory from the driver's zero-filled pages.  Testing only: it synchronises the device on every allocation.

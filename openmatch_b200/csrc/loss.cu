@@ -570,16 +570,11 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
   // aligned bf16 inputs are read in place by TMA (row pitch = d elements must be a multiple of 16 bytes)
   const bool direct = dtype == OM_BF16 && d % 8 == 0 && ((reinterpret_cast<uintptr_t>(Q) | reinterpret_cast<uintptr_t>(P)) & 15) == 0 &&
                       !loss_knobs().copy_inputs;
-  size_t off = 0;
-  auto carve = [&](size_t bytes) {
-    size_t o = off;
-    off += round_up(bytes, 256);
-    return o;
-  };
-  const size_t o_qb = carve(direct ? 0 : (size_t)nq * dpad * 2), o_pb = carve(direct ? 0 : (size_t)np * dpad * 2);
-  const size_t o_s = carve(scores_out ? 0 : (size_t)nq * np * 4);
-  const size_t o_g = carve((size_t)nq * npp * 2);
-  const size_t o_rl = carve((size_t)nq * 4), o_flag = carve(256);
+  Layout lay;
+  const size_t o_qb = lay.add(direct ? 0 : (size_t)nq * dpad * 2), o_pb = lay.add(direct ? 0 : (size_t)np * dpad * 2);
+  const size_t o_s = lay.add(scores_out ? 0 : (size_t)nq * np * 4);
+  const size_t o_g = lay.add((size_t)nq * npp * 2);
+  const size_t o_rl = lay.add((size_t)nq * 4), o_flag = lay.add(256);
   // split-K of dQ: enough slices to spread its few tiles over the grid, >= 8 k-blocks per slice, at most 4 slices
   // (OM_LOSS_SPLITK overrides, for measurements)
   int dq_split = 1;
@@ -594,7 +589,8 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
       dq_split = (num_k + kper - 1) / kper;  // no empty slice
     }
   }
-  const size_t o_part = carve(dq_split > 1 ? (size_t)dq_split * nq * d * 4 : 0);
+  const size_t o_part = lay.add(dq_split > 1 ? (size_t)dq_split * nq * d * 4 : 0);
+  const size_t off = lay.bytes;
   if (off > ws.bytes) {
     if (ws.p) {
       // the workspace is process-global: the call that last used it may have run on another stream
@@ -612,7 +608,6 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
     // on `st`, ahead of the launch below: a legacy-stream memset is not ordered before a launch on a non-blocking stream
     OM_CUDA(cudaMemsetAsync(ws.grid_bar, 0, kLossBarBytes, st));
   }
-  uint8_t* base = static_cast<uint8_t*>(ws.p);
   LossArgs a;
   a.Q = Q;
   a.P = P;
@@ -626,18 +621,18 @@ extern "C" int om_contrastive_loss_fwd_bwd(const void* Q, const void* P, om_dtyp
   a.target = target;
   a.w = reduction == OM_REDUCE_MEAN ? 1.0f / nq : 1.0f;
   a.loss_scale = loss_scale;
-  a.qb = reinterpret_cast<__nv_bfloat16*>(base + o_qb);
-  a.pb = reinterpret_cast<__nv_bfloat16*>(base + o_pb);
-  a.G = reinterpret_cast<__nv_bfloat16*>(base + o_g);
-  a.S = scores_out ? scores_out : reinterpret_cast<float*>(base + o_s);
-  a.row_loss = reinterpret_cast<float*>(base + o_rl);
+  a.qb = region<__nv_bfloat16>(ws.p, o_qb);
+  a.pb = region<__nv_bfloat16>(ws.p, o_pb);
+  a.G = region<__nv_bfloat16>(ws.p, o_g);
+  a.S = scores_out ? scores_out : region<float>(ws.p, o_s);
+  a.row_loss = region<float>(ws.p, o_rl);
   a.loss_out = loss_out;
   a.dQ = dQ;
   a.dP = dP;
-  a.bad_target = reinterpret_cast<int*>(base + o_flag);
+  a.bad_target = region<int>(ws.p, o_flag);
   a.grid_bar = ws.grid_bar;
   a.dq_split = dq_split;
-  a.dq_part = reinterpret_cast<float*>(base + o_part);
+  a.dq_part = region<float>(ws.p, o_part);
   a.dq_sem = ws.grid_bar + 64;
   a.ts = reinterpret_cast<unsigned long long*>(reinterpret_cast<uint8_t*>(ws.grid_bar) + kLossBarBytes - 64);
   a.sm_fast = (np % 4 == 0 && np <= kSoftmaxMaxCols && (reinterpret_cast<uintptr_t>(a.S) & 15) == 0 &&

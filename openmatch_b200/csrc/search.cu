@@ -612,32 +612,6 @@ __global__ void __launch_bounds__(256) certify_kernel(const float* __restrict__ 
   }
 }
 
-// list[0 .. count) = ascending indices i with flags[i] != 0 (one block; chunked block-wide scan)
-__global__ void __launch_bounds__(1024) compact_flags_kernel(const int* __restrict__ flags, int n, int* __restrict__ list) {
-  __shared__ int warp_sums[32];
-  __shared__ int base;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) base = 0;
-  __syncthreads();
-  for (int i0 = 0; i0 < n; i0 += 1024) {
-    const int i = i0 + tid;
-    const bool f = i < n && flags[i] != 0;
-    const unsigned b = __ballot_sync(0xffffffffu, f);
-    if (lane == 0) warp_sums[warp] = __popc(b);
-    __syncthreads();
-    int off = base;
-    for (int w = 0; w < warp; ++w) off += warp_sums[w];
-    if (f) list[off + __popc(b & ((1u << lane) - 1u))] = i;
-    __syncthreads();
-    if (tid == 0) {
-      int t = 0;
-      for (int w = 0; w < 32; ++w) t += warp_sums[w];
-      base += t;
-    }
-    __syncthreads();
-  }
-}
-
 // EXACT fp32 scan on the CUDA cores (the certificate's last resort and the "exact_only" test mode): one warp per
 // row group, queries of the tile in shared memory, rows of type RowT (as finalize_kernel reads them).
 // Per (query, row) the summation order is EXACTLY the one of finalize_kernel (lane-strided 4-element FMA chain, then the
@@ -782,7 +756,7 @@ __global__ void allow_block_counts_kernel(const uint32_t* __restrict__ allow, in
   }
 }
 
-// dst[i] = src[list[i]] (rows of d floats): the flagged queries of an escalation level
+// dst[i] = src[list[i]] (rows of d floats): the queries (or radii) of a sub-batch
 __global__ void gather_rows_kernel(const float* __restrict__ src, const int* __restrict__ list, int n, int d,
                                    float* __restrict__ dst) {
   for (int64_t i = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; i < static_cast<int64_t>(n) * d;
@@ -802,11 +776,6 @@ __global__ void scatter_results_kernel(const float* __restrict__ Dsub, const int
     D[o] = Dsub[i];
     I[o] = Isub[i];
   }
-}
-// out[i] = outer[inner[i]]: flagged-within-flagged -> indices into the full query set
-__global__ void compose_list_kernel(const int* __restrict__ outer, const int* __restrict__ inner, int n, int* out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = outer[inner[i]];
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1041,7 +1010,7 @@ struct DevBuf {  // grow-only device scratch
 };
 
 // One pass of the pipeline (scan -> select -> re-score [-> exchange -> merge] -> certify) over nq device-resident
-// queries; all pointers are carved from the index's level workspace.
+// queries; all pointers lie in the index's level workspace (level_layout).
 struct Level {
   int nq = 0, k = 0, kp = 0, kp_target = 0, C = 0, growth = 2, mode = 0, world = 1, kc = 0, nqc_max = 0;
   const float* qf = nullptr;  // [nq, d] fp32 (not owned by the workspace)
@@ -1069,8 +1038,9 @@ struct om_index {
   int8_t* xq = nullptr;  // int8 rows of quant_i8.cuh, pitch dpad + 16 bytes (dpad = d rounded up to 16)
   // device [4]: [0] max ||x||, [1] max ||x - x_h|| over the committed rows (float bit patterns); fp16 / int8 storage: [2]
   // rows with a non-finite element (fp16) or scale (int8) committed since the last reset (int), [3] scratch (int: rejected
-  // elements or rows of an add, the all-reduced [2] of a sharded search)
+  // elements or rows of an add, the all-reduced [2] of a sharded search, a filter's or the radii's check, an agreed error)
   float* gstats = nullptr;
+  int* scratch() const { return reinterpret_cast<int*>(gstats) + 3; }  // gstats[3]
   bool gstats_stale = false;  // set by om_index_reset: gstats[0..2] are zeroed on the stream of the next commit / search
   int64_t st_nonfinite = 0;   // gstats[2] as the last search read it
   int64_t rescore_slack = -1;
@@ -1095,7 +1065,7 @@ struct om_index {
   DevBuf ws, ows, sws;  // level workspace / whole-search staging / escalation sub-batch
   // filtered search with a bitmap: allowed rows in [0, min(256 b, n)) for b = 0 .. ceil(n / 256), set by check_filter
   std::vector<int64_t> allow_prefix;
-  int* h_status = nullptr;  // pinned host mirror of Level::status
+  int* h_status = nullptr;  // pinned host copy of the device ints a call decides on (read_decision)
   // range search: first list capacity per query; the last range search's results (D fp32 then I int64, r_total of each) in
   // rout, r_total = -1 when there are none (before any range search, after a search or a reset); rkeys: its key store
   int range_list = 4096;
@@ -1175,6 +1145,22 @@ static int settle_reset(om_index* ix, cudaStream_t st) {
   if (!ix->gstats_stale) return 0;
   OM_CUDA(cudaMemsetAsync(ix->gstats, 0, 3 * sizeof(float), st));
   ix->gstats_stale = false;
+  return 0;
+}
+
+#define OM_NCCL(expr)                                                                                   \
+  do {                                                                                                  \
+    int r__ = (expr);                                                                                   \
+    if (r__ != 0) return fail(OM_ECUDA, "%s failed: %s", #expr, nccl_api().GetErrorString(r__));        \
+  } while (0)
+
+// Reads the n device ints at `dev` into ix->h_status[0, n) with one host synchronisation, for the host to branch on.  With
+// a communicator (nullptr: none), dev[0] is first all-reduced over the ranks with op (kNcclMax or kNcclSum) into dev[to]
+// (0: in place, else an int within the n read), so that every rank takes the same decision.
+static int read_decision(om_index* ix, om_comm* comm, int* dev, int n, int op, int to, cudaStream_t st) {
+  if (comm) OM_NCCL(nccl_api().AllReduce(dev, dev + to, 1, kNcclInt32, op, comm->nccl, st));
+  OM_CUDA(cudaMemcpyAsync(ix->h_status, dev, n * sizeof(int), cudaMemcpyDeviceToHost, st));
+  OM_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -1304,7 +1290,7 @@ static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype 
   void* tmp = nullptr;
   OM_TRY(stage_input(x, kind, elems * (dtype == OM_F32 ? 4 : 2), st, &src, &tmp));
   const bool i8 = ix->storage == OM_I8;  // quantise, else convert to fp16
-  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
+  int* bad = ix->scratch();
   cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(int), st);
   if (e == cudaSuccess)
     e = with_input(src, dtype, [&](const auto* in) {
@@ -1315,16 +1301,16 @@ static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype 
                                                                                         ix->dpad, bad);
       return cudaGetLastError();
     });
-  if (e == cudaSuccess) e = cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  const int rc = e == cudaSuccess ? read_decision(ix, nullptr, bad, 1, kNcclMax, 0, st) : 0;
   if (tmp) cudaFree(tmp);
   OM_CUDA(e);
-  if (ix->h_status[4] > 0 && i8)
+  OM_TRY(rc);
+  if (ix->h_status[0] > 0 && i8)
     return fail(OM_EINVAL, "om_index_add: %d rows hold inf or NaN; int8 storage cannot hold them and no row was added",
-                ix->h_status[4]);
-  if (ix->h_status[4] > 0)
+                ix->h_status[0]);
+  if (ix->h_status[0] > 0)
     return fail(OM_EINVAL, "om_index_add: %d elements are NaN or round to +-inf in fp16 (|x| >= 65520); fp16 storage cannot "
-                "hold them and no row was added", ix->h_status[4]);
+                "hold them and no row was added", ix->h_status[0]);
   return om_index_commit(ix, n, st);
 }
 
@@ -1514,13 +1500,31 @@ int convert_queries(om_index* ix, Level& L, cudaStream_t st) {
   return 0;
 }
 
-// sizes the candidate lists of a level, carves the level workspace and converts the queries
+// A level's own buffers at the start of the level workspace: the scan operand and certificate norms of its nq queries,
+// the lists of C keys, counts and thresholds of nqc queries (one chunk), the status word.  Returns their bytes, after
+// which callers lay out their own regions; with the reserved workspace at base (else nullptr), points L's buffers there.
+size_t level_layout(Level& L, void* base, size_t nq, size_t nqc, int C, int dpad) {
+  Layout lay;
+  const size_t o_qh = lay.add(nq * dpad * 2), o_hn = lay.add(nq * 4), o_en = lay.add(nq * 4), o_cand = lay.add(nqc * C * 8),
+               o_count = lay.add(nqc * 4), o_thr = lay.add(nqc * 4), o_status = lay.add(256), o_sig = lay.add(nq * 8);
+  if (base) {
+    L.qh = region<__half>(base, o_qh);
+    L.q8 = region<int8_t>(base, o_qh);
+    L.qsig = region<float2>(base, o_sig);
+    L.hn = region<float>(base, o_hn);
+    L.en = region<float>(base, o_en);
+    L.cand = region<unsigned long long>(base, o_cand);
+    L.count = region<int>(base, o_count);
+    L.thr = region<float>(base, o_thr);
+    L.status = region<int>(base, o_status);
+  }
+  return lay.bytes;
+}
+
+// sizes the candidate lists of a level, lays out the level workspace and converts the queries
 int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp_target, int mode, int world,
                   cudaStream_t st) {
-  const int d = ix->d, dpad = ix->dpad;
-  if (d > 16384) return fail(OM_EINVAL, "om_index_search: d > 16384 unsupported");
   if (k > kMaxCandidates) return fail(OM_EINVAL, "om_index_search: k = %d exceeds %d", k, kMaxCandidates);
-  OM_TRY(once_attrs(ix));
   L.qf = qf;
   L.nq = nq;
   L.k = k;
@@ -1547,35 +1551,13 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   L.kc = std::min(k, L.kp_target);  // entries a shard ships per query (it cannot contribute more than k)
   L.nqc_max = std::min(nq, kQueryChunk);
   ix->st_capacity = L.C;
-  size_t off = 0;
-  auto carve = [&](size_t bytes) {
-    size_t o = off;
-    off += round_up(bytes, 256);
-    return o;
-  };
-  const size_t nqc = L.nqc_max;
-  const size_t o_qh = carve(static_cast<size_t>(nq) * dpad * 2), o_hn = carve(static_cast<size_t>(nq) * 4),
-               o_en = carve(static_cast<size_t>(nq) * 4), o_cand = carve(nqc * L.C * 8), o_count = carve(nqc * 4),
-               o_thr = carve(nqc * 4), o_status = carve(256), o_sig = carve(static_cast<size_t>(nq) * 8);
-  size_t o_send = 0, o_recv = 0;
-  if (world > 1) {
-    const size_t blk = exchange_block_bytes(nqc, L.kc);
-    o_send = carve(blk);
-    o_recv = carve(blk * world);
-  }
-  OM_TRY(ix->ws.reserve(off));
-  uint8_t* base = static_cast<uint8_t*>(ix->ws.p);
-  L.qh = reinterpret_cast<__half*>(base + o_qh);
-  L.q8 = reinterpret_cast<int8_t*>(base + o_qh);
-  L.qsig = reinterpret_cast<float2*>(base + o_sig);
-  L.hn = reinterpret_cast<float*>(base + o_hn);
-  L.en = reinterpret_cast<float*>(base + o_en);
-  L.cand = reinterpret_cast<unsigned long long*>(base + o_cand);
-  L.count = reinterpret_cast<int*>(base + o_count);
-  L.thr = reinterpret_cast<float*>(base + o_thr);
-  L.status = reinterpret_cast<int*>(base + o_status);
-  L.send = world > 1 ? base + o_send : nullptr;
-  L.recv = world > 1 ? base + o_recv : nullptr;
+  Layout lay{level_layout(L, nullptr, nq, L.nqc_max, L.C, ix->dpad)};
+  const size_t blk = world > 1 ? exchange_block_bytes(L.nqc_max, L.kc) : 0;
+  const size_t o_send = lay.add(blk), o_recv = lay.add(blk * world);
+  OM_TRY(ix->ws.reserve(lay.bytes));
+  level_layout(L, ix->ws.p, nq, L.nqc_max, L.C, ix->dpad);
+  L.send = world > 1 ? region<uint8_t>(ix->ws.p, o_send) : nullptr;
+  L.recv = world > 1 ? region<uint8_t>(ix->ws.p, o_recv) : nullptr;
   return mode == 0 ? convert_queries(ix, L, st) : 0;
 }
 
@@ -1730,12 +1712,6 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
   return 0;
 }
 
-#define OM_NCCL(expr)                                                                                   \
-  do {                                                                                                  \
-    int r__ = (expr);                                                                                   \
-    if (r__ != 0) return fail(OM_ECUDA, "%s failed: %s", #expr, nccl_api().GetErrorString(r__));        \
-  } while (0)
-
 // Merge of nparts [nq, k_in] lists -> [nq, k_out]; more than 8192 entries per query are merged hierarchically.
 int merge_parts(const float* Dp, const int64_t* Ip, int64_t stride_d, int64_t stride_i, int nparts, int nq, int k_in,
                 int k_out, float* D, int64_t* I, cudaStream_t st) {
@@ -1798,16 +1774,17 @@ int exchange_chunk(om_index* ix, om_comm* comm, const Level& L, int q0, int nqc,
   return 0;
 }
 
-// Runs one level over all its queries and returns the number of uncertified ones (their indices in flag_list).
-// One host synchronisation at the end (status word); a list overflow redoes the level with the safe schedule.
+// Runs one level over all its queries and lists the uncertified ones, ascending, in `uncertified`.  One host
+// synchronisation at the end (status word), and one more to read the certificate's per-query flags when a query is
+// uncertified; a list overflow redoes the level with the safe schedule.  comm: a row-sharded level (nullptr: one shard).
 int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int64_t id_offset, int* flags,
-              int* flag_list, int* nflag_out, cudaStream_t st) {
+              std::vector<int>& uncertified, cudaStream_t st) {
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   NvtxRange nvtx(L.mode == 1 ? "om.search.level_exact" : (L.kp_target >= kMaxCandidates ? "om.search.level_wide" : "om.search.level0"));
-  const bool sharded = comm && comm->world > 1;
+  const bool sharded = comm != nullptr;
   bool safe = ix->force_safe != 0;
-  const bool certify = ix->certify && L.mode == 0 && flags != nullptr && !ix->stage_scores;
+  const bool certify = ix->certify && L.mode == 0 && !ix->stage_scores;
   for (int attempt = 0; attempt < 4; ++attempt) {
     OM_CUDA(cudaMemsetAsync(L.status, 0, 32, st));
     for (int q0 = 0; q0 < L.nq; q0 += kQueryChunk) {
@@ -1831,10 +1808,8 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
         ix->st_launches += 1;
       }
     }
-    if (sharded)  // every rank must take the same retry decision (list overflow on any shard)
-      OM_NCCL(nccl_api().AllReduce(L.status, L.status, 1, kNcclInt32, kNcclMax, comm->nccl, st));
-    OM_CUDA(cudaMemcpyAsync(ix->h_status, L.status, 4 * sizeof(int), cudaMemcpyDeviceToHost, st));
-    OM_CUDA(cudaStreamSynchronize(st));
+    // every rank must take the same retry decision (list overflow on any shard)
+    OM_TRY(read_decision(ix, comm, L.status, 4, kNcclMax, 0, st));
     const unsigned int fault = read_clear_dev_fault();
     if (fault) return fail(OM_EFAULT, "scan kernel pipeline fault 0x%08x", fault);
     if (ix->h_status[0]) {
@@ -1843,11 +1818,13 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
       ix->st_retries++;
       continue;
     }
-    *nflag_out = certify ? ix->h_status[2] : 0;
-    if (*nflag_out > 0) {  // ascending list of the uncertified queries (identical on every rank)
-      compact_flags_kernel<<<1, 1024, 0, st>>>(flags, L.nq, flag_list);
-      OM_CUDA(cudaGetLastError());
-      ix->st_launches += 1;
+    uncertified.clear();
+    if (certify && ix->h_status[2] > 0) {  // the flags, and so the list, are identical on every rank
+      std::vector<int> flagged(L.nq);
+      OM_CUDA(cudaMemcpyAsync(flagged.data(), flags, flagged.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+      OM_CUDA(cudaStreamSynchronize(st));
+      for (int i = 0; i < L.nq; ++i)
+        if (flagged[i]) uncertified.push_back(i);
     }
     return 0;
   }
@@ -1856,33 +1833,29 @@ int run_level(om_index* ix, om_comm* comm, Level& L, float* dD, int64_t* dI, int
 
 // fp16 / int8 storage: rows written in place may hold values the storage cannot represent (inf from an overflowing encoder
 // output, NaN; int8: a non-finite scale), and there is no fp32 copy to answer from, so the search is refused until
-// om_index_reset.  Sharded: the shards' counts are summed so that every rank takes the same decision.  One host
-// synchronisation; fp32 indices skip the check.
+// om_index_reset.  Sharded: the shards' counts are summed into the scratch int so that every rank takes the same decision.
+// One host synchronisation; fp32 indices skip the check.
 int check_finite_rows(om_index* ix, om_comm* comm, cudaStream_t st) {
   if (ix->storage == OM_F32) return 0;
-  int* cnt = reinterpret_cast<int*>(ix->gstats) + 2;
   const bool sharded = comm && comm->world > 1;
-  if (sharded) OM_NCCL(nccl_api().AllReduce(cnt, cnt + 1, 1, kNcclInt32, kNcclSum, comm->nccl, st));
-  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, cnt, 2 * sizeof(int), cudaMemcpyDeviceToHost, st));
-  OM_CUDA(cudaStreamSynchronize(st));
-  ix->st_nonfinite = ix->h_status[4];
-  const int total = sharded ? ix->h_status[5] : ix->h_status[4];
+  OM_TRY(read_decision(ix, sharded ? comm : nullptr, reinterpret_cast<int*>(ix->gstats) + 2, 2, kNcclSum, 1, st));
+  ix->st_nonfinite = ix->h_status[0];
+  const int total = sharded ? ix->h_status[1] : ix->h_status[0];
   if (total > 0)
     return fail(OM_EINVAL, "search: %d committed %s rows hold inf or NaN (%d on this shard); the storage cannot answer "
-                "exactly over them: reset the index", total, ix->storage == OM_I8 ? "int8" : "fp16", ix->h_status[4]);
+                "exactly over them: reset the index", total, ix->storage == OM_I8 ? "int8" : "fp16", ix->h_status[0]);
   return 0;
 }
 
 // A search filter's argument rules (om_search_filter), checked on `st` before the search writes anything: the bitmap
 // covers the shard, and every query excludes at most kMaxExcluded ids, none negative, through monotone offsets.
-// Sharded: every rank takes part (its filter may be null or empty) and takes the decision of all of them.  A valid bitmap
-// also leaves its allowed rows per 256-row block in ix->allow_prefix, from which sweep_chunk sizes the rounds.  One host
-// synchronisation.
+// Sharded (comm): every rank takes part (its filter may be null or empty) and takes the decision of all of them.  A valid
+// bitmap also leaves its allowed rows per 256-row block in ix->allow_prefix, from which sweep_chunk sizes the rounds.  One
+// host synchronisation.
 int check_filter(om_index* ix, om_comm* comm, const om_search_filter* f, int nq, cudaStream_t st) {
   const om_search_filter none = {nullptr, 0, nullptr, nullptr};
   if (!f) f = &none;
-  const bool sharded = comm && comm->world > 1;
-  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
+  int* bad = ix->scratch();
   const bool short_bits = f->allow_bits && f->allow_words < (ix->n + 31) / 32;
   fill_i32<<<1, 1, 0, st>>>(bad, short_bits ? 8 : 0, 1);
   if (f->exclude_offsets)
@@ -1898,62 +1871,85 @@ int check_filter(om_index* ix, om_comm* comm, const om_search_filter* f, int nq,
     counts.resize(nblocks);
     OM_CUDA(cudaMemcpyAsync(counts.data(), ix->ows.p, static_cast<size_t>(nblocks) * 4, cudaMemcpyDeviceToHost, st));
   }
-  if (sharded) OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
-  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-  OM_CUDA(cudaStreamSynchronize(st));
+  OM_TRY(read_decision(ix, comm, bad, 1, kNcclMax, 0, st));
   ix->allow_prefix.assign(1, 0);
   for (int c : counts) ix->allow_prefix.push_back(ix->allow_prefix.back() + c);
-  const int b = ix->h_status[4];
+  const int b = ix->h_status[0];
   if (b & 8)
     return fail(OM_EINVAL, "search filter: allow_words = %lld is fewer than the %lld words of the %lld rows%s",
-                (long long)f->allow_words, (long long)((ix->n + 31) / 32), (long long)ix->n, sharded ? " (or on another rank)" : "");
+                (long long)f->allow_words, (long long)((ix->n + 31) / 32), (long long)ix->n, comm ? " (or on another rank)" : "");
   if (b & 2) return fail(OM_EINVAL, "search filter: a query excludes more than %d ids", kMaxExcluded);
   if (b & 1) return fail(OM_EINVAL, "search filter: exclude_offsets must be non-negative and non-decreasing, with exclude_ids given");
   if (b & 4) return fail(OM_EINVAL, "search filter: an excluded id is negative");
   return 0;
 }
 
-// The whole search: level 0 (all queries, k + slack candidates) -> level 1 (uncertified queries, widest list) ->
-// level 2 (still uncertified: exact fp32 scan).  comm == nullptr / world 1: single shard.  f: nullptr, or a checked filter
-// with at least one part.
-int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
-                om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
-  NvtxRange nvtx("om.search");
-  const int d = ix->d;
-  const int world = comm ? comm->world : 1;
+// The start of a search or a range search (`who` in the messages), before it writes anything: the per-call stats, the
+// shared-memory opt-ins, the d limit, the host queries staged in ix->ows after the caller's regions in `ows`, and the
+// stored rows' finiteness.  A range search passes its radii: staged likewise, and refused on every rank if one is NaN.
+// *qf (and *rho): the device queries (and radii).
+int call_prologue(om_index* ix, om_comm* comm, const char* who, const void* q, om_memkind q_kind, int nq, const float* radius,
+                  Layout& ows, const float** qf, const float** rho, cudaStream_t st) {
   ix->st_rounds = ix->st_retries = ix->st_launches = 0;
   ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
   ix->st_scan_cluster = ix->st_scan_clusters = 0;
   ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
   ix->ev_used = 0;
-  OM_TRY(check_finite_rows(ix, comm, st));
-  // whole-search staging: queries (if they arrive from the host), results (if they leave to the host), flag list
-  size_t off = 0;
-  auto carve = [&](size_t bytes) {
-    size_t o = off;
-    off += round_up(bytes, 256);
-    return o;
-  };
-  const size_t o_q = carve(q_kind == OM_HOST ? static_cast<size_t>(nq) * d * 4 : 0);
-  const size_t o_D = carve(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 4 : 0);
-  const size_t o_I = carve(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 8 : 0);
-  const size_t o_flags = carve(static_cast<size_t>(nq) * 4);  // per-query 0 / 1 written by the certificate of a level
-  const size_t o_flag = carve(static_cast<size_t>(nq) * 4);   // level-0 uncertified queries (ascending indices)
-  const size_t o_sub = carve(static_cast<size_t>(nq) * 4);    // uncertified within an escalation sub-batch
-  const size_t o_flag2 = carve(static_cast<size_t>(nq) * 4);  // ... composed back to indices into the full set
-  OM_TRY(ix->ows.reserve(off));
-  uint8_t* ob = static_cast<uint8_t*>(ix->ows.p);
-  const float* qf = static_cast<const float*>(q);
-  if (q_kind == OM_HOST) {
-    OM_CUDA(cudaMemcpyAsync(ob + o_q, q, static_cast<size_t>(nq) * d * 4, cudaMemcpyHostToDevice, st));
-    qf = reinterpret_cast<const float*>(ob + o_q);
+  OM_TRY(once_attrs(ix));
+  if (ix->d > 16384) return fail(OM_EINVAL, "%s: d > 16384 unsupported", who);
+  const bool host = q_kind == OM_HOST;
+  const size_t q_bytes = static_cast<size_t>(nq) * ix->d * 4, rho_bytes = static_cast<size_t>(nq) * 4;
+  const size_t o_q = ows.add(host ? q_bytes : 0), o_rho = ows.add(host && radius ? rho_bytes : 0);
+  OM_TRY(ix->ows.reserve(ows.bytes));
+  *qf = static_cast<const float*>(q);
+  if (host) {
+    OM_CUDA(cudaMemcpyAsync(region<void>(ix->ows.p, o_q), q, q_bytes, cudaMemcpyHostToDevice, st));
+    *qf = region<const float>(ix->ows.p, o_q);
   }
-  float* dD = out_kind == OM_HOST ? reinterpret_cast<float*>(ob + o_D) : D;
-  int64_t* dI = out_kind == OM_HOST ? reinterpret_cast<int64_t*>(ob + o_I) : I;
-  int* flags = reinterpret_cast<int*>(ob + o_flags);
-  int* flag_list = reinterpret_cast<int*>(ob + o_flag);
-  int* sub_flags = reinterpret_cast<int*>(ob + o_sub);
-  int* flag_list2 = reinterpret_cast<int*>(ob + o_flag2);
+  if (radius) {
+    *rho = radius;
+    if (host) {
+      OM_CUDA(cudaMemcpyAsync(region<void>(ix->ows.p, o_rho), radius, rho_bytes, cudaMemcpyHostToDevice, st));
+      *rho = region<const float>(ix->ows.p, o_rho);
+    }
+    int* bad = ix->scratch();
+    OM_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
+    check_radius_kernel<<<grid_for(nq, 256), 256, 0, st>>>(*rho, nq, bad);
+    OM_CUDA(cudaGetLastError());
+    OM_TRY(read_decision(ix, comm, bad, 1, kNcclMax, 0, st));
+    if (ix->h_status[0]) return fail(OM_EINVAL, "%s: a radius is NaN%s", who, comm ? " (on some rank)" : "");
+  }
+  return check_finite_rows(ix, comm, st);
+}
+
+// Uploads `list` (indices into the call's queries) to dlist and gathers the listed rows of src (rows of d floats) into
+// dst: the queries of a sub-batch.
+int gather_listed(const std::vector<int>& list, int* dlist, const float* src, int d, float* dst, cudaStream_t st) {
+  const int m = static_cast<int>(list.size());
+  OM_CUDA(cudaMemcpyAsync(dlist, list.data(), list.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  gather_rows_kernel<<<grid_for(static_cast<int64_t>(m) * d, 256), 256, 0, st>>>(src, dlist, m, d, dst);
+  OM_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The whole search: level 0 (all queries, k + slack candidates) -> level 1 (uncertified queries, widest list) ->
+// level 2 (still uncertified: exact fp32 scan).  comm == nullptr: single shard.  f: nullptr, or a checked filter with at
+// least one part.
+int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
+                om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
+  NvtxRange nvtx("om.search");
+  const int d = ix->d;
+  const int world = comm ? comm->world : 1;
+  // whole-search staging: results (if they leave to the host), the certificate's per-query flags, queries (in the prologue)
+  Layout ows;
+  const size_t o_D = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 4 : 0);
+  const size_t o_I = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 8 : 0);
+  const size_t o_flags = ows.add(static_cast<size_t>(nq) * 4);
+  const float* qf = nullptr;
+  OM_TRY(call_prologue(ix, comm, "om_index_search", q, q_kind, nq, nullptr, ows, &qf, nullptr, st));
+  float* dD = out_kind == OM_HOST ? region<float>(ix->ows.p, o_D) : D;
+  int64_t* dI = out_kind == OM_HOST ? region<int64_t>(ix->ows.p, o_I) : I;
+  int* flags = region<int>(ix->ows.p, o_flags);
 
   // the filter of every level: the bitmap, and the exclusions of the level's queries (qmap: the escalated ones)
   auto filter = [&](Level& L, const int* qmap) {
@@ -1963,69 +1959,51 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   };
   const int64_t slack = ix->rescore_slack >= 0 ? ix->rescore_slack : std::max<int64_t>(128, k / 5);
   const int kp0 = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(k) + slack, kMaxCandidates));
-  int nf = 0;
-  if (!ix->exact_only) {
+  std::vector<int> list, sub;  // uncertified queries: indices into the call's queries, into the last sub-batch
+  {  // level 0; exact_only: the exact scan of every query, which leaves none uncertified
     Level L;
-    OM_TRY(level_prepare(ix, L, qf, nq, k, kp0, 0, world, st));
+    if (ix->exact_only) ix->st_exact = nq;
+    OM_TRY(level_prepare(ix, L, qf, nq, k, ix->exact_only ? k : kp0, ix->exact_only ? 1 : 0, world, st));
     filter(L, nullptr);
-    OM_TRY(run_level(ix, comm, L, dD, dI, id_offset, flags, flag_list, &nf, st));
-    ix->st_flagged = nf;
+    OM_TRY(run_level(ix, comm, L, dD, dI, id_offset, flags, list, st));
+    ix->st_flagged = static_cast<int64_t>(list.size());
   }
-  // Escalation: the queries listed in `list` (indices into the full set; nullptr = all of them) are gathered into a
-  // compact sub-batch, answered by one more level and scattered back over their rows of (dD, dI).
-  auto run_sub = [&](const int* list, int n_sub, int kp_target, int mode, int* nf_out) -> int {
+  // Escalation: the queries in `list` are gathered into a compact sub-batch, answered by one more level and scattered back
+  // over their rows of (dD, dI); `sub` lists the ones the level left uncertified.  sws holds the uploaded list (the
+  // sub-batch's qmap), the gathered queries and the level's results.
+  auto run_sub = [&](int kp_target, int mode) -> int {
+    const size_t n_sub = list.size();
+    Layout sws;
+    const size_t s_list = sws.add(n_sub * 4), s_q = sws.add(n_sub * d * 4), s_D = sws.add(n_sub * k * 4),
+                 s_I = sws.add(n_sub * k * 8);
+    OM_TRY(ix->sws.reserve(sws.bytes));
+    int* dlist = region<int>(ix->sws.p, s_list);
+    float* qsub = region<float>(ix->sws.p, s_q);
+    float* Ds = region<float>(ix->sws.p, s_D);
+    int64_t* Is = region<int64_t>(ix->sws.p, s_I);
+    OM_TRY(gather_listed(list, dlist, qf, d, qsub, st));
     Level Ls;
-    if (!list) {
-      OM_TRY(level_prepare(ix, Ls, qf, n_sub, k, kp_target, mode, world, st));
-      filter(Ls, nullptr);
-      return run_level(ix, comm, Ls, dD, dI, id_offset, flags, sub_flags, nf_out, st);
-    }
-    size_t so = 0;
-    auto scarve = [&](size_t bytes) {
-      size_t o = so;
-      so += round_up(bytes, 256);
-      return o;
-    };
-    const size_t s_q = scarve(static_cast<size_t>(n_sub) * d * 4), s_D = scarve(static_cast<size_t>(n_sub) * k * 4),
-                 s_I = scarve(static_cast<size_t>(n_sub) * k * 8);
-    OM_TRY(ix->sws.reserve(so));
-    uint8_t* sb = static_cast<uint8_t*>(ix->sws.p);
-    float* qsub = reinterpret_cast<float*>(sb + s_q);
-    float* Ds = reinterpret_cast<float*>(sb + s_D);
-    int64_t* Is = reinterpret_cast<int64_t*>(sb + s_I);
-    gather_rows_kernel<<<grid_for(static_cast<int64_t>(n_sub) * d, 256), 256, 0, st>>>(qf, list, n_sub, d, qsub);
-    OM_CUDA(cudaGetLastError());
-    OM_TRY(level_prepare(ix, Ls, qsub, n_sub, k, kp_target, mode, world, st));
-    filter(Ls, list);
-    OM_TRY(run_level(ix, comm, Ls, Ds, Is, id_offset, flags, sub_flags, nf_out, st));
-    scatter_results_kernel<<<grid_for(static_cast<int64_t>(n_sub) * k, 256), 256, 0, st>>>(Ds, Is, list, n_sub, k, dD, dI);
+    OM_TRY(level_prepare(ix, Ls, qsub, static_cast<int>(n_sub), k, kp_target, mode, world, st));
+    filter(Ls, dlist);
+    OM_TRY(run_level(ix, comm, Ls, Ds, Is, id_offset, flags, sub, st));
+    scatter_results_kernel<<<grid_for(static_cast<int64_t>(n_sub) * k, 256), 256, 0, st>>>(Ds, Is, dlist, static_cast<int>(n_sub),
+                                                                                            k, dD, dI);
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 2;
     return 0;
   };
-  if (ix->exact_only) {
-    int dummy = 0;
-    ix->st_exact = nq;
-    OM_TRY(run_sub(nullptr, nq, k, 1, &dummy));
-  } else if (nf > 0) {
-    const int* list = flag_list;
+  if (!list.empty()) {
     // level 1: widest candidate list the select / sort kernels take.  (Sharded: the decision must not depend on this
     // rank's row count — every rank runs the same levels.)
     if (kp0 < kMaxCandidates && (world > 1 || ix->n > kp0)) {
-      int nf1 = 0;
-      OM_TRY(run_sub(list, nf, kMaxCandidates, 0, &nf1));
-      if (nf1 > 0) {
-        compose_list_kernel<<<(nf1 + 255) / 256, 256, 0, st>>>(list, sub_flags, nf1, flag_list2);
-        OM_CUDA(cudaGetLastError());
-        list = flag_list2;
-      }
-      nf = nf1;
+      OM_TRY(run_sub(kMaxCandidates, 0));
+      for (int& i : sub) i = list[i];
+      list.swap(sub);
     }
-    ix->st_flagged_wide = nf;
-    if (nf > 0) {  // level 2: exact fp32 scan
-      int dummy = 0;
-      ix->st_exact = nf;
-      OM_TRY(run_sub(list, nf, k, 1, &dummy));
+    ix->st_flagged_wide = static_cast<int64_t>(list.size());
+    if (!list.empty()) {  // level 2: exact fp32 scan
+      ix->st_exact = static_cast<int64_t>(list.size());
+      OM_TRY(run_sub(k, 1));
     }
   }
   if (out_kind == OM_HOST) {
@@ -2056,6 +2034,7 @@ int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const
   OM_TRY(device_sm_count());
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   OM_TRY(settle_reset(ix, st));
+  if (comm && comm->world == 1) comm = nullptr;  // one rank: no collective, the single-shard search
   if (check) OM_TRY(check_filter(ix, comm, filter, nq, st));
   return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
 }
@@ -2099,48 +2078,32 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
   const int m = static_cast<int>(list.size()), d = ix->d;
   const size_t M = m;
   const bool long_lists = C > kRangeSortKeys;
-  size_t off = 0;
-  auto carve = [&](size_t bytes) {
-    size_t o = off;
-    off += round_up(bytes, 256);
-    return o;
-  };
-  const size_t o_list = carve(M * 4), o_q = carve(M * d * 4), o_rho = carve(M * 4), o_qh = carve(M * ix->dpad * 2),
-               o_hn = carve(M * 4), o_en = carve(M * 4), o_sig = carve(M * 8), o_cand = carve(M * C * 8),
-               o_alt = carve(long_lists ? M * C * 8 : 0), o_count = carve(M * 4), o_filled = carve(M * 4),
-               o_total = carve(M * 8), o_thr = carve(M * 4), o_surv = carve(M * 4), o_exact = carve(M * 4),
-               o_off = carve(M * 8), o_status = carve(256);
-  if (C == ix->range_list) ix->r_keep_ws = std::max(ix->r_keep_ws, off);  // a first sweep's workspace
-  if (ix->ws.reserve(off) != 0) {
+  Level L;
+  Layout lay{level_layout(L, nullptr, M, M, C, ix->dpad)};
+  const size_t o_list = lay.add(M * 4), o_q = lay.add(M * d * 4), o_rho = lay.add(M * 4),
+               o_alt = lay.add(long_lists ? M * C * 8 : 0), o_filled = lay.add(M * 4), o_total = lay.add(M * 8),
+               o_surv = lay.add(M * 4), o_exact = lay.add(M * 4), o_off = lay.add(M * 8);
+  if (C == ix->range_list) ix->r_keep_ws = std::max(ix->r_keep_ws, lay.bytes);  // a first sweep's workspace
+  if (ix->ws.reserve(lay.bytes) != 0) {
     cudaGetLastError();
     return fail(OM_ENOMEM, "range search: cannot allocate candidate lists of %d queries x %d rows", m, C);
   }
-  uint8_t* b = static_cast<uint8_t*>(ix->ws.p);
-  int* dlist = reinterpret_cast<int*>(b + o_list);
-  float* q = reinterpret_cast<float*>(b + o_q);
-  float* rq = reinterpret_cast<float*>(b + o_rho);
-  int* filled = reinterpret_cast<int*>(b + o_filled);
-  long long* total = reinterpret_cast<long long*>(b + o_total);
-  int* surv = reinterpret_cast<int*>(b + o_surv);
-  int* to_exact = reinterpret_cast<int*>(b + o_exact);
-  long long* doff = reinterpret_cast<long long*>(b + o_off);
-  unsigned long long* alt = reinterpret_cast<unsigned long long*>(b + o_alt);
-  Level L;
+  void* b = ix->ws.p;
+  level_layout(L, b, M, M, C, ix->dpad);
+  int* dlist = region<int>(b, o_list);
+  float* q = region<float>(b, o_q);
+  float* rq = region<float>(b, o_rho);
+  int* filled = region<int>(b, o_filled);
+  long long* total = region<long long>(b, o_total);
+  int* surv = region<int>(b, o_surv);
+  int* to_exact = region<int>(b, o_exact);
+  long long* doff = region<long long>(b, o_off);
+  unsigned long long* alt = region<unsigned long long>(b, o_alt);
   L.nq = m;
   L.C = C;
   L.mode = mode;
   L.qf = q;
-  L.qh = reinterpret_cast<__half*>(b + o_qh);
-  L.q8 = reinterpret_cast<int8_t*>(b + o_qh);
-  L.qsig = reinterpret_cast<float2*>(b + o_sig);
-  L.hn = reinterpret_cast<float*>(b + o_hn);
-  L.en = reinterpret_cast<float*>(b + o_en);
-  L.cand = reinterpret_cast<unsigned long long*>(b + o_cand);
-  L.count = reinterpret_cast<int*>(b + o_count);
-  L.thr = reinterpret_cast<float*>(b + o_thr);
-  L.status = reinterpret_cast<int*>(b + o_status);
-  OM_CUDA(cudaMemcpyAsync(dlist, list.data(), M * 4, cudaMemcpyHostToDevice, st));
-  gather_rows_kernel<<<grid_for(static_cast<int64_t>(m) * d, 256), 256, 0, st>>>(qf, dlist, m, d, q);
+  OM_TRY(gather_listed(list, dlist, qf, d, q, st));
   gather_rows_kernel<<<grid_for(m, 256), 256, 0, st>>>(rho, dlist, m, 1, rq);
   OM_CUDA(cudaGetLastError());
   if (mode == 0) OM_TRY(convert_queries(ix, L, st));
@@ -2284,7 +2247,6 @@ int range_local(om_index* ix, const float* qf, const float* rho, int nq, std::ve
 int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, const float* radius, int64_t* lims,
                om_memkind out_kind, int64_t id_offset, cudaStream_t st) {
   NvtxRange nvtx("om.range_search");
-  const int d = ix->d;
   // the sharded entry runs the exchange at every world size, one rank included
   const bool sharded = comm != nullptr;
   const int W = sharded ? comm->world : 1;
@@ -2302,35 +2264,10 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
     }
   } scratch{ix, ix->ws.bytes};
   ix->r_keep_ws = 0;
-  ix->st_rounds = ix->st_retries = ix->st_launches = 0;
-  ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
-  ix->st_scan_cluster = ix->st_scan_clusters = 0;
-  ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
   ix->st_range_candidates = ix->st_range_resweeps = 0;
-  ix->ev_used = 0;
-  OM_TRY(once_attrs(ix));
-  if (d > 16384) return fail(OM_EINVAL, "om_index_range_search: d > 16384 unsupported");
-  // whole-call staging: queries and radii that arrive from the host
-  const size_t o_q = 0, o_rho = round_up(q_kind == OM_HOST ? static_cast<size_t>(nq) * d * 4 : 0, 256);
-  OM_TRY(ix->ows.reserve(o_rho + round_up(static_cast<size_t>(nq) * 4, 256)));
-  uint8_t* ob = static_cast<uint8_t*>(ix->ows.p);
-  const float* qf = static_cast<const float*>(q);
-  const float* rho = radius;
-  if (q_kind == OM_HOST) {
-    OM_CUDA(cudaMemcpyAsync(ob + o_q, q, static_cast<size_t>(nq) * d * 4, cudaMemcpyHostToDevice, st));
-    OM_CUDA(cudaMemcpyAsync(ob + o_rho, radius, static_cast<size_t>(nq) * 4, cudaMemcpyHostToDevice, st));
-    qf = reinterpret_cast<const float*>(ob + o_q);
-    rho = reinterpret_cast<const float*>(ob + o_rho);
-  }
-  int* bad = reinterpret_cast<int*>(ix->gstats) + 3;
-  OM_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
-  check_radius_kernel<<<grid_for(nq, 256), 256, 0, st>>>(rho, nq, bad);
-  OM_CUDA(cudaGetLastError());
-  if (sharded) OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
-  OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-  OM_CUDA(cudaStreamSynchronize(st));
-  if (ix->h_status[4]) return fail(OM_EINVAL, "om_index_range_search: a radius is NaN%s", sharded ? " (on some rank)" : "");
-  OM_TRY(check_finite_rows(ix, comm, st));
+  Layout ows;
+  const float *qf = nullptr, *rho = nullptr;
+  OM_TRY(call_prologue(ix, comm, "om_index_range_search", q, q_kind, nq, radius, ows, &qf, &rho, st));
 
   std::vector<int64_t> src, cnt;
   int64_t stored = 0;
@@ -2340,11 +2277,9 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
   auto agree = [&](int rc_local) -> int {
     if (!sharded) return rc_local;
     cudaGetLastError();
-    fill_i32<<<1, 1, 0, st>>>(bad, rc_local < 0 ? -rc_local : 0, 1);
-    OM_NCCL(nccl_api().AllReduce(bad, bad, 1, kNcclInt32, kNcclMax, comm->nccl, st));
-    OM_CUDA(cudaMemcpyAsync(ix->h_status + 4, bad, sizeof(int), cudaMemcpyDeviceToHost, st));
-    OM_CUDA(cudaStreamSynchronize(st));
-    if (rc_local == 0 && ix->h_status[4]) return fail(-ix->h_status[4], "om_index_range_search_sharded: another rank failed");
+    fill_i32<<<1, 1, 0, st>>>(ix->scratch(), rc_local < 0 ? -rc_local : 0, 1);
+    OM_TRY(read_decision(ix, comm, ix->scratch(), 1, kNcclMax, 0, st));
+    if (rc_local == 0 && ix->h_status[0]) return fail(-ix->h_status[0], "om_index_range_search_sharded: another rank failed");
     return rc_local;
   };
 
@@ -2352,20 +2287,15 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
   for (int i = 0; i < nq && rc == 0; ++i) ll[i + 1] = ll[i] + cnt[i];
   const size_t NQ1 = static_cast<size_t>(nq) + 1;
   std::vector<long long> plims, glims;  // every part's lims [W][nq + 1], the merged lims
-  size_t off = 0;
-  auto carve = [&](size_t bytes) {
-    size_t o = off;
-    off += round_up(bytes, 256);
-    return o;
-  };
-  const size_t o_src = carve(nq * 8), o_ll = carve(NQ1 * 8), o_plims = carve(W * NQ1 * 8), o_glims = carve(NQ1 * 8),
-               o_cnt = carve(nq * 8), o_all = carve(static_cast<size_t>(W) * nq * 8);
-  if (rc == 0 && ix->ws.reserve(off) != 0) {
+  Layout lay;
+  const size_t o_src = lay.add(nq * 8), o_ll = lay.add(NQ1 * 8), o_plims = lay.add(W * NQ1 * 8), o_glims = lay.add(NQ1 * 8),
+               o_cnt = lay.add(nq * 8), o_all = lay.add(static_cast<size_t>(W) * nq * 8);
+  if (rc == 0 && ix->ws.reserve(lay.bytes) != 0) {
     cudaGetLastError();
     rc = fail(OM_ENOMEM, "range search: cannot allocate the lims of %d queries", nq);
   }
   OM_TRY(agree(rc));
-  uint8_t* b = static_cast<uint8_t*>(ix->ws.p);
+  void* b = ix->ws.p;
   const unsigned long long* keys = static_cast<const unsigned long long*>(ix->rkeys.p);
   auto outputs = [&](int64_t T, float** D, int64_t** I) -> int {
     if (ix->rout.reserve(round_up(T * 4, 256) + T * 8 + 256) != 0) {
@@ -2383,11 +2313,11 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
                          static_cast<unsigned>(std::max<long long>(1, std::min<long long>({(cmax + 255) / 256,
                                                                                           (8LL * sms + nq - 1) / nq, 65535}))));
   auto gather = [&](float* D, int64_t* I) -> int {
-    OM_CUDA(cudaMemcpyAsync(b + o_src, src.data(), nq * 8, cudaMemcpyHostToDevice, st));
-    OM_CUDA(cudaMemcpyAsync(b + o_ll, ll.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(region<long long>(b, o_src), src.data(), nq * 8, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(region<long long>(b, o_ll), ll.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
     if (cmax > 0)
-      range_gather_kernel<<<gather_grid, 256, 0, st>>>(keys, reinterpret_cast<long long*>(b + o_src),
-                                                       reinterpret_cast<long long*>(b + o_ll), id_offset, D, I);
+      range_gather_kernel<<<gather_grid, 256, 0, st>>>(keys, region<long long>(b, o_src),
+                                                       region<long long>(b, o_ll), id_offset, D, I);
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 1;
     return 0;
@@ -2403,10 +2333,10 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
     NcclApi& nc = nccl_api();
     Timed t(ix, st, 3);
     // counts of every shard
-    OM_CUDA(cudaMemcpyAsync(b + o_cnt, cnt.data(), nq * 8, cudaMemcpyHostToDevice, st));
-    OM_NCCL(nc.AllGather(b + o_cnt, b + o_all, static_cast<size_t>(nq) * 8, kNcclInt8, comm->nccl, st));
+    OM_CUDA(cudaMemcpyAsync(region<long long>(b, o_cnt), cnt.data(), nq * 8, cudaMemcpyHostToDevice, st));
+    OM_NCCL(nc.AllGather(region<long long>(b, o_cnt), region<long long>(b, o_all), static_cast<size_t>(nq) * 8, kNcclInt8, comm->nccl, st));
     std::vector<long long> all(static_cast<size_t>(W) * nq);
-    OM_CUDA(cudaMemcpyAsync(all.data(), b + o_all, all.size() * 8, cudaMemcpyDeviceToHost, st));
+    OM_CUDA(cudaMemcpyAsync(all.data(), region<long long>(b, o_all), all.size() * 8, cudaMemcpyDeviceToHost, st));
     OM_CUDA(cudaStreamSynchronize(st));
     plims.assign(W * NQ1, 0);
     glims.assign(NQ1, 0);
@@ -2424,26 +2354,26 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
     // every shard's sorted results, padded to the longest: [D f32 tmax | I i64 tmax], and the merged results; both
     // allocated, and the outcome agreed, before the results' all-gather
     const size_t o_i = round_up(tmax * 4, 256), blk = o_i + round_up(tmax * 8, 256) + 256;
-    const size_t o_send = carve(blk), o_recv = carve(blk * W);
+    const size_t o_send = lay.add(blk), o_recv = lay.add(blk * W);
     float* D = nullptr;
     int64_t* I = nullptr;
     int rc2 = 0;
-    if (ix->ws.reserve(off) != 0) {
+    if (ix->ws.reserve(lay.bytes) != 0) {
       cudaGetLastError();
       rc2 = fail(OM_ENOMEM, "range search: cannot allocate the exchange of %lld results per shard", tmax);
     }
     if (rc2 == 0) rc2 = outputs(T, &D, &I);
     OM_TRY(agree(rc2));
-    b = static_cast<uint8_t*>(ix->ws.p);  // possibly a new buffer: the uploads above were read by the all-gather already
-    OM_CUDA(cudaMemcpyAsync(b + o_plims, plims.data(), W * NQ1 * 8, cudaMemcpyHostToDevice, st));
-    OM_CUDA(cudaMemcpyAsync(b + o_glims, glims.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
-    OM_TRY(gather(reinterpret_cast<float*>(b + o_send), reinterpret_cast<int64_t*>(b + o_send + o_i)));
-    OM_NCCL(nc.AllGather(b + o_send, b + o_recv, blk, kNcclInt8, comm->nccl, st));
+    b = ix->ws.p;  // possibly a new buffer: the uploads above were read by the all-gather already
+    OM_CUDA(cudaMemcpyAsync(region<long long>(b, o_plims), plims.data(), W * NQ1 * 8, cudaMemcpyHostToDevice, st));
+    OM_CUDA(cudaMemcpyAsync(region<long long>(b, o_glims), glims.data(), NQ1 * 8, cudaMemcpyHostToDevice, st));
+    OM_TRY(gather(region<float>(b, o_send), region<int64_t>(b, o_send + o_i)));
+    OM_NCCL(nc.AllGather(region<uint8_t>(b, o_send), region<uint8_t>(b, o_recv), blk, kNcclInt8, comm->nccl, st));
     if (tmax > 0)
       range_merge_parts_kernel<<<dim3(static_cast<unsigned>(std::min<long long>((tmax + 255) / 256, 4096)), W), 256, 0, st>>>(
-          reinterpret_cast<const float*>(b + o_recv), reinterpret_cast<const int64_t*>(b + o_recv + o_i),
-          static_cast<int64_t>(blk / 4), static_cast<int64_t>(blk / 8), reinterpret_cast<const long long*>(b + o_plims), W, nq,
-          reinterpret_cast<const long long*>(b + o_glims), D, I);
+          region<const float>(b, o_recv), region<const int64_t>(b, o_recv + o_i),
+          static_cast<int64_t>(blk / 4), static_cast<int64_t>(blk / 8), region<const long long>(b, o_plims), W, nq,
+          region<const long long>(b, o_glims), D, I);
     OM_CUDA(cudaGetLastError());
     ix->st_launches += 3;
   }

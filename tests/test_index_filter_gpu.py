@@ -302,6 +302,25 @@ def test_exclusions_on_the_exact_and_safe_paths(om, dtype):
     _check_sub(om, xd, ~np.isin(np.arange(n), dup[:2500]), qd, k, dtype, "near-duplicates, half disallowed", idx=idx)
 
 
+@pytest.mark.parametrize("dtype", DTYPES, ids=["f32", "f16", "i8"])
+def test_exclusions_on_an_escalated_subset(om, dtype):
+    """Only the odd queries meet thousands of near-duplicate rows, so the 4096-wide level and the exact level each answer
+    a proper subset of the batch: every escalated query must keep its own excluded ids there."""
+    n, k, nq = 20000, 50, 40
+    x, q, rng = _data(19, n, 64, nq)
+    dup = rng.choice(n, 5000, replace=False)
+    v = rng.standard_normal(64, dtype=np.float32)
+    x[dup] = v + 1e-6 * rng.standard_normal((5000, 64), dtype=np.float32)
+    q[1::2] = v + 0.05 * rng.standard_normal((nq // 2, 64), dtype=np.float32)
+    idx = _index(om, x, dtype)
+    ref = idx.search(q, k + 128)
+    excl = [list(rng.choice(ref[1][i, :k], 40, replace=False)) for i in range(nq)]
+    _check_excl(idx, q, k, excl, "escalated subset", ref=ref)
+    stats = {s: idx.stat(s) for s in STATS}
+    print("[filter escalated subset] %s: %s" % (dtype, stats))
+    assert stats["uncertified"] < nq and stats["exact_queries"] > 0, "premise: a proper subset reaches both levels"
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # contract edges
 # ---------------------------------------------------------------------------------------------------------------------
