@@ -24,6 +24,8 @@
  * stream; the library issues the work of a call on that stream only.  The calls without a stream order
  * themselves: om_encoder_set_weight runs after all work already issued on the device and has finished
  * reading the caller's data on return; om_index_reserve synchronises the device when it grows the shard;
+ * a search of a host-resident index (om_index_create_host) also uploads rows on a stream the index owns, ordered after
+ * the caller's earlier work on `stream` and finished on return;
  * om_index_reset touches no device memory (the error-norm maxima are zeroed on the stream of the next
  * commit or search).  One handle must not be used from two streams at once.  The loss workspace is
  * process-global: loss calls must not overlap across streams.
@@ -187,6 +189,25 @@ int om_index_create(int d, om_index** out); /* faiss.IndexFlatIP(d); lives on th
  * cores with a two-level int8 split of the query; "pair_scan" and "scan_cluster_*" do not apply.
  * OM_BF16 storage returns OM_EINVAL.  Every shard of a sharded search has the same storage. */
 int om_index_create_typed(int d, om_dtype storage, om_index** out);
+/* Host-resident index: the stored rows (same storages, row format and add rules as om_index_create_typed; fp32 storage
+ * keeps the master rows only) live in pinned host memory, in chunks of window_rows rows, so a corpus larger than the
+ * device memory can be searched on one GPU.  window_rows: a positive multiple of 256, or 0 = automatic (the largest
+ * multiple of 256 rows, at least 256, for which two device windows take at most a quarter of the device memory free at
+ * creation; a window row is the fp32 row plus its fp16 scan copy, dpad halves, or dpad + 16 bytes).
+ * om_index_search / om_index_search_filtered search the rows one partition of window_rows rows at a time: the partition is
+ * uploaded into one of two device windows while the previous one is searched, searched exactly, and merged into the
+ * running top-k.  D and I are bitwise what a device index given the same adds returns (ties by ascending id across
+ * partitions too); the stats that count work ("uncertified", "uncertified_wide", "exact_queries", "rounds", "launches")
+ * are summed over the partitions; "partitions" is the number searched and, with "profile" on, "upload_wait_ns" the device
+ * time the search waited for uploads.
+ * Streams: the uploads run on a non-blocking stream the index owns, ordered after the work issued on `stream` before the
+ * call, and the call returns with them finished — the one exception to "the work of a call runs on `stream` only".
+ * om_index_add converts on the device (through a window) and synchronises `stream`; a failed pinned allocation returns
+ * OM_ENOMEM and adds nothing.  om_index_reset keeps the host chunks; om_index_destroy frees them.
+ * Limits: om_index_reserve, om_index_reserve_rows and om_index_commit return OM_ESTATE (there are no device rows to write
+ * in place); om_index_search_sharded(_filtered) and om_index_range_search(_sharded) return OM_EINVAL; none writes
+ * anything. */
+int om_index_create_host(int d, om_dtype storage, int64_t window_rows, om_index** out);
 int om_index_storage(const om_index* idx); /* the om_dtype given at creation */
 /* index.add(x): x [n, d] row-major, fp32, bf16 or fp16 (host or device).  Rows get ids ntotal .. ntotal+n-1.
  * fp16 storage: converted to fp16 with round-to-nearest-even; int8 storage: quantised by the OM_I8 rule; both synchronise

@@ -50,6 +50,7 @@ SIGNATURES = {
     "om_encoder_destroy": (None, [c_void_p]),
     "om_index_create": (c_int, [c_int, POINTER(c_void_p)]),
     "om_index_create_typed": (c_int, [c_int, c_int, POINTER(c_void_p)]),
+    "om_index_create_host": (c_int, [c_int, c_int, c_int64, POINTER(c_void_p)]),
     "om_index_storage": (c_int, [c_void_p]),
     "om_index_reserve_rows": (c_int, [c_void_p, c_int64, POINTER(c_void_p), POINTER(c_int64)]),
     "om_index_add": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int64, c_void_p]),

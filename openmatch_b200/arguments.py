@@ -169,3 +169,7 @@ class InferenceArguments(RuntimeArguments):
         "help": "row storage of the search index: 'float32' (fp32 rows + fp16 scan copy, 6 bytes per element), "
                 "'float16' (fp16 rows only, 2 bytes per element; search is exact over the fp16-rounded rows) or 'int8' "
                 "(one byte per element + a per-row scale; search is exact over the dequantised rows)"})
+    index_memory: str = field(default="device", metadata={
+        "help": "where the search index keeps its rows: 'device' (GPU memory) or 'host' (pinned host memory, streamed "
+                "through the GPU by every search, for corpora larger than the GPU's memory; one process, built from "
+                "embedding files by driver.retrieve; results are bitwise those of 'device')"})

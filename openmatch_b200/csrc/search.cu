@@ -1009,9 +1009,19 @@ struct DevBuf {  // grow-only device scratch
   }
 };
 
+// The stored rows a search reads: n rows in the index's storage (fp32 master rows xf + fp16 scan copy xh, fp16 rows xh, or
+// int8 rows xq).  A device index's own buffers, or one partition of a host-resident index in its device window.
+struct Rows {
+  int64_t n = 0;
+  const float* xf = nullptr;
+  const __half* xh = nullptr;
+  const int8_t* xq = nullptr;
+};
+
 // One pass of the pipeline (scan -> select -> re-score [-> exchange -> merge] -> certify) over nq device-resident
-// queries; all pointers lie in the index's level workspace (level_layout).
+// queries and the rows X; all pointers lie in the index's level workspace (level_layout).
 struct Level {
+  Rows X;
   int nq = 0, k = 0, kp = 0, kp_target = 0, C = 0, growth = 2, mode = 0, world = 1, kc = 0, nqc_max = 0;
   const float* qf = nullptr;  // [nq, d] fp32 (not owned by the workspace)
   __half* qh = nullptr;       // [nq, dpad] scan operand
@@ -1023,7 +1033,9 @@ struct Level {
   float* thr = nullptr;
   int* status = nullptr;  // [0] list overflow, [2] uncertified queries
   uint8_t *send = nullptr, *recv = nullptr;
-  const uint32_t* allow = nullptr;  // filtered search: the shard's allowed-row bitmap
+  const uint32_t* allow = nullptr;  // filtered search: the allowed-row bitmap of X's rows
+  // with allow: allowed rows before each 256-row block of X, relative to allow_prefix[0] (a slice of ix->allow_prefix)
+  const int64_t* allow_prefix = nullptr;
   Excluded ex{};  // filtered search: excluded ids (ex.off nullptr: none), ex.qmap the level's queries in the caller's batch
 };
 
@@ -1073,6 +1085,17 @@ struct om_index {
   DevBuf rkeys, rout;
   size_t r_keep_ws = 0;  // the workspace of the last range search's first sweeps (kept after the call)
   int64_t st_range_candidates = 0, st_range_resweeps = 0;
+  // Host-resident index (om_index_create_host; window > 0): the stored rows live in pinned host chunks of `window` rows
+  // each, in the stored row format (fp32 storage: the master rows only), and xf / xh / xq stay null.  A search uploads
+  // partition p (rows [p window, (p + 1) window)) into device window p % 2 on copy_st while it searches the other one.
+  int64_t window = 0;
+  std::vector<void*> chunks;
+  DevBuf win[2];
+  int64_t win_rows[2] = {0, 0};  // rows each window holds
+  cudaStream_t copy_st = nullptr;
+  cudaEvent_t ev_entry = nullptr, ev_ready[2] = {nullptr, nullptr}, ev_free[2] = {nullptr, nullptr};
+  int64_t st_partitions = 0;
+  double st_upload_wait_us = 0;
 };
 
 // Calls f with the index's stored rows as a typed pointer: the fp32 master rows, the fp16 rows or the int8 rows.  Kernels
@@ -1085,6 +1108,17 @@ static decltype(auto) with_rows(const om_index* ix, F&& f) {
     default: return f(ix->xf);
   }
 }
+// The same for the rows of a view X in the index's storage.
+template <typename F>
+static decltype(auto) with_rows(const om_index* ix, const Rows& X, F&& f) {
+  switch (ix->storage) {
+    case OM_I8: return f(X.xq);
+    case OM_F16: return f(X.xh);
+    default: return f(X.xf);
+  }
+}
+// A device index's rows as a view.
+static Rows device_rows(const om_index* ix) { return Rows{ix->n, ix->xf, ix->xh, ix->xq}; }
 
 // row pitch in elements of the rows behind a typed pointer
 template <typename RowT>
@@ -1099,6 +1133,41 @@ struct RowBuf {
 template <typename RowT>
 static RowBuf row_buf(RowT** p, int d, const char* name) {
   return {reinterpret_cast<void**>(p), StoredRow<RowT>::pitch(d) * sizeof(RowT), name};
+}
+
+// Device window of a host-resident index for `rows` rows: the fp32 master rows then their fp16 scan copy (fp32 storage),
+// the fp16 rows, or the int8 rows.  Returns its bytes; with base, points X's buffers there.
+static size_t window_layout(const om_index* ix, int64_t rows, void* base, Rows* X) {
+  Layout lay;
+  const size_t r = static_cast<size_t>(rows);
+  const size_t o_f = lay.add(ix->storage == OM_F32 ? r * ix->d * 4 : 0);
+  const size_t o_h = lay.add(ix->storage != OM_I8 ? r * ix->dpad * 2 : 0);
+  const size_t o_q = lay.add(ix->storage == OM_I8 ? r * pitch_of(ix->xq, ix->d) : 0);
+  if (base) {
+    X->xf = ix->storage == OM_F32 ? region<const float>(base, o_f) : nullptr;
+    X->xh = ix->storage != OM_I8 ? region<const __half>(base, o_h) : nullptr;
+    X->xq = ix->storage == OM_I8 ? region<const int8_t>(base, o_q) : nullptr;
+  }
+  return lay.bytes;
+}
+
+// Bytes of one stored row in a host chunk of a host-resident index (fp32 storage: the master row only).
+static size_t host_row_bytes(const om_index* ix) {
+  return with_rows(ix, [&](const auto* xs) -> size_t { return pitch_of(xs, ix->d) * sizeof(*xs); });
+}
+
+// Makes device window w of a host-resident index hold at least `rows` rows (at most one partition); its view in *X, with
+// X->n = rows.  Growing a window frees it first: no upload or search may be using it.
+static int window_reserve(om_index* ix, int w, int64_t rows, Rows* X) {
+  const int64_t need = std::min(ix->window, round_up(rows, 256));
+  if (need > ix->win_rows[w]) {
+    ix->win_rows[w] = 0;
+    OM_TRY(ix->win[w].reserve(window_layout(ix, need, nullptr, nullptr)));
+    ix->win_rows[w] = need;
+  }
+  window_layout(ix, ix->win_rows[w], ix->win[w].p, X);
+  X->n = rows;
+  return 0;
 }
 
 // Grows every row buffer of the index's storage to hold at least `need` rows.
@@ -1208,8 +1277,49 @@ int om_index_create_typed(int d, om_dtype storage, om_index** out) {
   return 0;
 }
 
+int om_index_create_host(int d, om_dtype storage, int64_t window_rows, om_index** out) {
+  if (!out || d <= 0) return fail(OM_EINVAL, "om_index_create_host: d must be positive");
+  if (window_rows < 0 || window_rows % 256 != 0)
+    return fail(OM_EINVAL, "om_index_create_host: window_rows = %lld must be 0 (automatic) or a positive multiple of 256",
+                (long long)window_rows);
+  om_index* ix = nullptr;
+  OM_TRY(om_index_create_typed(d, storage, &ix));
+  if (window_rows == 0) {  // two windows in at most a quarter of the free device memory
+    size_t free_b = 0, total_b = 0;
+    if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) {
+      cudaGetLastError();
+      om_index_destroy(ix);
+      return fail(OM_ECUDA, "om_index_create_host: cannot read the free device memory");
+    }
+    const size_t row =window_layout(ix, 256, nullptr, nullptr) / 256;
+    window_rows = std::max<int64_t>(256, static_cast<int64_t>(free_b / 4 / (2 * row)) / 256 * 256);
+  }
+  ix->window = window_rows;
+  if (cudaStreamCreateWithFlags(&ix->copy_st, cudaStreamNonBlocking) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ix->ev_entry, cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ix->ev_ready[0], cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ix->ev_ready[1], cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ix->ev_free[0], cudaEventDisableTiming) != cudaSuccess ||
+      cudaEventCreateWithFlags(&ix->ev_free[1], cudaEventDisableTiming) != cudaSuccess) {
+    cudaGetLastError();
+    om_index_destroy(ix);
+    return fail(OM_ECUDA, "om_index_create_host: cannot create the upload stream and its events");
+  }
+  *out = ix;
+  return 0;
+}
+
 void om_index_destroy(om_index* ix) {
   if (!ix) return;
+  if (ix->copy_st) {
+    cudaStreamSynchronize(ix->copy_st);
+    cudaStreamDestroy(ix->copy_st);
+  }
+  for (cudaEvent_t e : {ix->ev_entry, ix->ev_ready[0], ix->ev_ready[1], ix->ev_free[0], ix->ev_free[1]})
+    if (e) cudaEventDestroy(e);
+  for (void* c : ix->chunks) cudaFreeHost(c);
+  ix->win[0].release();
+  ix->win[1].release();
   cudaFree(ix->xf);
   cudaFree(ix->xh);
   cudaFree(ix->xq);
@@ -1240,6 +1350,7 @@ int om_index_reset(om_index* ix) {
 
 int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row_pitch_elems) {
   if (!ix || n < 0 || !dev_rows || !row_pitch_elems) return fail(OM_EINVAL, "om_index_reserve_rows: bad arguments");
+  if (ix->window) return fail(OM_ESTATE, "om_index_reserve_rows: a host-resident index has no device rows to write in place");
   if (ix->n + n > 0xfffffff0ll) return fail(OM_EINVAL, "index shard limited to 2^32-16 rows; shard the corpus");
   OM_TRY(index_grow(ix, ix->n + n));
   with_rows(ix, [&](auto* xs) {
@@ -1251,6 +1362,7 @@ int om_index_reserve_rows(om_index* ix, int64_t n, void** dev_rows, int64_t* row
 
 int om_index_reserve(om_index* ix, int64_t n, float** dev_rows) {
   if (!ix || n < 0 || !dev_rows) return fail(OM_EINVAL, "om_index_reserve: bad arguments");
+  if (ix->window) return fail(OM_ESTATE, "om_index_reserve: a host-resident index has no device rows to write in place");
   if (ix->storage != OM_F32)
     return fail(OM_ESTATE, "om_index_reserve: the index stores %s rows; use om_index_reserve_rows",
                 ix->storage == OM_F16 ? "fp16" : "int8");
@@ -1262,6 +1374,7 @@ int om_index_reserve(om_index* ix, int64_t n, float** dev_rows) {
 }
 
 int om_index_commit(om_index* ix, int64_t n, void* stream) {
+  if (ix && ix->window) return fail(OM_ESTATE, "om_index_commit: a host-resident index has no rows written in place to commit");
   if (!ix || n < 0 || ix->n + n > ix->cap) return fail(OM_EINVAL, "om_index_commit: more rows than reserved");
   if (n == 0) return 0;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -1279,6 +1392,40 @@ int om_index_commit(om_index* ix, int64_t n, void* stream) {
   return 0;
 }
 
+// fp16 / int8 storage: n input rows at src (device) -> stored rows at `rows` (row pitch in elements), converting to fp16 or
+// quantising; elements (fp16) or rows (int8) the storage cannot hold are added to *bad.
+static cudaError_t convert_rows(const om_index* ix, const void* src, om_dtype dtype, int64_t n, void* rows, int64_t pitch, int* bad,
+                                cudaStream_t st) {
+  return with_input(src, dtype, [&](const auto* in) {
+    if (ix->storage == OM_I8)
+      quantize_rows_i8_kernel<<<grid_for(n, 8), 256, 0, st>>>(in, n, ix->d, static_cast<int8_t*>(rows), pitch, bad);
+    else
+      to_f16_rows_kernel<<<grid_for(n * ix->d, 256), 256, 0, st>>>(in, n, ix->d, static_cast<__half*>(rows), ix->dpad, bad);
+    return cudaGetLastError();
+  });
+}
+
+// fp32 storage: `elems` input values at src (device, or host fp32 when kind is OM_HOST) -> fp32 rows at dst.
+static int fp32_rows(float* dst, const void* src, om_memkind kind, om_dtype dtype, size_t elems, cudaStream_t st) {
+  return with_input(src, dtype, [&](const auto* in) -> int {
+    if constexpr (std::is_same<decltype(in), const float*>::value) {
+      OM_CUDA(cudaMemcpyAsync(dst, in, elems * 4, kind == OM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
+    } else {
+      to_f32<<<grid_for(elems, 256), 256, 0, st>>>(in, dst, (int64_t)elems);
+      OM_CUDA(cudaGetLastError());
+    }
+    return 0;
+  });
+}
+
+// The refusal of an add to fp16 / int8 storage that holds `bad` values the storage cannot hold.
+static int refuse_add(const om_index* ix, int bad) {
+  if (ix->storage == OM_I8)
+    return fail(OM_EINVAL, "om_index_add: %d rows hold inf or NaN; int8 storage cannot hold them and no row was added", bad);
+  return fail(OM_EINVAL, "om_index_add: %d elements are NaN or round to +-inf in fp16 (|x| >= 65520); fp16 storage cannot "
+              "hold them and no row was added", bad);
+}
+
 // om_index_add on fp16 / int8 storage: convert into the reserved rows, count what the storage cannot hold, and commit only
 // if nothing was out of range (the converted rows stay beyond ntotal otherwise).  Synchronises `st` to read the count.
 static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, cudaStream_t st) {
@@ -1289,29 +1436,88 @@ static int add_converted(om_index* ix, const void* x, om_memkind kind, om_dtype 
   const void* src = nullptr;
   void* tmp = nullptr;
   OM_TRY(stage_input(x, kind, elems * (dtype == OM_F32 ? 4 : 2), st, &src, &tmp));
-  const bool i8 = ix->storage == OM_I8;  // quantise, else convert to fp16
   int* bad = ix->scratch();
   cudaError_t e = cudaMemsetAsync(bad, 0, sizeof(int), st);
-  if (e == cudaSuccess)
-    e = with_input(src, dtype, [&](const auto* in) {
-      if (i8)
-        quantize_rows_i8_kernel<<<grid_for(n, 8), 256, 0, st>>>(in, n, ix->d, static_cast<int8_t*>(rows), pitch, bad);
-      else
-        to_f16_rows_kernel<<<grid_for(static_cast<int64_t>(elems), 256), 256, 0, st>>>(in, n, ix->d, static_cast<__half*>(rows),
-                                                                                        ix->dpad, bad);
-      return cudaGetLastError();
-    });
+  if (e == cudaSuccess) e = convert_rows(ix, src, dtype, n, rows, pitch, bad, st);
   const int rc = e == cudaSuccess ? read_decision(ix, nullptr, bad, 1, kNcclMax, 0, st) : 0;
   if (tmp) cudaFree(tmp);
   OM_CUDA(e);
   OM_TRY(rc);
-  if (ix->h_status[0] > 0 && i8)
-    return fail(OM_EINVAL, "om_index_add: %d rows hold inf or NaN; int8 storage cannot hold them and no row was added",
-                ix->h_status[0]);
-  if (ix->h_status[0] > 0)
-    return fail(OM_EINVAL, "om_index_add: %d elements are NaN or round to +-inf in fp16 (|x| >= 65520); fp16 storage cannot "
-                "hold them and no row was added", ix->h_status[0]);
+  if (ix->h_status[0] > 0) return refuse_add(ix, ix->h_status[0]);
   return om_index_commit(ix, n, st);
+}
+
+// om_index_add on a host-resident index.  The rows pass through device window 0 in pieces that each end inside one host
+// chunk: converted there by the kernels of a device index's add (fp32 storage: committed at once, which builds the scan copy
+// and the error-norm maxima), then copied out to the chunk, beyond ntotal.  fp16 / int8 storage counts what it cannot
+// hold over all pieces and, when nothing is refused, commits every piece (re-uploaded from its chunk unless the add was one
+// piece) with commit_rows_kernel.  A refused add leaves ntotal, the stored rows and the maxima as they were.  Synchronises st.
+static int add_host(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, cudaStream_t st) {
+  if (ix->n + n > 0xfffffff0ll) return fail(OM_EINVAL, "index shard limited to 2^32-16 rows; shard the corpus");
+  const int64_t W = ix->window, n0 = ix->n, end = n0 + n;
+  const size_t hrow = host_row_bytes(ix), in_row = static_cast<size_t>(ix->d) * (dtype == OM_F32 ? 4 : 2);
+  while (static_cast<int64_t>(ix->chunks.size()) * W < end) {  // growth adds chunks; the rows already held stay where they are
+    void* c = nullptr;
+    if (cudaHostAlloc(&c, static_cast<size_t>(W) * hrow, cudaHostAllocDefault) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(OM_ENOMEM, "om_index_add: cannot allocate %lld rows of pinned host memory for the host-resident index",
+                  (long long)W);
+    }
+    ix->chunks.push_back(c);
+  }
+  Rows X;
+  OM_TRY(window_reserve(ix, 0, std::min(W, n), &X));
+  void* rows = const_cast<void*>(with_rows(ix, X, [](const auto* xs) -> const void* { return xs; }));
+  const bool f32 = ix->storage == OM_F32;
+  // host input the window cannot take as it is goes through a device staging buffer of one piece
+  struct Tmp {
+    void* p = nullptr;
+    ~Tmp() { cudaFree(p); }
+  } tmp;
+  const bool staged = kind == OM_HOST && !(f32 && dtype == OM_F32);
+  if (staged) OM_CUDA(cudaMalloc(&tmp.p, static_cast<size_t>(std::min(W, n)) * in_row));
+  OM_TRY(settle_reset(ix, st));
+  int* bad = ix->scratch();
+  OM_CUDA(cudaMemsetAsync(bad, 0, sizeof(int), st));
+  auto piece_end = [&](int64_t a) { return std::min(end, (a / W + 1) * W); };
+  for (int64_t a = n0; a < end; a = piece_end(a)) {
+    const int64_t m = piece_end(a) - a;
+    const void* in = static_cast<const uint8_t*>(x) + static_cast<size_t>(a - n0) * in_row;
+    if (staged) {
+      OM_CUDA(cudaMemcpyAsync(tmp.p, in, static_cast<size_t>(m) * in_row, cudaMemcpyHostToDevice, st));
+      in = tmp.p;
+    }
+    if (f32) {
+      OM_TRY(fp32_rows(static_cast<float*>(rows), in, staged ? OM_DEVICE : kind, dtype, static_cast<size_t>(m) * ix->d, st));
+      rows_to_f16_kernel<<<grid_for(m, 8), 256, 0, st>>>(static_cast<float*>(rows), const_cast<__half*>(X.xh), m, ix->d, ix->dpad,
+                                                         nullptr, nullptr, ix->gstats);
+      OM_CUDA(cudaGetLastError());
+    } else {
+      const int64_t pitch = with_rows(ix, X, [&](const auto* xs) { return pitch_of(xs, ix->d); });
+      OM_CUDA(convert_rows(ix, in, dtype, m, rows, pitch, bad, st));
+    }
+    uint8_t* chunk = static_cast<uint8_t*>(ix->chunks[a / W]) + static_cast<size_t>(a % W) * hrow;
+    OM_CUDA(cudaMemcpyAsync(chunk, rows, static_cast<size_t>(m) * hrow, cudaMemcpyDeviceToHost, st));
+  }
+  OM_TRY(read_decision(ix, nullptr, bad, 1, kNcclMax, 0, st));
+  if (ix->h_status[0] > 0) return refuse_add(ix, ix->h_status[0]);
+  if (!f32) {
+    const bool one_piece = piece_end(n0) == end;  // the window still holds it
+    for (int64_t a = n0; a < end; a = piece_end(a)) {
+      const int64_t m = piece_end(a) - a;
+      if (!one_piece)
+        OM_CUDA(cudaMemcpyAsync(rows, static_cast<const uint8_t*>(ix->chunks[a / W]) + static_cast<size_t>(a % W) * hrow,
+                                static_cast<size_t>(m) * hrow, cudaMemcpyHostToDevice, st));
+      with_rows(ix, X, [&](const auto* xs) {
+        if constexpr (!std::is_same<decltype(xs), const float*>::value)
+          commit_rows_kernel<<<grid_for(m, 8), 256, 0, st>>>(xs, m, ix->d, ix->gstats, reinterpret_cast<int*>(ix->gstats) + 2);
+      });
+      OM_CUDA(cudaGetLastError());
+    }
+  }
+  OM_CUDA(cudaStreamSynchronize(st));
+  ix->n = end;
+  return 0;
 }
 
 int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, int64_t n, void* stream) {
@@ -1319,6 +1525,7 @@ int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, i
   if (n == 0) return 0;
   if (dtype != OM_F32 && dtype != OM_BF16 && dtype != OM_F16) return fail(OM_EINVAL, "om_index_add: unsupported dtype %d", (int)dtype);
   cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (ix->window) return add_host(ix, x, kind, dtype, n, st);
   if (ix->storage != OM_F32) return add_converted(ix, x, kind, dtype, n, st);
   float* dst = nullptr;
   OM_TRY(om_index_reserve(ix, n, &dst));
@@ -1326,15 +1533,7 @@ int om_index_add(om_index* ix, const void* x, om_memkind kind, om_dtype dtype, i
   const void* src = x;
   void* tmp = nullptr;
   if (dtype != OM_F32) OM_TRY(stage_input(x, kind, elems * 2, st, &src, &tmp));  // fp32 rows are copied straight in
-  OM_TRY(with_input(src, dtype, [&](const auto* in) -> int {
-    if constexpr (std::is_same<decltype(in), const float*>::value) {
-      OM_CUDA(cudaMemcpyAsync(dst, in, elems * 4, kind == OM_HOST ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, st));
-    } else {
-      to_f32<<<grid_for(elems, 256), 256, 0, st>>>(in, dst, (int64_t)elems);
-      OM_CUDA(cudaGetLastError());
-    }
-    return 0;
-  }));
+  OM_TRY(fp32_rows(dst, src, kind, dtype, elems, st));
   if (tmp) {
     OM_CUDA(cudaStreamSynchronize(st));
     cudaFree(tmp);
@@ -1396,6 +1595,8 @@ int64_t om_index_get_stat(const om_index* ix, const char* name) {
   if (!strcmp(name, "other_ns")) return static_cast<int64_t>(ix->st_other_us * 1e3);
   if (!strcmp(name, "range_candidates")) return ix->st_range_candidates;
   if (!strcmp(name, "range_resweeps")) return ix->st_range_resweeps;
+  if (!strcmp(name, "partitions")) return ix->st_partitions;
+  if (!strcmp(name, "upload_wait_ns")) return static_cast<int64_t>(ix->st_upload_wait_us * 1e3);
   return -1;
 }
 
@@ -1409,8 +1610,9 @@ struct Timed {
   cudaStream_t st;
   bool on;
   Timed(om_index* ix_, cudaStream_t st_, int kind) : ix(ix_), st(st_), on(ix_->profile != 0) {
-    static const char* nvtx_names[4] = {"om.search.scan", "om.search.select", "om.search.rescore", "om.search.exchange_certify"};
-    nvtxRangePushA(nvtx_names[kind & 3]);
+    static const char* nvtx_names[5] = {"om.search.scan", "om.search.select", "om.search.rescore", "om.search.exchange_certify",
+                                        "om.search.upload_wait"};
+    nvtxRangePushA(nvtx_names[kind]);
     if (!on) return;
     if (ix->ev_used + 2 > ix->ev.size()) {
       cudaEvent_t a, b;
@@ -1434,13 +1636,14 @@ struct Timed {
 };
 
 void collect_profile(om_index* ix) {
-  static const char* names[4] = {"scan", "select", "finalize", "exchange+certify"};
+  static const char* names[5] = {"scan", "select", "finalize", "exchange+certify", "upload wait"};
+  double* sums[5] = {&ix->st_scan_us, &ix->st_select_us, &ix->st_final_us, &ix->st_other_us, &ix->st_upload_wait_us};
   for (size_t i = 0; i + 1 < ix->ev_used; i += 2) {
     float ms = 0.f;
     if (cudaEventElapsedTime(&ms, ix->ev[i], ix->ev[i + 1]) != cudaSuccess) continue;
     const int kind = ix->ev_kind[i / 2];
-    (kind == 0 ? ix->st_scan_us : kind == 1 ? ix->st_select_us : kind == 2 ? ix->st_final_us : ix->st_other_us) += ms * 1e3;
-    if (ix->profile >= 2) fprintf(stderr, "[om profile] launch %zu %s %.3f ms\n", i / 2, names[kind & 3], ms);
+    *sums[kind] += ms * 1e3;
+    if (ix->profile >= 2) fprintf(stderr, "[om profile] launch %zu %s %.3f ms\n", i / 2, names[kind], ms);
   }
   ix->ev_used = 0;
 }
@@ -1521,7 +1724,7 @@ size_t level_layout(Level& L, void* base, size_t nq, size_t nqc, int C, int dpad
   return lay.bytes;
 }
 
-// sizes the candidate lists of a level, lays out the level workspace and converts the queries
+// sizes the candidate lists of a level over the rows L.X, lays out the level workspace and converts the queries
 int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp_target, int mode, int world,
                   cudaStream_t st) {
   if (k > kMaxCandidates) return fail(OM_EINVAL, "om_index_search: k = %d exceeds %d", k, kMaxCandidates);
@@ -1539,7 +1742,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
     const double m = static_cast<double>(L.kp_target) / world;
     L.kp_target = static_cast<int>(std::min<int64_t>(L.kp_target, round_up(static_cast<int64_t>(m + 6.0 * sqrt(m) + 32.0), 32)));
   }
-  L.kp = static_cast<int>(std::min<int64_t>(L.kp_target, std::max<int64_t>(ix->n, 1)));
+  L.kp = static_cast<int>(std::min<int64_t>(L.kp_target, std::max<int64_t>(L.X.n, 1)));
   // Expected list length after a round that multiplies the rows seen by g is ~g kp (kp kept + ~(g-1) kp new
   // survivors); 25 % + 512 entries of head-room cover its spread for exchangeable row order.
   for (L.growth = ix->growth > 0 ? ix->growth : (nq <= 256 ? 8 : 2);; --L.growth) {  // large k: slower-growing schedule that fits the 16384-entry select
@@ -1561,7 +1764,7 @@ int level_prepare(om_index* ix, Level& L, const float* qf, int nq, int k, int kp
   return mode == 0 ? convert_queries(ix, L, st) : 0;
 }
 
-// One scan round over rows [pos, pos + step) of the shard for queries [q0, q0 + nqc) of the level, on the kernel the level
+// One scan round over rows [pos, pos + step) of L.X for queries [q0, q0 + nqc) of the level, on the kernel the level
 // and the storage choose: mode 1 the exact fp32 scan; mode 0 the int8 scan on an int8 index, else the wide cluster scan
 // for threshold rounds of more than 128 queries with pair_scan on, else the GEMM core.  Survivors of thr go to the level's
 // lists; dense: every score at position = column.
@@ -1575,13 +1778,13 @@ int scan_round(om_index* ix, const Level& L, int q0, int nqc, int64_t pos, int64
     // every round on the int8 scan (pair_scan and the cluster shape do not apply)
     const int8_t* qhi = L.q8 + static_cast<size_t>(q0) * ix->dpad;
     const int8_t* qlo = L.q8 + (static_cast<size_t>(L.nq) + q0) * ix->dpad;
-    const int64_t pitch = pitch_of(ix->xq, ix->d);
-    const cudaError_t e = launch_scan_i8(dense, L.allow, qhi, qlo, ix->dpad, L.qsig + q0, ix->xq + pos * pitch, pitch,
+    const int64_t pitch = pitch_of(L.X.xq, ix->d);
+    const cudaError_t e = launch_scan_i8(dense, L.allow, qhi, qlo, ix->dpad, L.qsig + q0, L.X.xq + pos * pitch, pitch,
                                          ix->dpad, nqc, ncols, ix->d, L.thr, L.cand, L.count, overflow, C, row_base, sms, st);
     if (e != cudaSuccess) return fail(OM_ECUDA, "int8 scan kernel launch failed: %s", cudaGetErrorString(e));
   } else if (L.mode == 0) {
     const __half* qh = L.qh + static_cast<size_t>(q0) * ix->dpad;
-    const __half* xrows = ix->xh + static_cast<size_t>(pos) * ix->dpad;
+    const __half* xrows = L.X.xh + static_cast<size_t>(pos) * ix->dpad;
     cudaError_t e;
     // a cluster owns at least 2 x 128 query rows per tile: with <= 128 queries the peers' boxes would be padding (and the sweep is
     // HBM-bound there, where the dynamic tile order of the single-CTA kernel matters more than operand sharing).  The
@@ -1612,7 +1815,7 @@ int scan_round(om_index* ix, const Level& L, int q0, int nqc, int64_t pos, int64
     dim3 grid(static_cast<unsigned>(std::min<int64_t>((step + 15) / 16, static_cast<int64_t>(sms) * 4)),
               static_cast<unsigned>((nqc + nqt - 1) / nqt));
     const size_t smem = static_cast<size_t>(nqt) * ix->d * 4 + (exact_filter ? 8 * kMaxExcluded * 4 : 0);
-    with_rows(ix, [&](const auto* xs) {
+    with_rows(ix, L.X, [&](const auto* xs) {
       using RowT = std::decay_t<decltype(*xs)>;
       const auto kernel = exact_filter ? exact_scan_kernel<8, 2, RowT, true> : exact_scan_kernel<8, 2, RowT>;
       kernel<<<grid, 256, smem, st>>>(xs + pos * pitch_of(xs, ix->d), step, row_base, qf, nqc, ix->d, nqt, L.thr, L.cand,
@@ -1623,12 +1826,12 @@ int scan_round(om_index* ix, const Level& L, int q0, int nqc, int64_t pos, int64
   return 0;
 }
 
-// One sweep of the shard for queries [q0, q0 + nqc) of the level.  safe = false: doubling rounds; safe = true: fixed
+// One sweep of the rows L.X for queries [q0, q0 + nqc) of the level.  safe = false: doubling rounds; safe = true: fixed
 // rounds of C - kp rows, which cannot overflow.  mode 0: tensor-core scan (fp16; int8 index: scan_i8.cuh), 1: exact fp32
 // scan.
 int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sms, cudaStream_t st) {
   const int64_t growth = L.growth;
-  const int64_t N = ix->n;
+  const int64_t N = L.X.n;
   const int C = L.C, kp = L.kp;
   if (N == 0) {
     fill_i32<<<(nqc + 255) / 256, 256, 0, st>>>(L.count, 0, nqc);
@@ -1644,16 +1847,17 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
   // survives, and select counts the list, which holds allowed rows only.  Later rounds filter as usual.  The exact scan
   // drops excluded ids as well, so its lists (k rows) hold no excluded row either.
   const bool sparse_first = L.allow || (L.mode == 1 && L.ex.off);
-  // With a bitmap, rounds are sized in allowed rows (ix->allow_prefix, per 256-row block), as they would be in rows on an
+  // With a bitmap, rounds are sized in allowed rows (L.allow_prefix, per 256-row block), as they would be in rows on an
   // index of the allowed rows alone: the first round takes up to C allowed rows, a doubling round (growth - 1) x the
   // allowed rows seen, a safe round C - kp.  So a round at threshold -inf (fewer than kp allowed rows seen) cannot
   // overflow its list however the allowed rows are placed, and stretches of disallowed rows join the next round.
   // Returns the end of the round from pos: the last block boundary (or N) whose allowed rows since pos stay within
-  // budget, one block at least.
-  const std::vector<int64_t>& A = ix->allow_prefix;
+  // budget, one block at least.  seen(b): allowed rows of X before block b.
+  const int64_t* A = L.allow_prefix;
+  auto seen = [&](int64_t b) { return A[b] - A[0]; };
   auto allowed_end = [&](int64_t from, int64_t budget) -> int64_t {
     const int64_t b0 = from / 256;
-    int64_t b = std::upper_bound(A.begin() + b0 + 1, A.end(), A[b0] + budget) - A.begin() - 1;
+    int64_t b = std::upper_bound(A + b0 + 1, A + (N + 255) / 256 + 1, A[b0] + budget) - A - 1;
     b = std::max(b, b0 + 1);
     return std::min<int64_t>(b * 256, N);
   };
@@ -1665,7 +1869,7 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
   while (pos < N) {
     int64_t step;
     if (L.allow)
-      step = allowed_end(pos, first ? C : safe ? C - kp : (growth - 1) * (A[pos / 256])) - pos;
+      step = allowed_end(pos, first ? C : safe ? C - kp : (growth - 1) * seen(pos / 256)) - pos;
     else if (first)
       step = std::min<int64_t>(N, C);
     else if (safe)
@@ -1674,7 +1878,7 @@ int sweep_chunk(om_index* ix, const Level& L, int q0, int nqc, bool safe, int sm
       step = std::min<int64_t>(N - pos, (growth - 1) * pos);
     // a first round of allowed rows only (an allow-all bitmap, a sub-collection at the start of the shard) stores densely
     // as the unfiltered search does: nothing there for the filter to drop
-    const bool dense = first && (!sparse_first || (L.mode == 0 && L.allow && A[(pos + step + 255) / 256] == step));
+    const bool dense = first && (!sparse_first || (L.mode == 0 && L.allow && seen((pos + step + 255) / 256) == step));
     OM_TRY(scan_round(ix, L, q0, nqc, pos, step, dense, sms, st));
     {
       Timed t(ix, st, 1);
@@ -1700,7 +1904,7 @@ int finalize_chunk(om_index* ix, const Level& L, int q0, int nqc, float* D, int6
     const float* qf = L.qf + static_cast<size_t>(q0) * ix->d;
     Excluded ex = L.ex;
     ex.q_base = q0;
-    with_rows(ix, [&](const auto* xs) {
+    with_rows(ix, L.X, [&](const auto* xs) {
       using RowT = std::decay_t<decltype(*xs)>;
       const auto kernel = filter ? finalize_kernel<RowT, true> : finalize_kernel<RowT>;
       kernel<<<nqc, 256, fin_smem, st>>>(L.cand, L.count, L.C, qf, xs, ix->d, D, I, id_offset, k_out, ix->stage_scores,
@@ -1893,7 +2097,8 @@ int call_prologue(om_index* ix, om_comm* comm, const char* who, const void* q, o
   ix->st_rounds = ix->st_retries = ix->st_launches = 0;
   ix->st_flagged = ix->st_flagged_wide = ix->st_exact = 0;
   ix->st_scan_cluster = ix->st_scan_clusters = 0;
-  ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = 0;
+  ix->st_scan_us = ix->st_select_us = ix->st_final_us = ix->st_other_us = ix->st_upload_wait_us = 0;
+  ix->st_partitions = 1;
   ix->ev_used = 0;
   OM_TRY(once_attrs(ix));
   if (ix->d > 16384) return fail(OM_EINVAL, "%s: d > 16384 unsupported", who);
@@ -1932,41 +2137,32 @@ int gather_listed(const std::vector<int>& list, int* dlist, const float* src, in
   return 0;
 }
 
-// The whole search: level 0 (all queries, k + slack candidates) -> level 1 (uncertified queries, widest list) ->
-// level 2 (still uncertified: exact fp32 scan).  comm == nullptr: single shard.  f: nullptr, or a checked filter with at
-// least one part.
-int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
-                om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
-  NvtxRange nvtx("om.search");
+// The levels of a search over the rows X, the rows [p0, p0 + X.n) of the index (p0 a multiple of 256): level 0 (all
+// queries, k + slack candidates) -> level 1 (uncertified queries, widest list) -> level 2 (still uncertified: exact fp32
+// scan), into the device results (dD, dI) with ids id_offset + p0 + row.  comm == nullptr: single shard.  f: nullptr, or a
+// checked filter with at least one part, over all the index's rows.  flags: nq ints of scratch.
+int search_rows(om_index* ix, om_comm* comm, const Rows& X, int64_t p0, const float* qf, int nq, int k, float* dD, int64_t* dI,
+                int64_t id_offset, const om_search_filter* f, int* flags, cudaStream_t st) {
   const int d = ix->d;
   const int world = comm ? comm->world : 1;
-  // whole-search staging: results (if they leave to the host), the certificate's per-query flags, queries (in the prologue)
-  Layout ows;
-  const size_t o_D = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 4 : 0);
-  const size_t o_I = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 8 : 0);
-  const size_t o_flags = ows.add(static_cast<size_t>(nq) * 4);
-  const float* qf = nullptr;
-  OM_TRY(call_prologue(ix, comm, "om_index_search", q, q_kind, nq, nullptr, ows, &qf, nullptr, st));
-  float* dD = out_kind == OM_HOST ? region<float>(ix->ows.p, o_D) : D;
-  int64_t* dI = out_kind == OM_HOST ? region<int64_t>(ix->ows.p, o_I) : I;
-  int* flags = region<int>(ix->ows.p, o_flags);
-
-  // the filter of every level: the bitmap, and the exclusions of the level's queries (qmap: the escalated ones)
+  // the filter of every level: X's slice of the bitmap, and the exclusions of the level's queries (qmap: the escalated ones)
   auto filter = [&](Level& L, const int* qmap) {
     if (!f) return;
-    L.allow = f->allow_bits;
-    L.ex = Excluded{f->exclude_offsets, f->exclude_ids, qmap, 0, id_offset};
+    L.allow = f->allow_bits ? f->allow_bits + p0 / 32 : nullptr;
+    L.allow_prefix = ix->allow_prefix.data() + p0 / 256;
+    L.ex = Excluded{f->exclude_offsets, f->exclude_ids, qmap, 0, id_offset + p0};
   };
   const int64_t slack = ix->rescore_slack >= 0 ? ix->rescore_slack : std::max<int64_t>(128, k / 5);
   const int kp0 = static_cast<int>(std::min<int64_t>(static_cast<int64_t>(k) + slack, kMaxCandidates));
   std::vector<int> list, sub;  // uncertified queries: indices into the call's queries, into the last sub-batch
   {  // level 0; exact_only: the exact scan of every query, which leaves none uncertified
     Level L;
-    if (ix->exact_only) ix->st_exact = nq;
+    L.X = X;
+    if (ix->exact_only) ix->st_exact += nq;
     OM_TRY(level_prepare(ix, L, qf, nq, k, ix->exact_only ? k : kp0, ix->exact_only ? 1 : 0, world, st));
     filter(L, nullptr);
-    OM_TRY(run_level(ix, comm, L, dD, dI, id_offset, flags, list, st));
-    ix->st_flagged = static_cast<int64_t>(list.size());
+    OM_TRY(run_level(ix, comm, L, dD, dI, id_offset + p0, flags, list, st));
+    ix->st_flagged += static_cast<int64_t>(list.size());
   }
   // Escalation: the queries in `list` are gathered into a compact sub-batch, answered by one more level and scattered back
   // over their rows of (dD, dI); `sub` lists the ones the level left uncertified.  sws holds the uploaded list (the
@@ -1983,9 +2179,10 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
     int64_t* Is = region<int64_t>(ix->sws.p, s_I);
     OM_TRY(gather_listed(list, dlist, qf, d, qsub, st));
     Level Ls;
+    Ls.X = X;
     OM_TRY(level_prepare(ix, Ls, qsub, static_cast<int>(n_sub), k, kp_target, mode, world, st));
     filter(Ls, dlist);
-    OM_TRY(run_level(ix, comm, Ls, Ds, Is, id_offset, flags, sub, st));
+    OM_TRY(run_level(ix, comm, Ls, Ds, Is, id_offset + p0, flags, sub, st));
     scatter_results_kernel<<<grid_for(static_cast<int64_t>(n_sub) * k, 256), 256, 0, st>>>(Ds, Is, dlist, static_cast<int>(n_sub),
                                                                                             k, dD, dI);
     OM_CUDA(cudaGetLastError());
@@ -1995,17 +2192,116 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   if (!list.empty()) {
     // level 1: widest candidate list the select / sort kernels take.  (Sharded: the decision must not depend on this
     // rank's row count — every rank runs the same levels.)
-    if (kp0 < kMaxCandidates && (world > 1 || ix->n > kp0)) {
+    if (kp0 < kMaxCandidates && (world > 1 || X.n > kp0)) {
       OM_TRY(run_sub(kMaxCandidates, 0));
       for (int& i : sub) i = list[i];
       list.swap(sub);
     }
-    ix->st_flagged_wide = static_cast<int64_t>(list.size());
+    ix->st_flagged_wide += static_cast<int64_t>(list.size());
     if (!list.empty()) {  // level 2: exact fp32 scan
-      ix->st_exact = static_cast<int64_t>(list.size());
+      ix->st_exact += static_cast<int64_t>(list.size());
       OM_TRY(run_sub(k, 1));
     }
   }
+  return 0;
+}
+
+// The partition p upload of a host-resident index into window p % 2, on the copy stream: it waits until the search has
+// left the window (ev_free), copies the partition's chunk in one piece and marks the window ready (ev_ready).
+int upload_partition(om_index* ix, int64_t p) {
+  const int w = static_cast<int>(p & 1);
+  const int64_t rows = std::min(ix->window, ix->n - p * ix->window);
+  Rows X;
+  OM_TRY(window_reserve(ix, w, rows, &X));
+  const void* dst = with_rows(ix, X, [](const auto* xs) -> const void* { return xs; });
+  OM_CUDA(cudaStreamWaitEvent(ix->copy_st, ix->ev_free[w], 0));
+  OM_CUDA(cudaMemcpyAsync(const_cast<void*>(dst), ix->chunks[p], static_cast<size_t>(rows) * host_row_bytes(ix),
+                          cudaMemcpyHostToDevice, ix->copy_st));
+  OM_CUDA(cudaEventRecord(ix->ev_ready[w], ix->copy_st));
+  return 0;
+}
+
+// The search of a host-resident index: each partition of `window` rows is uploaded while the previous one is searched,
+// searched by search_rows with its row offset, and merged into the running result by (score desc, id asc).  Each
+// partition's result is the exact top-k of its rows, and an fp32 score does not depend on the rows around it, so the merge
+// is bitwise the search of one device index of all the rows.  R, RI: [2, nq, k] scratch (running result, partition result).
+int search_host(om_index* ix, const float* qf, int nq, int k, float* dD, int64_t* dI, int64_t id_offset,
+                const om_search_filter* f, int* flags, float* R, int64_t* RI, cudaStream_t st) {
+  const int64_t W = ix->window, N = ix->n;
+  const int64_t np = (N + W - 1) / W;
+  if (np <= 1) {
+    ix->st_partitions = 1;
+    if (N == 0) return search_rows(ix, nullptr, Rows{}, 0, qf, nq, k, dD, dI, id_offset, f, flags, st);
+  } else {
+    ix->st_partitions = np;
+  }
+  // whatever way the call ends, no upload is left running into the windows
+  struct CopyDone {
+    cudaStream_t s;
+    ~CopyDone() { cudaStreamSynchronize(s); }
+  } copy_done{ix->copy_st};
+  // both windows are sized before the first upload: a reservation that grows a window frees it
+  Rows X;
+  OM_TRY(window_reserve(ix, 0, std::min(W, N), &X));
+  if (np > 1) OM_TRY(window_reserve(ix, 1, std::min(W, N - W), &X));
+  OM_CUDA(cudaEventRecord(ix->ev_entry, st));  // uploads start after the caller's earlier work on st
+  OM_CUDA(cudaStreamWaitEvent(ix->copy_st, ix->ev_entry, 0));
+  OM_TRY(upload_partition(ix, 0));
+  const size_t slot = static_cast<size_t>(nq) * k;
+  for (int64_t p = 0; p < np; ++p) {
+    if (p + 1 < np) OM_TRY(upload_partition(ix, p + 1));
+    const int w = static_cast<int>(p & 1);
+    {
+      Timed t(ix, st, 4);
+      OM_CUDA(cudaStreamWaitEvent(st, ix->ev_ready[w], 0));
+    }
+    OM_TRY(window_reserve(ix, w, std::min(W, N - p * W), &X));
+    if (ix->storage == OM_F32) {  // the scan copy, as om_index_commit builds it
+      rows_to_f16_kernel<<<grid_for(X.n, 8), 256, 0, st>>>(X.xf, const_cast<__half*>(X.xh), X.n, ix->d, ix->dpad, nullptr,
+                                                           nullptr, nullptr);
+      OM_CUDA(cudaGetLastError());
+      ix->st_launches += 1;
+    }
+    float* Dp = np == 1 ? dD : R + (p > 0 ? slot : 0);
+    int64_t* Ip = np == 1 ? dI : RI + (p > 0 ? slot : 0);
+    OM_TRY(search_rows(ix, nullptr, X, p * W, qf, nq, k, Dp, Ip, id_offset, f, flags, st));
+    OM_CUDA(cudaEventRecord(ix->ev_free[w], st));
+    if (p > 0) {
+      OM_TRY(merge_parts(R, RI, static_cast<int64_t>(slot), static_cast<int64_t>(slot), 2, nq, k, k, dD, dI, st));
+      ix->st_launches += 1;
+      if (p + 1 < np) {
+        OM_CUDA(cudaMemcpyAsync(R, dD, slot * 4, cudaMemcpyDeviceToDevice, st));
+        OM_CUDA(cudaMemcpyAsync(RI, dI, slot * 8, cudaMemcpyDeviceToDevice, st));
+      }
+    }
+  }
+  return 0;
+}
+
+// The whole search of a device index (search_rows over its rows) or of a host-resident one (search_host), from the
+// caller's queries to the caller's results.
+int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
+                om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
+  NvtxRange nvtx("om.search");
+  const bool host_rows = ix->window > 0;
+  // whole-search staging: results (if they leave to the host), the certificate's per-query flags, a host-resident index's
+  // running and partition results, queries (in the prologue)
+  Layout ows;
+  const size_t o_D = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 4 : 0);
+  const size_t o_I = ows.add(out_kind == OM_HOST ? static_cast<size_t>(nq) * k * 8 : 0);
+  const size_t o_flags = ows.add(static_cast<size_t>(nq) * 4);
+  const size_t o_R = ows.add(host_rows ? 2 * static_cast<size_t>(nq) * k * 4 : 0);
+  const size_t o_RI = ows.add(host_rows ? 2 * static_cast<size_t>(nq) * k * 8 : 0);
+  const float* qf = nullptr;
+  OM_TRY(call_prologue(ix, comm, "om_index_search", q, q_kind, nq, nullptr, ows, &qf, nullptr, st));
+  float* dD = out_kind == OM_HOST ? region<float>(ix->ows.p, o_D) : D;
+  int64_t* dI = out_kind == OM_HOST ? region<int64_t>(ix->ows.p, o_I) : I;
+  int* flags = region<int>(ix->ows.p, o_flags);
+  if (host_rows)
+    OM_TRY(search_host(ix, qf, nq, k, dD, dI, id_offset, f, flags, region<float>(ix->ows.p, o_R), region<int64_t>(ix->ows.p, o_RI),
+                       st));
+  else
+    OM_TRY(search_rows(ix, comm, device_rows(ix), 0, qf, nq, k, dD, dI, id_offset, f, flags, st));
   if (out_kind == OM_HOST) {
     OM_CUDA(cudaMemcpyAsync(D, dD, static_cast<size_t>(nq) * k * 4, cudaMemcpyDeviceToHost, st));
     OM_CUDA(cudaMemcpyAsync(I, dI, static_cast<size_t>(nq) * k * 8, cudaMemcpyDeviceToHost, st));
@@ -2022,6 +2318,9 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
 // name the plain entry.
 int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
                  float* D, int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter, void* stream) {
+  if (ix && ix->window && sharded)  // refused before the communicator is read
+    return fail(OM_EINVAL, "%s: a host-resident index cannot be a shard of a sharded search",
+                filtered ? "om_index_search_sharded_filtered" : "om_index_search_sharded");
   const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
   const bool check = local || (filtered && comm && comm->world > 1);
   const char* who = sharded ? (check ? "om_index_search_sharded_filtered" : "om_index_search_sharded")
@@ -2099,6 +2398,7 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
   int* to_exact = region<int>(b, o_exact);
   long long* doff = region<long long>(b, o_off);
   unsigned long long* alt = region<unsigned long long>(b, o_alt);
+  L.X = device_rows(ix);
   L.nq = m;
   L.C = C;
   L.mode = mode;
@@ -2115,8 +2415,8 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
   OM_CUDA(cudaMemsetAsync(L.status, 0, 32, st));
   ix->st_launches += 4;
   // the sweep: one pass over the shard at the fixed thresholds, in rounds only to keep the column counts in an int
-  for (int64_t pos = 0; pos < ix->n; pos += kRangeRound) {
-    OM_TRY(scan_round(ix, L, 0, m, pos, std::min(ix->n - pos, kRangeRound), false, sms, st));
+  for (int64_t pos = 0; pos < L.X.n; pos += kRangeRound) {
+    OM_TRY(scan_round(ix, L, 0, m, pos, std::min(L.X.n - pos, kRangeRound), false, sms, st));
     range_fold_kernel<<<(m + 255) / 256, 256, 0, st>>>(L.count, filled, total, C, m);
     OM_CUDA(cudaGetLastError());
     ix->st_rounds++;
@@ -2124,7 +2424,7 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
   }
   {
     Timed t(ix, st, 2);
-    with_rows(ix, [&](const auto* xs) {
+    with_rows(ix, L.X, [&](const auto* xs) {
       using RowT = std::decay_t<decltype(*xs)>;
       // at least 32 CTAs per query, more when few queries would leave SMs idle (a handful of long lists)
       const int gx = std::min((C + 63) / 64, std::max(32, (8 * sms + m - 1) / m));
@@ -2392,6 +2692,7 @@ int range_entry(bool sharded, om_index* ix, om_comm* comm, const void* q, om_mem
   const char* who = sharded ? "om_index_range_search_sharded" : "om_index_range_search";
   if (!ix || (sharded && !comm) || nq < 0 || !lims || (nq > 0 && (!q || !radius)))
     return fail(OM_EINVAL, "%s: bad arguments (nq=%d)", who, nq);
+  if (ix->window) return fail(OM_EINVAL, "%s: range search is not available on a host-resident index", who);
   ix->r_total = -1;
   OM_TRY(device_sm_count());
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -139,17 +139,30 @@ class FlatIPIndex:
     -127, 127)`` (a zero row: s = 0); search is exact with respect to the dequantised values ``fp32(s * c)``, bitwise
     what a float32 index of ``rows_f32()`` returns.  ``add`` of a row holding inf or NaN raises and adds nothing; rows
     written in place (the encoder quantises into an int8 ``reserve_rows`` view) and committed with a non-finite scale
-    make ``search`` raise until ``reset``."""
+    make ``search`` raise until ``reset``.
 
-    def __init__(self, d: int, dtype: torch.dtype = torch.float32):
+    ``memory="host"`` (``om_index_create_host``) keeps the stored rows in pinned host memory, for corpora larger than
+    the GPU's memory: a search streams them through the GPU ``window_rows`` rows at a time (a multiple of 256; 0 = sized
+    from the free device memory) and returns bitwise what the ``memory="device"`` index of the same adds returns.
+    ``add``, ``search`` (filters included), ``search_device``, ``search_pinned``, ``reset``, ``set_param`` and
+    ``stat`` work as for a device index; the calls that need device rows (``reserve_rows``, ``commit_rows``,
+    ``master_rows``, ``rows_f32``), range search and the sharded searches raise the library's error."""
+
+    def __init__(self, d: int, dtype: torch.dtype = torch.float32, memory: str = "device", window_rows: int = 0):
         if dtype not in _STORAGE:
             raise ValueError("index storage must be torch.float32, torch.float16 or torch.int8, got %s" % dtype)
+        if memory not in ("device", "host"):
+            raise ValueError("index memory must be 'device' or 'host', got %r" % (memory,))
         self._lib = _lib.load()
         h = ctypes.c_void_p()
-        _lib.check(self._lib.om_index_create_typed(int(d), _STORAGE[dtype], ctypes.byref(h)))
+        if memory == "host":
+            _lib.check(self._lib.om_index_create_host(int(d), _STORAGE[dtype], int(window_rows), ctypes.byref(h)))
+        else:
+            _lib.check(self._lib.om_index_create_typed(int(d), _STORAGE[dtype], ctypes.byref(h)))
         self._h = h
         self.d = int(d)
         self.dtype = dtype
+        self.memory = memory
 
     def __del__(self):
         h, self._h = getattr(self, "_h", None), None

@@ -84,6 +84,23 @@ def _index_dtype(args) -> torch.dtype:
     return dtypes[name]
 
 
+def _index_memory(args, writes_rows: bool = False) -> str:
+    """``--index_memory``: 'device' (the rows in HBM) or 'host' (the rows in pinned host memory, streamed through the GPU
+    by every search).  A host-resident index is built from embedding files on one process: the paths that write rows in
+    place on the GPU (``writes_rows``) and row-sharded retrieval need the device index."""
+    memory = getattr(args, "index_memory", "device")
+    if memory not in ("device", "host"):
+        raise ValueError("--index_memory must be 'device' or 'host', got %r" % (memory,))
+    if memory == "host" and args.world_size > 1:
+        raise ValueError("--index_memory host searches on one process; world_size is %d (row-sharded retrieval needs "
+                         "--index_memory device)" % args.world_size)
+    if memory == "host" and writes_rows:
+        raise ValueError("--index_memory host: a host-resident index is built from embedding files (driver.retrieve); "
+                         "encoding the corpus into the index writes its rows in place on the GPU and needs "
+                         "--index_memory device")
+    return memory
+
+
 class RankArrays:
     """Search output kept as arrays (``Retriever.search(..., as_arrays=True)``): row ``i`` of ``I`` / ``D`` holds the
     ranked rows of ``doc_names`` / scores for ``query_ids[i]``; ``to_dict()`` gives the reference's dict-of-dicts."""
@@ -125,8 +142,8 @@ class Retriever:
     # ------------------------------------------------------------------ index plumbing
     def _initialize_faiss_index(self, dim: int):
         """Name kept from the reference (:38-41); the index is the HBM-resident flat IP index with the row storage
-        ``--index_dtype`` names (float32, float16 or int8)."""
-        self.index = FlatIPIndex(dim, dtype=_index_dtype(self.args))
+        ``--index_dtype`` names (float32, float16 or int8), in the memory ``--index_memory`` names."""
+        self.index = FlatIPIndex(dim, dtype=_index_dtype(self.args), memory=_index_memory(self.args))
 
     def _move_index_to_gpu(self):
         """The reference clones a CPU faiss index to all GPUs here (:43-58).  Ours is born in HBM, one row
@@ -253,7 +270,8 @@ class Retriever:
     def doc_embedding_inference(self):
         if self.corpus_dataset is None:
             raise ValueError("No corpus dataset provided")
-        ids, _ = self._encode_dataset(self.corpus_dataset, is_query=False, into_index=True)
+        _index_memory(self.args, writes_rows=True)
+        ids, _ =self._encode_dataset(self.corpus_dataset, is_query=False, into_index=True)
         self.doc_lookup = list(ids)
         self._resident_rows = len(ids)
         os.makedirs(self.args.output_dir, exist_ok=True)
@@ -284,13 +302,15 @@ class Retriever:
                 continue
             if self.index is None or self.index.d != encoded.shape[1]:
                 self._initialize_faiss_index(encoded.shape[1])
-            self.index.reserve_rows(ef.shape[0])  # capacity for the whole file: one allocation
+            if getattr(self.index, "memory", "device") == "device":
+                self.index.reserve_rows(ef.shape[0])  # capacity for the whole file: one allocation
             for chunk in ef.chunks():
                 self.index.add(np.ascontiguousarray(chunk))
             self.doc_lookup.extend(lookup)
 
     @classmethod
     def build_all(cls, model: DRModelForInference, corpus_dataset: IterableDataset, args: EncodingArguments):
+        _index_memory(args, writes_rows=True)
         retriever = cls(model, corpus_dataset, args)
         retriever.doc_embedding_inference()  # leaves this rank's rows in its HBM shard
         if args.world_size > 1:
@@ -299,12 +319,14 @@ class Retriever:
 
     @classmethod
     def build_embeddings(cls, model: DRModelForInference, corpus_dataset: IterableDataset, args: EncodingArguments):
+        _index_memory(args, writes_rows=True)
         retriever = cls(model, corpus_dataset, args)
         retriever.doc_embedding_inference()
         return retriever
 
     @classmethod
     def from_embeddings(cls, model: DRModelForInference, args: EncodingArguments):
+        _index_memory(args)
         retriever = cls(model, None, args)
         if args.world_size > 1:
             # rank r loads the files r, r+W, ... : the corpus ends up row-sharded across the GPUs
