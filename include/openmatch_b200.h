@@ -205,8 +205,8 @@ int om_index_create_typed(int d, om_dtype storage, om_index** out);
  * om_index_add converts on the device (through a window) and synchronises `stream`; a failed pinned allocation returns
  * OM_ENOMEM and adds nothing.  om_index_reset keeps the host chunks; om_index_destroy frees them.
  * Limits: om_index_reserve, om_index_reserve_rows and om_index_commit return OM_ESTATE (there are no device rows to write
- * in place); om_index_search_sharded(_filtered) and om_index_range_search(_sharded) return OM_EINVAL; none writes
- * anything. */
+ * in place); om_index_search_sharded(_filtered) and om_index_range_search(_sharded)(_filtered) return OM_EINVAL; none
+ * writes anything. */
 int om_index_create_host(int d, om_dtype storage, int64_t window_rows, om_index** out);
 int om_index_storage(const om_index* idx); /* the om_dtype given at creation */
 /* index.add(x): x [n, d] row-major, fp32, bf16 or fp16 (host or device).  Rows get ids ntotal .. ntotal+n-1.
@@ -300,6 +300,25 @@ int om_index_range_search(om_index* idx, const void* q, om_memkind q_kind, int n
                           om_memkind out_kind, int64_t id_offset, void* stream);
 int om_index_range_search_sharded(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                   const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream);
+/* Filtered range search: for query i every row that the filter's bitmap allows and query i does not exclude, and whose
+ * fp32 score is strictly greater than radius[i], ordered by (score desc, id asc).  The filter is om_search_filter with
+ * the rules of om_index_search_filtered (bitmap over the local rows, allow_words >= ceil(ntotal / 32), at most 128
+ * excluded ids per query in the result id space, >= 0, non-decreasing offsets; ids outside the shard are ignored and
+ * duplicates are allowed).  lims and the results are bitwise what om_index_range_search returns on an index built from
+ * the eligible rows only, with ids mapped back, on every storage; for every j <= min(count, 4096) the first j results of
+ * a query are bitwise om_index_search_filtered(q, j)'s with the same filter.  Disallowed rows are never collected, so
+ * their count does not send a query to a second sweep.  A broken rule, a NaN radius or non-finite fp16 / int8 rows
+ * return OM_EINVAL before lims is written.  A null filter, or one with both parts null, is om_index_range_search /
+ * om_index_range_search_sharded.  Sharded: allow_bits covers this rank's rows, exclusions are global ids; every rank
+ * calls om_index_range_search_sharded_filtered, and a rank may pass a null or empty filter while others pass one (with
+ * more than one rank the filters are always checked together, one all-reduce).  Everything else (results kept in the
+ * handle, tunables, stats, the synchronous return) is as for the unfiltered calls. */
+int om_index_range_search_filtered(om_index* idx, const void* q, om_memkind q_kind, int nq, const float* radius,
+                                   int64_t* lims, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
+                                   void* stream);
+int om_index_range_search_sharded_filtered(om_index* idx, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                                           const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset,
+                                           const om_search_filter* filter, void* stream);
 /* D fp32 [lims[nq]], I int64 [lims[nq]] of the last range search on idx; OM_ESTATE if there is none. */
 int om_index_range_results(const om_index* idx, float* D, int64_t* I, om_memkind out_kind, void* stream);
 

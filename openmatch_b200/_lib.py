@@ -73,6 +73,10 @@ SIGNATURES = {
     "om_index_range_search": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int64, c_void_p]),
     "om_index_range_search_sharded": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int,
                                               c_int64, c_void_p]),
+    "om_index_range_search_filtered": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int64,
+                                               POINTER(SearchFilter), c_void_p]),
+    "om_index_range_search_sharded_filtered": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                                       c_int, c_int64, POINTER(SearchFilter), c_void_p]),
     "om_index_range_results": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p]),
     "om_index_set_param": (c_int, [c_void_p, c_char_p, c_int64]),
     "om_index_get_stat": (c_int64, [c_void_p, c_char_p]),

@@ -819,17 +819,22 @@ __global__ void range_fold_kernel(int* __restrict__ count, int* __restrict__ fil
 // RE-SCORE and CUT: one warp per candidate (grid.y = query), the query in shared memory, the score of FINAL (row_dot).  A
 // candidate becomes make_key(s, row) if s > rho, else 0, which is no row's key and sorts last; surv counts the kept ones.
 // Queries whose list overflowed (total > C) are swept again and skipped here.
-template <typename RowT>
+// FILTER: candidates whose rows the query excludes (ex, <= kMaxExcluded ids in shared memory after the query) become 0
+// before their re-score and are not counted, as finalize_kernel<RowT, true> drops them.
+template <typename RowT, bool FILTER = false>
 __global__ void __launch_bounds__(256, 4) range_rescore_kernel(unsigned long long* __restrict__ cand, const int* __restrict__ count,
                                                             const long long* __restrict__ total, int C,
                                                             const float* __restrict__ qf, const RowT* __restrict__ xs, int d,
-                                                            const float* __restrict__ rho, int* __restrict__ surv) {
+                                                            const float* __restrict__ rho, int* __restrict__ surv, Excluded ex) {
   extern __shared__ float4 rsm[];
   float* sq = reinterpret_cast<float*>(rsm);
   const int q = blockIdx.y;
   const int cnt = count[q];
   if (total[q] > C || static_cast<int>(blockIdx.x) * 8 >= cnt) return;
   for (int i = threadIdx.x; i < d; i += blockDim.x) sq[i] = qf[static_cast<size_t>(q) * d + i];
+  uint32_t* sx = reinterpret_cast<uint32_t*>(sq + d);
+  int nx = 0;
+  if constexpr (FILTER) nx = ex.load(q, sx, 1, threadIdx.x, blockDim.x);
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const float r = rho[q];
@@ -837,6 +842,14 @@ __global__ void __launch_bounds__(256, 4) range_rescore_kernel(unsigned long lon
   int kept = 0;
   for (int j = blockIdx.x * 8 + warp; j < cnt; j += gridDim.x * 8) {
     const uint32_t row = key_row(mine[j]);
+    if constexpr (FILTER) {
+      bool hit = false;
+      for (int e = lane; e < nx; e += 32) hit |= sx[e] == row;
+      if (__any_sync(0xffffffffu, hit)) {
+        if (lane == 0) mine[j] = 0ull;
+        continue;
+      }
+    }
     const float s = row_dot(xs, row, d, sq, lane);
     const bool keep = s > r;
     if (lane == 0) mine[j] = keep ? make_key(s, row) : 0ull;
@@ -1669,6 +1682,8 @@ int once_attrs(const om_index* ix) {
     OM_CUDA(cudaFuncSetAttribute(exact_scan_kernel<8, 2, RowT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                  96 * 1024 + 8 * kMaxExcluded * 4));
     OM_CUDA(cudaFuncSetAttribute(range_rescore_kernel<RowT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 4));
+    OM_CUDA(cudaFuncSetAttribute(range_rescore_kernel<RowT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                 16384 * 4 + kMaxExcluded * 4));
     rows_done = true;
     return 0;
   });
@@ -2371,9 +2386,12 @@ struct RangeSweep {
 // One sweep of a range search over queries list[0, m) (rows of qf / rho) with lists of C keys: mode 0 the tensor-core
 // scan at t(q), mode 1 the exact scan at rho; then re-score, cut and sort of every list that holds all its query's
 // candidates.  One host synchronisation; the answered queries' sorted keys are appended to ix->rkeys at *stored, and
-// src[g] / cnt[g] record where and how many for query g.
+// src[g] / cnt[g] record where and how many for query g.  f: nullptr, or a checked filter with at least one part; the
+// scans then store allowed rows only (the exact scan also drops excluded ids), and the re-score drops excluded ids.
+// Exclusions are read through the uploaded list (qmap: sweep query i is the caller's query list[i]), as ids id_offset + row.
 int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vector<int>& list, int mode, int C, int sms,
-                int64_t* stored, std::vector<int64_t>& src, std::vector<int64_t>& cnt, RangeSweep& r, cudaStream_t st) {
+                const om_search_filter* f, int64_t id_offset, int64_t* stored, std::vector<int64_t>& src,
+                std::vector<int64_t>& cnt, RangeSweep& r, cudaStream_t st) {
   const int m = static_cast<int>(list.size()), d = ix->d;
   const size_t M = m;
   const bool long_lists = C > kRangeSortKeys;
@@ -2403,6 +2421,11 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
   L.C = C;
   L.mode = mode;
   L.qf = q;
+  if (f) {
+    L.allow = f->allow_bits;
+    L.ex = Excluded{f->exclude_offsets, f->exclude_ids, dlist, 0, id_offset};
+  }
+  const bool exclude = L.ex.off != nullptr;
   OM_TRY(gather_listed(list, dlist, qf, d, q, st));
   gather_rows_kernel<<<grid_for(m, 256), 256, 0, st>>>(rho, dlist, m, 1, rq);
   OM_CUDA(cudaGetLastError());
@@ -2428,8 +2451,9 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
       using RowT = std::decay_t<decltype(*xs)>;
       // at least 32 CTAs per query, more when few queries would leave SMs idle (a handful of long lists)
       const int gx = std::min((C + 63) / 64, std::max(32, (8 * sms + m - 1) / m));
-      range_rescore_kernel<RowT><<<dim3(gx, m), 256, static_cast<size_t>(d) * 4, st>>>(
-          L.cand, L.count, total, C, q, xs, d, rq, surv);
+      const auto kernel = exclude ? range_rescore_kernel<RowT, true> : range_rescore_kernel<RowT>;
+      kernel<<<dim3(gx, m), 256, static_cast<size_t>(d) * 4 + (exclude ? kMaxExcluded * 4 : 0), st>>>(
+          L.cand, L.count, total, C, q, xs, d, rq, surv, exclude ? L.ex : Excluded{});
     });
     int P = 2;
     while (P < std::min(C, kRangeSortKeys)) P <<= 1;
@@ -2481,9 +2505,9 @@ int range_sweep(om_index* ix, const float* qf, const float* rho, const std::vect
 // overflowed their list are swept again in groups that fit the device, with lists sized from their counts (a re-sweep may
 // run another scan kernel, whose stage scores can differ in the last bit: hence the head-room and a bounded number of
 // attempts); queries without a finite certificate bound are swept by the exact scan.  cnt[g] rows above rho for query g
-// end sorted at ix->rkeys + src[g]; *stored keys in all.
-int range_local(om_index* ix, const float* qf, const float* rho, int nq, std::vector<int64_t>& src, std::vector<int64_t>& cnt,
-                int64_t* stored, cudaStream_t st) {
+// end sorted at ix->rkeys + src[g]; *stored keys in all.  f: as for range_sweep, every sweep's.
+int range_local(om_index* ix, const float* qf, const float* rho, int nq, const om_search_filter* f, int64_t id_offset,
+                std::vector<int64_t>& src, std::vector<int64_t>& cnt, int64_t* stored, cudaStream_t st) {
   const int sms = device_sm_count();
   if (sms < 0) return sms;
   struct Job {
@@ -2505,7 +2529,7 @@ int range_local(om_index* ix, const float* qf, const float* rho, int nq, std::ve
   for (size_t j = 0; j < jobs.size(); ++j) {
     const Job job = jobs[j];  // a copy: jobs grows below
     RangeSweep r;
-    OM_TRY(range_sweep(ix, qf, rho, job.qs, job.mode, job.C, sms, stored, src, cnt, r, st));
+    OM_TRY(range_sweep(ix, qf, rho, job.qs, job.mode, job.C, sms, f, id_offset, stored, src, cnt, r, st));
     std::vector<int> exact;
     std::vector<std::pair<long long, int>> over;  // (candidates, query)
     for (size_t i = 0; i < job.qs.size(); ++i) {
@@ -2543,9 +2567,9 @@ int range_local(om_index* ix, const float* qf, const float* rho, int nq, std::ve
 // The whole range search, unsharded or this rank's part of a sharded one: argument rules (a NaN radius, fp16 / int8 rows
 // holding inf or NaN) checked before anything is written, the shard's results, then with several ranks one all-gather of
 // the per-query counts, one all-gather of every shard's sorted results (padded to the largest) and the merge.  The lims
-// go to the caller, the results stay in the index (rout).
+// go to the caller, the results stay in the index (rout).  f: nullptr, or a checked filter with at least one part.
 int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, const float* radius, int64_t* lims,
-               om_memkind out_kind, int64_t id_offset, cudaStream_t st) {
+               om_memkind out_kind, int64_t id_offset, const om_search_filter* f, cudaStream_t st) {
   NvtxRange nvtx("om.range_search");
   // the sharded entry runs the exchange at every world size, one rank included
   const bool sharded = comm != nullptr;
@@ -2571,7 +2595,7 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
 
   std::vector<int64_t> src, cnt;
   int64_t stored = 0;
-  int rc = range_local(ix, qf, rho, nq, src, cnt, &stored, st);
+  int rc = range_local(ix, qf, rho, nq, f, id_offset, src, cnt, &stored, st);
   // Every rank takes the same decision after a step that can fail on one rank alone (a re-sweep, an allocation): the
   // largest error code of all ranks, through one all-reduce, before the next collective.
   auto agree = [&](int rc_local) -> int {
@@ -2687,9 +2711,16 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
   return 0;
 }
 
-int range_entry(bool sharded, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, const float* radius,
-                int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream) {
-  const char* who = sharded ? "om_index_range_search_sharded" : "om_index_range_search";
+// The four exported range searches, as search_entry: the filter is checked when it has a part and, through the sharded
+// filtered entry with more than one rank, always (one all-reduce with every rank's filter, null or empty ones included);
+// the check comes before anything is written.  Any other call is the plain range search.
+int range_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
+                void* stream) {
+  const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
+  const bool check = local || (filtered && sharded && comm && comm->world > 1);
+  const char* who = sharded ? (check ? "om_index_range_search_sharded_filtered" : "om_index_range_search_sharded")
+                            : (check ? "om_index_range_search_filtered" : "om_index_range_search");
   if (!ix || (sharded && !comm) || nq < 0 || !lims || (nq > 0 && (!q || !radius)))
     return fail(OM_EINVAL, "%s: bad arguments (nq=%d)", who, nq);
   if (ix->window) return fail(OM_EINVAL, "%s: range search is not available on a host-resident index", who);
@@ -2707,20 +2738,33 @@ int range_entry(bool sharded, om_index* ix, om_comm* comm, const void* q, om_mem
     return 0;
   }
   OM_TRY(settle_reset(ix, st));
-  return range_impl(ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, st);
+  if (check) OM_TRY(check_filter(ix, comm, filter, nq, st));
+  return range_impl(ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, local ? filter : nullptr, st);
 }
 
 }  // namespace
 
 extern "C" int om_index_range_search(om_index* ix, const void* q, om_memkind q_kind, int nq, const float* radius,
                                      int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream) {
-  return range_entry(false, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, stream);
+  return range_entry(false, false, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, nullptr, stream);
+}
+
+extern "C" int om_index_range_search_filtered(om_index* ix, const void* q, om_memkind q_kind, int nq, const float* radius,
+                                              int64_t* lims, om_memkind out_kind, int64_t id_offset,
+                                              const om_search_filter* filter, void* stream) {
+  return range_entry(false, true, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, filter, stream);
 }
 
 extern "C" int om_index_range_search_sharded(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                              const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset,
                                              void* stream) {
-  return range_entry(true, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, stream);
+  return range_entry(true, false, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, nullptr, stream);
+}
+
+extern "C" int om_index_range_search_sharded_filtered(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
+                                                      const float* radius, int64_t* lims, om_memkind out_kind,
+                                                      int64_t id_offset, const om_search_filter* filter, void* stream) {
+  return range_entry(true, true, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, filter, stream);
 }
 
 extern "C" int om_index_range_results(const om_index* ix, float* D, int64_t* I, om_memkind out_kind, void* stream) {

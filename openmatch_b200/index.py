@@ -294,35 +294,54 @@ class FlatIPIndex:
                      _lib.OM_HOST, id_offset)
 
     # ---- range search ----
-    def range_search(self, q, radius, id_offset: int = 0) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    def range_search(self, q, radius, id_offset: int = 0, allow=None,
+                     exclude=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """``lims, D, I = index.range_search(q, radius)`` (faiss's signature): for query i every row whose score is
         strictly greater than ``radius`` (a float, or one per query), at ``D[lims[i]:lims[i + 1]]`` /
         ``I[lims[i]:lims[i + 1]]`` ordered by (score desc, id asc).  The first j results of a query are bitwise
-        ``search(q, j)``'s for j <= 4096.  numpy outputs (int64 [nq + 1], float32, int64)."""
+        ``search(q, j)``'s for j <= 4096.  numpy outputs (int64 [nq + 1], float32, int64).
+
+        ``allow`` / ``exclude``: the filter of :meth:`search` (``om_index_range_search_filtered``).  The result is then
+        every eligible row above the radius, bitwise what an index of the eligible rows alone returns with ids mapped
+        back, and its first j results are ``search(q, j, allow=allow, exclude=exclude)``'s.  ``None`` keeps the
+        unfiltered range search."""
         if not isinstance(q, torch.Tensor):
             q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        lims, D, I = self.range_search_device(q.cuda(), radius, id_offset)
+        lims, D, I = self.range_search_device(q.cuda(), radius, id_offset, allow=allow, exclude=exclude)
         return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()
 
-    def range_search_device(self, q: torch.Tensor, radius, id_offset: int = 0):
-        """:meth:`range_search` with CUDA tensors in and out: (lims int64 [nq + 1], D float32, I int64)."""
-        return self._range(None, q, radius, id_offset)
+    def range_search_device(self, q: torch.Tensor, radius, id_offset: int = 0, allow=None, exclude=None):
+        """:meth:`range_search` with CUDA tensors in and out: (lims int64 [nq + 1], D float32, I int64).  ``allow`` /
+        ``exclude``: the filter of :meth:`range_search`, packed on the query's device."""
+        return self._range(None, q, radius, id_offset, allow, exclude)
 
-    def range_search_sharded_device(self, comm: "Comm", q: torch.Tensor, radius, id_offset: int = 0):
+    def range_search_sharded_device(self, comm: "Comm", q: torch.Tensor, radius, id_offset: int = 0, allow=None,
+                                    exclude=None):
         """This rank's call of the row-sharded range search (``om_index_range_search_sharded``): collective over
-        ``comm``; every rank passes the same queries and radii and receives the same global (lims, D, I)."""
-        return self._range(comm, q, radius, id_offset)
+        ``comm``; every rank passes the same queries and radii and receives the same global (lims, D, I).  ``allow``
+        covers THIS rank's rows and ``exclude`` holds global ids, as for :meth:`search_sharded_device`; every rank
+        passes a filter or none does."""
+        return self._range(comm, q, radius, id_offset, allow, exclude)
 
-    def _range(self, comm, q: torch.Tensor, radius, id_offset: int):
+    def _range(self, comm, q: torch.Tensor, radius, id_offset: int, allow=None, exclude=None):
+        """One range search call of the C ABI: ``om_index_range_search``, ``_sharded`` with ``comm``, ``_filtered``
+        with a filter; an unfiltered call never takes a ``_filtered`` entry."""
         q = q.detach().contiguous().float()
         self._check_shape(q.shape)
         nq = q.shape[0]
         rho = range_radius(radius, nq, q.device)
+        f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         lims = torch.empty(nq + 1, dtype=torch.int64)
-        head = (self._h,) if comm is None else (self._h, comm._h)
-        fn = self._lib.om_index_range_search if comm is None else self._lib.om_index_range_search_sharded
+        lib = self._lib
+        if comm is None:
+            head = (self._h,)
+            fn = lib.om_index_range_search if f is None else lib.om_index_range_search_filtered
+        else:
+            head = (self._h, comm._h)
+            fn = lib.om_index_range_search_sharded if f is None else lib.om_index_range_search_sharded_filtered
+        tail = (_stream(),) if f is None else (ctypes.byref(f), _stream())
         _lib.check(fn(*head, q.data_ptr(), _lib.OM_DEVICE, nq, rho.data_ptr(), lims.data_ptr(), _lib.OM_HOST,
-                      int(id_offset), _stream()))
+                      int(id_offset), *tail))
         total = int(lims[-1])
         D = torch.empty(total, dtype=torch.float32, device=q.device)
         I = torch.empty(total, dtype=torch.int64, device=q.device)
@@ -485,14 +504,17 @@ def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offs
     return index.search_sharded_device(comm_for(group), q, k, id_offset, allow=allow, exclude=exclude)
 
 
-def sharded_range_search_device(index: "FlatIPIndex", q: torch.Tensor, radius, id_offset: int, group=None):
+def sharded_range_search_device(index: "FlatIPIndex", q: torch.Tensor, radius, id_offset: int, group=None, allow=None,
+                                exclude=None):
     """Row-sharded exact range search: every rank passes the same queries and radii and its own shard's ``id_offset``
     and receives the same global (lims, D, I), bitwise one index's range search over the concatenated shards.  Without
-    a process group, or with one rank: the single-shard range search."""
+    a process group, or with one rank: the single-shard range search.  ``allow`` (over global ids; each rank takes its
+    slice) and ``exclude`` (global ids) filter as in :meth:`FlatIPIndex.range_search`."""
     import torch.distributed as dist
+    allow = local_allow(allow, int(id_offset), index.ntotal, q.device)
     if not dist.is_initialized() or dist.get_world_size(group) == 1:
-        return index.range_search_device(q, radius, id_offset)
-    return index.range_search_sharded_device(comm_for(group), q, radius, id_offset)
+        return index.range_search_device(q, radius, id_offset, allow=allow, exclude=exclude)
+    return index.range_search_sharded_device(comm_for(group), q, radius, id_offset, allow=allow, exclude=exclude)
 
 
 def shard_offsets(n_local: int, group=None):
@@ -542,12 +564,13 @@ class ShardedFlatIPIndex:
         D, I = self.search_device(q.cuda(), k, allow=allow, exclude=exclude)
         return D.cpu().numpy(), I.cpu().numpy()
 
-    def range_search_device(self, q: torch.Tensor, radius):
-        return sharded_range_search_device(self.local, q, radius, self.offset, self.group)
+    def range_search_device(self, q: torch.Tensor, radius, allow=None, exclude=None):
+        """``allow``: bitmap over the global ids (each rank uses its slice); ``exclude``: global ids per query."""
+        return sharded_range_search_device(self.local, q, radius, self.offset, self.group, allow=allow, exclude=exclude)
 
-    def range_search(self, q, radius):
+    def range_search(self, q, radius, allow=None, exclude=None):
         """(lims, D, I) numpy over the global ids, the same on every rank."""
         if not isinstance(q, torch.Tensor):
             q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        lims, D, I = self.range_search_device(q.cuda(), radius)
+        lims, D, I = self.range_search_device(q.cuda(), radius, allow=allow, exclude=exclude)
         return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()

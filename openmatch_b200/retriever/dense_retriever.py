@@ -409,27 +409,37 @@ class Retriever:
         result = RankArrays(self.query_lookup, names, D.cpu().numpy(), I.cpu().numpy())
         return result if as_arrays else result.to_dict()
 
-    def range_search(self, radius):
+    def range_search(self, radius, allowed_docs=None, exclude=None):
         """Every document whose score is strictly above ``radius`` (a float, or one per query in query order) as
         ``{qid: {docid: score}}``, each query's documents in rank order (``FlatIPIndex.range_search``).  Sharded: every
-        rank takes part and rank 0 builds the result; the other ranks return ``{}``."""
+        rank takes part and rank 0 builds the result; the other ranks return ``{}``.
+
+        ``allowed_docs`` / ``exclude`` filter as in :meth:`search`: only the allowed documents, less each query's
+        excluded ones (at most 128 per query, e.g. the query itself in near-duplicate detection), are returned."""
         if self.index is None:
             raise ValueError("Index is not initialized")
         encoded = self._load_queries()
         radius = range_radius(radius, encoded.shape[0]).numpy()
         if self.args.world_size > 1:
-            return self._range_search_sharded(encoded, radius)
-        lims, D, I = self.index.range_search(encoded, radius)
+            return self._range_search_sharded(encoded, radius, allowed_docs, exclude)
+        if allowed_docs is None and exclude is None:
+            lims, D, I = self.index.range_search(encoded, radius)
+        else:
+            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude)
+            lims, D, I = self.index.range_search(encoded, radius, allow=allow, exclude=excluded)
         return _range_dict(self.query_lookup, np.array(self.doc_lookup), lims, D, I)
 
-    def _range_search_sharded(self, encoded: np.ndarray, radius: np.ndarray):
+    def _range_search_sharded(self, encoded: np.ndarray, radius: np.ndarray, allowed_docs=None, exclude=None):
         dist = torch.distributed
         W, r = self.args.world_size, self.args.process_index
         if self.index is None:  # this rank holds no rows (fewer embedding files than ranks)
             self._initialize_faiss_index(encoded.shape[1])
         offset, _ = shard_offsets(len(self.doc_lookup))
         q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
-        lims, D, I = self.index.range_search_sharded_device(comm_for(None), q, torch.from_numpy(radius), offset)
+        # each rank maps the filter on its own rows, as _search_sharded does
+        allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
+        lims, D, I = self.index.range_search_sharded_device(comm_for(None), q, torch.from_numpy(radius), offset,
+                                                            allow=allow, exclude=excluded)
         lookups = [None] * W if r == 0 else None
         dist.gather_object(self.doc_lookup, lookups, dst=0)
         if r != 0:
