@@ -2326,33 +2326,6 @@ int search_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, i
   return 0;
 }
 
-// The four exported searches: sharded, the entries that take a communicator (required); filtered, the _filtered entries.
-// The filter is checked before the search when it has a part and, through the sharded entry with more than one rank,
-// always: every rank checks the filters together (one all-reduce), also a rank whose filter is null or empty, so the
-// ranks' collectives stay in step when only some pass a filter.  Any other call is the plain search, and its messages
-// name the plain entry.
-int search_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
-                 float* D, int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter, void* stream) {
-  if (ix && ix->window && sharded)  // refused before the communicator is read
-    return fail(OM_EINVAL, "%s: a host-resident index cannot be a shard of a sharded search",
-                filtered ? "om_index_search_sharded_filtered" : "om_index_search_sharded");
-  const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
-  const bool check = local || (filtered && comm && comm->world > 1);
-  const char* who = sharded ? (check ? "om_index_search_sharded_filtered" : "om_index_search_sharded")
-                            : (check ? "om_index_search_filtered" : "om_index_search");
-  if (!ix || (sharded && !comm) || (nq > 0 && (!q || !D || !I)) || nq < 0 || k <= 0)
-    return fail(OM_EINVAL, "%s: bad arguments (nq=%d k=%d)", who, nq, k);
-  ix->r_total = -1;  // a search ends the last range search's results
-  ix->rout.release();
-  if (nq == 0) return 0;
-  OM_TRY(device_sm_count());
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  OM_TRY(settle_reset(ix, st));
-  if (comm && comm->world == 1) comm = nullptr;  // one rank: no collective, the single-shard search
-  if (check) OM_TRY(check_filter(ix, comm, filter, nq, st));
-  return search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, local ? filter : nullptr, st);
-}
-
 // ---- range search ---------------------------------------------------------------------------------------------------
 // A list count starts a round at most kRangeMaxList (its fill) and a round adds at most kRangeRound: 2^30 + 2^29 < 2^31, so
 // the scans' int counters cannot wrap.
@@ -2711,23 +2684,40 @@ int range_impl(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, in
   return 0;
 }
 
-// The four exported range searches, as search_entry: the filter is checked when it has a part and, through the sharded
-// filtered entry with more than one rank, always (one all-reduce with every rank's filter, null or empty ones included);
-// the check comes before anything is written.  Any other call is the plain range search.
-int range_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
-                const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
-                void* stream) {
+// The eight exported searches: a top-k search or a range search (range), sharded (the entries that take a
+// communicator, required) or not, filtered (the _filtered entries) or not.  The filter is checked before the search when
+// it has a part and, through a sharded filtered entry with more than one rank, always: every rank checks the filters
+// together (one all-reduce), also a rank whose filter is null or empty, so the ranks' collectives stay in step when only
+// some pass a filter.  Any other call is the unfiltered search, and its messages name the unfiltered entry.  What differs
+// by kind: a top-k search refuses a host-resident index only as a shard, before the communicator is read, needs k > 0,
+// ends the last range search's results and drops a one-rank communicator (no collective); a range search refuses a
+// host-resident index always, needs lims and the radii, writes lims = {0} for nq = 0 and keeps its collectives at every
+// world size.
+int search_entry(bool range, bool sharded, bool filtered, om_index* ix, om_comm* comm, const void* q, om_memkind q_kind,
+                 int nq, int k, float* D, int64_t* I, const float* radius, int64_t* lims, om_memkind out_kind,
+                 int64_t id_offset, const om_search_filter* filter, void* stream) {
+  static const char* const kNames[2][2][2] = {  // [range][sharded][filtered]
+      {{"om_index_search", "om_index_search_filtered"}, {"om_index_search_sharded", "om_index_search_sharded_filtered"}},
+      {{"om_index_range_search", "om_index_range_search_filtered"},
+       {"om_index_range_search_sharded", "om_index_range_search_sharded_filtered"}}};
+  if (!range && sharded && ix && ix->window)  // refused before the communicator is read
+    return fail(OM_EINVAL, "%s: a host-resident index cannot be a shard of a sharded search", kNames[0][1][filtered]);
   const bool local = filter && (filter->allow_bits || filter->exclude_offsets);
-  const bool check = local || (filtered && sharded && comm && comm->world > 1);
-  const char* who = sharded ? (check ? "om_index_range_search_sharded_filtered" : "om_index_range_search_sharded")
-                            : (check ? "om_index_range_search_filtered" : "om_index_range_search");
-  if (!ix || (sharded && !comm) || nq < 0 || !lims || (nq > 0 && (!q || !radius)))
-    return fail(OM_EINVAL, "%s: bad arguments (nq=%d)", who, nq);
-  if (ix->window) return fail(OM_EINVAL, "%s: range search is not available on a host-resident index", who);
-  ix->r_total = -1;
+  const bool check = local || (filtered && comm && comm->world > 1);
+  const char* who = kNames[range][sharded][check];
+  const bool bad = range ? !lims || (nq > 0 && (!q || !radius)) : k <= 0 || (nq > 0 && (!q || !D || !I));
+  if (!ix || (sharded && !comm) || nq < 0 || bad)
+    return range ? fail(OM_EINVAL, "%s: bad arguments (nq=%d)", who, nq)
+                 : fail(OM_EINVAL, "%s: bad arguments (nq=%d k=%d)", who, nq, k);
+  if (range && ix->window) return fail(OM_EINVAL, "%s: range search is not available on a host-resident index", who);
+  ix->r_total = -1;  // the last range search's results end here
+  if (!range) {      // a search frees their buffer too; a range search reuses it
+    ix->rout.release();
+    if (nq == 0) return 0;
+  }
   OM_TRY(device_sm_count());
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (nq == 0) {  // lims = {0}, no results
+  if (nq == 0) {  // a range search: lims = {0}, no results
     if (out_kind == OM_HOST) {
       lims[0] = 0;
     } else {
@@ -2738,33 +2728,40 @@ int range_entry(bool sharded, bool filtered, om_index* ix, om_comm* comm, const 
     return 0;
   }
   OM_TRY(settle_reset(ix, st));
+  if (!range && comm && comm->world == 1) comm = nullptr;  // one rank: no collective, the single-shard search
   if (check) OM_TRY(check_filter(ix, comm, filter, nq, st));
-  return range_impl(ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, local ? filter : nullptr, st);
+  const om_search_filter* f = local ? filter : nullptr;
+  return range ? range_impl(ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, f, st)
+               : search_impl(ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, f, st);
 }
 
 }  // namespace
 
 extern "C" int om_index_range_search(om_index* ix, const void* q, om_memkind q_kind, int nq, const float* radius,
                                      int64_t* lims, om_memkind out_kind, int64_t id_offset, void* stream) {
-  return range_entry(false, false, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, nullptr, stream);
+  return search_entry(true, false, false, ix, nullptr, q, q_kind, nq, 0, nullptr, nullptr, radius, lims, out_kind, id_offset,
+                      nullptr, stream);
 }
 
 extern "C" int om_index_range_search_filtered(om_index* ix, const void* q, om_memkind q_kind, int nq, const float* radius,
                                               int64_t* lims, om_memkind out_kind, int64_t id_offset,
                                               const om_search_filter* filter, void* stream) {
-  return range_entry(false, true, ix, nullptr, q, q_kind, nq, radius, lims, out_kind, id_offset, filter, stream);
+  return search_entry(true, false, true, ix, nullptr, q, q_kind, nq, 0, nullptr, nullptr, radius, lims, out_kind, id_offset,
+                      filter, stream);
 }
 
 extern "C" int om_index_range_search_sharded(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                              const float* radius, int64_t* lims, om_memkind out_kind, int64_t id_offset,
                                              void* stream) {
-  return range_entry(true, false, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, nullptr, stream);
+  return search_entry(true, true, false, ix, comm, q, q_kind, nq, 0, nullptr, nullptr, radius, lims, out_kind, id_offset,
+                      nullptr, stream);
 }
 
 extern "C" int om_index_range_search_sharded_filtered(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                                       const float* radius, int64_t* lims, om_memkind out_kind,
                                                       int64_t id_offset, const om_search_filter* filter, void* stream) {
-  return range_entry(true, true, ix, comm, q, q_kind, nq, radius, lims, out_kind, id_offset, filter, stream);
+  return search_entry(true, true, true, ix, comm, q, q_kind, nq, 0, nullptr, nullptr, radius, lims, out_kind, id_offset,
+                      filter, stream);
 }
 
 extern "C" int om_index_range_results(const om_index* ix, float* D, int64_t* I, om_memkind out_kind, void* stream) {
@@ -2785,13 +2782,15 @@ extern "C" int om_index_range_results(const om_index* ix, float* D, int64_t* I, 
 
 extern "C" int om_index_search(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D, int64_t* I,
                                om_memkind out_kind, int64_t id_offset, void* stream) {
-  return search_entry(false, false, ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, stream);
+  return search_entry(false, false, false, ix, nullptr, q, q_kind, nq, k, D, I, nullptr, nullptr, out_kind, id_offset,
+                      nullptr, stream);
 }
 
 extern "C" int om_index_search_filtered(om_index* ix, const void* q, om_memkind q_kind, int nq, int k, float* D,
                                         int64_t* I, om_memkind out_kind, int64_t id_offset, const om_search_filter* filter,
                                         void* stream) {
-  return search_entry(false, true, ix, nullptr, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, stream);
+  return search_entry(false, false, true, ix, nullptr, q, q_kind, nq, k, D, I, nullptr, nullptr, out_kind, id_offset,
+                      filter, stream);
 }
 
 // ---- row-sharded search with the exchange inside the library (NCCL over NVLink) -----------------------------------
@@ -2833,13 +2832,15 @@ extern "C" void om_comm_destroy(om_comm* c) {
 
 extern "C" int om_index_search_sharded(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq, int k,
                                        float* D, int64_t* I, om_memkind out_kind, int64_t id_offset, void* stream) {
-  return search_entry(true, false, ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, nullptr, stream);
+  return search_entry(false, true, false, ix, comm, q, q_kind, nq, k, D, I, nullptr, nullptr, out_kind, id_offset,
+                      nullptr, stream);
 }
 
 extern "C" int om_index_search_sharded_filtered(om_index* ix, om_comm* comm, const void* q, om_memkind q_kind, int nq,
                                                 int k, float* D, int64_t* I, om_memkind out_kind, int64_t id_offset,
                                                 const om_search_filter* filter, void* stream) {
-  return search_entry(true, true, ix, comm, q, q_kind, nq, k, D, I, out_kind, id_offset, filter, stream);
+  return search_entry(false, true, true, ix, comm, q, q_kind, nq, k, D, I, nullptr, nullptr, out_kind, id_offset,
+                      filter, stream);
 }
 
 extern "C" int om_topk_merge_n(const float* D_parts, const int64_t* I_parts, int nparts, int nq, int k_in, int k_out,

@@ -106,6 +106,13 @@ def _filter(n: int, nq: int, device, allow, exclude):
     return f, keep
 
 
+def _cuda_queries(q) -> torch.Tensor:
+    """Queries given as a numpy array or a tensor, as a contiguous float32 tensor on the current CUDA device."""
+    if not isinstance(q, torch.Tensor):
+        q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
+    return q.detach().cuda().contiguous().float()
+
+
 def range_radius(radius, nq: int, device=None) -> torch.Tensor:
     """The per-query radii of a range search as float32 ``[nq]``: a number is broadcast, an array must hold ``nq``."""
     if isinstance(radius, (int, float, np.floating, np.integer)):
@@ -208,13 +215,8 @@ class FlatIPIndex:
         query (a list of ``nq`` id lists, or an ``(offsets, ids)`` CSR pair; at most 128 ids per query; ids are
         ``id_offset`` + row).  The result is the exact top-k among the eligible rows, bitwise what an index of those rows
         alone returns with ids mapped back; missing slots hold id -1.  ``None`` keeps the unfiltered search."""
-        if allow is not None or exclude is not None:
-            if not isinstance(q, torch.Tensor):
-                q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-            D, I = self.search_device(q.cuda(), k, id_offset, allow=allow, exclude=exclude)
-            return D.cpu().numpy(), I.cpu().numpy()
-        if isinstance(q, torch.Tensor) and q.is_cuda:
-            D, I = self.search_device(q, k, id_offset)
+        if allow is not None or exclude is not None or (isinstance(q, torch.Tensor) and q.is_cuda):
+            D, I = self.search_device(_cuda_queries(q), k, id_offset, allow=allow, exclude=exclude)
             return D.cpu().numpy(), I.cpu().numpy()
         if isinstance(q, torch.Tensor):
             q = q.detach().cpu().numpy()
@@ -223,22 +225,18 @@ class FlatIPIndex:
         nq = q.shape[0]
         D = np.empty((nq, k), dtype=np.float32)
         I = np.empty((nq, k), dtype=np.int64)
-        self._search(None, q.ctypes.data, _lib.OM_HOST, nq, k, D.ctypes.data, I.ctypes.data, _lib.OM_HOST, id_offset)
+        self._call("search", None, None, q.ctypes.data, _lib.OM_HOST, nq, int(k), D.ctypes.data, I.ctypes.data,
+                   _lib.OM_HOST, int(id_offset))
         return D, I
 
-    def _search(self, comm, q_ptr, q_kind, nq, k, D_ptr, I_ptr, out_kind, id_offset, f=None) -> None:
-        """One search call of the C ABI: ``om_index_search``, ``_sharded`` with ``comm``, ``_filtered`` with the
-        filter ``f``.  An unfiltered call never takes a ``_filtered`` entry: with more than one rank that would add a
-        collective filter check."""
-        lib = self._lib
-        if comm is None:
-            head = (self._h,)
-            fn = lib.om_index_search if f is None else lib.om_index_search_filtered
-        else:
-            head = (self._h, comm._h)
-            fn = lib.om_index_search_sharded if f is None else lib.om_index_search_sharded_filtered
+    def _call(self, kind: str, comm, f, *args) -> None:
+        """One call of the C ABI's ``om_index_<kind>`` (``search`` or ``range_search``), ``_sharded`` with ``comm``,
+        ``_filtered`` with the filter ``f``; ``args`` go between the handles and the filter.  An unfiltered call never
+        takes a ``_filtered`` entry: with more than one rank that would add a collective filter check."""
+        name = "om_index_" + kind + ("" if comm is None else "_sharded") + ("" if f is None else "_filtered")
+        head = (self._h,) if comm is None else (self._h, comm._h)
         tail = (_stream(),) if f is None else (ctypes.byref(f), _stream())
-        _lib.check(fn(*head, q_ptr, q_kind, nq, int(k), D_ptr, I_ptr, out_kind, int(id_offset), *tail))
+        _lib.check(getattr(self._lib, name)(*head, *args, *tail))
 
     # ---- device-resident variants ----
     @staticmethod
@@ -256,13 +254,7 @@ class FlatIPIndex:
                       exclude=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """``out=(D, I)``: write into caller-owned CUDA tensors (no allocation on the search path).  ``allow`` /
         ``exclude``: the filter of :meth:`search`, packed on the query's device."""
-        q = q.contiguous().float()
-        self._check_shape(q.shape)
-        nq = q.shape[0]
-        f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
-        D, I = self._outputs(nq, int(k), q.device, out)
-        self._search(None, q.data_ptr(), _lib.OM_DEVICE, nq, k, D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, id_offset, f)
-        return D, I
+        return self._search(None, q, k, id_offset, allow, exclude, out)
 
     def search_sharded_device(self, comm: "Comm", q: torch.Tensor, k: int, id_offset: int = 0, out=None, allow=None,
                               exclude=None):
@@ -271,27 +263,34 @@ class FlatIPIndex:
         rank's rows (``ntotal`` of them); ``exclude`` holds global ids and may be the same on every rank.  Every rank
         passes a filter or none does; a rank's filter may be empty (a shard without rows packs to no words), which
         still takes the filtered call, so the ranks' collectives stay in step."""
-        q = q.contiguous().float()
+        return self._search(comm, q, k, id_offset, allow, exclude, out)
+
+    def _search(self, comm, q: torch.Tensor, k: int, id_offset: int, allow, exclude, out=None):
+        q = q.detach().contiguous().float()
         self._check_shape(q.shape)
-        nq = q.shape[0]
+        nq, k = q.shape[0], int(k)
         f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
-        D, I = self._outputs(nq, int(k), q.device, out)
-        self._search(comm, q.data_ptr(), _lib.OM_DEVICE, nq, k, D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE, id_offset, f)
+        D, I = self._outputs(nq, k, q.device, out)
+        self._call("search", comm, f, q.data_ptr(), _lib.OM_DEVICE, nq, k, D.data_ptr(), I.data_ptr(), _lib.OM_DEVICE,
+                   int(id_offset))
         return D, I
 
     def search_sharded_pinned(self, comm: "Comm", q_host: torch.Tensor, k: int, D_out: torch.Tensor, I_out: torch.Tensor,
                               id_offset: int = 0) -> None:
         """Host (pinned) queries in; results into ``D_out`` / ``I_out`` (pinned host on the rank that wants them,
         device tensors elsewhere)."""
-        kind = _lib.OM_DEVICE if D_out.is_cuda else _lib.OM_HOST
-        self._search(comm, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], k, D_out.data_ptr(), I_out.data_ptr(), kind,
-                     id_offset)
+        self._search_pinned(comm, q_host, k, D_out, I_out, id_offset)
 
     def search_pinned(self, q_host: torch.Tensor, k: int, D_host: torch.Tensor, I_host: torch.Tensor,
                       id_offset: int = 0) -> None:
         """Host (pinned) in, host (pinned) out — the end-to-end call the benchmark times."""
-        self._search(None, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], k, D_host.data_ptr(), I_host.data_ptr(),
-                     _lib.OM_HOST, id_offset)
+        self._search_pinned(None, q_host, k, D_host, I_host, id_offset)
+
+    def _search_pinned(self, comm, q_host: torch.Tensor, k: int, D_out: torch.Tensor, I_out: torch.Tensor,
+                       id_offset: int) -> None:
+        kind = _lib.OM_DEVICE if D_out.is_cuda else _lib.OM_HOST
+        self._call("search", comm, None, q_host.data_ptr(), _lib.OM_HOST, q_host.shape[0], int(k), D_out.data_ptr(),
+                   I_out.data_ptr(), kind, int(id_offset))
 
     # ---- range search ----
     def range_search(self, q, radius, id_offset: int = 0, allow=None,
@@ -305,9 +304,7 @@ class FlatIPIndex:
         every eligible row above the radius, bitwise what an index of the eligible rows alone returns with ids mapped
         back, and its first j results are ``search(q, j, allow=allow, exclude=exclude)``'s.  ``None`` keeps the
         unfiltered range search."""
-        if not isinstance(q, torch.Tensor):
-            q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        lims, D, I = self.range_search_device(q.cuda(), radius, id_offset, allow=allow, exclude=exclude)
+        lims, D, I = self.range_search_device(_cuda_queries(q), radius, id_offset, allow=allow, exclude=exclude)
         return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()
 
     def range_search_device(self, q: torch.Tensor, radius, id_offset: int = 0, allow=None, exclude=None):
@@ -323,25 +320,15 @@ class FlatIPIndex:
         passes a filter or none does."""
         return self._range(comm, q, radius, id_offset, allow, exclude)
 
-    def _range(self, comm, q: torch.Tensor, radius, id_offset: int, allow=None, exclude=None):
-        """One range search call of the C ABI: ``om_index_range_search``, ``_sharded`` with ``comm``, ``_filtered``
-        with a filter; an unfiltered call never takes a ``_filtered`` entry."""
+    def _range(self, comm, q: torch.Tensor, radius, id_offset: int, allow, exclude):
         q = q.detach().contiguous().float()
         self._check_shape(q.shape)
         nq = q.shape[0]
         rho = range_radius(radius, nq, q.device)
         f, _keep = _filter(self.ntotal, nq, q.device, allow, exclude)
         lims = torch.empty(nq + 1, dtype=torch.int64)
-        lib = self._lib
-        if comm is None:
-            head = (self._h,)
-            fn = lib.om_index_range_search if f is None else lib.om_index_range_search_filtered
-        else:
-            head = (self._h, comm._h)
-            fn = lib.om_index_range_search_sharded if f is None else lib.om_index_range_search_sharded_filtered
-        tail = (_stream(),) if f is None else (ctypes.byref(f), _stream())
-        _lib.check(fn(*head, q.data_ptr(), _lib.OM_DEVICE, nq, rho.data_ptr(), lims.data_ptr(), _lib.OM_HOST,
-                      int(id_offset), *tail))
+        self._call("range_search", comm, f, q.data_ptr(), _lib.OM_DEVICE, nq, rho.data_ptr(), lims.data_ptr(), _lib.OM_HOST,
+                   int(id_offset))
         total = int(lims[-1])
         D = torch.empty(total, dtype=torch.float32, device=q.device)
         I = torch.empty(total, dtype=torch.int64, device=q.device)
@@ -497,11 +484,7 @@ def sharded_search_device(index: "FlatIPIndex", q: torch.Tensor, k: int, id_offs
     use whatever the group's backend.  Without a process group, or with one rank: the single-shard search.
     ``allow`` (over global ids; each rank takes its slice) and ``exclude`` (global ids) filter as in
     :meth:`FlatIPIndex.search`."""
-    import torch.distributed as dist
-    allow = local_allow(allow, int(id_offset), index.ntotal, q.device)
-    if not dist.is_initialized() or dist.get_world_size(group) == 1:
-        return index.search_device(q, k, id_offset=id_offset, allow=allow, exclude=exclude)
-    return index.search_sharded_device(comm_for(group), q, k, id_offset, allow=allow, exclude=exclude)
+    return _on_shards(index._search, index, q, k, id_offset, group, allow, exclude)
 
 
 def sharded_range_search_device(index: "FlatIPIndex", q: torch.Tensor, radius, id_offset: int, group=None, allow=None,
@@ -510,11 +493,17 @@ def sharded_range_search_device(index: "FlatIPIndex", q: torch.Tensor, radius, i
     and receives the same global (lims, D, I), bitwise one index's range search over the concatenated shards.  Without
     a process group, or with one rank: the single-shard range search.  ``allow`` (over global ids; each rank takes its
     slice) and ``exclude`` (global ids) filter as in :meth:`FlatIPIndex.range_search`."""
+    return _on_shards(index._range, index, q, radius, id_offset, group, allow, exclude)
+
+
+def _on_shards(call, index: "FlatIPIndex", q: torch.Tensor, arg, id_offset: int, group, allow, exclude):
+    """``call(comm, q, arg, id_offset, allow, exclude)`` (``FlatIPIndex._search`` or ``_range``) on this rank's shard,
+    with its slice of the bitmap ``allow``: without a process group, or with one rank, the single-shard call (``comm``
+    None), else the sharded one over the library's communicator for ``group``."""
     import torch.distributed as dist
     allow = local_allow(allow, int(id_offset), index.ntotal, q.device)
-    if not dist.is_initialized() or dist.get_world_size(group) == 1:
-        return index.range_search_device(q, radius, id_offset, allow=allow, exclude=exclude)
-    return index.range_search_sharded_device(comm_for(group), q, radius, id_offset, allow=allow, exclude=exclude)
+    sharded = dist.is_initialized() and dist.get_world_size(group) > 1
+    return call(comm_for(group) if sharded else None, q, arg, id_offset, allow, exclude)
 
 
 def shard_offsets(n_local: int, group=None):
@@ -559,9 +548,7 @@ class ShardedFlatIPIndex:
         return sharded_search_device(self.local, q, k, self.offset, self.group, allow=allow, exclude=exclude)
 
     def search(self, q, k: int, allow=None, exclude=None):
-        if not isinstance(q, torch.Tensor):
-            q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        D, I = self.search_device(q.cuda(), k, allow=allow, exclude=exclude)
+        D, I = self.search_device(_cuda_queries(q), k, allow=allow, exclude=exclude)
         return D.cpu().numpy(), I.cpu().numpy()
 
     def range_search_device(self, q: torch.Tensor, radius, allow=None, exclude=None):
@@ -570,7 +557,5 @@ class ShardedFlatIPIndex:
 
     def range_search(self, q, radius, allow=None, exclude=None):
         """(lims, D, I) numpy over the global ids, the same on every rank."""
-        if not isinstance(q, torch.Tensor):
-            q = torch.from_numpy(np.ascontiguousarray(q, dtype=np.float32))
-        lims, D, I = self.range_search_device(q.cuda(), radius, allow=allow, exclude=exclude)
+        lims, D, I = self.range_search_device(_cuda_queries(q), radius, allow=allow, exclude=exclude)
         return lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy()

@@ -375,38 +375,14 @@ class Retriever:
         most 128 per query) drops documents per query, e.g. the query's positives or the query itself; the ranking is the
         exact top-k among the remaining documents (``FlatIPIndex.search``'s filter).  Unknown doc ids are ignored."""
         logger.info("Searching")
-        if self.index is None:
-            raise ValueError("Index is not initialized")
-        encoded = self._load_queries()
-        if self.args.world_size > 1:
-            return self._search_sharded(encoded, topk, as_arrays, allowed_docs, exclude)
-        if allowed_docs is None and exclude is None:
-            D, I = self.index.search(encoded, topk)
-        else:
-            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude)
-            D, I = self.index.search(encoded, topk, allow=allow, exclude=excluded)
-        result = RankArrays(self.query_lookup, np.array(self.doc_lookup), D, I)
-        logger.info("End searching with %d queries", len(result))
-        return result if as_arrays else result.to_dict()
-
-    def _search_sharded(self, encoded: np.ndarray, topk: int, as_arrays: bool = False, allowed_docs=None, exclude=None):
-        """Every rank: all queries x local shard -> all-gather [nq, k] lists over NCCL -> merge; doc-id strings
-        are gathered to rank 0, which alone builds the result dict (like the reference, :200-203)."""
-        dist = torch.distributed
-        W, r = self.args.world_size, self.args.process_index
-        if self.index is None:  # this rank holds no rows (fewer embedding files than ranks)
-            self._initialize_faiss_index(encoded.shape[1])
-        offset, _ = shard_offsets(len(self.doc_lookup))
-        q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
-        # each rank maps the filter on its own rows (its slice of the bitmap, exclusions among its own documents)
-        allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
-        D, I = self.index.search_sharded_device(comm_for(None), q, topk, offset, allow=allow, exclude=excluded)
-        lookups = [None] * W if r == 0 else None
-        dist.gather_object(self.doc_lookup, lookups, dst=0)
-        if r != 0:
+        out = self._search_index(lambda q, **f: self.index.search(q, topk, **f),
+                                 lambda comm, q, offset, **f: self.index.search_sharded_device(comm, q, topk, offset, **f),
+                                 allowed_docs, exclude)
+        if out is None:
             return RankArrays([], [], None, None) if as_arrays else {}
-        names = np.array([d for part in lookups for d in part])
-        result = RankArrays(self.query_lookup, names, D.cpu().numpy(), I.cpu().numpy())
+        names, (D, I) = out
+        result = RankArrays(self.query_lookup, names, D, I)
+        logger.info("End searching with %d queries", len(result))
         return result if as_arrays else result.to_dict()
 
     def range_search(self, radius, allowed_docs=None, exclude=None):
@@ -416,36 +392,42 @@ class Retriever:
 
         ``allowed_docs`` / ``exclude`` filter as in :meth:`search`: only the allowed documents, less each query's
         excluded ones (at most 128 per query, e.g. the query itself in near-duplicate detection), are returned."""
+        def radii(q):
+            return range_radius(radius, q.shape[0]).numpy()
+
+        out = self._search_index(lambda q, **f: self.index.range_search(q, radii(q), **f),
+                                 lambda comm, q, offset, **f: self.index.range_search_sharded_device(
+                                     comm, q, torch.from_numpy(radii(q)), offset, **f),
+                                 allowed_docs, exclude)
+        if out is None:
+            return {}
+        names, (lims, D, I) = out
+        return _range_dict(self.query_lookup, names, lims, D, I)
+
+    def _search_index(self, local, sharded, allowed_docs, exclude):
+        """One search of the saved queries, with the filter mapped onto this rank's rows.  One process:
+        ``local(queries, **filter)`` with numpy queries and results.  ``world_size > 1``: every rank searches all queries
+        against its row shard, ``sharded(comm, queries, id_offset, **filter)`` with CUDA tensors, and the doc-id strings
+        are gathered to rank 0, which alone builds the result (like the reference, :200-203).  Returns (doc names, numpy
+        results), or None on the other ranks.  An unfiltered search passes no filter arguments."""
         if self.index is None:
             raise ValueError("Index is not initialized")
         encoded = self._load_queries()
-        radius = range_radius(radius, encoded.shape[0]).numpy()
-        if self.args.world_size > 1:
-            return self._range_search_sharded(encoded, radius, allowed_docs, exclude)
-        if allowed_docs is None and exclude is None:
-            lims, D, I = self.index.range_search(encoded, radius)
-        else:
-            allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude)
-            lims, D, I = self.index.range_search(encoded, radius, allow=allow, exclude=excluded)
-        return _range_dict(self.query_lookup, np.array(self.doc_lookup), lims, D, I)
-
-    def _range_search_sharded(self, encoded: np.ndarray, radius: np.ndarray, allowed_docs=None, exclude=None):
-        dist = torch.distributed
-        W, r = self.args.world_size, self.args.process_index
-        if self.index is None:  # this rank holds no rows (fewer embedding files than ranks)
-            self._initialize_faiss_index(encoded.shape[1])
-        offset, _ = shard_offsets(len(self.doc_lookup))
-        q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
-        # each rank maps the filter on its own rows, as _search_sharded does
+        W = self.args.world_size
+        offset = shard_offsets(len(self.doc_lookup))[0] if W > 1 else 0
+        # each rank maps the filter on its own rows (its slice of the bitmap, exclusions among its own documents)
         allow, excluded = doc_filter(self.doc_lookup, self.query_lookup, allowed_docs, exclude, offset)
-        lims, D, I = self.index.range_search_sharded_device(comm_for(None), q, torch.from_numpy(radius), offset,
-                                                            allow=allow, exclude=excluded)
-        lookups = [None] * W if r == 0 else None
-        dist.gather_object(self.doc_lookup, lookups, dst=0)
-        if r != 0:
-            return {}
-        names = np.array([d for part in lookups for d in part])
-        return _range_dict(self.query_lookup, names, lims.cpu().numpy(), D.cpu().numpy(), I.cpu().numpy())
+        f = {} if allow is None and excluded is None else {"allow": allow, "exclude": excluded}
+        if W <= 1:
+            return np.array(self.doc_lookup), local(encoded, **f)
+        q = torch.from_numpy(np.ascontiguousarray(encoded, dtype=np.float32)).to(self.args.device)
+        results = sharded(comm_for(None), q, offset, **f)
+        rank0 = self.args.process_index == 0
+        lookups = [None] * W if rank0 else None
+        torch.distributed.gather_object(self.doc_lookup, lookups, dst=0)
+        if not rank0:
+            return None
+        return np.array([d for part in lookups for d in part]), tuple(t.cpu().numpy() for t in results)
 
     def retrieve(self, query_dataset: IterableDataset, topk: int = 100, as_arrays: bool = False, allowed_docs=None,
                  exclude=None):
